@@ -571,7 +571,14 @@ __global__ void split_to_f32_kernel(const __half* __restrict__ x, long long npix
 }
 
 // ------------------------------------------------------------------ GroupNorm(+ReLU) for 8 channels per group (FCOS towers)
-// pass 1: per (image, group) sum and sum of squares (fp32 per thread over <= 64 values, double across threads)
+// pivot of (image b, group g): the group's first channel at the image's first pixel.  The sums are taken around it so that they stay at the
+// scale of the group's spread: E[x^2] - mean^2 would lose (mean / std)^2 times the fp32 accumulation error.
+__device__ __forceinline__ float gn_pivot(const __half* __restrict__ x, int b, int g, int npix, int xp, long long xplane) {
+  const size_t o = (size_t)b * npix * xp + g * 8;
+  return __half2float(x[o]) + __half2float(x[o + xplane]);
+}
+
+// pass 1: per (image, group) sum and sum of squares of x - pivot (fp32 per thread over <= 64 values, double across threads)
 __global__ void gn_stats_kernel(const __half* __restrict__ x, int npix, int C, int xp, long long xplane, double* __restrict__ stats) {
   const int groups = C / 8;
   const int b = blockIdx.y;
@@ -580,6 +587,7 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, int npix, int C, i
   const int pl = threadIdx.x / groups;
   const int chunk = (npix + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * chunk, p1 = min(npix, p0 + chunk);
+  const float k = gn_pivot(x, b, g, npix, xp, xplane);
   double s = 0.0, ss = 0.0;
   float fs = 0.0f, fss = 0.0f;
   int cnt = 0;
@@ -593,7 +601,7 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, int npix, int C, i
     for (int e = 0; e < 4; ++e) {
       const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[e]));
       const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(&lw[e]));
-      const float v0 = hf.x + lf.x, v1 = hf.y + lf.y;
+      const float v0 = (hf.x + lf.x) - k, v1 = (hf.y + lf.y) - k;
       fs += v0 + v1;
       fss += v0 * v0 + v1 * v1;
     }
@@ -621,9 +629,9 @@ __global__ void gn_apply_kernel(const __half* __restrict__ x, int npix, int C, i
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int g = (int)(i % groups);
     const long long p = i / groups;
-    const double m = stats[((size_t)b * groups + g) * 2] * inv_n;
-    const double var = fmax(stats[((size_t)b * groups + g) * 2 + 1] * inv_n - m * m, 0.0);
-    const float mean = (float)m, rstd = (float)(1.0 / sqrt(var + (double)eps));
+    const double d = stats[((size_t)b * groups + g) * 2] * inv_n;  // mean - pivot
+    const double var = fmax(stats[((size_t)b * groups + g) * 2 + 1] * inv_n - d * d, 0.0);
+    const float mean = (float)((double)gn_pivot(x, b, g, npix, xp, xplane) + d), rstd = (float)(1.0 / sqrt(var + (double)eps));
     const size_t o = ((size_t)b * npix + p) * xp + g * 8;
     const uint4 hv = __ldg(reinterpret_cast<const uint4*>(x + o));
     const uint4 lv = __ldg(reinterpret_cast<const uint4*>(x + o + xplane));

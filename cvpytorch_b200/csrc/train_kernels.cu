@@ -198,8 +198,9 @@ struct alignas(64) TWgradArgs {
   int tiles_w, tiles_h, tiles_b;  // over the OUTPUT pixels (dy)
   int TW, TH, NB;
   int cin, cout, taps;
-  int nblocks;  // cout / (64 * NPAN): output-channel blocks of one launch (cout = 512 runs as two 256-wide blocks), folded into blockIdx.z
+  int nblocks;  // cout / (64 * NPAN): output-channel blocks of one launch (cout = 512 runs as two 256-wide blocks, 192 as three 64-wide), folded into blockIdx.z
   int8_t tap_dh[9], tap_dw[9], tap_map[9];
+  int8_t tap_idx[9];  // filter tap (dw block) of grid row blockIdx.y; `taps` = k * k is the dw layout's
   int splits;
   float* dw;  // [cout][taps][cin] fp32, accumulated with atomics (zeroed by the caller)
 };
@@ -233,10 +234,10 @@ __global__ void __launch_bounds__(kTThreads, 1) twgrad_kernel(const __grid_const
   }
   __syncthreads();
 
-  const int split = blockIdx.x, tap = blockIdx.y, c0 = ((int)blockIdx.z / a.nblocks) * 128, n0 = ((int)blockIdx.z % a.nblocks) * N;
+  const int split = blockIdx.x, ti = blockIdx.y, tap = a.tap_idx[ti], c0 = ((int)blockIdx.z / a.nblocks) * 128, n0 = ((int)blockIdx.z % a.nblocks) * N;
   const int m_pan = (a.cin - c0) >= 128 ? 2 : 1;  // valid 64-channel panels of this cin block
-  const int dh = a.tap_dh[tap], dw_ = a.tap_dw[tap];
-  const CUtensorMap* mapX = &a.tmX[a.tap_map[tap]];
+  const int dh = a.tap_dh[ti], dw_ = a.tap_dw[ti];
+  const CUtensorMap* mapX = &a.tmX[a.tap_map[ti]];
   const int m_tiles = a.tiles_w * a.tiles_h * a.tiles_b;
   const int per = (m_tiles + a.splits - 1) / a.splits;
   const int t_begin = split * per, t_end = min(m_tiles, t_begin + per);
@@ -356,7 +357,9 @@ __device__ __forceinline__ void red_finish(float (&a1)[8], float (&a2)[8], int v
   }
 }
 
-// sums[c] += sum_p y[p][c], sums[C + c] += sum_p y[p][c]^2
+// sums[c] += sum_p (y[p][c] - y[0][c]), sums[C + c] += sum_p (y[p][c] - y[0][c])^2
+// The pivot y[0][c] (a sample of the channel) keeps the sums at the scale of the channel's spread, not of its mean: E[y^2] - mean^2 in fp32
+// loses (mean / std)^2 times the accumulation error, which a channel with mean = 100 * std turns into a 1e-3 error of rstd.
 __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat16* __restrict__ y, long long npix, int C, float* __restrict__ sums) {
   __shared__ float s_part[kRedSmemFloats];
   const int cv = C / 8;
@@ -369,6 +372,8 @@ __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat1
 #pragma unroll
   for (int i = 0; i < 8; ++i) a1[i] = a2[i] = 0.0f;
   if (active) {
+    float k[8];
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y) + v), k);
     long long p = p0 + pl;
     for (; p + np < p1; p += 2 * np) {  // two independent 16-byte loads in flight
       float f[8], h[8];
@@ -378,8 +383,9 @@ __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat1
       bf16x8_to_float(u1, h);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        a1[i] += f[i] + h[i];
-        a2[i] = fmaf(f[i], f[i], fmaf(h[i], h[i], a2[i]));
+        const float d0 = f[i] - k[i], d1 = h[i] - k[i];
+        a1[i] += d0 + d1;
+        a2[i] = fmaf(d0, d0, fmaf(d1, d1, a2[i]));
       }
     }
     if (p < p1) {
@@ -387,8 +393,9 @@ __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat1
       bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y + p * C) + v), f);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        a1[i] += f[i];
-        a2[i] = fmaf(f[i], f[i], a2[i]);
+        const float d0 = f[i] - k[i];
+        a1[i] += d0;
+        a2[i] = fmaf(d0, d0, a2[i]);
       }
     }
   }
@@ -396,14 +403,15 @@ __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat1
 }
 
 // batch statistics -> mean, rstd, folded scale / shift; running statistics updated like nn.BatchNorm2d (unbiased variance, momentum)
-__global__ void bn_finalize_kernel(const float* __restrict__ sums, long long npix, int C, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   float eps, float momentum, float* __restrict__ running_mean, float* __restrict__ running_var,
+__global__ void bn_finalize_kernel(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ y, long long npix, int C, const float* __restrict__ gamma,
+                                   const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean, float* __restrict__ running_var,
                                    float* __restrict__ stat /* [4][C]: mean, rstd, scale, shift */) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const double n = (double)npix;
-  const double mean = (double)sums[c] / n;
-  double var = (double)sums[C + c] / n - mean * mean;
+  const double d1 = (double)sums[c] / n;  // mean - pivot
+  const double mean = (double)__bfloat162float(y[c]) + d1;
+  double var = (double)sums[C + c] / n - d1 * d1;
   if (var < 0.0) var = 0.0;
   const float rstd = (float)(1.0 / sqrt(var + (double)eps));
   const float s = gamma[c] * rstd;
@@ -604,7 +612,7 @@ extern "C" int cvb_train_pack_weights(const float* w, int32_t cout, int32_t cin,
 // tensor map of one parity class (py, px) of an NHWC tensor: pixels (2i + py, 2j + px); (0, 0) with step 1 is the plain map
 static int act_map_strided(CUtensorMap* m, const void* base, int B, int H, int W, int C, int step, int py, int px, int TW, int TH, int NB) {
   const int Wp = (W - px + step - 1) / step, Hp = (H - py + step - 1) / step;
-  if (Wp <= 0 || Hp <= 0) return act_map(m, base, B, H, W, C, TW, TH, NB);  // never addressed (no pixel of this parity): any valid map
+  if (Wp <= 0 || Hp <= 0) return act_map(m, base, B, H, W, C, TW, TH, NB);  // no pixel of this parity, no tap reads it (s2_taps): any valid map
   const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
   const cuuint64_t str[3] = {(cuuint64_t)C * 2 * step, (cuuint64_t)C * 2 * W * step, (cuuint64_t)C * 2 * W * H};
   const cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB};
@@ -612,15 +620,21 @@ static int act_map_strided(CUtensorMap* m, const void* base, int B, int H, int W
 }
 
 // stride-2 3x3 / pad 1: tap (ky, kx) reads input pixel (2h + ky - 1, 2w + kx - 1) = parity class ((ky + 1) & 1, (kx + 1) & 1) at index
-// (h + (ky == 0 ? -1 : 0), w + (kx == 0 ? -1 : 0)) of that class
-static void s2_taps(int8_t* dh, int8_t* dw, int8_t* map) {
+// (h + (ky == 0 ? -1 : 0), w + (kx == 0 ? -1 : 0)) of that class.  When H or W is 1 the odd class has no pixel: its taps read only padding
+// and are left out.  -> number of taps kept; tap[i] = ky * 3 + kx of kept tap i
+static int s2_taps(int H, int W, int8_t* dh, int8_t* dw, int8_t* map, int8_t* tap) {
+  int n = 0;
   for (int ky = 0; ky < 3; ++ky)
     for (int kx = 0; kx < 3; ++kx) {
-      const int t = ky * 3 + kx;
-      dh[t] = (int8_t)(ky == 0 ? -1 : 0);
-      dw[t] = (int8_t)(kx == 0 ? -1 : 0);
-      map[t] = (int8_t)((((ky + 1) & 1) << 1) | ((kx + 1) & 1));
+      const int py = (ky + 1) & 1, px = (kx + 1) & 1;
+      if (H - py <= 0 || W - px <= 0) continue;
+      dh[n] = (int8_t)(ky == 0 ? -1 : 0);
+      dw[n] = (int8_t)(kx == 0 ? -1 : 0);
+      map[n] = (int8_t)((py << 1) | px);
+      tap[n] = (int8_t)(ky * 3 + kx);
+      ++n;
     }
+  return n;
 }
 
 static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const void* y_prev, const float* bn_stat_prev, void* stream) {
@@ -685,8 +699,7 @@ extern "C" int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, in
     }
     rc = act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
   } else {
-    s2_taps(a.tap_dh, a.tap_dw, a.tap_map);
-    for (int t = 0; t < 9; ++t) a.tap_wblk[t] = (int8_t)t;
+    a.taps = s2_taps(H, W, a.tap_dh, a.tap_dw, a.tap_map, a.tap_wblk);
     for (int py = 0; py < 2 && rc == CVB_OK; ++py)
       for (int px = 0; px < 2 && rc == CVB_OK; ++px) rc = act_map_strided(&a.tmA[py * 2 + px], x, B, H, W, cin, 2, py, px, a.TW, a.TH, a.NB);
   }
@@ -744,7 +757,7 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
 extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t stride, float* dw,
                                     void* stream) {
   CVB_REQUIRE(x && dy && dw, "train_conv_wgrad: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && cin % 64 == 0 && (cout == 64 || cout == 128 || cout % 256 == 0), "train_conv_wgrad: k in {1,3}, cin %% 64 == 0, cout in {64, 128, multiples of 256}");
+  CVB_REQUIRE((k == 1 || k == 3) && cin % 64 == 0 && cout % 64 == 0 && cout > 0, "train_conv_wgrad: k in {1,3}, cin and cout multiples of 64 (cin=%d cout=%d)", cin, cout);
   CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv_wgrad: stride 1, or stride 2 with k = 3");
   CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15) == 0, "train_conv_wgrad: pointers must be 16-byte aligned");
   TWgradArgs a;
@@ -760,22 +773,24 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   a.dw = dw;
   const int m_tiles = a.tiles_w * a.tiles_h * a.tiles_b;
   const int cblocks = ceil_div(cin, 128);
-  const int npan = cout >= 256 ? 4 : cout / 64;
+  // widest block (4, 2 or 1 panels of 64) that divides cout: 192 runs as three 64-wide blocks, 384 as three 128-wide ones
+  const int npan = (cout / 64) % 4 == 0 ? 4 : ((cout / 64) % 2 == 0 ? 2 : 1);
   a.nblocks = cout / (64 * npan);
   int splits = (2 * num_sms()) / (a.taps * cblocks * a.nblocks);  // ~two waves of CTAs: (split, tap, cin block x cout block)
   if (splits < 1) splits = 1;
   if (splits > m_tiles) splits = m_tiles;
   a.splits = splits;
-  int rc = CVB_OK;
+  int rc = CVB_OK, ntaps = k * k;
   if (stride == 1) {
     for (int t = 0; t < k * k; ++t) {
       a.tap_dh[t] = (int8_t)(t / k - k / 2);
       a.tap_dw[t] = (int8_t)(t % k - k / 2);
       a.tap_map[t] = 0;
+      a.tap_idx[t] = (int8_t)t;
     }
     rc = act_map(&a.tmX[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
   } else {
-    s2_taps(a.tap_dh, a.tap_dw, a.tap_map);
+    ntaps = s2_taps(H, W, a.tap_dh, a.tap_dw, a.tap_map, a.tap_idx);  // the taps left out keep dw = 0
     for (int py = 0; py < 2 && rc == CVB_OK; ++py)
       for (int px = 0; px < 2 && rc == CVB_OK; ++px) rc = act_map_strided(&a.tmX[py * 2 + px], x, B, H, W, cin, 2, py, px, a.TW, a.TH, a.NB);
   }
@@ -787,7 +802,7 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   CVB_REQUIRE(smem <= 232448, "train_conv_wgrad: cout=%d needs %d bytes of shared memory", cout, smem);
   CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   void* kargs[1] = {&a};
-  const dim3 grid((unsigned)splits, (unsigned)a.taps, (unsigned)(cblocks * a.nblocks));
+  const dim3 grid((unsigned)splits, (unsigned)ntaps, (unsigned)(cblocks * a.nblocks));
   CVB_CHECK_CUDA(cudaLaunchKernel(fn, grid, dim3(kTThreads), kargs, (size_t)smem, as_stream(stream)));
   count_launch();
   return CVB_OK;
@@ -814,7 +829,7 @@ extern "C" int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const 
   const int np = kEwThreads / (C / 8) > 0 ? kEwThreads / (C / 8) : 1;
   CVB_REQUIRE(C / 8 <= kEwThreads, "train_bn_stats: C too large");
   bn_stats_kernel<<<red_grid(npix, np), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
-  bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, st>>>(sums_scratch, npix, C, gamma, beta, eps, momentum, running_mean, running_var, stat);
+  bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, st>>>(sums_scratch, static_cast<const __nv_bfloat16*>(y), npix, C, gamma, beta, eps, momentum, running_mean, running_var, stat);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
   return CVB_OK;

@@ -340,10 +340,11 @@ int cvb_coco_pack(const float* rows, int32_t B, int32_t M, int32_t row_stride, c
  * cvb_train_conv_dgrad_s2: backward-data of that stride-2 convolution, dx[B,H,W,cin] from dy[B,Ho,Wo,cout] and w_bwd: four dense
  *   sub-convolutions, one per parity class of dx (1 + 2 + 2 + 4 taps), same optional SiLU' epilogue.
  * cvb_train_conv_wgrad: dw[cout][k*k][cin] (fp32, ZEROED BY THE CALLER, accumulated with atomics) += sum over pixels of dy x (shifted x);
- *   x is [B,H,W,cin], dy the conv output's gradient (stride 1: same H, W; stride 2: (H-1)/2+1 etc.); cout in {64, 128, multiples of 256}.
+ *   x is [B,H,W,cin], dy the conv output's gradient (stride 1: same H, W; stride 2: (H-1)/2+1 etc.); cout a multiple of 64 (blocks of
+ *   256, 128 or 64 output channels, the widest that divides cout).
  * cvb_train_bn_stats: batch mean / biased variance of y over npix = B*H*W -> stat [4][C] fp32 = (mean, rstd, scale = gamma*rstd,
  *   shift = beta - mean*scale); running_mean / running_var (may be NULL) updated like nn.BatchNorm2d (momentum, unbiased variance).
- *   sums_scratch: [2][C] fp32.
+ *   sums_scratch: [2][C] fp32 (sums of y - y[pixel 0] and of its square: the variance keeps its precision when |mean| >> std).
  * cvb_train_bn_silu_fwd: out = silu(y * scale + shift).
  * cvb_train_bn_silu_bwd: g = d(loss)/d(out) (or, g_is_dz != 0, already multiplied by silu'): sums [2][C] = (dbeta, dgamma) and
  *   dy = gamma * rstd * (dz - dbeta / N - xhat * dgamma / N)   (the batch-norm backward of torch.autograd).

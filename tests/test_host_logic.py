@@ -339,7 +339,36 @@ def test_training_c_abi_rejects_bad_arguments_before_touching_the_device():
     assert L.cvb_train_conv(one, 1, 8, 8, 64, one, 64, 1, 2, one, None, None, None) != 0      # stride 2 needs k = 3
     assert b'stride' in L.cvb_last_error_string()
     assert L.cvb_train_conv(one, 1, 8, 8, 64, one, 64, 3, 1, one, one, None, None) != 0       # SiLU' epilogue needs both operands
-    assert L.cvb_train_conv_wgrad(one, one, 1, 8, 8, 64, 192, 3, 1, one, None) != 0          # unsupported cout
+    assert L.cvb_train_conv_wgrad(one, one, 1, 8, 8, 64, 96, 3, 1, one, None) != 0           # cout not a multiple of 64
+    assert b'multiples of 64' in L.cvb_last_error_string()
     assert L.cvb_train_conv_dgrad_s2(one, 1, 5, 5, 64, one, 64, 8, 8, one, None, None, None) != 0  # Ho != (H - 1) / 2 + 1
     assert b'geometry' in L.cvb_last_error_string()
     assert L.cvb_train_pack_weights(one, 64, 64, 5, one, one, None) != 0                      # k in {1, 3}
+
+
+def test_fp64_reference_helpers_and_wgrad_split_geometry():
+    """tests/fp64ref.py (the float64 references and element-wise bound of the training-kernel tests) on CPU tensors: the references agree
+    with torch.autograd in float64, the bound accepts a bf16-rounded result and names the element it rejects, and the backward-weight
+    split that test_train_gpu.py's docstring states for its per > 1 cases."""
+    import sys
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import fp64ref as R
+    g = torch.Generator().manual_seed(0)
+    x = torch.randn(2, 64, 5, 7, generator=g).to(torch.bfloat16).double().requires_grad_(True)
+    w = torch.randn(32, 64, 3, 3, generator=g).to(torch.bfloat16).double().requires_grad_(True)
+    yr, ya = R.conv_fwd(x.detach(), w.detach(), 2, 1)
+    dy = torch.randn(yr.shape, generator=g).to(torch.bfloat16).double()
+    F.conv2d(x, w, None, 2, 1).backward(dy)
+    dxr, _ = R.conv_dgrad(dy, w.detach(), x.shape, 2, 1)
+    dwr, dwa = R.conv_wgrad(x.detach(), dy, w.shape, 2, 1)
+    assert torch.allclose(dxr, x.grad, rtol=1e-12, atol=1e-12) and torch.allclose(dwr, w.grad, rtol=1e-12, atol=1e-12)
+    assert bool((ya >= yr.abs()).all()) and bool((dwa >= dwr.abs()).all())
+    bound = R.BF16_REL * yr.abs() + R.mma_gamma(9 * 64) * ya
+    assert R.check(yr.float().to(torch.bfloat16), yr, bound, 'bf16-rounded') <= 1.0
+    bad = yr.clone()
+    bad[1, 3, 2, 1] += 1.5 * bound[1, 3, 2, 1]
+    with pytest.raises(AssertionError, match=r'at \(1, 3, 2, 1\)'):
+        R.check(bad, yr, bound, 'perturbed')
+    assert R.choose_box128(16, 48, 48) == (16, 1, 8) and R.wgrad_split(16, 48, 48, 64, 64, 1, 132) == (288, 264, 2)
+    assert R.choose_box128(16, 40, 40) == (8, 1, 16) and R.wgrad_split(16, 40, 40, 64, 64, 3, 132) == (200, 29, 7)
+    assert R.wgrad_split(2, 10, 10, 64, 192, 3, 132)[1:] == (3, 1)  # cout 192: three 64-wide blocks, no split beyond the 3 tiles
