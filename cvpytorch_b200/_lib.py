@@ -54,6 +54,9 @@ SYMBOLS = {
     'cvb_train_bn_stats': (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_train_bn_silu_fwd': (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_bn_silu_bwd': (c_int32, [c_void_p, c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_focus_s2d': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    'cvb_train_spp_pool_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_spp_pool_bwd': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

@@ -101,8 +101,9 @@ __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_consta
   const int n0 = blockIdx.y * BN;
   if (SILU_BWD) {
     for (int i = threadIdx.x; i < BN; i += kTThreads) {
-      st_s[i] = a.s_prev[n0 + i];
-      st_s[BN + i] = a.t_prev[n0 + i];
+      const bool in = BN != 32 || i < a.cout;  // BN = 32: the whole (16- or 32-channel) output in one tile
+      st_s[i] = in ? a.s_prev[n0 + i] : 0.0f;
+      st_s[BN + i] = in ? a.t_prev[n0 + i] : 0.0f;
     }
   }
   __syncthreads();
@@ -111,7 +112,9 @@ __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_consta
   const int wt = mt % a.tiles_w, t2 = mt / a.tiles_w;
   const int ht = t2 % a.tiles_h, bt = t2 / a.tiles_h;
   const int w0 = wt * a.TW, h0 = ht * a.TH, b0 = bt * a.NB;
-  const int chunks = a.cin / 64;
+  // cin = 16 or 32: one chunk whose channels past cin TMA zero-fills (the 64-channel box is wider than the tensor), and the weights' K
+  // blocks are padded to the chunk width with zeros (cvb_train_pack_weights)
+  const int chunks = (a.cin + 63) / 64;
   const int k_iters = a.taps * chunks;
 
   if (warp == kTProducerWarp) {
@@ -121,7 +124,7 @@ __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_consta
       for (int tap = 0; tap < a.taps; ++tap) {
         const int dh = a.tap_dh[tap], dw = a.tap_dw[tap];
         const CUtensorMap* mapA = &a.tmA[a.tap_map[tap]];
-        const int kb = a.tap_wblk[tap] * a.cin;
+        const int kb = a.tap_wblk[tap] * chunks * 64;
         for (int ck = 0; ck < chunks; ++ck) {
           mbar_wait(&empty[stage], phase ^ 1, 100 + stage);
           mbar_expect_tx(&full[stage], A_BYTES + B_BYTES);
@@ -176,6 +179,7 @@ __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_consta
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int c = 8 * j + cq;
+        if (BN == 32 && c >= a.cout) continue;  // cout = 16: the upper half of the tile is the zero-filled weight rows
         float d0 = d[4 * j + 2 * h], d1 = d[4 * j + 2 * h + 1];
         if (SILU_BWD) {
           const float2 yf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.y_prev + pix * a.cout + n0 + c));
@@ -208,7 +212,8 @@ struct alignas(64) TWgradArgs {
 // dW^T block [128 cin rows, cout columns] of one filter tap += sum over this CTA's pixel tiles of x_tile^T * dy_tile  (K = 128 pixels per
 // stage, 8 MMAs of K = 16).  Both operands are the NHWC tiles exactly as TMA lands them: MN-major (channels contiguous), 64-channel panels;
 // warpgroup w owns the cin panel w (accumulator rows 64w..64w+63).
-template <int NPAN>  // cout / 64
+// NARROW (NPAN = 1): cout = 16 or 32; the dy panel's channels past cout are zero-filled by TMA and their columns are not stored.
+template <int NPAN, bool NARROW = false>  // cout / 64
 __global__ void __launch_bounds__(kTThreads, 1) twgrad_kernel(const __grid_constant__ TWgradArgs a) {
   constexpr int PANEL = 128 * 128;  // 128 pixel rows x 64 channels bf16
   constexpr int X_BYTES = 2 * PANEL;
@@ -307,6 +312,7 @@ __global__ void __launch_bounds__(kTThreads, 1) twgrad_kernel(const __grid_const
 #pragma unroll
         for (int j = 0; j < N / 8; ++j) {
           const int c = 8 * j + cq;
+          if (NARROW && c >= a.cout) continue;
           atomicAdd(base + (size_t)c * cstride, d[4 * j + 2 * h]);
           atomicAdd(base + (size_t)(c + 1) * cstride, d[4 * j + 2 * h + 1]);
         }
@@ -537,17 +543,156 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_apply_kernel(const __n
   }
 }
 
+// ------------------------------------------------------------------------------------------------ Focus stem and SPPF pooling
+// Focus (src/models/modules/yolo_modules.py:19-37): fp32 NCHW [B,3,H,W] -> bf16 NHWC [B,H/2,W/2,16], channel 3 * patch + c in the reference's
+// patch order tl, bl, tr, br (patch = 2 * dx + dy), channels 12..15 zero: the 12 -> cout stem conv then runs as a 16-channel conv whose
+// weight is the reference's, zero-padded.  One thread per output pixel; a float2 load holds the dx = 0 / 1 pair of one (c, dy) row.
+__global__ void __launch_bounds__(kEwThreads) focus_s2d_kernel(const float* __restrict__ img, int B, int H, int W, __nv_bfloat16* __restrict__ out) {
+  const int Ho = H / 2, Wo = W / 2;
+  const long long n = (long long)B * Ho * Wo;
+  for (long long p = blockIdx.x * (long long)kEwThreads + threadIdx.x; p < n; p += (long long)gridDim.x * kEwThreads) {
+    const int ow = (int)(p % Wo);
+    const long long t = p / Wo;
+    const int oh = (int)(t % Ho), b = (int)(t / Ho);
+    float lo[8], hi[8];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int dy = 0; dy < 2; ++dy) {
+        const float2 v = __ldg(reinterpret_cast<const float2*>(img + (((size_t)b * 3 + c) * H + 2 * oh + dy) * W + 2 * ow));
+        const int c0 = 3 * dy + c, c1 = 3 * (2 + dy) + c;  // (dx = 0: patch dy; dx = 1: patch 2 + dy)
+        if (c0 < 8) lo[c0] = v.x; else hi[c0 - 8] = v.x;
+        if (c1 < 8) lo[c1] = v.y; else hi[c1 - 8] = v.y;
+      }
+#pragma unroll
+    for (int i = 4; i < 8; ++i) hi[i] = 0.0f;
+    uint4* o = reinterpret_cast<uint4*>(out + p * 16);
+    o[0] = float_to_bf16x8(lo);
+    o[1] = float_to_bf16x8(hi);
+  }
+}
+
+// SPPF pooling (yolo_modules.py:165-194, kernel_sizes (5, 9, 13), stride 1, padding k // 2, the three pools in parallel on conv1's output):
+// a [B,H,W,C] -> cat [B,H,W,4C] = [a | mp5 | mp9 | mp13] (conv2's input, no separate concat) and, per pool and element, the winner's
+// row-major offset inside its window, idx [3][B*H*W][C] uint8 (13 * 13 = 169 offsets).  The windows are nested and centred on the same
+// pixel, so one row-major scan of the 13 x 13 neighbourhood serves all three; a value replaces the running maximum only if it is strictly
+// greater (or NaN), so the first maximal element in row-major window order wins -- the rule of PyTorch's max_pool2d, which decides where the
+// backward routes a tie.  Positions outside the map are skipped (the padding never wins: the centre is always inside).
+// Thread = one 8-channel vector of one pixel.
+__global__ void __launch_bounds__(kEwThreads) spp_pool_fwd_kernel(const __nv_bfloat16* __restrict__ a, int B, int H, int W, int C, __nv_bfloat16* __restrict__ cat,
+                                                                  uint8_t* __restrict__ idx) {
+  const int cv = C / 8;
+  const long long npix = (long long)B * H * W, n = npix * cv;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int v = (int)(i % cv);
+    const long long p = i / cv;
+    const int w = (int)(p % W);
+    const long long t = p / W;
+    const int h = (int)(t % H);
+    const long long img = (t / H) * H * W;
+    float m[3][8];
+    int k[3][8];
+#pragma unroll
+    for (int s = 0; s < 3; ++s)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        m[s][j] = -INFINITY;
+        k[s][j] = 0;
+      }
+    for (int dy = -6; dy <= 6; ++dy) {
+      const int y = h + dy;
+      if (y < 0 || y >= H) continue;
+      for (int dx = -6; dx <= 6; ++dx) {
+        const int x = w + dx;
+        if (x < 0 || x >= W) continue;
+        float f[8];
+        bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(a + ((img + (long long)y * W + x) * C)) + v), f);
+        const bool in9 = dy >= -4 && dy <= 4 && dx >= -4 && dx <= 4, in5 = dy >= -2 && dy <= 2 && dx >= -2 && dx <= 2;
+        const int o13 = (dy + 6) * 13 + dx + 6, o9 = (dy + 4) * 9 + dx + 4, o5 = (dy + 2) * 5 + dx + 2;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const bool nan = f[j] != f[j];
+          if (in5 && (f[j] > m[0][j] || nan)) { m[0][j] = f[j]; k[0][j] = o5; }
+          if (in9 && (f[j] > m[1][j] || nan)) { m[1][j] = f[j]; k[1][j] = o9; }
+          if (f[j] > m[2][j] || nan) { m[2][j] = f[j]; k[2][j] = o13; }
+        }
+      }
+    }
+    uint4* crow = reinterpret_cast<uint4*>(cat + p * 4 * C) + v;
+    crow[0] = __ldg(reinterpret_cast<const uint4*>(a + p * C) + v);
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      crow[(s + 1) * cv] = float_to_bf16x8(m[s]);  // (bf16 values: the conversion is exact)
+      uint2 u;
+      u.x = (uint32_t)k[s][0] | ((uint32_t)k[s][1] << 8) | ((uint32_t)k[s][2] << 16) | ((uint32_t)k[s][3] << 24);
+      u.y = (uint32_t)k[s][4] | ((uint32_t)k[s][5] << 8) | ((uint32_t)k[s][6] << 16) | ((uint32_t)k[s][7] << 24);
+      reinterpret_cast<uint2*>(idx + ((long long)s * npix + p) * C)[v] = u;
+    }
+  }
+}
+
+// da = g[:, :C] + sum over pools s and the windows q that contain p and chose p: g[q][(s + 1) C + c] -- a gather in a fixed order (q row-major,
+// then s), summed in fp32 and rounded to bf16 once: bitwise reproducible, no atomics.
+__global__ void __launch_bounds__(kEwThreads) spp_pool_bwd_kernel(const __nv_bfloat16* __restrict__ g, const uint8_t* __restrict__ idx, int B, int H, int W, int C,
+                                                                  __nv_bfloat16* __restrict__ da) {
+  const int cv = C / 8;
+  const long long npix = (long long)B * H * W, n = npix * cv;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int v = (int)(i % cv);
+    const long long p = i / cv;
+    const int w = (int)(p % W);
+    const long long t = p / W;
+    const int h = (int)(t % H);
+    const long long img = (t / H) * H * W;
+    float acc[8];
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(g + p * 4 * C) + v), acc);
+    for (int ey = -6; ey <= 6; ++ey) {  // q = (h + ey, w + ex): p sits at (-ey, -ex) from q's centre
+      const int y = h + ey;
+      if (y < 0 || y >= H) continue;
+      for (int ex = -6; ex <= 6; ++ex) {
+        const int x = w + ex;
+        if (x < 0 || x >= W) continue;
+        const long long q = img + (long long)y * W + x;
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+          const int r = 2 + 2 * s, kk = 2 * r + 1;  // 5, 9, 13
+          if (ey < -r || ey > r || ex < -r || ex > r) continue;
+          const uint32_t off = (uint32_t)((r - ey) * kk + (r - ex));
+          const uint2 u = __ldg(reinterpret_cast<const uint2*>(idx + ((long long)s * npix + q) * C) + v);
+          const uint32_t want = off * 0x01010101u;
+          // bytes of u equal to `off`: one bit per channel (a byte of x ^ want is zero)
+          uint32_t hit = 0;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            hit |= ((((u.x ^ want) >> (8 * j)) & 0xffu) == 0u ? 1u : 0u) << j;
+            hit |= ((((u.y ^ want) >> (8 * j)) & 0xffu) == 0u ? 1u : 0u) << (4 + j);
+          }
+          if (hit == 0) continue;
+          float f[8];
+          bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(g + q * 4 * C + (s + 1) * C) + v), f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (hit & (1u << j)) acc[j] += f[j];
+        }
+      }
+    }
+    reinterpret_cast<uint4*>(da + p * C)[v] = float_to_bf16x8(acc);
+  }
+}
+
 // fp32 master weights [cout][cin][kh][kw] (nn.Conv2d) -> bf16 [cout][kh*kw][cin] (forward / wgrad layout) and the backward-data operand
-// bf16 [cin][kh*kw][cout] with the taps rotated by 180 degrees
-__global__ void pack_train_weights_kernel(const float* __restrict__ w, int cout, int cin, int taps, __nv_bfloat16* __restrict__ wf, __nv_bfloat16* __restrict__ wb) {
+// bf16 [cin][kh*kw][cout] with the taps rotated by 180 degrees.  The K rows are kin_pad = kpad(cin) / kout_pad = kpad(cout) long (16 and 32
+// channels: one zero-padded 64-channel chunk; the padding is zeroed by the caller)
+__global__ void pack_train_weights_kernel(const float* __restrict__ w, int cout, int cin, int taps, int kin_pad, int kout_pad, __nv_bfloat16* __restrict__ wf,
+                                          __nv_bfloat16* __restrict__ wb) {
   const long long n = (long long)cout * cin * taps;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int t = (int)(i % taps);
     const int ci = (int)((i / taps) % cin);
     const int co = (int)(i / ((long long)taps * cin));
     const __nv_bfloat16 v = __float2bfloat16_rn(w[i]);
-    wf[((size_t)co * taps + t) * cin + ci] = v;
-    wb[((size_t)ci * taps + (taps - 1 - t)) * cout + co] = v;
+    wf[((size_t)co * taps + t) * kin_pad + ci] = v;
+    wb[((size_t)ci * taps + (taps - 1 - t)) * kout_pad + co] = v;
   }
 }
 
@@ -599,11 +744,20 @@ static int num_sms() {
 
 using namespace cvb;
 
+// channel counts of the training convolutions: 16, 32 (one partial K chunk / N tile) or multiples of 64
+static bool train_channels_ok(int c) { return c == 16 || c == 32 || (c > 0 && c % 64 == 0); }
+static int kpad64(int c) { return (c + 63) / 64 * 64; }
+
 extern "C" int cvb_train_pack_weights(const float* w, int32_t cout, int32_t cin, int32_t k, void* w_fwd, void* w_bwd, void* stream) {
   CVB_REQUIRE(w && w_fwd && w_bwd && cout > 0 && cin > 0 && (k == 1 || k == 3), "train_pack_weights: bad argument");
+  CVB_REQUIRE(train_channels_ok(cin) && train_channels_ok(cout), "train_pack_weights: channels must be 16, 32 or multiples of 64 (cin=%d cout=%d)", cin, cout);
   const long long n = (long long)cout * cin * k * k;
-  pack_train_weights_kernel<<<(int)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184), 256, 0, as_stream(stream)>>>(
-      w, cout, cin, k * k, static_cast<__nv_bfloat16*>(w_fwd), static_cast<__nv_bfloat16*>(w_bwd));
+  const int kin = kpad64(cin), kout = kpad64(cout);
+  cudaStream_t st = as_stream(stream);
+  if (kin != cin) CVB_CHECK_CUDA(cudaMemsetAsync(w_fwd, 0, (size_t)cout * k * k * kin * 2, st));
+  if (kout != cout) CVB_CHECK_CUDA(cudaMemsetAsync(w_bwd, 0, (size_t)cin * k * k * kout * 2, st));
+  pack_train_weights_kernel<<<(int)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184), 256, 0, st>>>(
+      w, cout, cin, k * k, kin, kout, static_cast<__nv_bfloat16*>(w_fwd), static_cast<__nv_bfloat16*>(w_bwd));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
@@ -645,9 +799,9 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
   a.y_prev = static_cast<const __nv_bfloat16*>(y_prev);
   a.s_prev = bn_stat_prev ? bn_stat_prev + 2 * (size_t)a.cout : nullptr;
   a.t_prev = bn_stat_prev ? bn_stat_prev + 3 * (size_t)a.cout : nullptr;
-  const int bn = a.cout % 128 == 0 ? 128 : 64;
+  const int bn = a.cout % 128 == 0 ? 128 : (a.cout % 64 == 0 ? 64 : 32);  // 32: cout = 16 or 32, one tile (rows past cout zero-filled)
   {
-    const long long K = (long long)wblocks * a.cin;
+    const long long K = (long long)wblocks * kpad64(a.cin);
     const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)a.cout};
     const cuuint64_t str[1] = {(cuuint64_t)K * 2};
     const cuuint32_t box[2] = {64, (cuuint32_t)bn};
@@ -656,13 +810,14 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
   }
   const void* fn;
   if (bn == 128) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<128, true>) : reinterpret_cast<const void*>(&tconv_kernel<128, false>);
-  else fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<64, true>) : reinterpret_cast<const void*>(&tconv_kernel<64, false>);
-  const int k_iters = a.taps * (a.cin / 64);
+  else if (bn == 64) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<64, true>) : reinterpret_cast<const void*>(&tconv_kernel<64, false>);
+  else fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<32, true>) : reinterpret_cast<const void*>(&tconv_kernel<32, false>);
+  const int k_iters = a.taps * (kpad64(a.cin) / 64);
   a.stages = k_iters < kTStagesFwd ? k_iters : kTStagesFwd;
   const int smem = a.stages * (128 * 128 + bn * 128) + 256 + 2 * bn * 4;
   CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   void* kargs[1] = {&a};
-  const dim3 grid((unsigned)(a.tiles_w * a.tiles_h * a.tiles_b), (unsigned)(a.cout / bn));
+  const dim3 grid((unsigned)(a.tiles_w * a.tiles_h * a.tiles_b), (unsigned)ceil_div(a.cout, bn));
   CVB_CHECK_CUDA(cudaLaunchKernel(fn, grid, dim3(kTThreads), kargs, (size_t)smem, as_stream(stream)));
   count_launch();
   return CVB_OK;
@@ -671,7 +826,8 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
 extern "C" int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t stride, void* out,
                               const void* y_prev, const float* bn_stat_prev, void* stream) {
   CVB_REQUIRE(x && w_packed && out, "train_conv: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && cin % 64 == 0 && cout % 64 == 0 && B > 0 && H > 0 && W > 0, "train_conv: k in {1,3}, channels multiples of 64 (cin=%d cout=%d k=%d)", cin, cout, k);
+  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout) && B > 0 && H > 0 && W > 0,
+              "train_conv: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", cin, cout, k);
   CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv: stride 1, or stride 2 with k = 3");
   CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, "train_conv: pointers must be 16-byte aligned");
   CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv: the SiLU' epilogue needs both y_prev and its BN statistics");
@@ -713,7 +869,8 @@ extern "C" int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, in
 extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, int32_t Wo, int32_t cout, const void* w_bwd, int32_t cin, int32_t H, int32_t W, void* dx,
                                        const void* y_prev, const float* bn_stat_prev, void* stream) {
   CVB_REQUIRE(dy && w_bwd && dx, "train_conv_dgrad_s2: null tensor");
-  CVB_REQUIRE(cin % 64 == 0 && cout % 64 == 0 && B > 0 && Ho == (H - 1) / 2 + 1 && Wo == (W - 1) / 2 + 1, "train_conv_dgrad_s2: bad geometry");
+  CVB_REQUIRE(train_channels_ok(cin) && train_channels_ok(cout), "train_conv_dgrad_s2: channels must be 16, 32 or multiples of 64 (cin=%d cout=%d)", cin, cout);
+  CVB_REQUIRE(B > 0 && Ho == (H - 1) / 2 + 1 && Wo == (W - 1) / 2 + 1, "train_conv_dgrad_s2: bad geometry");
   CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv_dgrad_s2: the SiLU' epilogue needs both y_prev and its BN statistics");
   for (int pi = 0; pi < 2; ++pi)
     for (int pj = 0; pj < 2; ++pj) {
@@ -757,7 +914,8 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
 extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t stride, float* dw,
                                     void* stream) {
   CVB_REQUIRE(x && dy && dw, "train_conv_wgrad: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && cin % 64 == 0 && cout % 64 == 0 && cout > 0, "train_conv_wgrad: k in {1,3}, cin and cout multiples of 64 (cin=%d cout=%d)", cin, cout);
+  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout),
+              "train_conv_wgrad: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d)", cin, cout);
   CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv_wgrad: stride 1, or stride 2 with k = 3");
   CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15) == 0, "train_conv_wgrad: pointers must be 16-byte aligned");
   TWgradArgs a;
@@ -774,8 +932,10 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   const int m_tiles = a.tiles_w * a.tiles_h * a.tiles_b;
   const int cblocks = ceil_div(cin, 128);
   // widest block (4, 2 or 1 panels of 64) that divides cout: 192 runs as three 64-wide blocks, 384 as three 128-wide ones
-  const int npan = (cout / 64) % 4 == 0 ? 4 : ((cout / 64) % 2 == 0 ? 2 : 1);
-  a.nblocks = cout / (64 * npan);
+  // (cout = 16 or 32: one 64-wide block whose columns past cout are not stored)
+  const bool narrow = cout < 64;
+  const int npan = narrow ? 1 : ((cout / 64) % 4 == 0 ? 4 : ((cout / 64) % 2 == 0 ? 2 : 1));
+  a.nblocks = narrow ? 1 : cout / (64 * npan);
   int splits = (2 * num_sms()) / (a.taps * cblocks * a.nblocks);  // ~two waves of CTAs: (split, tap, cin block x cout block)
   if (splits < 1) splits = 1;
   if (splits > m_tiles) splits = m_tiles;
@@ -796,7 +956,9 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   }
   if (rc == CVB_OK) rc = act_map(&a.tmD, dy, B, Ho, Wo, cout, a.TW, a.TH, a.NB);
   if (rc != CVB_OK) return rc;
-  const void* fn = npan == 1 ? reinterpret_cast<const void*>(&twgrad_kernel<1>) : (npan == 2 ? reinterpret_cast<const void*>(&twgrad_kernel<2>) : reinterpret_cast<const void*>(&twgrad_kernel<4>));
+  const void* fn = narrow ? reinterpret_cast<const void*>(&twgrad_kernel<1, true>)
+                          : (npan == 1 ? reinterpret_cast<const void*>(&twgrad_kernel<1>)
+                                       : (npan == 2 ? reinterpret_cast<const void*>(&twgrad_kernel<2>) : reinterpret_cast<const void*>(&twgrad_kernel<4>)));
   const int stages = npan == 4 ? 2 : kTStagesWg;
   const int smem = stages * ((2 + npan) * 128 * 128) + 256;
   CVB_REQUIRE(smem <= 232448, "train_conv_wgrad: cout=%d needs %d bytes of shared memory", cout, smem);
@@ -857,5 +1019,42 @@ extern "C" int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void*
                                                                  (float)(1.0 / (double)npix), g_is_dz, static_cast<__nv_bfloat16*>(dy));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream) {
+  CVB_REQUIRE(img && out && B > 0 && H > 0 && W > 0, "train_focus_s2d: bad argument");
+  CVB_REQUIRE(H % 2 == 0 && W % 2 == 0, "train_focus_s2d: H and W must be even (H=%d W=%d)", H, W);
+  CVB_REQUIRE((reinterpret_cast<uintptr_t>(img) & 7) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "train_focus_s2d: img must be 8-byte, out 16-byte aligned");
+  const long long n = (long long)B * (H / 2) * (W / 2);
+  focus_s2d_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(img, B, H, W, static_cast<__nv_bfloat16*>(out));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream) {
+  CVB_REQUIRE(a && cat && idx && B > 0 && H > 0 && W > 0 && C > 0, "train_spp_pool_fwd: bad argument");
+  CVB_REQUIRE(C % 8 == 0, "train_spp_pool_fwd: C must be a multiple of 8 (C=%d)", C);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0 && (reinterpret_cast<uintptr_t>(idx) & 7) == 0,
+              "train_spp_pool_fwd: a / cat must be 16-byte, idx 8-byte aligned");
+  const long long n = (long long)B * H * W * (C / 8);
+  spp_pool_fwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat),
+                                                                         static_cast<uint8_t*>(idx));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, void* da, void* stream) {
+  CVB_REQUIRE(g && idx && da && B > 0 && H > 0 && W > 0 && C > 0, "train_spp_pool_bwd: bad argument");
+  CVB_REQUIRE(C % 8 == 0, "train_spp_pool_bwd: C must be a multiple of 8 (C=%d)", C);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da)) & 15) == 0 && (reinterpret_cast<uintptr_t>(idx) & 7) == 0,
+              "train_spp_pool_bwd: g / da must be 16-byte, idx 8-byte aligned");
+  const long long n = (long long)B * H * W * (C / 8);
+  spp_pool_bwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), static_cast<const uint8_t*>(idx), B, H, W, C,
+                                                                         static_cast<__nv_bfloat16*>(da));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
   return CVB_OK;
 }

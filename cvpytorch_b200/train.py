@@ -1,9 +1,14 @@
-"""Training-step drop-ins for the YOLOX C3 block (SURVEY.md 8(f) rank 3, BASELINE.json configs[3]): forward AND backward on the H100 kernels.
+"""Training-step drop-ins for the YOLOX backbone (SURVEY.md 8(f) rank 3, BASELINE.json configs[3]): forward AND backward on the H100 kernels.
 
 Mirrors (paths relative to the reference checkout), with the same constructor arguments and state_dict keys:
   BaseConv     src/models/modules/yolox_modules.py:35-55    nn.Conv2d(bias=False) -> nn.BatchNorm2d -> SiLU, training mode (batch statistics)
   Bottleneck   src/models/modules/yolox_modules.py:79-96    1x1 -> 3x3 (+ shortcut)
   CSPLayer     src/models/modules/yolox_modules.py:99-129   conv1 | conv2 -> bottlenecks -> cat -> conv3
+  Focus        src/models/modules/yolo_modules.py:19-37     2x2 space-to-depth (patches tl, bl, tr, br) -> 3x3 conv 12 -> cout
+  SPPF         src/models/modules/yolo_modules.py:165-194   conv1 -> cat[x, maxpool5, maxpool9, maxpool13] (parallel pools) -> conv2
+  CSPDarknet   src/models/backbones/det/csp_darknet.py:25-129   stem, four stages, SPPF in stage4
+
+Channel counts of every convolution: 16, 32 or multiples of 64 (YOLOX-n, -s and -l; the 24 / 48 / 80-wide -t, -m and -x raise).
 
 What runs where: every convolution (forward, backward-data, backward-weight) is a bf16 wgmma implicit GEMM and every BatchNorm / SiLU pass
 (statistics, apply, backward reductions, backward apply) is a kernel of libcvb200.so (csrc/train_kernels.cu).  torch.autograd only chains the
@@ -34,11 +39,20 @@ def _check_cuda(t, what):
         raise _lib.CvbError(f'{what}: CUDA tensor required (the H100 training path has no CPU fallback)')
 
 
+def kpad(c):
+    """K width of a packed weight row: 16 and 32 channels are one zero-padded 64-channel chunk."""
+    return -(-c // 64) * 64
+
+
+def channels_ok(c):
+    return c in (16, 32) or (c > 0 and c % 64 == 0)
+
+
 def pack_weights(w):
-    """fp32 [cout,cin,k,k] -> (bf16 [cout,k*k,cin] forward / wgrad layout, bf16 [cin,k*k,cout] backward-data operand)."""
+    """fp32 [cout,cin,k,k] -> (bf16 [cout,k*k,kpad(cin)] forward / wgrad layout, bf16 [cin,k*k,kpad(cout)] backward-data operand)."""
     cout, cin, k, _ = w.shape
-    wf = torch.empty((cout, k * k, cin), dtype=torch.bfloat16, device=w.device)
-    wb = torch.empty((cin, k * k, cout), dtype=torch.bfloat16, device=w.device)
+    wf = torch.empty((cout, k * k, kpad(cin)), dtype=torch.bfloat16, device=w.device)
+    wb = torch.empty((cin, k * k, kpad(cout)), dtype=torch.bfloat16, device=w.device)
     _lib.check(_lib.lib().cvb_train_pack_weights(_p(w.detach().float().contiguous()), cout, cin, k, _p(wf), _p(wb), _stream()), 'cvb_train_pack_weights')
     return wf, wb
 
@@ -173,8 +187,8 @@ class BaseConv(nn.Module):
         super().__init__()
         if not (stride == 1 or (stride == 2 and ksize == 3)) or groups != 1 or bias or act != 'silu' or ksize not in (1, 3):
             raise NotImplementedError('H100 training BaseConv: ksize in {1,3}, stride 1 (or 2 with ksize 3), groups 1, no bias, SiLU')
-        if in_channels % 64 or out_channels % 64:
-            raise NotImplementedError('H100 training BaseConv: channel counts must be multiples of 64')
+        if not (channels_ok(in_channels) and channels_ok(out_channels)):
+            raise NotImplementedError(f'H100 training BaseConv: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
         self.conv = nn.Conv2d(in_channels, out_channels, kernel_size=ksize, stride=stride, padding=(ksize - 1) // 2, groups=groups, bias=bias)
         self.bn = nn.BatchNorm2d(out_channels)
         self.act = nn.SiLU(inplace=True)  # (parameter-free; kept for module-tree parity with the reference)
@@ -242,3 +256,179 @@ class CSPLayer(nn.Module):
         _check_cuda(x, 'CSPLayer (H100 training)')
         xh = x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)
         return self.forward_nhwc(xh).permute(0, 3, 1, 2).to(x.dtype)
+
+
+# ------------------------------------------------------------------------------------------------ whole backbone: Focus stem, SPPF, CSPDarknet
+def focus_s2d(img):
+    """fp32 NCHW [B,3,H,W] (H, W even) -> bf16 NHWC [B,H/2,W/2,16]: channel 3 * patch + c in the reference's patch order (tl, bl, tr, br),
+    channels 12..15 zero."""
+    _check_cuda(img, 'Focus (H100 training)')
+    B, C, H, W = img.shape
+    if C != 3:
+        raise ValueError(f'Focus: a 3-channel image expected, got {C} channels')
+    img = img.detach().float().contiguous()
+    out = torch.empty((B, H // 2, W // 2, 16), dtype=torch.bfloat16, device=img.device)
+    _lib.check(_lib.lib().cvb_train_focus_s2d(_p(img), B, H, W, _p(out), _stream()), 'cvb_train_focus_s2d')
+    return out
+
+
+def spp_pool(a):
+    """a NHWC bf16 [B,H,W,C] -> (cat [B,H,W,4C] = [a | maxpool5 | maxpool9 | maxpool13], idx uint8 [3,B,H,W,C]: each window's winner)."""
+    B, H, W, C = a.shape
+    cat = torch.empty((B, H, W, 4 * C), dtype=torch.bfloat16, device=a.device)
+    idx = torch.empty((3, B, H, W, C), dtype=torch.uint8, device=a.device)
+    _lib.check(_lib.lib().cvb_train_spp_pool_fwd(_p(a), B, H, W, C, _p(cat), _p(idx), _stream()), 'cvb_train_spp_pool_fwd')
+    return cat, idx
+
+
+def spp_pool_backward(g, idx):
+    """g = d(loss)/d(cat) [B,H,W,4C], idx of spp_pool -> d(loss)/d(a) [B,H,W,C] (deterministic gather, fp32 sums)."""
+    B, H, W, C4 = g.shape
+    da = torch.empty((B, H, W, C4 // 4), dtype=torch.bfloat16, device=g.device)
+    _lib.check(_lib.lib().cvb_train_spp_pool_bwd(_p(g), _p(idx), B, H, W, C4 // 4, _p(da), _stream()), 'cvb_train_spp_pool_bwd')
+    return da
+
+
+class _SppPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, a):
+        _check_cuda(a, 'SPPF (H100 training)')
+        cat, idx = spp_pool(a.contiguous())
+        ctx.save_for_backward(idx)
+        return cat
+
+    @staticmethod
+    def backward(ctx, g):
+        idx, = ctx.saved_tensors
+        return spp_pool_backward(g.contiguous(), idx)
+
+
+def _bn_momentum(bn):
+    bn.num_batches_tracked += 1
+    return bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
+
+
+class _StemConv(nn.Module):
+    """The Focus stem's ConvModule (keys conv.weight [cout,12,3,3], bn.*): on the kernels a 16 -> cout BaseConv over cvb_train_focus_s2d's
+    output, with the weight zero-padded to 16 input channels (its gradient is the first 12).  Computes no input gradient."""
+
+    def __init__(self, in_channels, out_channels):
+        super().__init__()
+        self.conv = nn.Conv2d(in_channels, out_channels, kernel_size=3, stride=1, padding=1, bias=False)
+        self.bn = nn.BatchNorm2d(out_channels)
+        self.act = nn.SiLU(inplace=True)  # (parameter-free; module-tree parity)
+
+    def forward(self, s2d):
+        if not self.training:
+            raise RuntimeError('cvpytorch_b200.train.Focus is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
+        bn = self.bn
+        mom = _bn_momentum(bn)
+        w16 = nn.functional.pad(self.conv.weight, (0, 0, 0, 0, 0, s2d.shape[3] - self.conv.weight.shape[1]))
+        return _ConvBnSiLU.apply(s2d, w16, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, mom, 3, 1)
+
+
+class Focus(nn.Module):
+    """src/models/modules/yolo_modules.py:19-37 (3-channel image, 3x3 stride-1 conv).  forward: NCHW fp32 image -> NCHW; forward_nhwc -> NHWC bf16.
+    The image gets no gradient (an input with requires_grad raises)."""
+
+    def __init__(self, in_channels, out_channels, kernel_sizes=1, stride=1, conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True), act_cfg=dict(type='Swish')):
+        super().__init__()
+        if in_channels != 3 or kernel_sizes != 3 or stride != 1:
+            raise NotImplementedError('H100 training Focus: the 3-channel image, 3x3 conv, stride 1 (the YOLOX stem)')
+        if not channels_ok(out_channels):
+            raise NotImplementedError(f'H100 training Focus: out_channels must be 16, 32 or a multiple of 64 (got {out_channels})')
+        self.conv = _StemConv(in_channels * 4, out_channels)
+
+    def forward_nhwc(self, x):
+        if x.requires_grad:
+            raise NotImplementedError('H100 training Focus computes no gradient for the input image: pass an image without requires_grad')
+        return self.conv(focus_s2d(x))
+
+    def forward(self, x):
+        return self.forward_nhwc(x).permute(0, 3, 1, 2).to(x.dtype)
+
+
+class SPPF(nn.Module):
+    """src/models/modules/yolo_modules.py:165-194 with kernel_sizes (5, 9, 13): conv1 (C -> C/2) -> [x | mp5 | mp9 | mp13] (parallel pools,
+    one kernel that writes the concatenation conv2 reads) -> conv2 (2C -> C).  forward: NCHW; forward_nhwc: NHWC bf16."""
+
+    def __init__(self, in_channels, out_channels, kernel_sizes=(5, 9, 13), conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True),
+                 act_cfg=dict(type='Swish'), init_cfg=None):
+        super().__init__()
+        if isinstance(kernel_sizes, int) or tuple(kernel_sizes) != (5, 9, 13):
+            raise NotImplementedError(f'H100 training SPPF: kernel_sizes (5, 9, 13) only (got {kernel_sizes})')
+        self.kernel_sizes = kernel_sizes
+        hidden_channels = in_channels // 2
+        self.conv1 = BaseConv(in_channels, hidden_channels, 1, stride=1)
+        self.m = nn.ModuleList([nn.MaxPool2d(kernel_size=ks, stride=1, padding=ks // 2) for ks in kernel_sizes])  # (parameter-free; module-tree parity)
+        self.conv2 = BaseConv(hidden_channels * 4, out_channels, 1, stride=1)
+
+    def forward_nhwc(self, x):
+        return self.conv2(_SppPool.apply(self.conv1(x)))
+
+    def forward(self, x):
+        _check_cuda(x, 'SPPF (H100 training)')
+        return self.forward_nhwc(x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)).permute(0, 3, 1, 2).to(x.dtype)
+
+
+def _nhwc(m, x):
+    return m.forward_nhwc(x) if isinstance(m, (CSPLayer, SPPF)) else m(x)
+
+
+class CSPDarknet(nn.Module):
+    """src/models/backbones/det/csp_darknet.py:25-129, training mode, same constructor and state_dict keys.  Every BatchNorm gets eps 1e-3 and
+    momentum 0.03 (the reference's init_weights).  forward(x): NCHW fp32 image -> list of NCHW outputs of `out_stages` (one tensor if a single
+    stage); forward_nhwc(x): the same outputs as NHWC bf16, for chaining into later drop-ins.  Evaluation goes through the inference
+    cvpytorch_b200.yolox_models.CSPDarknet, which loads this module's state_dict with strict=True."""
+    cfg = {"n": [0.33, 0.25], "t": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
+
+    def __init__(self, subtype='cspdark_s', out_channels=[64, 128, 256, 512, 1024], layers=[3, 9, 9, 3], spp_ksizes=(5, 9, 13), depthwise=False,
+                 conv_cfg=None, norm_cfg=dict(type='BN', momentum=0.03, eps=0.001), act_cfg=dict(type='Swish'), out_stages=[2, 3, 4], output_stride=32,
+                 backbone_path=None, pretrained=False, frozen_stages=-1, norm_eval=False):
+        super().__init__()
+        if depthwise:
+            raise NotImplementedError('H100 training CSPDarknet: depthwise convolutions are not on the training path')
+        if norm_eval:
+            raise NotImplementedError('H100 training CSPDarknet: norm_eval=True (frozen BatchNorm statistics) is not on the training path')
+        if frozen_stages >= 0:
+            raise NotImplementedError('H100 training CSPDarknet: frozen_stages >= 0 is not on the training path')
+        if isinstance(spp_ksizes, int) or tuple(spp_ksizes) != (5, 9, 13):
+            raise NotImplementedError(f'H100 training CSPDarknet: spp_ksizes (5, 9, 13) only (got {spp_ksizes})')
+        if (norm_cfg or {}).get('type', 'BN') != 'BN' or (act_cfg or {}).get('type') not in ('Swish', 'SiLU') or conv_cfg is not None:
+            raise NotImplementedError('H100 training CSPDarknet: plain Conv2d, BatchNorm and Swish / SiLU only')
+        self.subtype, self.out_stages, self.output_stride = subtype, out_stages, output_stride
+        self.backbone_path, self.pretrained, self.frozen_stages, self.norm_eval = backbone_path, pretrained, frozen_stages, norm_eval
+        depth_mul, width_mul = self.cfg[subtype.split('_')[1]]
+        ch = list(map(lambda x: int(x * width_mul), out_channels))
+        nl = list(map(lambda x: max(round(x * depth_mul), 1), layers))
+        self.layers = nl
+        bad = sorted({c for c in ch + [c // 2 for c in ch[1:]] if not channels_ok(c)})
+        if bad:
+            raise NotImplementedError(f'H100 training CSPDarknet {subtype}: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        self.stem = Focus(3, ch[0], kernel_sizes=3)
+        self.stage1 = nn.Sequential(BaseConv(ch[0], ch[1], 3, 2), CSPLayer(ch[1], ch[1], n=nl[0], shortcut=True))
+        self.stage2 = nn.Sequential(BaseConv(ch[1], ch[2], 3, 2), CSPLayer(ch[2], ch[2], n=nl[1], shortcut=True))
+        self.stage3 = nn.Sequential(BaseConv(ch[2], ch[3], 3, 2), CSPLayer(ch[3], ch[3], n=nl[2], shortcut=True))
+        self.stage4 = nn.Sequential(BaseConv(ch[3], ch[4], 3, 2), SPPF(ch[4], ch[4], kernel_sizes=spp_ksizes), CSPLayer(ch[4], ch[4], n=nl[3], shortcut=False))
+        self.out_channels = ch[out_stages[0]:out_stages[-1] + 1]
+        for m in self.modules():
+            if isinstance(m, nn.BatchNorm2d):
+                m.eps, m.momentum = 1e-3, 0.03
+
+    def forward_nhwc(self, x):
+        if not self.training:
+            raise RuntimeError('cvpytorch_b200.train.CSPDarknet is the TRAINING drop-in (batch statistics); load its state_dict into '
+                               'cvpytorch_b200.yolox_models.CSPDarknet for eval()')
+        _check_cuda(x, 'CSPDarknet (H100 training)')
+        h = self.stem.forward_nhwc(x)
+        outs = []
+        for i in range(1, 5):
+            for m in getattr(self, f'stage{i}'):
+                h = _nhwc(m, h)
+            if i in self.out_stages:
+                outs.append(h)
+        return outs
+
+    def forward(self, x):
+        outs = [o.permute(0, 3, 1, 2).to(x.dtype) for o in self.forward_nhwc(x)]
+        return outs if len(self.out_stages) > 1 else outs[0]

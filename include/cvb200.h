@@ -328,10 +328,12 @@ int cvb_coco_pack(const float* rows, int32_t B, int32_t M, int32_t row_stride, c
  * Training step of the YOLOX C3 block (SURVEY.md 8(f) rank 3; BASELINE.json configs[3]): one  BaseConv = nn.Conv2d(bias=False) ->
  * nn.BatchNorm2d (batch statistics) -> SiLU  (src/models/modules/yolox_modules.py:35-55) forward and backward, i.e. what
  * trainer.py:177-207 gets from cuDNN / ATen autograd, as bf16 wgmma implicit GEMMs + element-wise passes (csrc/train_kernels.cu).
- * All activations / gradients: device bf16 NHWC, dense ([B,H,W,C], C a multiple of 64); convolutions k = 1 or 3, stride 1, pad k/2.
+ * All activations / gradients: device bf16 NHWC, dense ([B,H,W,C]); convolutions k = 1 or 3, stride 1, pad k/2.  Every channel count of the
+ * convolutions (cin, cout) is 16, 32 or a multiple of 64: a 16- or 32-channel tensor is one partial 64-channel K chunk / N tile.
  *
- * cvb_train_pack_weights: fp32 master weights [cout,cin,k,k] -> w_fwd bf16 [cout][k*k][cin] and w_bwd bf16 [cin][k*k][cout] (taps rotated
- *   by 180 degrees: the operand of the backward-data convolution).
+ * cvb_train_pack_weights: fp32 master weights [cout,cin,k,k] -> w_fwd bf16 [cout][k*k][kpad(cin)] and w_bwd bf16 [cin][k*k][kpad(cout)]
+ *   (taps rotated by 180 degrees: the operand of the backward-data convolution); kpad(c) = c rounded up to a multiple of 64, the padding
+ *   zero (16 and 32 channels only; kpad(c) = c otherwise).
  * cvb_train_conv: out[B,H,W,cout] = conv(x[B,H,W,cin], w_packed [cout][k*k][cin]).  Forward: (x, w_fwd).  Backward-data: (dy, w_bwd) with
  *   cin/cout swapped.  y_prev / bn_stat_prev != NULL: SiLU' epilogue -- the result is multiplied by silu'(y_prev * scale + shift) of the
  *   layer that produced this conv's input (bn_stat layout below), giving dz of that layer directly.
@@ -340,14 +342,24 @@ int cvb_coco_pack(const float* rows, int32_t B, int32_t M, int32_t row_stride, c
  * cvb_train_conv_dgrad_s2: backward-data of that stride-2 convolution, dx[B,H,W,cin] from dy[B,Ho,Wo,cout] and w_bwd: four dense
  *   sub-convolutions, one per parity class of dx (1 + 2 + 2 + 4 taps), same optional SiLU' epilogue.
  * cvb_train_conv_wgrad: dw[cout][k*k][cin] (fp32, ZEROED BY THE CALLER, accumulated with atomics) += sum over pixels of dy x (shifted x);
- *   x is [B,H,W,cin], dy the conv output's gradient (stride 1: same H, W; stride 2: (H-1)/2+1 etc.); cout a multiple of 64 (blocks of
- *   256, 128 or 64 output channels, the widest that divides cout).
+ *   x is [B,H,W,cin], dy the conv output's gradient (stride 1: same H, W; stride 2: (H-1)/2+1 etc.); output channels in blocks of 256,
+ *   128 or 64, the widest that divides cout (cout = 16 or 32: one block).
  * cvb_train_bn_stats: batch mean / biased variance of y over npix = B*H*W -> stat [4][C] fp32 = (mean, rstd, scale = gamma*rstd,
  *   shift = beta - mean*scale); running_mean / running_var (may be NULL) updated like nn.BatchNorm2d (momentum, unbiased variance).
  *   sums_scratch: [2][C] fp32 (sums of y - y[pixel 0] and of its square: the variance keeps its precision when |mean| >> std).
  * cvb_train_bn_silu_fwd: out = silu(y * scale + shift).
  * cvb_train_bn_silu_bwd: g = d(loss)/d(out) (or, g_is_dz != 0, already multiplied by silu'): sums [2][C] = (dbeta, dgamma) and
  *   dy = gamma * rstd * (dz - dbeta / N - xhat * dgamma / N)   (the batch-norm backward of torch.autograd).
+ *
+ * Whole-backbone training (CSPDarknet, src/models/backbones/det/csp_darknet.py:25-129) adds the Focus stem and the SPPF pools:
+ * cvb_train_focus_s2d: img fp32 NCHW [B,3,H,W] (H, W even) -> out bf16 NHWC [B,H/2,W/2,16], channel 3 * patch + c in the reference's patch
+ *   order (top-left, bottom-left, top-right, bottom-right; src/models/modules/yolo_modules.py:19-37), channels 12..15 zero.  The stem conv
+ *   then runs as a 16 -> cout cvb_train_conv with the reference weight zero-padded to 16 input channels.  No input gradient.
+ * cvb_train_spp_pool_fwd: a bf16 NHWC [B,H,W,C] (C % 8 == 0) -> cat [B,H,W,4C] = [a | maxpool5(a) | maxpool9(a) | maxpool13(a)] (stride 1,
+ *   padding k/2, the pools in parallel: yolo_modules.py:165-194) and idx uint8 [3][B*H*W][C], the winner's row-major offset in its window
+ *   (ties: the first maximal element, as torch's max_pool2d).
+ * cvb_train_spp_pool_bwd: g = d(loss)/d(cat) [B,H,W,4C], idx of the forward -> da [B,H,W,C] = g[..., :C] + the pooled gradients routed to
+ *   their winners; a gather summed in fp32 in a fixed order (bitwise reproducible).
  */
 int cvb_train_pack_weights(const float* w, int32_t cout, int32_t cin, int32_t k, void* w_fwd, void* w_bwd, void* stream);
 int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t stride, void* out,
@@ -361,6 +373,9 @@ int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const float* gamm
 int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream);
 int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, float* sums,
                           void* dy, void* stream);
+int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream);
+int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream);
+int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, void* da, void* stream);
 
 /* Library info / errors */
 const char* cvb_last_error_string(void);
