@@ -30,7 +30,7 @@ class CvbConvDesc(ctypes.Structure):
     _fields_ = [('inp', CvbView), ('out', CvbView), ('weights', c_void_p), ('cout_pad', c_int32),
                 ('bias', c_void_p), ('kh', c_int32), ('kw', c_int32), ('stride', c_int32), ('pad', c_int32),
                 ('dilation', c_int32), ('act', c_int32), ('out_kind', c_int32), ('residual', CvbView),
-                ('up_partial', CvbView), ('block_n', c_int32), ('sm_limit', c_int32), ('no_resident', c_int32), ('residual_before_act', c_int32), ('w_window', c_int32), ('halo', c_int32), ('yolo', POINTER(CvbYoloDecode)), ('residual_scale', c_float)]
+                ('up_partial', CvbView), ('block_n', c_int32), ('sm_limit', c_int32), ('no_resident', c_int32), ('residual_before_act', c_int32), ('w_window', c_int32), ('halo', c_int32), ('yolo', POINTER(CvbYoloDecode)), ('residual_scale', c_float), ('schedule', c_int32)]
 
 
 class CvbNmsParams(ctypes.Structure):

@@ -188,31 +188,36 @@ __device__ __forceinline__ void issue_tap(float (&dm)[BLOCK_N / 2], float (&dc)[
   }
 }
 
-template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO>
+// PP: ping-pong schedule -- a tile is 64 pixels and belongs to one warpgroup, so every per-tile buffer below exists once per warpgroup
+template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, bool PP = false>
 struct ConvCfg {
+  static constexpr int TILE_M = PP ? kTileM / 2 : kTileM;  // output pixels of one tile
   static constexpr int SWZ = BLOCK_K * 2;  // swizzle span == bytes of one K chunk row
-  static constexpr int A_BYTES = kTileM * SWZ;
+  static constexpr int A_BYTES = TILE_M * SWZ;
   static constexpr int B_BYTES = BLOCK_N * SWZ;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr int OUT_GROUP_CH = OUT_F32 ? 32 : (BLOCK_N >= 64 ? 64 : 32);
   static constexpr int OUT_ROW_BYTES = OUT_F32 ? 128 : OUT_GROUP_CH * 2;
-  static constexpr int OUT_PLANE_BYTES = kTileM * OUT_ROW_BYTES;
-  static constexpr int OUT_STAGE_BYTES = OUT_PLANE_BYTES * (OUT_F32 ? 1 : 2);
+  static constexpr int OUT_PLANE_BYTES = TILE_M * OUT_ROW_BYTES;
+  static constexpr int OUT_TILE_BYTES = OUT_PLANE_BYTES * (OUT_F32 ? 1 : 2);  // staging tile of one output group of one tile
+  static constexpr int OUT_STAGE_BYTES = OUT_TILE_BYTES * (PP ? 2 : 1);       // one staging buffer (ping-pong: one tile per warpgroup)
   // fp32 accumulator tile the epilogue reads (one output group, or the 96 decoded columns of a fused-decode tile); rows padded by
-  // 16 bytes so that the row-per-thread reads of eight consecutive rows hit distinct banks
+  // 16 bytes so that the row-per-thread reads of eight consecutive rows hit distinct banks.  Ping-pong: rows 64*wg.. are warpgroup wg's tile.
   static constexpr int ACC_COLS = YOLO ? 96 : OUT_GROUP_CH;
   static constexpr int ACC_PITCH = ACC_COLS + 4;
   static constexpr int ACC_BYTES = kTileM * ACC_PITCH * 4;
-  static constexpr int TAIL_BYTES = ACC_BYTES + BLOCK_N * 4 + 64 * 8 + 16;  // accumulator tile + bias + barriers
+  static constexpr int TAIL_BYTES = ACC_BYTES + (PP ? 2 : 1) * BLOCK_N * 4 + 64 * 8 + 16;  // accumulator tile + bias + barriers
 };
 
 // EPI selects a compile-time specialisation of the epilogue (the hot layers run a compact, branch-free instruction stream; the generic
 // stream with its run-time mode checks costs more issue slots per tile, and the HBM-bound layers are issue bound in the epilogue):
 //   0 generic   1 act = SiLU, no residual, no up-partial   2 act = SiLU, residual tile by TMA added after the activation (Darknet bottleneck)
 //   3 act = ReLU, no residual, no up-partial   4 act = ReLU, residual tile by TMA added BEFORE the activation (ResNet bottleneck)
-template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0>
+// PP selects the ping-pong schedule (one-CTA-per-SM plans, not for the fused decode or the halo loader): a tile is 64 pixels, the
+// CTA's tiles alternate between the two warpgroups, and a warpgroup runs its epilogue while the other one's MMAs run (DESIGN.md 4.1).
+template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0, bool PP = false>
 __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
-  using Cfg = ConvCfg<BLOCK_N, BLOCK_K, OUT_F32, YOLO>;
+  using Cfg = ConvCfg<BLOCK_N, BLOCK_K, OUT_F32, YOLO, PP>;
   constexpr int SWZ = Cfg::SWZ;
   constexpr int A_BYTES = Cfg::A_BYTES;
   constexpr int B_BYTES = Cfg::B_BYTES;
@@ -220,9 +225,10 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
   constexpr int OUT_GROUP_CH = Cfg::OUT_GROUP_CH;
   constexpr int OUT_ROW_BYTES = Cfg::OUT_ROW_BYTES;
   constexpr int ACC_PITCH = Cfg::ACC_PITCH;
-  constexpr int EPI_THREADS = kEpiThreads;
+  constexpr int EPI_THREADS = PP ? kEpiThreads / 2 : kEpiThreads;  // threads that share one tile's epilogue
   constexpr bool SPLIT = BLOCK_N <= 128;
   static_assert(EPI == 0 || (!OUT_F32 && !YOLO), "epilogue specialisations exist for the split16 output only");
+  static_assert(!(PP && YOLO), "the fused decode runs the cooperative schedule");
   // run-time mode flags, folded to constants in the specialised kernels
   const bool resid_tma = (EPI == 2 || EPI == 4) ? true : ((EPI == 1 || EPI == 3) ? false : a.resid_tma != 0);
   const int act_mode = (EPI == 1 || EPI == 2) ? CVB_ACT_SILU : ((EPI == 3 || EPI == 4) ? CVB_ACT_RELU : a.act);
@@ -237,21 +243,22 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
   }
   const int dbg = kDiag ? a.dbg : 0;  // diagnostics switches: compiled out of the product library
   const int STAGES = a.stages;
-  const int stage_bytes = a.halo ? (int)a.a_slot_bytes : (a.b_resident ? 2 * A_BYTES : STAGE_BYTES);
+  const bool halo = PP ? false : a.halo != 0;
+  const int stage_bytes = halo ? (int)a.a_slot_bytes : (a.b_resident ? 2 * A_BYTES : STAGE_BYTES);
   uint8_t* stage_base = smem;
   uint8_t* b_res = smem + STAGES * stage_bytes;                                  // resident weights: k_iters x {hi, lo} tiles (halo mode: or the weight ring)
-  uint8_t* out_stage0 = b_res + (a.b_resident ? a.taps * a.chunks * 2 * B_BYTES : (a.halo ? a.sb_stages * 2 * B_BYTES : 0));
+  uint8_t* out_stage0 = b_res + (a.b_resident ? a.taps * a.chunks * 2 * B_BYTES : (halo ? a.sb_stages * 2 * B_BYTES : 0));
   uint8_t* res_stage = out_stage0 + (YOLO ? kYoloStageBytes + kNmsBins * 4 + kYoloBiasBytes : a.out_bufs * Cfg::OUT_STAGE_BYTES);  // residual tile (same layout as an output tile)
   float* acc_s = reinterpret_cast<float*>(res_stage + (resid_tma ? Cfg::OUT_STAGE_BYTES : 0));  // (fused decode: staging tile + histogram instead of output tiles)
   float* bias_s = acc_s + Cfg::ACC_BYTES / 4;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + BLOCK_N);
-  const int SB = a.halo ? a.sb_stages : 0;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + (PP ? 2 : 1) * BLOCK_N);
+  const int SB = halo ? a.sb_stages : 0;
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
   uint64_t* fullB = bars + 2 * STAGES;  // halo mode: separate ring of weight tiles
   uint64_t* emptyB = fullB + SB;
   uint64_t* bfull = emptyB + SB;  // resident weights have landed
-  uint64_t* rfull = bfull + 1;    // residual tile has landed
+  uint64_t* rfull = bfull + 1;    // residual tile has landed (ping-pong: one per warpgroup)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -263,10 +270,10 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
     if (resid_tma) tma_prefetch_desc(&a.tmR);
   }
   if (threadIdx.x == 0) {
-    // a ring slot is free once every MMA warp has seen its wgmma group complete
+    // a ring slot is free once every MMA warp that reads it has seen its wgmma group complete (ping-pong: the 4 warps of one warpgroup)
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], kMmaWarps);
+      mbar_init(&empty[s], PP ? kMmaWarps / 2 : kMmaWarps);
     }
     for (int s = 0; s < SB; ++s) {
       mbar_init(&fullB[s], 1);
@@ -274,6 +281,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
     }
     mbar_init(bfull, 1);
     mbar_init(rfull, 1);
+    if (PP) mbar_init(rfull + 1, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -314,7 +322,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
         }
       }
       grid_dep_wait();  // activations are written by the previous kernel(s)
-      if (a.halo) {
+      if (halo) {
         // copy / tap mode: per (tile, K chunk) one box per copy (all filter rows -- and in mode 2 all filter columns -- of that
         // chunk), then the weight tiles of the copy's taps in the order the MMA warp consumes them
         int sb = 0;
@@ -382,23 +390,34 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           }
         }
       }
-      if (prof_on) {  // producer: total cycles, waiting for a free A slot, waiting for a free weight slot
-        a.prof[blockIdx.x * 16 + 0] = clock64() - prof_t0;
-        a.prof[blockIdx.x * 16 + 1] = prof_acc[0];
-        a.prof[blockIdx.x * 16 + 2] = prof_acc[1];
+      if (prof_on) {  // producer: total cycles, waiting for a free A slot, waiting for a free weight slot (ping-pong: in both counter rows)
+        const long long t = clock64() - prof_t0;
+        for (int r = 0; r < (PP ? 2 : 1); ++r) {
+          long long* pr = a.prof + ((size_t)r * gridDim.x + blockIdx.x) * 16;
+          pr[0] = t;
+          pr[1] = prof_acc[0];
+          pr[2] = prof_acc[1];
+        }
       }
     }
   } else {
     // ------------------------------------------------------------------ MMA + epilogue (warps 0..7: two warpgroups)
     // Warpgroup wg issues the wgmmas of accumulator rows 64*wg .. +63 of every tile (register accumulators), then all eight warps
     // run the epilogue from a shared-memory copy of the accumulators; the producer warp keeps the ring full meanwhile.
+    // Ping-pong: warpgroup wg owns every other tile of the CTA (64 pixels, all BLOCK_N columns) and runs its MMAs and its epilogue
+    // alone, with its own accumulator rows 64*wg.., staging tiles, residual tile, bias and epilogue barrier.
     const int wg = warp >> 2;
     // fused decode: the rows of warpgroup wg are decode group wg (its staging half, barrier and bulk store); plain epilogue: two warps
-    // per row quarter, each converting half of the columns of every staged group
+    // per row quarter (ping-pong: per row half), each converting half of the columns of every staged group
     const int q = warp & 3;
-    const int half = YOLO ? ((warp >> 1) & 1) : (warp >> 2);
-    const int row = YOLO ? 64 * wg + 32 * (warp & 1) + lane : q * 32 + lane;  // accumulator row == pixel index inside the tile box
-    const int tid_e = threadIdx.x;
+    const int half = YOLO ? ((warp >> 1) & 1) : (PP ? (q >> 1) : (warp >> 2));
+    const int row = YOLO ? 64 * wg + 32 * (warp & 1) + lane : (PP ? (q & 1) * 32 + lane : q * 32 + lane);  // pixel index inside the tile box
+    const int tid_e = PP ? (int)threadIdx.x & (EPI_THREADS - 1) : (int)threadIdx.x;
+    const int ebar = PP ? 2 + wg : 1;                                         // epilogue barrier of the tile's EPI_THREADS threads
+    float* const acc_t = acc_s + (PP ? 64 * wg * ACC_PITCH : 0);               // accumulator rows of the tile
+    float* const bias_t = bias_s + (PP ? wg * BLOCK_N : 0);
+    uint64_t* const rfull_t = rfull + (PP ? wg : 0);
+    uint8_t* const res_t = res_stage + (PP ? wg * Cfg::OUT_TILE_BYTES : 0);
     const int tw = row % a.TW;
     const int r2 = row / a.TW;
     const int th = r2 % a.TH;
@@ -446,14 +465,16 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
     };
     // One tile: dm = gain * (hi*hi chain) + cross terms.  The tensor core's fp32 adder rounds toward zero, so a long accumulation chain
     // shrinks |sum| slightly per MMA; rz_gain undoes the mean shrink and the (2^-11 smaller) cross terms have their own accumulator.
-    auto mainloop = [&]() {
+    // Ping-pong: `pass_turn` hands the tensor pipe to the other warpgroup (named barrier 4 + other) once every MMA of the tile has been
+    // issued, before this warpgroup waits for them to complete.
+    auto mainloop = [&](bool pass_turn) {
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) dm[i] = 0.0f;
       if constexpr (SPLIT) {
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) dc[i] = 0.0f;
       }
-      if (a.halo) {
+      if (halo) {
         // copy / tap mode: every tap is a row-shifted descriptor view of the copy in the current A slot; weight tiles come from the
         // resident slab or from their own ring.  The taps of a copy form an ny x nx grid (filter rows x filter columns) whose view
         // offsets and weight indices are affine in (y, x): two running descriptor words, no per-tap table.
@@ -496,7 +517,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
         }
       } else {
         const uint32_t lo16 = a.a_lo_off >> 4;
-        const uint32_t wg16 = (uint32_t)wg * (4u * SWZ);  // rows 64*wg..: eight 8-row groups of 8 * SWZ bytes
+        const uint32_t wg16 = PP ? 0u : (uint32_t)wg * (4u * SWZ);  // rows 64*wg..: eight 8-row groups of 8 * SWZ bytes
         uint32_t bres_it16 = bres16;
         for (int i = 0; i < k_iters; ++i, bres_it16 += 2u * kB16) {
           mbar_wait(&full[stage], phase, 300 + stage);
@@ -512,6 +533,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           }
         }
       }
+      if (PP && pass_turn) named_bar_arrive(4 + (wg ^ 1), kEpiThreads);
       wgmma_wait<0>();
       wgmma_fence_regs(dm);
       if constexpr (SPLIT) wgmma_fence_regs(dc);
@@ -528,7 +550,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
       }
     };
     // accumulator columns [c0, c0 + ncols) of this thread's fragment -> acc_s (columns relative to c0).  wgmma fragment: rows
-    // 64*wg + 16*(warp&3) + lane/4 (+8), columns 8*j + 2*(lane&3) (+1)
+    // 64*wg + 16*(warp&3) + lane/4 (+8), columns 8*j + 2*(lane&3) (+1); in both schedules accumulator row 64*wg + r holds wgmma row r
     const int fr = 64 * wg + 16 * q + (lane >> 2), fc = 2 * (lane & 3);
     auto dump = [&](int c0, int ncols) {
 #pragma unroll
@@ -557,9 +579,9 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
       const int t2_ = fast_div(mt_, a.tiles_w, a.mg_w), wt_ = mt_ - t2_ * a.tiles_w;
       const int bt_ = fast_div(t2_, a.tiles_h, a.mg_h), ht_ = t2_ - bt_ * a.tiles_h;
       const int c0 = nt_ * BLOCK_N + g * OUT_GROUP_CH;
-      mbar_expect_tx(rfull, (uint32_t)(2 * a.rows_valid * OUT_ROW_BYTES));
-      tma_load_5d(&a.tmR, rfull, res_stage, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 0);
-      tma_load_5d(&a.tmR, rfull, res_stage + Cfg::OUT_PLANE_BYTES, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 1);
+      mbar_expect_tx(rfull_t, (uint32_t)(2 * a.rows_valid * OUT_ROW_BYTES));
+      tma_load_5d(&a.tmR, rfull_t, res_t, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 0);
+      tma_load_5d(&a.tmR, rfull_t, res_t + Cfg::OUT_PLANE_BYTES, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 1);
     };
     // fused YOLOv5 decode (YOLO kernels): staging tile [128 rows][85] fp32 + per-row partial best scores + per-image NMS histogram
     float* y_stage = reinterpret_cast<float*>(out_stage0);
@@ -586,12 +608,15 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
       for (int i = tid_e; i < a.tiles_n * BLOCK_N; i += EPI_THREADS)
         y_bias[i] = ((i & (BLOCK_N - 1)) < a.y_no && i < a.bias_len) ? a.bias[i] : -CUDART_INF_F;
     }
-    if (resid_tma && tid_e == 0 && t_begin < t_end) issue_residual(t_begin, 0);
+    // this thread's tiles: all of the CTA's, or (ping-pong) every other one, starting with the warpgroup's index
+    const int my_begin = PP ? t_begin + wg * t_step : t_begin;
+    const int my_step = PP ? 2 * t_step : t_step;
+    if (resid_tma && tid_e == 0 && my_begin < t_end) issue_residual(my_begin, 0);
     if (a.b_resident && t_begin < t_end) mbar_wait(bfull, 0, 250);
     // per-thread pixel coordinates are needed only by the operands read with per-thread loads (up-partial, non-TMA residual) and by the
     // fused decode; the plain path knows its tile through the TMA store coordinates alone
     const bool need_rows = EPI != 0 ? false : (YOLO || a.up != nullptr || (a.resid != nullptr && !resid_tma));
-    for (int tile = (dbg & 16) ? t_end : t_begin; tile < t_end; tile += t_step) {
+    for (int tile = (dbg & 16) ? t_end : my_begin, kt = PP ? wg : 0; tile < t_end; tile += my_step, kt += PP ? 2 : 1) {
       const int mt = fast_div(tile, a.tiles_n, a.mg_n);
       const int nt = tile - mt * a.tiles_n;
       const int t2 = fast_div(mt, a.tiles_w, a.mg_w);
@@ -604,17 +629,25 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
 
       {
         const long long pt0 = prof_on ? clock64() : 0;
-        mainloop();
-        if (prof_on) prof_acc[0] += clock64() - pt0;  // MMA main loop (including the waits for operands)
+        if constexpr (PP) {
+          // the producer fills the ring in the CTA's tile order: this tile (the CTA's kt-th) starts at ring position kt * k_iters
+          const int pos = kt * k_iters;
+          stage = pos % STAGES;
+          phase = (uint32_t)(pos / STAGES) & 1u;
+          a_ring16 = ring16 + (uint32_t)stage * stage16;
+          if (kt > 0) named_bar_sync(4 + wg, kEpiThreads);  // wait for the turn: the other warpgroup has issued the previous tile
+        }
+        mainloop(tile + t_step < t_end);
+        if (prof_on) prof_acc[0] += clock64() - pt0;  // MMA main loop (including the waits for operands and, ping-pong, for the turn)
       }
 
       if (!YOLO && n0 != cur_n0) {
-        named_bar_sync(1, EPI_THREADS);
+        named_bar_sync(ebar, EPI_THREADS);
         for (int i = tid_e; i < BLOCK_N; i += EPI_THREADS) {
           float bv = (n0 + i < a.bias_len) ? a.bias[n0 + i] : 0.0f;
-          bias_s[i] = bv;
+          bias_t[i] = bv;
         }
-        named_bar_sync(1, EPI_THREADS);
+        named_bar_sync(ebar, EPI_THREADS);
         cur_n0 = n0;
       }
       const float* up_row = nullptr;
@@ -783,7 +816,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
         load_extras(0);
         if constexpr (!OUT_F32) {
           if (resid_tma) {
-            mbar_wait(rfull, res_phase, 500);
+            mbar_wait(rfull_t, res_phase, 500);
             res_phase ^= 1;
           }
         }
@@ -795,13 +828,13 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           if (a.out_bufs == 2) tma_store_wait_read1();
           else tma_store_wait_read0();
         }
-        named_bar_sync(1, EPI_THREADS);
+        named_bar_sync(ebar, EPI_THREADS);
         if (prof_on) {
           const long long t = clock64();
           prof_acc[1] += t - pt0;  // staging tile free (TMA store read + barrier)
           pt0 = t;
         }
-        uint8_t* out_stage = out_stage0 + (gcount & (a.out_bufs - 1)) * Cfg::OUT_STAGE_BYTES;
+        uint8_t* out_stage = out_stage0 + (gcount & (a.out_bufs - 1)) * Cfg::OUT_STAGE_BYTES + (PP ? wg * Cfg::OUT_TILE_BYTES : 0);
         ++gcount;
 #pragma unroll
         for (int sc = 0; sc < CW / SUB; ++sc) {
@@ -810,7 +843,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           if (sc > 0) load_extras(sc);
           if constexpr (!OUT_F32) {
             if (resid_tma) {  // same swizzled chunk addressing as the output staging tile below
-              const uint8_t* rh = res_stage + row * OUT_ROW_BYTES;
+              const uint8_t* rh = res_t + row * OUT_ROW_BYTES;
 #pragma unroll
               for (int j = 0; j < SUB / 8; ++j) {
                 const int cj = half * (CW / 8) + sc * (SUB / 8) + j;
@@ -824,7 +857,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           }
           float f[SUB];
           {
-            const float* ap = acc_s + row * ACC_PITCH + (col - g * OUT_GROUP_CH);
+            const float* ap = acc_t + row * ACC_PITCH + (col - g * OUT_GROUP_CH);
 #pragma unroll
             for (int j = 0; j < SUB / 4; ++j) {
               const float4 v4 = *reinterpret_cast<const float4*>(ap + 4 * j);
@@ -837,7 +870,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           float bv[SUB];  // bias of this thread's columns: 16-byte shared-memory loads
 #pragma unroll
           for (int j = 0; j < SUB / 4; ++j) {
-            const float4 b4 = *reinterpret_cast<const float4*>(bias_s + col + 4 * j);
+            const float4 b4 = *reinterpret_cast<const float4*>(bias_t + col + 4 * j);
             bv[4 * j] = b4.x;
             bv[4 * j + 1] = b4.y;
             bv[4 * j + 2] = b4.z;
@@ -926,7 +959,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           prof_acc[2] += t - pt0;  // accumulator reads + conversion + staging
           pt0 = t;
         }
-        named_bar_sync(1, EPI_THREADS);
+        named_bar_sync(ebar, EPI_THREADS);
         if (prof_on) {
           const long long t = clock64();
           prof_acc[3] += t - pt0;  // barrier after the conversion
@@ -941,7 +974,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
           tma_store_commit();
           if (resid_tma) {  // every epilogue thread has consumed the residual tile (barrier above): fetch the next one
             if (g + 1 < kGroups) issue_residual(tile, g + 1);
-            else if (tile + t_step < t_end) issue_residual(tile + t_step, 0);
+            else if (tile + my_step < t_end) issue_residual(tile + my_step, 0);
           }
         }
         if (prof_on) prof_acc[4] += clock64() - pt0;  // store issue
@@ -953,9 +986,10 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_ker
     }
     if (tid_e == 0) tma_store_wait_all0();
     if (prof_on && tid_e == 0) {  // epilogue: total cycles, MMA main loop, staging waits, conversion, barrier, store issue
-      a.prof[blockIdx.x * 16 + 8] = clock64() - prof_t0;
-      a.prof[blockIdx.x * 16 + 9] = prof_acc[0];
-      for (int i = 1; i < 5; ++i) a.prof[blockIdx.x * 16 + 9 + i] = prof_acc[i];
+      long long* pr = a.prof + ((size_t)(PP ? wg : 0) * gridDim.x + blockIdx.x) * 16;  // ping-pong: one counter row per warpgroup
+      pr[8] = clock64() - prof_t0;
+      pr[9] = prof_acc[0];
+      for (int i = 1; i < 5; ++i) pr[9 + i] = prof_acc[i];
     }
   }
 }
@@ -966,31 +1000,46 @@ struct KernelEntry {
   int stage_bytes, out_stage_bytes, tail_bytes;
 };
 
-template <int BN, int BK, bool F32, bool YOLO = false, int EPI = 0>
+template <int BN, int BK, bool F32, bool YOLO = false, int EPI = 0, bool PP = false>
 static KernelEntry entry() {
-  using Cfg = ConvCfg<BN, BK, F32, YOLO>;
-  return KernelEntry{reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, F32, YOLO, EPI>), Cfg::STAGE_BYTES, Cfg::OUT_STAGE_BYTES,
+  using Cfg = ConvCfg<BN, BK, F32, YOLO, PP>;
+  return KernelEntry{reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, F32, YOLO, EPI, PP>), Cfg::STAGE_BYTES, Cfg::OUT_STAGE_BYTES,
                      Cfg::TAIL_BYTES};
 }
 
-static bool lookup_kernel(int bn, int bk, bool f32, KernelEntry* e, bool yolo = false, int epi = 0) {
+template <int BN, int BK, bool PP>
+static KernelEntry entry_epi(bool f32, int epi) {
+  return f32 ? entry<BN, BK, true, false, 0, PP>()
+             : (epi == 1 ? entry<BN, BK, false, false, 1, PP>() : (epi == 2 ? entry<BN, BK, false, false, 2, PP>() : (epi == 3 ? entry<BN, BK, false, false, 3, PP>()
+             : (epi == 4 ? entry<BN, BK, false, false, 4, PP>() : entry<BN, BK, false, false, 0, PP>()))));
+}
+
+// pp: the ping-pong schedule, instantiated for block_n = 128 (at 256 its generic and residual epilogues spill more than the
+// cooperative kernel's)
+static bool lookup_kernel(int bn, int bk, bool f32, KernelEntry* e, bool yolo = false, int epi = 0, bool pp = false) {
   if (yolo) {  // fused-decode epilogue: one anchor per 128-wide n-tile
+    if (pp) return false;
     if (bn == 128 && bk == 32) { *e = entry<128, 32, true, true>(); return true; }
     if (bn == 128 && bk == 64) { *e = entry<128, 64, true, true>(); return true; }
     return false;
   }
-#define CVB_CASE(BN, BK)                                                                                          \
-  if (bn == BN && bk == BK) {                                                                                     \
-    *e = f32 ? entry<BN, BK, true>()                                                                              \
-             : (epi == 1 ? entry<BN, BK, false, false, 1>() : (epi == 2 ? entry<BN, BK, false, false, 2>() : (epi == 3 ? entry<BN, BK, false, false, 3>() \
-             : (epi == 4 ? entry<BN, BK, false, false, 4>() : entry<BN, BK, false>())))); \
-    return true;                                                                                                  \
+#define CVB_CASE(BN, BK)                                  \
+  if (bn == BN && bk == BK) {                             \
+    *e = entry_epi<BN, BK, false>(f32, epi);              \
+    return true;                                          \
   }
+#define CVB_CASE_PP(BN, BK)                               \
+  if (bn == BN && bk == BK) {                             \
+    *e = pp ? entry_epi<BN, BK, true>(f32, epi) : entry_epi<BN, BK, false>(f32, epi); \
+    return true;                                          \
+  }
+  if (pp && bn != 128) return false;
   CVB_CASE(32, 16) CVB_CASE(32, 32) CVB_CASE(32, 64)
   CVB_CASE(64, 16) CVB_CASE(64, 32) CVB_CASE(64, 64)
-  CVB_CASE(128, 16) CVB_CASE(128, 32) CVB_CASE(128, 64)
+  CVB_CASE_PP(128, 16) CVB_CASE_PP(128, 32) CVB_CASE_PP(128, 64)
   CVB_CASE(256, 16) CVB_CASE(256, 32) CVB_CASE(256, 64)
 #undef CVB_CASE
+#undef CVB_CASE_PP
   return false;
 }
 
@@ -1002,6 +1051,7 @@ struct CvbConvPlan {
   int grid;
   int smem;
   int threads;
+  int schedule;  // CVB_SCHED_COOPERATIVE or CVB_SCHED_PINGPONG
 };
 
 namespace cvb {
@@ -1028,21 +1078,21 @@ static CUtensorMapSwizzle swizzle_for_bytes(int bytes) {
   return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// Pick the output pixel box (TW x TH x NB <= 128) that wastes the fewest accumulator rows.
-static void choose_box(int B, int H, int W, int* TW, int* TH, int* NB) {
+// Pick the output pixel box (TW x TH x NB <= rows: the tile's accumulator rows) that wastes the fewest accumulator rows.
+static void choose_box(int B, int H, int W, int rows, int* TW, int* TH, int* NB) {
   double best = -1.0;
   int bw = 1, bh = 1, bb = 1;
-  for (int tw = 1; tw <= 128; ++tw) {
+  for (int tw = 1; tw <= rows; ++tw) {
     if (tw > W && tw != 1) break;
     if (!(tw == W || (tw & (tw - 1)) == 0)) continue;  // powers of two, or the full row
-    for (int th = 1; th * tw <= 128; ++th) {
+    for (int th = 1; th * tw <= rows; ++th) {
       if (th > H) break;
-      int nb = 128 / (tw * th);
+      int nb = rows / (tw * th);
       if (nb > B) nb = B;
       if (nb < 1) nb = 1;
       // keep all box dims <= 256 (TMA limit) -- implied by <= 128
       const long long tiles = (long long)ceil_div(W, tw) * ceil_div(H, th) * ceil_div(B, nb);
-      const double util = (double)B * H * W / ((double)tiles * 128.0);
+      const double util = (double)B * H * W / ((double)tiles * rows);
       const double score = util + 1e-4 * tw / 128.0;  // tie-break: longer contiguous rows
       if (score > best) {
         best = score;
@@ -1387,7 +1437,7 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
       if (have) {
         // classic estimate: one 128-row box per (tap, chunk); weights resident only below 64 KB
         int cTW, cTH, cNB;
-        choose_box(out.B, Ho, Wo, &cTW, &cTH, &cNB);
+        choose_box(out.B, Ho, Wo, kTileM, &cTW, &cTH, &cNB);
         const long long tiles_c = (long long)ceil_div(Wo, cTW) * ceil_div(Ho, cTH) * ceil_div(out.B, cNB) * ceil_div(cout, bn);
         const int chunks_c = cin / bk;
         const long long w_c = (long long)n_taps * chunks_c * 2 * bn * bk * 2;
@@ -1402,24 +1452,40 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     }
   }
   if (use_halo) bk = hc.bk;
-  if (!use_halo && !yolo) {
-    // the fp32 accumulator tile of the epilogue shares the 227 KB with the ring: halve the K chunk until two streamed stages fit
+  // the fp32 accumulator tile of the epilogue shares the 227 KB with the ring: halve the K chunk until two streamed stages fit
+  auto fit_bk = [&](bool pp_) {
     const bool rt = has_resid && !f32 && resid_tma_on;
+    const int tile_m = pp_ ? kTileM / 2 : kTileM;
+    int b = bk;
     KernelEntry kt;
-    while (bk > 16 && cin % (bk / 2) == 0 && lookup_kernel(bn, bk, f32, &kt) &&
-           kt.tail_bytes + (rt ? 2 : 1) * kt.out_stage_bytes + 2 * (2 * kTileM * bk * 2 + 2 * bn * bk * 2) > kSmemBudget)
-      bk /= 2;
-  }
+    while (b > 16 && cin % (b / 2) == 0 && lookup_kernel(bn, b, f32, &kt, false, 0, pp_) &&
+           kt.tail_bytes + (rt ? 2 : 1) * kt.out_stage_bytes + 2 * (2 * tile_m * b * 2 + 2 * bn * b * 2) > kSmemBudget)
+      b /= 2;
+    return b;
+  };
+  // ---- schedule.  Cooperative: both warpgroups share each 128-pixel tile and run its epilogue together, so the tensor pipe idles
+  // during every epilogue.  Ping-pong: 64-pixel tiles alternate between the warpgroups and one warpgroup's epilogue overlaps the other's
+  // MMAs.  It streams each weight tile from L2 once per 64 instead of 128 pixels, but its half-height activation stages also buy a
+  // deeper ring (or 64-wide K chunks) in the same shared memory.  Measured on the YOLOv5-s stack (DESIGN.md 6): faster on every
+  // block_n = 128 layer, streamed 3x3 and stride-2 ones included, except the 3x3 layers with a residual (the staging tile of the
+  // residual leaves the ring too shallow), which auto keeps cooperative.
+  CVB_REQUIRE(d->schedule >= CVB_SCHED_AUTO && d->schedule <= CVB_SCHED_PINGPONG, "conv: schedule %d unsupported", d->schedule);
+  const bool pp_ok = !yolo && !use_halo && bn == 128;  // (one CTA per SM)
+  CVB_REQUIRE(d->schedule != CVB_SCHED_PINGPONG || pp_ok,
+              "conv: the ping-pong schedule needs block_n = 128 and no halo loader or fused decode");
+  const bool pp = pp_ok && (d->schedule == CVB_SCHED_PINGPONG || (d->schedule == CVB_SCHED_AUTO && !(has_resid && n_taps > 1)));
+  if (!use_halo && !yolo) bk = fit_bk(pp);
   KernelEntry ke;
-  CVB_REQUIRE(lookup_kernel(bn, bk, f32, &ke, yolo), "conv: no kernel for block_n=%d block_k=%d yolo=%d", bn, bk, (int)yolo);
+  CVB_REQUIRE(lookup_kernel(bn, bk, f32, &ke, yolo, 0, pp), "conv: no kernel for block_n=%d block_k=%d yolo=%d", bn, bk, (int)yolo);
 
   CvbConvPlan* p = new (std::nothrow) CvbConvPlan();
   CVB_REQUIRE(p != nullptr, "out of host memory");
   ConvKArgs& a = p->args;
   memset(&a, 0, sizeof(a));
 
+  const int tile_m = pp ? kTileM / 2 : kTileM;  // output pixels of one tile
   int TW, TH, NB;
-  choose_box(out.B, Ho, Wo, &TW, &TH, &NB);
+  choose_box(out.B, Ho, Wo, tile_m, &TW, &TH, &NB);
   if (yolo) {  // one image per tile (the epilogue keeps a per-image histogram), 128 consecutive pixels of the flattened level
     TW = Wo < kTileM ? Wo : kTileM;
     TH = 1;
@@ -1459,7 +1525,7 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   a.rows_valid = TW * TH * NB;
   a.a_box_bytes = (uint32_t)(TW * TH * NB * bk * 2);
   a.a_fused = (a.rows_valid % 8 == 0) ? 1 : 0;  // the lo plane must start on a swizzle-atom boundary (8 rows)
-  a.a_lo_off = a.a_fused ? a.a_box_bytes : (uint32_t)(kTileM * bk * 2);
+  a.a_lo_off = a.a_fused ? a.a_box_bytes : (uint32_t)(tile_m * bk * 2);
   a.bias = d->bias;
   a.bias_len = d->cout_pad;
 
@@ -1606,7 +1672,7 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   }
   // ---- shared-memory plan: ring depth, resident weights, output staging
   const int k_iters = a.taps * a.chunks;
-  const int a_stage = 2 * kTileM * bk * 2;   // hi + lo activation tiles of one K chunk
+  const int a_stage = 2 * tile_m * bk * 2;   // hi + lo activation tiles of one K chunk
   const int b_stage = 2 * bn * bk * 2;       // hi + lo weight tiles of one K chunk
   const int base = ke.tail_bytes + (a.resid_tma ? ke.out_stage_bytes : 0);
   const bool can_pin_n = (a.tiles_n == 1 || a.tiles_n == 2 || a.tiles_n == 4);
@@ -1716,10 +1782,11 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     }
     if (epi) {
       KernelEntry k2;
-      if (lookup_kernel(bn, bk, f32, &k2, false, epi)) p->fn = k2.fn;
+      if (lookup_kernel(bn, bk, f32, &k2, false, epi, pp)) p->fn = k2.fn;
     }
   }
   p->threads = kThreads;
+  p->schedule = pp ? CVB_SCHED_PINGPONG : CVB_SCHED_COOPERATIVE;
   {
     const char* e = getenv("CVB_DBG");  // diagnostics only (tools/conv_pipeline_profile.py): results are wrong when set
     a.dbg = e ? atoi(e) : 0;
@@ -1762,9 +1829,9 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     static const bool dbg = [] { const char* e = getenv("CVB_PLAN_DEBUG"); return e && atoi(e) != 0; }();
     if (dbg)
       fprintf(stderr, "[cvb plan] cin=%d cout=%d k=%dx%d s=%d out=%dx%dx%d bn=%d bk=%d stages=%d resident=%d out_bufs=%d ctas/sm=%d "
-              "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d\n", cin, cout, d->kh, d->kw, d->stride, out.B, Ho, Wo, bn, bk,
+              "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s\n", cin, cout, d->kh, d->kw, d->stride, out.B, Ho, Wo, bn, bk,
               stages, a.b_resident, a.out_bufs, ctas_per_sm, p->smem, p->grid, total, a.resid_tma, a.halo,
-              a.n_copies, a.sb_stages, a.a_slot_bytes, a.kskip);
+              a.n_copies, a.sb_stages, a.a_slot_bytes, a.kskip, pp ? "pingpong" : "cooperative");
   }
   *out_plan = p;
   return CVB_OK;
@@ -1809,6 +1876,6 @@ extern "C" void cvb_conv_plan_destroy(CvbConvPlan* p) { delete p; }
 extern "C" int cvb_conv_plan_set_profile(CvbConvPlan* p, long long* counters, int32_t* grid) {
   CVB_REQUIRE(p != nullptr, "null plan");
   p->args.prof = counters;
-  if (grid) *grid = p->grid;
+  if (grid) *grid = p->schedule == CVB_SCHED_PINGPONG ? 2 * p->grid : p->grid;  // counter rows: one per warpgroup in ping-pong
   return CVB_OK;
 }

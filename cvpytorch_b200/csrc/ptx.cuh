@@ -143,5 +143,6 @@ __device__ __forceinline__ uint64_t make_kmajor_desc_sbo(uint32_t smem_addr, uin
   return d;
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 }  // namespace cvb

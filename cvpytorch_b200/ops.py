@@ -169,9 +169,10 @@ class ConvPlan:
 
     def __init__(self, inp, out, weights, bias, k, stride=1, pad=0, dilation=1, act=None, residual=None,
                  up_partial=None, block_n=0, sm_limit=0, keepalive=(), w_window=0, no_resident=0, residual_before_act=0, halo=0, residual_scale=1.0,
-                 yolo=None):
+                 yolo=None, schedule=0):
         """yolo: a CvbYoloDecode -> the conv's epilogue is the YOLOv5 decode (out_kind CVB_OUT_YOLO, see include/cvb200.h); `out` then only
-        carries B/H/W with C = na * 128 and `weights` / `bias` must come from pack_yolo_head_weights."""
+        carries B/H/W with C = na * 128 and `weights` / `bias` must come from pack_yolo_head_weights.
+        schedule: 0 = auto, 1 = cooperative, 2 = ping-pong (CvbConvDesc.schedule)."""
         d = CvbConvDesc()
         d.inp, d.out = inp, out
         d.weights = weights.data_ptr()
@@ -193,6 +194,7 @@ class ConvPlan:
         d.residual_before_act = residual_before_act
         d.halo = halo
         d.residual_scale = float(residual_scale)
+        d.schedule = schedule
         self._keep = (weights, bias) + tuple(keepalive)
         self.handle = c_void_p()
         _lib.check(_lib.lib().cvb_conv_plan_create(byref(d), byref(self.handle)), 'cvb_conv_plan_create')

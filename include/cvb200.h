@@ -113,17 +113,27 @@ typedef struct CvbConvDesc {
   const CvbYoloDecode* yolo; /* required iff out_kind == CVB_OUT_YOLO */
   float residual_scale; /* out = act(...) + residual_scale * residual (0 is read as 1): the learnable shortcut weight `alpha` of the YOLOv6
                            BottleRep block (src/models/modules/yolo_modules.py:474-492) */
+  int32_t schedule;     /* CVB_SCHED_*: how the two MMA warpgroups share the work.  0 = auto (cost model), 1 = cooperative: both
+                           warpgroups compute each 128-pixel tile and run its epilogue together, 2 = ping-pong: 64-pixel tiles alternate
+                           between the warpgroups and one's epilogue overlaps the other's MMAs (block_n = 128 plans, which run one CTA per
+                           SM, without the halo loader or the fused decode; anything else is rejected).  Both give bit-identical outputs. */
 } CvbConvDesc;
+
+#define CVB_SCHED_AUTO 0
+#define CVB_SCHED_COOPERATIVE 1
+#define CVB_SCHED_PINGPONG 2
 
 typedef struct CvbConvPlan CvbConvPlan;
 
 int cvb_conv_plan_create(const CvbConvDesc* desc, CvbConvPlan** plan);
 int cvb_conv_plan_run(const CvbConvPlan* plan, void* stream);
 void cvb_conv_plan_destroy(CvbConvPlan* plan);
-/* Diagnostics: attach a device buffer of grid * 16 int64 cycle counters (NULL detaches); every CTA then records how long its TMA
+/* Diagnostics: attach a device buffer of rows * 16 int64 cycle counters (NULL detaches); every CTA then records how long its TMA
  * producer, MMA issuer and epilogue spent in total and waiting on each pipeline barrier
  * ([0..2] producer: total, wait free A slot, wait free weight slot; [4..7] MMA: total, wait accumulator, wait activations, wait
- * weights; [8..9] epilogue: total, wait accumulator).  *grid receives the number of CTAs.  Used by tools/conv_pipeline_profile.py. */
+ * weights; [8..9] epilogue: total, wait accumulator).  *grid receives the number of counter rows: one per CTA, or with the ping-pong
+ * schedule one per warpgroup (row r + grid * w for warpgroup w of CTA r; both rows carry the CTA's producer counters).
+ * Used by tools/conv_pipeline_profile.py. */
 int cvb_conv_plan_set_profile(CvbConvPlan* plan, long long* counters, int32_t* grid);
 /* Run n plans back to back on one stream (one C call per forward instead of one per layer). */
 int cvb_conv_plan_run_many(CvbConvPlan* const* plans, int32_t n, void* stream);
