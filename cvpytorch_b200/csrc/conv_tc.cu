@@ -215,8 +215,9 @@ struct ConvCfg {
 //   3 act = ReLU, no residual, no up-partial   4 act = ReLU, residual tile by TMA added BEFORE the activation (ResNet bottleneck)
 // PP selects the ping-pong schedule (one-CTA-per-SM plans, not for the fused decode or the halo loader): a tile is 64 pixels, the
 // CTA's tiles alternate between the two warpgroups, and a warpgroup runs its epilogue while the other one's MMAs run (DESIGN.md 4.1).
+// Only the cooperative narrow kernels may share an SM; a ping-pong plan always runs one CTA per SM and gets the full register budget.
 template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0, bool PP = false>
-__global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 ? 2 : 1)) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
+__global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
   using Cfg = ConvCfg<BLOCK_N, BLOCK_K, OUT_F32, YOLO, PP>;
   constexpr int SWZ = Cfg::SWZ;
   constexpr int A_BYTES = Cfg::A_BYTES;
@@ -1014,7 +1015,7 @@ static KernelEntry entry_epi(bool f32, int epi) {
              : (epi == 4 ? entry<BN, BK, false, false, 4, PP>() : entry<BN, BK, false, false, 0, PP>()))));
 }
 
-// pp: the ping-pong schedule, instantiated for block_n = 128 (at 256 its generic and residual epilogues spill more than the
+// pp: the ping-pong schedule, instantiated for block_n <= 128 (at 256 its generic and residual epilogues spill more than the
 // cooperative kernel's)
 static bool lookup_kernel(int bn, int bk, bool f32, KernelEntry* e, bool yolo = false, int epi = 0, bool pp = false) {
   if (yolo) {  // fused-decode epilogue: one anchor per 128-wide n-tile
@@ -1033,10 +1034,10 @@ static bool lookup_kernel(int bn, int bk, bool f32, KernelEntry* e, bool yolo = 
     *e = pp ? entry_epi<BN, BK, true>(f32, epi) : entry_epi<BN, BK, false>(f32, epi); \
     return true;                                          \
   }
-  if (pp && bn != 128) return false;
-  CVB_CASE(32, 16) CVB_CASE(32, 32) CVB_CASE(32, 64)
-  CVB_CASE(64, 16) CVB_CASE(64, 32) CVB_CASE(64, 64)
+  CVB_CASE_PP(32, 16) CVB_CASE_PP(32, 32) CVB_CASE_PP(32, 64)
+  CVB_CASE_PP(64, 16) CVB_CASE_PP(64, 32) CVB_CASE_PP(64, 64)
   CVB_CASE_PP(128, 16) CVB_CASE_PP(128, 32) CVB_CASE_PP(128, 64)
+  if (pp) return false;
   CVB_CASE(256, 16) CVB_CASE(256, 32) CVB_CASE(256, 64)
 #undef CVB_CASE
 #undef CVB_CASE_PP
@@ -1173,14 +1174,18 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   if (bn == 0) {
     bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : 128);
     static const int split128 = [] {
-      // 128-wide 1x1 layers with cin <= 128 run as two pinned 64-wide n-tiles so that two CTAs share an SM (measured +3-10 % on
-      // those layers; the activation tile is read twice, from L2).  CVB_SPLIT_N128=0 restores one 128-wide tile per CTA.
+      // 128-wide 1x1 layers with cin <= 128 and an up-sampled partial run as two pinned 64-wide n-tiles (one CTA per SM, ping-pong):
+      // the partial needs the generic epilogue, which spills at block_n = 128 and not at 64 (0.26 vs 0.50 ms at 80x80, B = 64).
+      // Without the partial, one 128-wide ping-pong tile measured between 2 % slower and 11 % faster than two 64-wide ones, 0.03 ms
+      // less over the eight such layers of the YOLOv5-s step (DESIGN.md 6).  Both give bitwise-equal outputs.  CVB_SPLIT_N128=0 keeps
+      // one 128-wide tile per CTA.
       const char* e = getenv("CVB_SPLIT_N128");
       return e ? atoi(e) : 1;
     }();
-    if (split128 && !f32 && d->kh * d->kw == 1 && cout == 128 && cin <= 128 && cin % 64 == 0) bn = 64;
+    if (split128 && !f32 && d->kh * d->kw == 1 && cout == 128 && cin <= 128 && cin % 64 == 0 && d->up_partial.base) bn = 64;
   }
   int bk = (cin % 64 == 0) ? 64 : (cin % 32 == 0 ? 32 : 16);
+  const int bk_full = bk;
   if (yolo) {
     bn = 128;  // one anchor per n-tile
     CVB_REQUIRE(cin % 32 == 0, "conv(yolo): cin must be a multiple of 32");
@@ -1192,9 +1197,9 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
       const int v = e ? atoi(e) : 0;
       return (v == 16 || v == 32 || v == 64) ? v : 32;
     }();
-    // 64-channel inputs into narrow tiles (1x1 convs and the row-window stems): half-size K chunks let two CTAs share an SM
-    // (see plan_smem below), which hides the epilogue latency these HBM-bound layers are limited by.  Multi-tap 3x3 layers
-    // keep 64-wide chunks: measured slower with twice the TMA operations.
+    // 64-channel inputs into narrow cooperative tiles (1x1 convs and the row-window stems): half-size K chunks shrink the ring
+    // stages, so that more of these plans fit two CTAs per SM (see plan_smem below); ping-pong plans go back to full chunks.
+    // Multi-tap 3x3 layers keep 64-wide chunks: measured slower with twice the TMA operations.
     if (bn <= 64 && (cin == 64 || (cin == 128 && cout > 64)) && (d->kh * d->kw == 1 || win > 0)) bk = bk_small;
   }
   // ---- filter taps: (input map, row offset, column offset) of every tap; stride 2 reads four "parity" maps
@@ -1452,29 +1457,86 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     }
   }
   if (use_halo) bk = hc.bk;
+  const bool rt = has_resid && !f32 && resid_tma_on;  // (classic loader) the residual tile arrives by TMA into its own staging tile
   // the fp32 accumulator tile of the epilogue shares the 227 KB with the ring: halve the K chunk until two streamed stages fit
-  auto fit_bk = [&](bool pp_) {
-    const bool rt = has_resid && !f32 && resid_tma_on;
+  auto fit_bk = [&](int b, bool pp_) {
     const int tile_m = pp_ ? kTileM / 2 : kTileM;
-    int b = bk;
     KernelEntry kt;
     while (b > 16 && cin % (b / 2) == 0 && lookup_kernel(bn, b, f32, &kt, false, 0, pp_) &&
            kt.tail_bytes + (rt ? 2 : 1) * kt.out_stage_bytes + 2 * (2 * tile_m * b * 2 + 2 * bn * b * 2) > kSmemBudget)
       b /= 2;
     return b;
   };
+  // ring depth / resident weights / staging buffers of a classic-loader plan (kernel ke_, tile_m-pixel tiles, K chunk bk_) that fit
+  // `budget` bytes of dynamic shared memory (0 stages = no fit)
+  auto plan_smem = [&](int budget, int tile_m, int bk_, const KernelEntry& ke_, int& resident, int& out_bufs) -> int {
+    const int k_it = n_taps * (cin / bk_);
+    const int a_st = 2 * tile_m * bk_ * 2, b_st = 2 * bn * bk_ * 2;
+    const int base_ = ke_.tail_bytes + (rt ? ke_.out_stage_bytes : 0);
+    const bool can_res = can_pin && !d->no_resident && (long long)k_it * b_st <= 64 * 1024;
+    resident = 0;
+    out_bufs = 1;
+    if (can_res) {
+      // the CTA's n-tile never changes and its whole weight slab fits: keep it resident, stream only activations
+      const int st = (budget - base_ - 2 * ke_.out_stage_bytes - k_it * b_st) / a_st;
+      if (st >= 3 || (st >= 2 && k_it == 1)) {
+        resident = 1;
+        out_bufs = 2;
+        return st;
+      }
+    }
+    const int st2 = (budget - base_ - 2 * ke_.out_stage_bytes) / (a_st + b_st);
+    if (st2 >= 3) {
+      out_bufs = 2;
+      return st2;
+    }
+    if (can_res) {
+      const int st = (budget - base_ - ke_.out_stage_bytes - k_it * b_st) / a_st;
+      if (st >= 3) {
+        resident = 1;
+        return st;
+      }
+    }
+    return (budget - base_ - ke_.out_stage_bytes) / (a_st + b_st);
+  };
+  // ---- CTAs per SM of the cooperative plan.  Narrow tiles whose ring, staging and accumulator tiles fit in half the shared memory
+  // run two CTAs per SM, so one CTA's epilogue overlaps the other's main loop.  On the H100 every CTA also holds the fp32
+  // accumulator tile, so most block_n = 64 plans do not fit and run one CTA per SM.
+  int st_two = 0, res_two = 0, ob_two = 1;
+  bool two_ctas = use_halo && hc.ctas == 2;
+  if (!use_halo && !yolo) {
+    bk = fit_bk(bk, false);
+    KernelEntry kc;
+    if (bn <= 64 && two_ctas_on && lookup_kernel(bn, bk, f32, &kc)) {
+      st_two = plan_smem(kSmemBudget2, kTileM, bk, kc, res_two, ob_two);
+      two_ctas = st_two >= 3 || (st_two >= 2 && ob_two == 2);
+    }
+  }
   // ---- schedule.  Cooperative: both warpgroups share each 128-pixel tile and run its epilogue together, so the tensor pipe idles
-  // during every epilogue.  Ping-pong: 64-pixel tiles alternate between the warpgroups and one warpgroup's epilogue overlaps the other's
-  // MMAs.  It streams each weight tile from L2 once per 64 instead of 128 pixels, but its half-height activation stages also buy a
-  // deeper ring (or 64-wide K chunks) in the same shared memory.  Measured on the YOLOv5-s stack (DESIGN.md 6): faster on every
-  // block_n = 128 layer, streamed 3x3 and stride-2 ones included, except the 3x3 layers with a residual (the staging tile of the
-  // residual leaves the ring too shallow), which auto keeps cooperative.
+  // during every epilogue (unless a second CTA on the SM fills it).  Ping-pong: 64-pixel tiles alternate between the warpgroups and one
+  // warpgroup's epilogue overlaps the other's MMAs.  It streams each weight tile from L2 once per 64 instead of 128 pixels, but its
+  // half-height activation stages also buy a deeper ring (or 64-wide K chunks) in the same shared memory.  Eligible: every one-CTA-per-SM
+  // plan on the classic loader with block_n = 128, or with block_n <= 64 on a layer of at most 128 output channels -- the narrow plans
+  // auto picks (narrow layers and the 128 -> 128 split).  A wider layer forced to narrow tiles would read every 64-pixel activation tile
+  // from L2 once per n-tile; it has its 128-wide ping-pong plan, so the forced narrow plan stays cooperative.
+  // Measured per layer on the YOLOv5-s stack (DESIGN.md 6): faster on every 1x1
+  // layer.  Multi-tap layers depend on the width and the residual.  At block_n = 128, ping-pong is faster on every 3x3 and stride-2
+  // layer except those with a residual, where the residual's staging tile leaves the ping-pong ring too shallow.  At block_n <= 64 it is
+  // the other way round.  Ping-pong re-streams the whole weight slab per 64 pixels, and the 3x3 layers without a residual measured
+  // 11-19 % slower.  With a residual, the cooperative ring is only two stages deep, and ping-pong measured 28 % faster.
   CVB_REQUIRE(d->schedule >= CVB_SCHED_AUTO && d->schedule <= CVB_SCHED_PINGPONG, "conv: schedule %d unsupported", d->schedule);
-  const bool pp_ok = !yolo && !use_halo && bn == 128;  // (one CTA per SM)
+  const bool narrow_wide = bn < 128 && cout > 128;  // a layer of more than 128 channels in narrow n-tiles
+  const bool pp_ok = !yolo && !use_halo && bn <= 128 && !narrow_wide && !two_ctas;
   CVB_REQUIRE(d->schedule != CVB_SCHED_PINGPONG || pp_ok,
-              "conv: the ping-pong schedule needs block_n = 128 and no halo loader or fused decode");
-  const bool pp = pp_ok && (d->schedule == CVB_SCHED_PINGPONG || (d->schedule == CVB_SCHED_AUTO && !(has_resid && n_taps > 1)));
-  if (!use_halo && !yolo) bk = fit_bk(pp);
+              "conv: the ping-pong schedule needs a one-CTA-per-SM plan on the classic loader with block_n = 128, or block_n <= 64 on a "
+              "layer of at most 128 channels (this plan %s)",
+              yolo ? "runs the fused decode" : (use_halo ? "uses the halo loader" : (bn > 128 ? "has block_n = 256"
+              : (narrow_wide ? "has narrow n-tiles on a layer of more than 128 channels"
+              : "runs two CTAs per SM, which already overlap one CTA's epilogue with the other's MMAs"))));
+  const bool pp_auto = n_taps == 1 || (bn == 128 ? !has_resid : has_resid);
+  const bool pp = pp_ok && (d->schedule == CVB_SCHED_PINGPONG || (d->schedule == CVB_SCHED_AUTO && pp_auto));
+  // a ping-pong plan runs one CTA per SM: no reason for the half-size K chunks of the narrow cooperative plans
+  if (pp) bk = fit_bk(bk_full, true);
   KernelEntry ke;
   CVB_REQUIRE(lookup_kernel(bn, bk, f32, &ke, yolo, 0, pp), "conv: no kernel for block_n=%d block_k=%d yolo=%d", bn, bk, (int)yolo);
 
@@ -1675,34 +1737,6 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   const int a_stage = 2 * tile_m * bk * 2;   // hi + lo activation tiles of one K chunk
   const int b_stage = 2 * bn * bk * 2;       // hi + lo weight tiles of one K chunk
   const int base = ke.tail_bytes + (a.resid_tma ? ke.out_stage_bytes : 0);
-  const bool can_pin_n = (a.tiles_n == 1 || a.tiles_n == 2 || a.tiles_n == 4);
-  // ring depth / resident weights / staging buffers that fit `budget` bytes of dynamic shared memory (0 stages = no fit)
-  auto plan_smem = [&](int budget, int& resident, int& out_bufs) -> int {
-    resident = 0;
-    out_bufs = 1;
-    if (can_pin_n && !d->no_resident && (long long)k_iters * b_stage <= 64 * 1024) {
-      // the CTA's n-tile never changes and its whole weight slab fits: keep it resident, stream only activations
-      const int st = (budget - base - 2 * ke.out_stage_bytes - k_iters * b_stage) / a_stage;
-      if (st >= 3 || (st >= 2 && k_iters == 1)) {
-        resident = 1;
-        out_bufs = 2;
-        return st;
-      }
-    }
-    const int st2 = (budget - base - 2 * ke.out_stage_bytes) / (a_stage + b_stage);
-    if (st2 >= 3) {
-      out_bufs = 2;
-      return st2;
-    }
-    if (can_pin_n && !d->no_resident && (long long)k_iters * b_stage <= 64 * 1024) {
-      const int st = (budget - base - ke.out_stage_bytes - k_iters * b_stage) / a_stage;
-      if (st >= 3) {
-        resident = 1;
-        return st;
-      }
-    }
-    return (budget - base - ke.out_stage_bytes) / (a_stage + b_stage);
-  };
   int stages = 0, ctas_per_sm = 1;
   if (yolo) {
     const CvbYoloDecode& y = *d->yolo;
@@ -1728,19 +1762,14 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     a.b_resident = hc.resident;
     a.out_bufs = hc.out_bufs;
     ctas_per_sm = hc.ctas;
-  } else if (bn <= 64 && two_ctas_on) {
-    // small-N tiles are bound by epilogue latency, not by smem capacity: two co-resident CTAs (each <= half the SM's shared
-    // memory) overlap one tile's epilogue with the other's main loop
-    int res, ob;
-    const int st = plan_smem(kSmemBudget2, res, ob);
-    if (st >= 3 || (st >= 2 && ob == 2)) {
-      stages = st;
-      a.b_resident = res;
-      a.out_bufs = ob;
-      ctas_per_sm = 2;
-    }
+  } else if (two_ctas) {
+    // the cooperative narrow plan that fits half the SM's shared memory (decided with the schedule above)
+    stages = st_two;
+    a.b_resident = res_two;
+    a.out_bufs = ob_two;
+    ctas_per_sm = 2;
   }
-  if (stages == 0) stages = plan_smem(kSmemBudget, a.b_resident, a.out_bufs);
+  if (stages == 0) stages = plan_smem(kSmemBudget, tile_m, bk, ke, a.b_resident, a.out_bufs);
   if (stages > 8) stages = 8;
   if (use_halo && (a.resid_tma != hc.resid_tma)) {
     delete p;

@@ -115,8 +115,10 @@ typedef struct CvbConvDesc {
                            BottleRep block (src/models/modules/yolo_modules.py:474-492) */
   int32_t schedule;     /* CVB_SCHED_*: how the two MMA warpgroups share the work.  0 = auto (cost model), 1 = cooperative: both
                            warpgroups compute each 128-pixel tile and run its epilogue together, 2 = ping-pong: 64-pixel tiles alternate
-                           between the warpgroups and one's epilogue overlaps the other's MMAs (block_n = 128 plans, which run one CTA per
-                           SM, without the halo loader or the fused decode; anything else is rejected).  Both give bit-identical outputs. */
+                           between the warpgroups and one's epilogue overlaps the other's MMAs (plans that run one CTA per SM, without
+                           the halo loader or the fused decode, with block_n = 128, or block_n <= 64 on a layer of at most 128 channels;
+                           a plan that fits two CTAs per SM already overlaps one CTA's epilogue with the other's MMAs; anything else is
+                           rejected).  Both give bit-identical outputs. */
 } CvbConvDesc;
 
 #define CVB_SCHED_AUTO 0

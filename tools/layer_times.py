@@ -33,8 +33,9 @@ def main():
     g.run()
     torch.cuda.synchronize()
     peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))) if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else {}
-    P = float(peaks.get('bf16_tflops', 1590.0))
-    BW = float(peaks.get('hbm_gbs', 6650.0))
+    # without measured peaks: the H100 SXM data-sheet rates (dense bf16, HBM3) that DESIGN.md and BASELINE.md use
+    P = float(peaks.get('bf16_tflops', 989.0))
+    BW = float(peaks.get('hbm_gbs', 3350.0))
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     rows = []
     li = 0
