@@ -23,6 +23,7 @@
 #include <math_constants.h>
 
 #include <cstdlib>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <type_traits>
@@ -47,6 +48,46 @@ constexpr int kYoloBiasBytes = 4 * 128 * 4;  // fused decode: bias of all (<= 4)
 constexpr int kYoloStageBytes = 45056;  // fused decode: [128][85] fp32 staging tile + 3 x 128 partial row maxima, rounded to 1 KB
 constexpr int kSmemBudget = 232448;  // 227 KB opt-in limit per CTA on sm_90
 constexpr int kSmemBudget2 = 115712;  // per CTA when two share an SM: (228 KB - 2 x 1 KB reserved) / 2
+constexpr int kMaxBars = 64;                  // mbarrier slots of a CTA
+constexpr int kBarBytes = kMaxBars * 8 + 16;  // mbarrier area
+
+// Per-tile shared-memory geometry of a kernel instantiation: the kernel's compile-time constants, and what the planner sizes plans with.
+// pp: ping-pong schedule -- a tile is 64 pixels and belongs to one warpgroup, so every per-tile buffer exists once per warpgroup.
+struct ConvGeom {
+  int tile_m;           // output pixels of one tile
+  int swz;              // swizzle span == bytes of one K chunk row
+  int a_bytes, b_bytes; // one plane of the activation / weight tile of one K chunk
+  int out_group_ch, out_row_bytes, out_plane_bytes;
+  int out_tile_bytes;   // staging tile of one output group of one tile
+  int out_buf_bytes;  // one staging buffer (ping-pong: one tile per warpgroup)
+  int acc_pitch, acc_bytes;
+  int bias_bytes;
+};
+__host__ __device__ constexpr ConvGeom conv_geom(int block_n, int block_k, bool f32, bool yolo, bool pp) {
+  const int tile_m = pp ? kTileM / 2 : kTileM;
+  const int gch = f32 ? 32 : (block_n >= 64 ? 64 : 32);
+  const int row = f32 ? 128 : gch * 2;
+  const int tile = tile_m * row * (f32 ? 1 : 2);
+  // fp32 accumulator tile the epilogue reads (one output group, or the 96 decoded columns of a fused-decode tile); rows padded by
+  // 16 bytes so that the row-per-thread reads of eight consecutive rows hit distinct banks.  Ping-pong: rows 64*wg.. are warpgroup wg's tile.
+  const int acc_pitch = (yolo ? 96 : gch) + 4;
+  return ConvGeom{tile_m, block_k * 2, tile_m * block_k * 2, block_n * block_k * 2, gch, row, tile_m * row, tile, tile * (pp ? 2 : 1),
+                  acc_pitch, kTileM * acc_pitch * 4, (pp ? 2 : 1) * block_n * 4};
+}
+
+// Byte offsets of the regions of a CTA's dynamic shared memory, in address order; the ring starts at offset 0.  smem_layout builds it on
+// the host.  The plan carries it in ConvKArgs::sm: the kernel reads the ring slot, and the diagnostics build checks its region pointers
+// against the offsets.
+struct SmemLayout {
+  int slot;     // bytes of one ring slot
+  int weights;  // resident weight slab, or the halo loader's weight ring
+  int out;      // output staging tiles (fused decode: staging tile, NMS histogram and bias)
+  int resid;    // residual staging tile
+  int acc;      // fp32 accumulator tile
+  int bias;     // bias of the current n-tile
+  int bars;     // mbarriers
+  int total;
+};
 
 struct alignas(64) ConvKArgs {
   CUtensorMap tmA[4];  // input, one per (row parity, col parity) for stride 2; only [0] for stride 1
@@ -88,7 +129,6 @@ struct alignas(64) ConvKArgs {
   int n_copies;
   int sb_stages;         // depth of the separate weight-tile ring (0: weights resident)
   int kskip;             // K steps (of 16) skipped at the end of every chunk (zero weight columns of the row-window stems)
-  uint32_t a_slot_bytes; // bytes of one A ring slot (hi + lo planes of the largest copy)
   uint32_t cp_bytes[6];  // bytes of ONE plane of copy c
   uint32_t cp_lo_off[6]; // offset of the lo plane inside the slot
   uint32_t cp_sbo[6];    // byte stride between the 8-row groups of a tap view of copy c (= one row of the copy's halo image)
@@ -112,11 +152,24 @@ struct alignas(64) ConvKArgs {
   uint32_t wait_hint;          // suspend-time hint (ns) of the producer's free-slot waits (CVB_WAIT_HINT, 0 = spin)
   int dbg;                     // diagnostics (CVB_DBG, results are WRONG): bit 0 = no TMA stores, bit 1 = activations loaded only for the first ring pass, bit 2 = epilogue skips the math / staging, bit 5 = fused decode without histogram atomics, bit 6 = without the z copy-out
   long long* prof;             // diagnostics (cvb_conv_plan_set_profile): per-CTA cycle counters of the three pipeline roles, or NULL
+  SmemLayout sm;
 };
 
 // x / d for 0 <= x with x * d < 2^32 (checked on the host, else magic = 0; magic = 1 means d == 1): one multiply-high instead of a
 // ~20-instruction division
 __device__ __forceinline__ int fast_div(int x, int d, uint32_t magic) { return magic == 1u ? x : (magic ? (int)__umulhi((uint32_t)x, magic) : x / d); }
+
+// first output column, row, image and channel of a tile; tile = ((bt * tiles_h + ht) * tiles_w + wt) * tiles_n + nt
+struct TileOrigin {
+  int w0, h0, b0, n0;
+};
+template <int BLOCK_N>
+__device__ __forceinline__ TileOrigin tile_origin(const ConvKArgs& a, int tile) {
+  const int mt = fast_div(tile, a.tiles_n, a.mg_n), nt = tile - mt * a.tiles_n;
+  const int t2 = fast_div(mt, a.tiles_w, a.mg_w), wt = mt - t2 * a.tiles_w;
+  const int bt = fast_div(t2, a.tiles_h, a.mg_h), ht = t2 - bt * a.tiles_h;
+  return TileOrigin{wt * a.TW, ht * a.TH, bt * a.NB, nt * BLOCK_N};
+}
 
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == CVB_ACT_SILU) return __fdividef(x, 1.0f + __expf(-x));
@@ -188,27 +241,6 @@ __device__ __forceinline__ void issue_tap(float (&dm)[BLOCK_N / 2], float (&dc)[
   }
 }
 
-// PP: ping-pong schedule -- a tile is 64 pixels and belongs to one warpgroup, so every per-tile buffer below exists once per warpgroup
-template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, bool PP = false>
-struct ConvCfg {
-  static constexpr int TILE_M = PP ? kTileM / 2 : kTileM;  // output pixels of one tile
-  static constexpr int SWZ = BLOCK_K * 2;  // swizzle span == bytes of one K chunk row
-  static constexpr int A_BYTES = TILE_M * SWZ;
-  static constexpr int B_BYTES = BLOCK_N * SWZ;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int OUT_GROUP_CH = OUT_F32 ? 32 : (BLOCK_N >= 64 ? 64 : 32);
-  static constexpr int OUT_ROW_BYTES = OUT_F32 ? 128 : OUT_GROUP_CH * 2;
-  static constexpr int OUT_PLANE_BYTES = TILE_M * OUT_ROW_BYTES;
-  static constexpr int OUT_TILE_BYTES = OUT_PLANE_BYTES * (OUT_F32 ? 1 : 2);  // staging tile of one output group of one tile
-  static constexpr int OUT_STAGE_BYTES = OUT_TILE_BYTES * (PP ? 2 : 1);       // one staging buffer (ping-pong: one tile per warpgroup)
-  // fp32 accumulator tile the epilogue reads (one output group, or the 96 decoded columns of a fused-decode tile); rows padded by
-  // 16 bytes so that the row-per-thread reads of eight consecutive rows hit distinct banks.  Ping-pong: rows 64*wg.. are warpgroup wg's tile.
-  static constexpr int ACC_COLS = YOLO ? 96 : OUT_GROUP_CH;
-  static constexpr int ACC_PITCH = ACC_COLS + 4;
-  static constexpr int ACC_BYTES = kTileM * ACC_PITCH * 4;
-  static constexpr int TAIL_BYTES = ACC_BYTES + (PP ? 2 : 1) * BLOCK_N * 4 + 64 * 8 + 16;  // accumulator tile + bias + barriers
-};
-
 // EPI selects a compile-time specialisation of the epilogue (the hot layers run a compact, branch-free instruction stream; the generic
 // stream with its run-time mode checks costs more issue slots per tile, and the HBM-bound layers are issue bound in the epilogue):
 //   0 generic   1 act = SiLU, no residual, no up-partial   2 act = SiLU, residual tile by TMA added after the activation (Darknet bottleneck)
@@ -218,14 +250,18 @@ struct ConvCfg {
 // Only the cooperative narrow kernels may share an SM; a ping-pong plan always runs one CTA per SM and gets the full register budget.
 template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0, bool PP = false>
 __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
-  using Cfg = ConvCfg<BLOCK_N, BLOCK_K, OUT_F32, YOLO, PP>;
-  constexpr int SWZ = Cfg::SWZ;
-  constexpr int A_BYTES = Cfg::A_BYTES;
-  constexpr int B_BYTES = Cfg::B_BYTES;
-  constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
-  constexpr int OUT_GROUP_CH = Cfg::OUT_GROUP_CH;
-  constexpr int OUT_ROW_BYTES = Cfg::OUT_ROW_BYTES;
-  constexpr int ACC_PITCH = Cfg::ACC_PITCH;
+  constexpr ConvGeom G = conv_geom(BLOCK_N, BLOCK_K, OUT_F32, YOLO, PP);
+  constexpr int SWZ = G.swz;
+  constexpr int A_BYTES = G.a_bytes;
+  constexpr int B_BYTES = G.b_bytes;
+  constexpr int OUT_GROUP_CH = G.out_group_ch;
+  constexpr int OUT_ROW_BYTES = G.out_row_bytes;
+  constexpr int OUT_PLANE_BYTES = G.out_plane_bytes;
+  constexpr int OUT_TILE_BYTES = G.out_tile_bytes;
+  constexpr int ACC_PITCH = G.acc_pitch;
+  // ring slots, weight tiles and staging tiles are multiples of the 1024-byte swizzle atom, so every TMA-swizzled region the host lays
+  // out starts on a 1024-byte boundary
+  static_assert(A_BYTES % 1024 == 0 && B_BYTES % 1024 == 0 && OUT_TILE_BYTES % 1024 == 0, "swizzled tiles must be 1024-byte multiples");
   constexpr int EPI_THREADS = PP ? kEpiThreads / 2 : kEpiThreads;  // threads that share one tile's epilogue
   constexpr bool SPLIT = BLOCK_N <= 128;
   static_assert(EPI == 0 || (!OUT_F32 && !YOLO), "epilogue specialisations exist for the split16 output only");
@@ -245,14 +281,24 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
   const int dbg = kDiag ? a.dbg : 0;  // diagnostics switches: compiled out of the product library
   const int STAGES = a.stages;
   const bool halo = PP ? false : a.halo != 0;
-  const int stage_bytes = halo ? (int)a.a_slot_bytes : (a.b_resident ? 2 * A_BYTES : STAGE_BYTES);
+  // Region pointers in smem_layout's order, chained from the plan's ring / weight / staging parameters and the compile-time geometry.
+  // Taking them from a.sm, or from smem_layout made a __host__ __device__ function, costs registers at the 168-register cap: ptxas adds
+  // spills to 23 to 53 of the instantiations.  The diagnostics build checks the chain against the plan's offsets.
+  const int stage_bytes = halo ? (int)a.sm.slot : (a.b_resident ? 2 * A_BYTES : 2 * A_BYTES + 2 * B_BYTES);
   uint8_t* stage_base = smem;
-  uint8_t* b_res = smem + STAGES * stage_bytes;                                  // resident weights: k_iters x {hi, lo} tiles (halo mode: or the weight ring)
+  uint8_t* b_res = smem + STAGES * stage_bytes;
   uint8_t* out_stage0 = b_res + (a.b_resident ? a.taps * a.chunks * 2 * B_BYTES : (halo ? a.sb_stages * 2 * B_BYTES : 0));
-  uint8_t* res_stage = out_stage0 + (YOLO ? kYoloStageBytes + kNmsBins * 4 + kYoloBiasBytes : a.out_bufs * Cfg::OUT_STAGE_BYTES);  // residual tile (same layout as an output tile)
-  float* acc_s = reinterpret_cast<float*>(res_stage + (resid_tma ? Cfg::OUT_STAGE_BYTES : 0));  // (fused decode: staging tile + histogram instead of output tiles)
-  float* bias_s = acc_s + Cfg::ACC_BYTES / 4;
+  uint8_t* res_stage = out_stage0 + (YOLO ? kYoloStageBytes + kNmsBins * 4 + kYoloBiasBytes : a.out_bufs * G.out_buf_bytes);
+  float* acc_s = reinterpret_cast<float*>(res_stage + (resid_tma ? G.out_buf_bytes : 0));
+  float* bias_s = acc_s + G.acc_bytes / 4;
   uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + (PP ? 2 : 1) * BLOCK_N);
+  if (kDiag && threadIdx.x == 0 &&
+      (b_res != smem + a.sm.weights || out_stage0 != smem + a.sm.out || res_stage != smem + a.sm.resid ||
+       reinterpret_cast<uint8_t*>(acc_s) != smem + a.sm.acc || reinterpret_cast<uint8_t*>(bias_s) != smem + a.sm.bias ||
+       reinterpret_cast<uint8_t*>(bars) != smem + a.sm.bars || stage_bytes != a.sm.slot)) {
+    printf("conv_tc_kernel: shared-memory regions differ from the plan's layout\n");
+    __trap();
+  }
   const int SB = halo ? a.sb_stages : 0;
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
@@ -329,10 +375,8 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
         int sb = 0;
         uint32_t phase_b = 0;
         for (int tile = t_begin; tile < t_end; tile += t_step) {
-          const int mt = fast_div(tile, a.tiles_n, a.mg_n), nt = tile - mt * a.tiles_n;
-          const int t2 = fast_div(mt, a.tiles_w, a.mg_w), wt = mt - t2 * a.tiles_w;
-          const int bt = fast_div(t2, a.tiles_h, a.mg_h), ht = t2 - bt * a.tiles_h;
-          const int w0 = wt * a.TW, h0 = ht * a.TH, b0 = bt * a.NB, n0 = nt * BLOCK_N;
+          const TileOrigin to = tile_origin<BLOCK_N>(a, tile);
+          const int w0 = to.w0, h0 = to.h0, b0 = to.b0, n0 = to.n0;
           for (int ck = 0; ck < a.chunks; ++ck) {
             int t = 0;
             for (int c = 0; c < a.n_copies; ++c) {
@@ -366,10 +410,8 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
         }
       } else
       for (int tile = t_begin; tile < t_end; tile += t_step) {
-        const int mt = fast_div(tile, a.tiles_n, a.mg_n), nt = tile - mt * a.tiles_n;
-        const int t2 = fast_div(mt, a.tiles_w, a.mg_w), wt = mt - t2 * a.tiles_w;
-        const int bt = fast_div(t2, a.tiles_h, a.mg_h), ht = t2 - bt * a.tiles_h;
-        const int w0 = wt * a.TW, h0 = ht * a.TH, b0 = bt * a.NB, n0 = nt * BLOCK_N;
+        const TileOrigin to = tile_origin<BLOCK_N>(a, tile);
+        const int w0 = to.w0, h0 = to.h0, b0 = to.b0, n0 = to.n0;
         for (int tap = 0; tap < a.taps; ++tap) {
           const CUtensorMap* mapA = &a.tmA[a.tap_map[tap]];
           const int cw = w0 + a.tap_dw[tap];
@@ -418,7 +460,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
     float* const acc_t = acc_s + (PP ? 64 * wg * ACC_PITCH : 0);               // accumulator rows of the tile
     float* const bias_t = bias_s + (PP ? wg * BLOCK_N : 0);
     uint64_t* const rfull_t = rfull + (PP ? wg : 0);
-    uint8_t* const res_t = res_stage + (PP ? wg * Cfg::OUT_TILE_BYTES : 0);
+    uint8_t* const res_t = res_stage + (PP ? wg * OUT_TILE_BYTES : 0);
     const int tw = row % a.TW;
     const int r2 = row / a.TW;
     const int th = r2 % a.TH;
@@ -576,13 +618,11 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
     const float rscale = (EPI == 2 || EPI == 4) ? 1.0f : a.resid_scale;  // (the specialised kernels are selected for unit shortcuts only)
     // residual tile of (tile, group): two TMA boxes (hi, lo) with the output tile's geometry; OOB parts are zero-filled
     auto issue_residual = [&](int tile_i, int g) {
-      const int mt_ = fast_div(tile_i, a.tiles_n, a.mg_n), nt_ = tile_i - mt_ * a.tiles_n;
-      const int t2_ = fast_div(mt_, a.tiles_w, a.mg_w), wt_ = mt_ - t2_ * a.tiles_w;
-      const int bt_ = fast_div(t2_, a.tiles_h, a.mg_h), ht_ = t2_ - bt_ * a.tiles_h;
-      const int c0 = nt_ * BLOCK_N + g * OUT_GROUP_CH;
+      const TileOrigin to = tile_origin<BLOCK_N>(a, tile_i);
+      const int c0 = to.n0 + g * OUT_GROUP_CH;
       mbar_expect_tx(rfull_t, (uint32_t)(2 * a.rows_valid * OUT_ROW_BYTES));
-      tma_load_5d(&a.tmR, rfull_t, res_t, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 0);
-      tma_load_5d(&a.tmR, rfull_t, res_t + Cfg::OUT_PLANE_BYTES, c0, wt_ * a.TW, ht_ * a.TH, bt_ * a.NB, 1);
+      tma_load_5d(&a.tmR, rfull_t, res_t, c0, to.w0, to.h0, to.b0, 0);
+      tma_load_5d(&a.tmR, rfull_t, res_t + OUT_PLANE_BYTES, c0, to.w0, to.h0, to.b0, 1);
     };
     // fused YOLOv5 decode (YOLO kernels): staging tile [128 rows][85] fp32 + per-row partial best scores + per-image NMS histogram
     float* y_stage = reinterpret_cast<float*>(out_stage0);
@@ -618,13 +658,8 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
     // fused decode; the plain path knows its tile through the TMA store coordinates alone
     const bool need_rows = EPI != 0 ? false : (YOLO || a.up != nullptr || (a.resid != nullptr && !resid_tma));
     for (int tile = (dbg & 16) ? t_end : my_begin, kt = PP ? wg : 0; tile < t_end; tile += my_step, kt += PP ? 2 : 1) {
-      const int mt = fast_div(tile, a.tiles_n, a.mg_n);
-      const int nt = tile - mt * a.tiles_n;
-      const int t2 = fast_div(mt, a.tiles_w, a.mg_w);
-      const int wt = mt - t2 * a.tiles_w;
-      const int bt = fast_div(t2, a.tiles_h, a.mg_h);
-      const int ht = t2 - bt * a.tiles_h;
-      const int w0 = wt * a.TW, h0 = ht * a.TH, b0 = bt * a.NB, n0 = nt * BLOCK_N;
+      const TileOrigin to = tile_origin<BLOCK_N>(a, tile);
+      const int w0 = to.w0, h0 = to.h0, b0 = to.b0, n0 = to.n0;
       const int ow = w0 + tw, oh = h0 + th, ob = b0 + nb;
       const bool valid = need_rows && (row < a.rows_valid) && (ow < a.Wo) && (oh < a.Ho) && (ob < a.Bn);
 
@@ -669,7 +704,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
           flush_hist(cur_img);
           cur_img = b0;
         }
-        const int an = nt, no = a.y_no;
+        const int an = n0 / BLOCK_N, no = a.y_no;
         const float conf = a.y_conf;
         const float* bias_a = y_bias + an * BLOCK_N;
         const int grp = wg;                                      // rows 64 * grp .. + 63
@@ -835,7 +870,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
           prof_acc[1] += t - pt0;  // staging tile free (TMA store read + barrier)
           pt0 = t;
         }
-        uint8_t* out_stage = out_stage0 + (gcount & (a.out_bufs - 1)) * Cfg::OUT_STAGE_BYTES + (PP ? wg * Cfg::OUT_TILE_BYTES : 0);
+        uint8_t* out_stage = out_stage0 + (gcount & (a.out_bufs - 1)) * G.out_buf_bytes + (PP ? wg * OUT_TILE_BYTES : 0);
         ++gcount;
 #pragma unroll
         for (int sc = 0; sc < CW / SUB; ++sc) {
@@ -852,7 +887,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
                 if constexpr (OUT_GROUP_CH == 64) chunk = cj ^ (row & 7);
                 else chunk = cj ^ ((row >> 1) & 3);
                 rhv[j] = *reinterpret_cast<const uint4*>(rh + (chunk << 4));
-                rlv[j] = *reinterpret_cast<const uint4*>(rh + Cfg::OUT_PLANE_BYTES + (chunk << 4));
+                rlv[j] = *reinterpret_cast<const uint4*>(rh + OUT_PLANE_BYTES + (chunk << 4));
               }
             }
           }
@@ -939,7 +974,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
             }
           } else {
             uint8_t* rowh = out_stage + row * OUT_ROW_BYTES;
-            uint8_t* rowl = rowh + Cfg::OUT_PLANE_BYTES;
+            uint8_t* rowl = rowh + OUT_PLANE_BYTES;
 #pragma unroll
             for (int j = 0; j < SUB / 8; ++j) {
               uint32_t hq[4], lq[4];
@@ -970,7 +1005,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
           const int c0 = n0 + g * OUT_GROUP_CH;
           if (c0 < a.cout && !(dbg & 1)) {
             tma_store_5d(&a.tmO, out_stage, c0, w0, h0, b0, 0);
-            if constexpr (!OUT_F32) tma_store_5d(&a.tmO, out_stage + Cfg::OUT_PLANE_BYTES, c0, w0, h0, b0, 1);
+            if constexpr (!OUT_F32) tma_store_5d(&a.tmO, out_stage + OUT_PLANE_BYTES, c0, w0, h0, b0, 1);
           }
           tma_store_commit();
           if (resid_tma) {  // every epilogue thread has consumed the residual tile (barrier above): fetch the next one
@@ -996,53 +1031,59 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
 }
 
 // ---------------------------------------------------------------------------------------------- host
-struct KernelEntry {
-  const void* fn;
-  int stage_bytes, out_stage_bytes, tail_bytes;
-};
-
-template <int BN, int BK, bool F32, bool YOLO = false, int EPI = 0, bool PP = false>
-static KernelEntry entry() {
-  using Cfg = ConvCfg<BN, BK, F32, YOLO, PP>;
-  return KernelEntry{reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, F32, YOLO, EPI, PP>), Cfg::STAGE_BYTES, Cfg::OUT_STAGE_BYTES,
-                     Cfg::TAIL_BYTES};
-}
-
 template <int BN, int BK, bool PP>
-static KernelEntry entry_epi(bool f32, int epi) {
-  return f32 ? entry<BN, BK, true, false, 0, PP>()
-             : (epi == 1 ? entry<BN, BK, false, false, 1, PP>() : (epi == 2 ? entry<BN, BK, false, false, 2, PP>() : (epi == 3 ? entry<BN, BK, false, false, 3, PP>()
-             : (epi == 4 ? entry<BN, BK, false, false, 4, PP>() : entry<BN, BK, false, false, 0, PP>()))));
+static const void* kernel_epi(bool f32, int epi) {
+  if (f32) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, true, false, 0, PP>);
+  switch (epi) {
+    case 1: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 1, PP>);
+    case 2: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 2, PP>);
+    case 3: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 3, PP>);
+    case 4: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 4, PP>);
+    default: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 0, PP>);
+  }
 }
 
-// pp: the ping-pong schedule, instantiated for block_n <= 128 (at 256 its generic and residual epilogues spill more than the
-// cooperative kernel's)
-static bool lookup_kernel(int bn, int bk, bool f32, KernelEntry* e, bool yolo = false, int epi = 0, bool pp = false) {
+// the kernel instantiation, or nullptr.  pp: the ping-pong schedule, instantiated for block_n <= 128 (at 256 its generic and residual
+// epilogues spill more than the cooperative kernel's)
+static const void* lookup_kernel(int bn, int bk, bool f32, bool yolo = false, int epi = 0, bool pp = false) {
   if (yolo) {  // fused-decode epilogue: one anchor per 128-wide n-tile
-    if (pp) return false;
-    if (bn == 128 && bk == 32) { *e = entry<128, 32, true, true>(); return true; }
-    if (bn == 128 && bk == 64) { *e = entry<128, 64, true, true>(); return true; }
-    return false;
+    if (pp) return nullptr;
+    if (bn == 128 && bk == 32) return reinterpret_cast<const void*>(&conv_tc_kernel<128, 32, true, true>);
+    if (bn == 128 && bk == 64) return reinterpret_cast<const void*>(&conv_tc_kernel<128, 64, true, true>);
+    return nullptr;
   }
-#define CVB_CASE(BN, BK)                                  \
-  if (bn == BN && bk == BK) {                             \
-    *e = entry_epi<BN, BK, false>(f32, epi);              \
-    return true;                                          \
-  }
-#define CVB_CASE_PP(BN, BK)                               \
-  if (bn == BN && bk == BK) {                             \
-    *e = pp ? entry_epi<BN, BK, true>(f32, epi) : entry_epi<BN, BK, false>(f32, epi); \
-    return true;                                          \
-  }
+#define CVB_CASE(BN, BK) \
+  if (bn == BN && bk == BK) return kernel_epi<BN, BK, false>(f32, epi);
+#define CVB_CASE_PP(BN, BK) \
+  if (bn == BN && bk == BK) return pp ? kernel_epi<BN, BK, true>(f32, epi) : kernel_epi<BN, BK, false>(f32, epi);
   CVB_CASE_PP(32, 16) CVB_CASE_PP(32, 32) CVB_CASE_PP(32, 64)
   CVB_CASE_PP(64, 16) CVB_CASE_PP(64, 32) CVB_CASE_PP(64, 64)
   CVB_CASE_PP(128, 16) CVB_CASE_PP(128, 32) CVB_CASE_PP(128, 64)
-  if (pp) return false;
+  if (pp) return nullptr;
   CVB_CASE(256, 16) CVB_CASE(256, 32) CVB_CASE(256, 64)
 #undef CVB_CASE
 #undef CVB_CASE_PP
-  return false;
+  return nullptr;
 }
+
+// A CTA's dynamic shared memory: `stages` ring slots of `slot` bytes, the weight region (resident slab or halo weight ring), the output
+// staging tiles (fused decode: staging tile, NMS histogram and bias), the residual tile, the accumulator tile, the bias and the
+// mbarriers.  Every plan is sized with it; the kernel chains the same regions in the same order (see its prologue).
+static SmemLayout smem_layout(const ConvGeom& g, int stages, int slot, int weight_bytes, int out_bufs, bool resid_tma, bool yolo) {
+  SmemLayout l;
+  l.slot = slot;
+  l.weights = stages * slot;
+  l.out = l.weights + weight_bytes;
+  l.resid = l.out + (yolo ? kYoloStageBytes + kNmsBins * 4 + kYoloBiasBytes : out_bufs * g.out_buf_bytes);
+  l.acc = l.resid + (resid_tma ? g.out_buf_bytes : 0);
+  l.bias = l.acc + g.acc_bytes;
+  l.bars = l.bias + g.bias_bytes;
+  l.total = l.bars + kBarBytes;
+  return l;
+}
+
+// ring slots that fit in `budget` next to the other regions of l0 (a layout of 0 stages); 0 or less: no fit
+static int stages_fitting(int budget, const SmemLayout& l0) { return (budget - l0.total) / l0.slot; }
 
 }  // namespace cvb
 
@@ -1079,6 +1120,15 @@ static CUtensorMapSwizzle swizzle_for_bytes(int bytes) {
   return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
+// 5-D (C, W, H, B, plane) tensor map: extents, byte strides of a W / H / B / plane step, and the box
+static int encode_5d(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int C, int W, int H, int B, int planes, long long s_w,
+                     long long s_h, long long s_b, long long s_plane, const int (&box)[5], CUtensorMapSwizzle swz) {
+  const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B, (cuuint64_t)planes};
+  const cuuint64_t str[4] = {(cuuint64_t)s_w, (cuuint64_t)s_h, (cuuint64_t)s_b, (cuuint64_t)s_plane};
+  const cuuint32_t bx[5] = {(cuuint32_t)box[0], (cuuint32_t)box[1], (cuuint32_t)box[2], (cuuint32_t)box[3], (cuuint32_t)box[4]};
+  return encode_map(m, dt, 5, const_cast<void*>(base), dims, str, bx, swz);
+}
+
 // Pick the output pixel box (TW x TH x NB <= rows: the tile's accumulator rows) that wastes the fewest accumulator rows.
 static void choose_box(int B, int H, int W, int rows, int* TW, int* TH, int* NB) {
   double best = -1.0;
@@ -1110,43 +1160,69 @@ static void choose_box(int B, int H, int W, int rows, int* TW, int* TH, int* NB)
 
 static int g_num_sms = 0;
 
-}  // namespace cvb
+// A/B knobs read once per process
+static bool two_ctas_on() {
+  static const bool on = [] {
+    const char* e = getenv("CVB_CTAS_PER_SM");  // A/B knob: 1 = always one CTA per SM
+    return !(e && atoi(e) == 1);
+  }();
+  return on;
+}
+static bool resid_tma_on() {
+  static const bool on = [] {
+    const char* e = getenv("CVB_RESID_TMA");  // A/B knob: 0 = per-thread residual loads
+    return !(e && atoi(e) == 0);
+  }();
+  return on;
+}
 
-extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan) {
-  using namespace cvb;
-  CVB_REQUIRE(d != nullptr && out_plan != nullptr, "null argument");
-  *out_plan = nullptr;
-  CvbConvDesc flat;
-  int yolo_nx = 0;
-  if (d->out_kind == CVB_OUT_YOLO) {
+// The validated descriptor (the fused-decode level flattened to one row) and the GEMM view of the layer.
+struct ConvProblem {
+  CvbConvDesc d;
+  int yolo_nx;  // fused decode: width of the level
+  int win;      // >0: K chunk of a filter row = `win` horizontally adjacent input pixels (see cvb200.h)
+  int cin;      // K per tap as seen by the GEMM
+  int cout, Ho, Wo, n_taps;
+  bool yolo, f32, has_resid;
+};
+
+// the K chunk that divides cin best
+static int full_bk(int cin) { return (cin % 64 == 0) ? 64 : (cin % 32 == 0 ? 32 : 16); }
+
+// the CTA's n-tile can stay the same along its stride over the tiles, so its weights may stay resident
+static bool can_pin(int cout, int bn) { return ceil_div(cout, bn) == 1 || ceil_div(cout, bn) == 2 || ceil_div(cout, bn) == 4; }
+
+static int validate_desc(const CvbConvDesc& desc, ConvProblem* P) {
+  P->d = desc;
+  CvbConvDesc* d = &P->d;
+  P->yolo = d->out_kind == CVB_OUT_YOLO;
+  P->yolo_nx = 0;
+  if (P->yolo) {
     // fused decode: a 1x1 / stride 1 conv does not care about the image geometry, so the level is planned as ONE row of H * W pixels.
     // A tile is then 128 consecutive pixels = 128 consecutive z rows (one contiguous 43 KB store) and no accumulator row is wasted
     // on partial boxes (80x80: 50 full tiles per image and anchor).
     CVB_REQUIRE(d->in.H >= 1 && d->in.W >= 1 && d->in.H == d->out.H && d->in.W == d->out.W && (long long)d->in.H * d->in.W < (1 << 24),
                 "conv(yolo): bad level geometry");
-    flat = *d;
-    yolo_nx = d->in.W;
-    flat.in.W = flat.out.W = d->in.H * d->in.W;
-    flat.in.H = flat.out.H = 1;
-    d = &flat;
+    P->yolo_nx = d->in.W;
+    d->in.W = d->out.W = d->in.H * d->in.W;
+    d->in.H = d->out.H = 1;
   }
   const CvbView& in = d->in;
   const CvbView& out = d->out;
-  CVB_REQUIRE(in.base && (out.base || d->out_kind == CVB_OUT_YOLO) && d->weights && d->bias, "conv: null tensor pointer");
+  CVB_REQUIRE(in.base && (out.base || P->yolo) && d->weights && d->bias, "conv: null tensor pointer");
   CVB_REQUIRE(d->kh >= 1 && d->kw >= 1 && (d->w_window > 0 ? d->kh : d->kh * d->kw) <= kMaxTaps,
               "conv: kernel %dx%d unsupported (max %d taps)", d->kh, d->kw, kMaxTaps);
   CVB_REQUIRE(d->stride == 1 || d->stride == 2, "conv: stride %d unsupported", d->stride);
   CVB_REQUIRE(d->dilation >= 1, "conv: bad dilation");
-  const int win = d->w_window;  // >0: K chunk of a filter row = `win` horizontally adjacent input pixels (see cvb200.h)
+  const int win = d->w_window;
   if (win > 0) {
     CVB_REQUIRE(d->stride == 1 && d->dilation == 1 && d->kw <= win && d->pad >= 0 && d->pad < d->kh,
                 "conv: w_window needs a stride-1 convolution with kw <= w_window (filter row ky reads input row h + ky - pad)");
     CVB_REQUIRE(in.c_pitch == in.C && (win * in.C == 64 || win * in.C == 32), "conv: w_window needs contiguous pixels and window*C in {32,64}");
     CVB_REQUIRE(in.W > win - 1, "conv: padded input too narrow");
   }
-  const int cin = win > 0 ? win * in.C : in.C;  // K per tap as seen by the GEMM
-  const bool yolo = d->out_kind == CVB_OUT_YOLO;
-  if (yolo) {
+  const int cin = win > 0 ? win * in.C : in.C;
+  if (P->yolo) {
     CVB_REQUIRE(d->yolo != nullptr && d->yolo->z != nullptr, "conv: out_kind CVB_OUT_YOLO needs CvbConvDesc.yolo with a z pointer");
     CVB_REQUIRE(d->yolo->na >= 1 && d->yolo->na <= 4 && d->yolo->no >= 6 && d->yolo->no <= 85, "conv(yolo): na <= 4 and 6 <= no <= 85 supported");
     CVB_REQUIRE(d->kh == 1 && d->kw == 1 && d->stride == 1 && d->pad == 0 && win == 0, "conv(yolo): the detect conv is 1x1 / stride 1");
@@ -1156,8 +1232,8 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   }
   const int cout = out.C;
   CVB_REQUIRE(cin % 16 == 0, "conv: cin=%d must be a multiple of 16", cin);
-  CVB_REQUIRE(in.c_pitch % 8 == 0 && (yolo || out.c_pitch % 8 == 0), "conv: channel pitch must be a multiple of 8");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(in.base) & 15) == 0 && (yolo || (reinterpret_cast<uintptr_t>(out.base) & 15) == 0) &&
+  CVB_REQUIRE(in.c_pitch % 8 == 0 && (P->yolo || out.c_pitch % 8 == 0), "conv: channel pitch must be a multiple of 8");
+  CVB_REQUIRE((reinterpret_cast<uintptr_t>(in.base) & 15) == 0 && (P->yolo || (reinterpret_cast<uintptr_t>(out.base) & 15) == 0) &&
                   (reinterpret_cast<uintptr_t>(d->weights) & 15) == 0,
               "conv: pointers must be 16-byte aligned");
   // window mode: the caller fixes the output height (asymmetric vertical padding is expressed by `pad` = rows above; rows
@@ -1167,9 +1243,33 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   CVB_REQUIRE(Ho == out.H && Wo == out.W && in.B == out.B, "conv: output view %dx%dx%d does not match computed %dx%dx%d", out.B, out.H,
               out.W, in.B, Ho, Wo);
   CVB_REQUIRE(d->cout_pad >= cout && d->cout_pad % 8 == 0, "conv: bad cout_pad");
-  const bool f32 = d->out_kind == CVB_OUT_F32 || yolo;
-  if (f32) CVB_REQUIRE(out.c_pitch % 4 == 0, "conv: fp32 output pitch must be a multiple of 4");
+  P->f32 = d->out_kind == CVB_OUT_F32 || P->yolo;
+  if (P->f32) CVB_REQUIRE(out.c_pitch % 4 == 0, "conv: fp32 output pitch must be a multiple of 4");
+  if (d->residual.base) {
+    const CvbView& r = d->residual;
+    CVB_REQUIRE(r.B == out.B && r.H == Ho && r.W == Wo && r.C == cout && r.c_pitch % 8 == 0 && cout % 32 == 0 &&
+                    (reinterpret_cast<uintptr_t>(r.base) & 15) == 0 && r.plane_stride % 16 == 0,
+                "conv: residual view mismatch");
+  }
+  if (d->up_partial.base) {
+    const CvbView& u = d->up_partial;
+    CVB_REQUIRE(u.B == out.B && u.H == (Ho + 1) / 2 && u.W == (Wo + 1) / 2 && u.C == cout && u.c_pitch % 4 == 0 && cout % 32 == 0 &&
+                    (reinterpret_cast<uintptr_t>(u.base) & 15) == 0,
+                "conv: up_partial view mismatch");
+  }
+  P->win = win;
+  P->cin = cin;
+  P->cout = cout;
+  P->Ho = Ho;
+  P->Wo = Wo;
+  P->n_taps = win > 0 ? d->kh : d->kh * d->kw;
+  P->has_resid = d->residual.base != nullptr;
+  return CVB_OK;
+}
 
+static int choose_block(const ConvProblem& P, int* bn_out, int* bk_out) {
+  const CvbConvDesc* d = &P.d;
+  const int cin = P.cin, cout = P.cout;
   int bn = d->block_n;
   if (bn == 0) {
     bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : 128);
@@ -1182,78 +1282,84 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
       const char* e = getenv("CVB_SPLIT_N128");
       return e ? atoi(e) : 1;
     }();
-    if (split128 && !f32 && d->kh * d->kw == 1 && cout == 128 && cin <= 128 && cin % 64 == 0 && d->up_partial.base) bn = 64;
+    if (split128 && !P.f32 && d->kh * d->kw == 1 && cout == 128 && cin <= 128 && cin % 64 == 0 && d->up_partial.base) bn = 64;
   }
-  int bk = (cin % 64 == 0) ? 64 : (cin % 32 == 0 ? 32 : 16);
-  const int bk_full = bk;
-  if (yolo) {
+  int bk = full_bk(cin);
+  if (P.yolo) {
     bn = 128;  // one anchor per n-tile
     CVB_REQUIRE(cin % 32 == 0, "conv(yolo): cin must be a multiple of 32");
     bk = 32;   // the 64 KB NMS histogram + 44 KB staging tile leave room for three 32 KB stages
-  }
-  if (!yolo) {
+  } else {
     static const int bk_small = [] {
       const char* e = getenv("CVB_BK_SMALLN");  // tuning knob: K chunk of the block_n <= 64 kernels for 64-channel inputs (default 32)
       const int v = e ? atoi(e) : 0;
       return (v == 16 || v == 32 || v == 64) ? v : 32;
     }();
     // 64-channel inputs into narrow cooperative tiles (1x1 convs and the row-window stems): half-size K chunks shrink the ring
-    // stages, so that more of these plans fit two CTAs per SM (see plan_smem below); ping-pong plans go back to full chunks.
+    // stages, so that more of these plans fit two CTAs per SM (see plan_ring below); ping-pong plans go back to full chunks.
     // Multi-tap 3x3 layers keep 64-wide chunks: measured slower with twice the TMA operations.
-    if (bn <= 64 && (cin == 64 || (cin == 128 && cout > 64)) && (d->kh * d->kw == 1 || win > 0)) bk = bk_small;
+    if (bn <= 64 && (cin == 64 || (cin == 128 && cout > 64)) && (d->kh * d->kw == 1 || P.win > 0)) bk = bk_small;
   }
-  // ---- filter taps: (input map, row offset, column offset) of every tap; stride 2 reads four "parity" maps
-  const int s = d->stride;
-  const int n_taps = win > 0 ? d->kh : d->kh * d->kw;
-  int8_t t_map[kMaxTaps], t_dh[kMaxTaps], t_dw[kMaxTaps];
-  if (win > 0) {
-    for (int ky = 0; ky < d->kh; ++ky) {
-      t_map[ky] = 0;
-      t_dh[ky] = (int8_t)(ky - d->pad);
-      t_dw[ky] = 0;  // the physical tensor carries the left zero column: window of output w starts at padded column w
-    }
-  } else {
-    for (int ky = 0; ky < d->kh; ++ky)
-      for (int kx = 0; kx < d->kw; ++kx) {
-        const int t = ky * d->kw + kx;
-        const int qy = ky * d->dilation - d->pad, qx = kx * d->dilation - d->pad;
-        CVB_REQUIRE(qy >= -127 && qy <= 127 && qx >= -127 && qx <= 127, "conv: tap offset %d/%d out of the supported range", qy, qx);
-        if (s == 1) {
-          t_map[t] = 0;
-          t_dh[t] = (int8_t)qy;
-          t_dw[t] = (int8_t)qx;
-        } else {
-          const int py = ((qy % 2) + 2) % 2, px = ((qx % 2) + 2) % 2;
-          t_map[t] = (int8_t)(py * 2 + px);
-          t_dh[t] = (int8_t)((qy - py) / 2);
-          t_dw[t] = (int8_t)((qx - px) / 2);
-        }
-      }
-  }
+  *bn_out = bn;
+  *bk_out = bk;
+  return CVB_OK;
+}
 
-  // ---- halo (copy / tap) mode decision: see ConvKArgs.  Geometry is fixed to 8 x 16 output pixels of one image per tile, so the
-  // 8-row groups of every tap view are 8 horizontally adjacent pixels and consecutive groups are one (halo) image row apart.
-  struct HaloCfg {
-    int mode = 0, bk = 0, resident = 0, sa = 0, sb = 0, out_bufs = 1, resid_tma = 0, ctas = 1, smem = 0;
-    int n_copies = 0, fused = 1;
-    int cp_map[6], cp_dw[6], cp_dh[6], cp_ntaps[6], cp_boxw[6], cp_boxh[6];
-    int cp_ny[6], cp_nx[6], cp_w0[6], cp_wy[6], cp_wx[6];  // taps of a copy as an ny x nx grid, weight tap = w0 + y*wy + x*wx
-    uint32_t cp_bytes[6], cp_lo_off[6], slot = 0;
-    int tap_w[kMaxTaps], tap_off[kMaxTaps];
-    int map_boxw[4], map_boxh[4];
-    int kskip = 0;
-    double cost = 0.0;
-    KernelEntry ke;
-  } hc;
-  static const bool two_ctas_on = [] {
-    const char* e = getenv("CVB_CTAS_PER_SM");  // A/B knob: 1 = always one CTA per SM
-    return !(e && atoi(e) == 1);
-  }();
-  static const bool resid_tma_on = [] {
-    const char* e = getenv("CVB_RESID_TMA");  // A/B knob: 0 = per-thread residual loads
-    return !(e && atoi(e) == 0);
-  }();
-  const bool can_pin = (ceil_div(cout, bn) == 1 || ceil_div(cout, bn) == 2 || ceil_div(cout, bn) == 4);
+// ---- filter taps: (input map, row offset, column offset) of every tap; stride 2 reads four "parity" maps
+struct TapTable {
+  int8_t map[kMaxTaps], dh[kMaxTaps], dw[kMaxTaps];
+};
+
+static int build_taps(const ConvProblem& P, TapTable* T) {
+  const CvbConvDesc* d = &P.d;
+  if (P.win > 0) {
+    for (int ky = 0; ky < d->kh; ++ky) {
+      T->map[ky] = 0;
+      T->dh[ky] = (int8_t)(ky - d->pad);
+      T->dw[ky] = 0;  // the physical tensor carries the left zero column: window of output w starts at padded column w
+    }
+    return CVB_OK;
+  }
+  for (int ky = 0; ky < d->kh; ++ky)
+    for (int kx = 0; kx < d->kw; ++kx) {
+      const int t = ky * d->kw + kx;
+      const int qy = ky * d->dilation - d->pad, qx = kx * d->dilation - d->pad;
+      CVB_REQUIRE(qy >= -127 && qy <= 127 && qx >= -127 && qx <= 127, "conv: tap offset %d/%d out of the supported range", qy, qx);
+      if (d->stride == 1) {
+        T->map[t] = 0;
+        T->dh[t] = (int8_t)qy;
+        T->dw[t] = (int8_t)qx;
+      } else {
+        const int py = ((qy % 2) + 2) % 2, px = ((qx % 2) + 2) % 2;
+        T->map[t] = (int8_t)(py * 2 + px);
+        T->dh[t] = (int8_t)((qy - py) / 2);
+        T->dw[t] = (int8_t)((qx - px) / 2);
+      }
+    }
+  return CVB_OK;
+}
+
+// ---- halo (copy / tap) mode: see ConvKArgs.  Geometry is fixed to 8 x 16 output pixels of one image per tile, so the 8-row groups of
+// every tap view are 8 horizontally adjacent pixels and consecutive groups are one (halo) image row apart.
+constexpr int kHaloTW = 8, kHaloTH = 16;
+
+struct HaloCfg {
+  int mode = 0, bk = 0, resident = 0, sa = 0, sb = 0, out_bufs = 1, resid_tma = 0, ctas = 1;
+  int n_copies = 0, fused = 1;
+  int cp_map[6], cp_dw[6], cp_dh[6], cp_ntaps[6], cp_boxw[6], cp_boxh[6];
+  int cp_ny[6], cp_nx[6], cp_w0[6], cp_wy[6], cp_wx[6];  // taps of a copy as an ny x nx grid, weight tap = w0 + y*wy + x*wx
+  uint32_t cp_bytes[6], cp_lo_off[6], slot = 0;
+  int tap_w[kMaxTaps], tap_off[kMaxTaps];
+  int map_boxw[4], map_boxh[4];
+  int kskip = 0;
+  double cost = 0.0;
+};
+
+// The halo plan of the layer if the cost model (or a request) picks the halo loader; bk: the classic loader's K chunk.
+static bool plan_halo(const ConvProblem& P, const TapTable& T, int bn, int bk, HaloCfg* out) {
+  const CvbConvDesc* d = &P.d;
+  const int n_taps = P.n_taps, cin = P.cin, cout = P.cout, win = P.win;
+  const bool pin = can_pin(cout, bn);
   auto f_mma = [](int n) { return n / 2 > 50 ? n / 2 : 50; };  // cost model: cycles of one M=128, K=16 MMA step (floor of 50)
   const int chain_all = n_taps * cin / 16;
   const bool pair_mode_est = chain_all <= 160 && bn <= 128 && (bn == 128 || n_taps > 1);
@@ -1263,253 +1369,259 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     const char* e = getenv("CVB_HALO");  // A/B knob: 0 = classic one-box-per-tap loads everywhere, 1 / 2 = force that halo mode where possible
     return e ? atoi(e) : -1;
   }();
-  const bool has_resid = d->residual.base != nullptr;
-  const int HTW = 8, HTH = 16;
-  bool use_halo = false;
+  const int HTW = kHaloTW, HTH = kHaloTH;
   const int halo_req = d->halo != 0 ? d->halo : halo_env;  // per-plan request wins over the environment knob
-  if (n_taps > 1 && d->dilation == 1 && halo_req != 0 && halo_req != -2 && d->halo != -1) {
-    // the halo loader pays off where two CTAs share an SM (BLOCK_N <= 64: the
-    // second CTA's MMAs fill the tensor-pipe bubbles of the first); mode 1 (aligned copies) wins for 32-channel inputs, mode 2 above
-    const int mode = halo_req == 1 ? 1 : (halo_req == 2 ? 2 : (cin <= 32 && win == 0 ? 1 : 2));
-    // copies: mode 2 = one per input map (box covers every tap of the map); mode 1 = one per (map, column offset)
-    HaloCfg h;
-    h.mode = mode;
-    int nc = 0;
-    int order[kMaxTaps], n_ord = 0;
-    for (int m = 0; m < 4; ++m) {
-      int dwmin = 127, dwmax = -127, dhmin = 127, dhmax = -127, cnt = 0;
+  if (!(n_taps > 1 && d->dilation == 1 && halo_req != 0 && halo_req != -2 && d->halo != -1)) return false;
+  // the halo loader pays off where two CTAs share an SM (BLOCK_N <= 64: the
+  // second CTA's MMAs fill the tensor-pipe bubbles of the first); mode 1 (aligned copies) wins for 32-channel inputs, mode 2 above
+  const int mode = halo_req == 1 ? 1 : (halo_req == 2 ? 2 : (cin <= 32 && win == 0 ? 1 : 2));
+  // copies: mode 2 = one per input map (box covers every tap of the map); mode 1 = one per (map, column offset)
+  HaloCfg h;
+  h.mode = mode;
+  int nc = 0;
+  int n_ord = 0;
+  for (int m = 0; m < 4; ++m) {
+    int dwmin = 127, dwmax = -127, dhmin = 127, dhmax = -127, cnt = 0;
+    for (int t = 0; t < n_taps; ++t)
+      if (T.map[t] == m) {
+        dwmin = T.dw[t] < dwmin ? T.dw[t] : dwmin;
+        dwmax = T.dw[t] > dwmax ? T.dw[t] : dwmax;
+        dhmin = T.dh[t] < dhmin ? T.dh[t] : dhmin;
+        dhmax = T.dh[t] > dhmax ? T.dh[t] : dhmax;
+        ++cnt;
+      }
+    h.map_boxw[m] = h.map_boxh[m] = 0;
+    if (!cnt) continue;
+    h.map_boxh[m] = HTH + (dhmax - dhmin);
+    h.map_boxw[m] = mode == 2 ? HTW + (dwmax - dwmin) : HTW;
+    const int n_groups = mode == 2 ? 1 : (dwmax - dwmin + 1);
+    for (int gi = 0; gi < n_groups; ++gi) {
+      const int gdw = dwmin + gi;
+      int nt = 0;
+      int dhs[kMaxTaps], dws[kMaxTaps], ndh = 0, ndw = 0;
       for (int t = 0; t < n_taps; ++t)
-        if (t_map[t] == m) {
-          dwmin = t_dw[t] < dwmin ? t_dw[t] : dwmin;
-          dwmax = t_dw[t] > dwmax ? t_dw[t] : dwmax;
-          dhmin = t_dh[t] < dhmin ? t_dh[t] : dhmin;
-          dhmax = t_dh[t] > dhmax ? t_dh[t] : dhmax;
-          ++cnt;
+        if (T.map[t] == m && (mode == 2 || T.dw[t] == gdw)) {
+          h.tap_w[n_ord] = t;
+          h.tap_off[n_ord] = (T.dh[t] - dhmin) * h.map_boxw[m] + (mode == 2 ? T.dw[t] - dwmin : 0);
+          ++n_ord;
+          ++nt;
+          bool seen = false;
+          for (int i = 0; i < ndh; ++i) seen |= dhs[i] == T.dh[t];
+          if (!seen) dhs[ndh++] = T.dh[t];
+          seen = false;
+          for (int i = 0; i < ndw; ++i) seen |= dws[i] == T.dw[t];
+          if (!seen) dws[ndw++] = T.dw[t];
         }
-      h.map_boxw[m] = h.map_boxh[m] = 0;
-      if (!cnt) continue;
-      h.map_boxh[m] = HTH + (dhmax - dhmin);
-      h.map_boxw[m] = mode == 2 ? HTW + (dwmax - dwmin) : HTW;
-      const int n_groups = mode == 2 ? 1 : (dwmax - dwmin + 1);
-      for (int gi = 0; gi < n_groups; ++gi) {
-        const int gdw = dwmin + gi;
-        int nt = 0;
-        int dhs[kMaxTaps], dws[kMaxTaps], ndh = 0, ndw = 0;
-        for (int t = 0; t < n_taps; ++t)
-          if (t_map[t] == m && (mode == 2 || t_dw[t] == gdw)) {
-            h.tap_w[n_ord] = t;
-            h.tap_off[n_ord] = (t_dh[t] - dhmin) * h.map_boxw[m] + (mode == 2 ? t_dw[t] - dwmin : 0);
-            order[n_ord++] = t;
-            ++nt;
-            bool seen = false;
-            for (int i = 0; i < ndh; ++i) seen |= dhs[i] == t_dh[t];
-            if (!seen) dhs[ndh++] = t_dh[t];
-            seen = false;
-            for (int i = 0; i < ndw; ++i) seen |= dws[i] == t_dw[t];
-            if (!seen) dws[ndw++] = t_dw[t];
-          }
-        if (!nt) continue;
-        if (nc >= 6) {
+      if (!nt) continue;
+      if (nc >= 6) {
+        nc = 7;
+        break;
+      }
+      {
+        // the kernel walks the taps of a copy as an ny x nx grid with affine view offsets / weight indices: verify that structure
+        auto find = [&](int dh, int dw) {
+          for (int t = 0; t < n_taps; ++t)
+            if (T.map[t] == m && T.dh[t] == dh && T.dw[t] == dw) return t;
+          return -1;
+        };
+        bool affine = ndh * ndw == nt;
+        const int t00 = find(dhs[0], dws[0]);
+        const int wy = ndh > 1 ? find(dhs[1], dws[0]) - t00 : 0, wx = ndw > 1 ? find(dhs[0], dws[1]) - t00 : 0;
+        for (int y = 0; affine && y < ndh; ++y)
+          for (int x = 0; affine && x < ndw; ++x)
+            affine = find(dhs[y], dws[x]) == t00 + y * wy + x * wx && dhs[y] == dhmin + y && dws[x] == (mode == 2 ? dwmin + x : gdw);
+        if (!affine || t00 < 0 || t00 > 127 || wy > 127 || wx > 127 || wy < 0 || wx < 0) {
           nc = 7;
           break;
         }
-        {
-          // the kernel walks the taps of a copy as an ny x nx grid with affine view offsets / weight indices: verify that structure
-          auto find = [&](int dh, int dw) {
-            for (int t = 0; t < n_taps; ++t)
-              if (t_map[t] == m && t_dh[t] == dh && t_dw[t] == dw) return t;
-            return -1;
-          };
-          bool affine = ndh * ndw == nt;
-          const int t00 = find(dhs[0], dws[0]);
-          const int wy = ndh > 1 ? find(dhs[1], dws[0]) - t00 : 0, wx = ndw > 1 ? find(dhs[0], dws[1]) - t00 : 0;
-          for (int y = 0; affine && y < ndh; ++y)
-            for (int x = 0; affine && x < ndw; ++x)
-              affine = find(dhs[y], dws[x]) == t00 + y * wy + x * wx && dhs[y] == dhmin + y && dws[x] == (mode == 2 ? dwmin + x : gdw);
-          if (!affine || t00 < 0 || t00 > 127 || wy > 127 || wx > 127 || wy < 0 || wx < 0) {
-            nc = 7;
-            break;
-          }
-          h.cp_ny[nc] = ndh;
-          h.cp_nx[nc] = ndw;
-          h.cp_w0[nc] = t00;
-          h.cp_wy[nc] = wy;
-          h.cp_wx[nc] = wx;
-        }
-        h.cp_map[nc] = m;
-        h.cp_dw[nc] = gdw;
-        h.cp_dh[nc] = dhmin;
-        h.cp_ntaps[nc] = nt;
-        h.cp_boxw[nc] = h.map_boxw[m];
-        h.cp_boxh[nc] = h.map_boxh[m];
-        ++nc;
+        h.cp_ny[nc] = ndh;
+        h.cp_nx[nc] = ndw;
+        h.cp_w0[nc] = t00;
+        h.cp_wy[nc] = wy;
+        h.cp_wx[nc] = wx;
       }
+      h.cp_map[nc] = m;
+      h.cp_dw[nc] = gdw;
+      h.cp_dh[nc] = dhmin;
+      h.cp_ntaps[nc] = nt;
+      h.cp_boxw[nc] = h.map_boxw[m];
+      h.cp_boxh[nc] = h.map_boxh[m];
+      ++nc;
     }
-    (void)order;
-    bool ok = nc >= 1 && nc <= 6 && n_ord == n_taps;
-    for (int c = 0; ok && c < nc; ++c) ok = h.cp_boxw[c] <= 256 && h.cp_boxh[c] <= 256;
-    if (ok) {
-      h.n_copies = nc;
-      h.fused = 1;
-      for (int c = 0; c < nc; ++c)
-        if ((h.cp_boxw[c] * h.cp_boxh[c]) % 8 != 0) h.fused = 0;
-      // candidate K chunks: the classic choice first, then smaller ones (they may let the weights stay resident)
-      int bks[3], n_bk = 0;
-      if (win > 0) bks[n_bk++] = cin;  // row-window stems: one chunk per filter row, trailing zero weight columns are skipped
-      else {
-        for (int c : {64, 32, 16})
-          if (cin % c == 0 && (c >= 32 || n_bk == 0)) bks[n_bk++] = c;  // 16-wide chunks (32-byte rows) only when nothing else divides cin
+  }
+  bool ok = nc >= 1 && nc <= 6 && n_ord == n_taps;
+  for (int c = 0; ok && c < nc; ++c) ok = h.cp_boxw[c] <= 256 && h.cp_boxh[c] <= 256;
+  if (!ok) return false;
+  h.n_copies = nc;
+  h.fused = 1;
+  for (int c = 0; c < nc; ++c)
+    if ((h.cp_boxw[c] * h.cp_boxh[c]) % 8 != 0) h.fused = 0;
+  // candidate K chunks: the classic choice first, then smaller ones (they may let the weights stay resident)
+  int bks[3], n_bk = 0;
+  if (win > 0) bks[n_bk++] = cin;  // row-window stems: one chunk per filter row, trailing zero weight columns are skipped
+  else {
+    for (int c : {64, 32, 16})
+      if (cin % c == 0 && (c >= 32 || n_bk == 0)) bks[n_bk++] = c;  // 16-wide chunks (32-byte rows) only when nothing else divides cin
+  }
+  // A/B knobs (read at every plan creation so one process can sweep them): K chunk, weight residency, CTAs per SM of the halo plans
+  const int bk_env = [] { const char* e = getenv("CVB_HALO_BK"); return e ? atoi(e) : 0; }();
+  const int res_env = [] { const char* e = getenv("CVB_HALO_RES"); return e ? atoi(e) : 1; }();
+  const int ctas_env = [] { const char* e = getenv("CVB_HALO_CTAS"); return e ? atoi(e) : 0; }();
+  const long long tiles_h = (long long)ceil_div(P.Wo, HTW) * ceil_div(P.Ho, HTH) * d->out.B * ceil_div(cout, bn);
+  HaloCfg best;
+  bool have = false;
+  for (int ctas = 2; ctas >= 1; --ctas) {
+    if (ctas == 2 && !(bn <= 64 && two_ctas_on())) continue;
+    if (ctas_env && ctas != ctas_env) continue;
+    if (!ctas_env && halo_req <= 0 && ctas == 1) continue;  // auto mode: only the two-CTAs-per-SM plans have been measured faster
+    const int budget = ctas == 2 ? kSmemBudget2 : kSmemBudget;
+    for (int bi = 0; bi < n_bk; ++bi) {
+      const int bkh = bks[bi];
+      if (bk_env && bkh != bk_env && win == 0) continue;
+      if (!lookup_kernel(bn, bkh, P.f32)) continue;
+      const ConvGeom g = conv_geom(bn, bkh, P.f32, false, false);
+      const int swz = bkh * 2;
+      const int chunks = cin / bkh;
+      uint32_t slot = 0;
+      double a_bytes = 0.0;
+      HaloCfg cand = h;
+      for (int c = 0; c < nc; ++c) {
+        const int rows = cand.cp_boxw[c] * cand.cp_boxh[c];
+        cand.cp_bytes[c] = (uint32_t)(rows * swz);
+        cand.cp_lo_off[c] = (uint32_t)(((rows + 7) / 8 * 8) * swz);
+        const uint32_t need = (cand.cp_lo_off[c] + cand.cp_bytes[c] + 1023u) / 1024u * 1024u;
+        slot = need > slot ? need : slot;
+        a_bytes += 2.0 * rows * swz;
       }
-      // A/B knobs (read at every plan creation so one process can sweep them): K chunk, weight residency, CTAs per SM of the halo plans
-      const int bk_env = [] { const char* e = getenv("CVB_HALO_BK"); return e ? atoi(e) : 0; }();
-      const int res_env = [] { const char* e = getenv("CVB_HALO_RES"); return e ? atoi(e) : 1; }();
-      const int ctas_env = [] { const char* e = getenv("CVB_HALO_CTAS"); return e ? atoi(e) : 0; }();
-      const long long tiles_h = (long long)ceil_div(Wo, HTW) * ceil_div(Ho, HTH) * out.B * ceil_div(cout, bn);
-      HaloCfg best;
-      bool have = false;
-      for (int ctas = 2; ctas >= 1; --ctas) {
-        if (ctas == 2 && !(bn <= 64 && two_ctas_on)) continue;
-        if (ctas_env && ctas != ctas_env) continue;
-        if (!ctas_env && halo_req <= 0 && ctas == 1) continue;  // auto mode: only the two-CTAs-per-SM plans have been measured faster
-        const int budget = ctas == 2 ? kSmemBudget2 : kSmemBudget;
-        for (int bi = 0; bi < n_bk; ++bi) {
-          const int bkh = bks[bi];
-          if (bk_env && bkh != bk_env && win == 0) continue;
-          KernelEntry keh;
-          if (!lookup_kernel(bn, bkh, f32, &keh)) continue;
-          const int swz = bkh * 2;
-          const int chunks = cin / bkh;
-          uint32_t slot = 0;
-          double a_bytes = 0.0;
-          HaloCfg cand = h;
-          for (int c = 0; c < nc; ++c) {
-            const int rows = cand.cp_boxw[c] * cand.cp_boxh[c];
-            cand.cp_bytes[c] = (uint32_t)(rows * swz);
-            cand.cp_lo_off[c] = (uint32_t)(((rows + 7) / 8 * 8) * swz);
-            const uint32_t need = (cand.cp_lo_off[c] + cand.cp_bytes[c] + 1023u) / 1024u * 1024u;
-            slot = need > slot ? need : slot;
-            a_bytes += 2.0 * rows * swz;
-          }
-          a_bytes *= chunks;
-          const int b_stage = 2 * bn * swz;
-          const long long w_tot = (long long)n_taps * chunks * b_stage;
-          const int kskip = win > 0 ? ((win - d->kw) * in.C) / 16 : 0;
-          const double mma = ((double)n_taps * chunks * (bkh / 16 - kskip)) * kstep_clk;
-          for (int cfg = 0; cfg < 4; ++cfg) {
-            const int ob = (cfg & 2) ? 1 : 2;
-            const int rt = (cfg & 1) ? 0 : 1;
-            if (rt && !(has_resid && !f32 && resid_tma_on)) continue;
-            const int fixed = keh.tail_bytes + ob * keh.out_stage_bytes + (rt ? keh.out_stage_bytes : 0);
-            for (int res = 1; res >= 0; --res) {
-              int sa, sb = 0;
-              if (res) {
-                if (!(can_pin && !d->no_resident && res_env)) continue;
-                sa = (int)((budget - fixed - w_tot) / (long long)slot);
-              } else {
-                sb = 4;
-                sa = (budget - fixed - sb * b_stage) / (int)slot;
-                if (sa < 2) {
-                  sb = 3;
-                  sa = (budget - fixed - sb * b_stage) / (int)slot;
-                }
-              }
-              if (sa < 2) continue;
-              if (sa > 6) sa = 6;
-              const double fill = (a_bytes + (res ? 0.0 : (double)w_tot)) / kFillBpc;
-              double cost = (mma > fill ? mma : fill) + 300.0;
-              cost *= (ctas == 2 ? 0.93 : 1.0) * (ob == 2 ? 0.97 : 1.0) * ((rt || !has_resid) ? 1.0 : 1.02) * (sa >= 3 ? 1.0 : 1.05) *
-                      (bkh == 64 ? 1.0 : (bkh == 32 ? 1.01 : 1.03));
-              if (!have || cost < best.cost) {
-                best = cand;
-                best.bk = bkh;
-                best.resident = res;
-                best.sa = sa;
-                best.sb = sb;
-                best.out_bufs = ob;
-                best.resid_tma = rt;
-                best.ctas = ctas;
-                best.slot = slot;
-                best.kskip = kskip;
-                best.cost = cost;
-                best.ke = keh;
-                best.smem = fixed + sa * (int)slot + (res ? (int)w_tot : sb * b_stage);
-                have = true;
-              }
+      a_bytes *= chunks;
+      const int b_stage = 2 * g.b_bytes;
+      const long long w_tot = (long long)n_taps * chunks * b_stage;
+      const int kskip = win > 0 ? ((win - d->kw) * P.d.in.C) / 16 : 0;
+      const double mma = ((double)n_taps * chunks * (bkh / 16 - kskip)) * kstep_clk;
+      for (int cfg = 0; cfg < 4; ++cfg) {
+        const int ob = (cfg & 2) ? 1 : 2;
+        const int rt = (cfg & 1) ? 0 : 1;
+        if (rt && !(P.has_resid && !P.f32 && resid_tma_on())) continue;
+        for (int res = 1; res >= 0; --res) {
+          int sa, sb = 0;
+          if (res) {
+            if (!(pin && !d->no_resident && res_env) || w_tot > budget) continue;
+            sa = stages_fitting(budget, smem_layout(g, 0, (int)slot, (int)w_tot, ob, rt, false));
+          } else {
+            sb = 4;
+            sa = stages_fitting(budget, smem_layout(g, 0, (int)slot, sb * b_stage, ob, rt, false));
+            if (sa < 2) {
+              sb = 3;
+              sa = stages_fitting(budget, smem_layout(g, 0, (int)slot, sb * b_stage, ob, rt, false));
             }
           }
+          if (sa < 2) continue;
+          if (sa > 6) sa = 6;
+          const double fill = (a_bytes + (res ? 0.0 : (double)w_tot)) / kFillBpc;
+          double cost = (mma > fill ? mma : fill) + 300.0;
+          cost *= (ctas == 2 ? 0.93 : 1.0) * (ob == 2 ? 0.97 : 1.0) * ((rt || !P.has_resid) ? 1.0 : 1.02) * (sa >= 3 ? 1.0 : 1.05) *
+                  (bkh == 64 ? 1.0 : (bkh == 32 ? 1.01 : 1.03));
+          if (!have || cost < best.cost) {
+            best = cand;
+            best.bk = bkh;
+            best.resident = res;
+            best.sa = sa;
+            best.sb = sb;
+            best.out_bufs = ob;
+            best.resid_tma = rt;
+            best.ctas = ctas;
+            best.slot = slot;
+            best.kskip = kskip;
+            best.cost = cost;
+            have = true;
+          }
         }
-      }
-      if (have) {
-        // classic estimate: one 128-row box per (tap, chunk); weights resident only below 64 KB
-        int cTW, cTH, cNB;
-        choose_box(out.B, Ho, Wo, kTileM, &cTW, &cTH, &cNB);
-        const long long tiles_c = (long long)ceil_div(Wo, cTW) * ceil_div(Ho, cTH) * ceil_div(out.B, cNB) * ceil_div(cout, bn);
-        const int chunks_c = cin / bk;
-        const long long w_c = (long long)n_taps * chunks_c * 2 * bn * bk * 2;
-        const bool res_c = can_pin && !d->no_resident && w_c <= 64 * 1024;
-        const double fill_c = ((double)n_taps * chunks_c * kTileM * bk * 4 + (res_c ? 0.0 : (double)w_c)) / kFillBpc;
-        const double mma_c = (double)n_taps * cin / 16 * kstep_clk;
-        const double cost_c = (double)tiles_c * ((mma_c > fill_c ? mma_c : fill_c) + 300.0);
-        const double cost_h = (double)tiles_h * best.cost;
-        use_halo = halo_req > 0 ? true : cost_h < 0.95 * cost_c;
-        if (use_halo) hc = best;
       }
     }
   }
-  if (use_halo) bk = hc.bk;
-  const bool rt = has_resid && !f32 && resid_tma_on;  // (classic loader) the residual tile arrives by TMA into its own staging tile
-  // the fp32 accumulator tile of the epilogue shares the 227 KB with the ring: halve the K chunk until two streamed stages fit
-  auto fit_bk = [&](int b, bool pp_) {
-    const int tile_m = pp_ ? kTileM / 2 : kTileM;
-    KernelEntry kt;
-    while (b > 16 && cin % (b / 2) == 0 && lookup_kernel(bn, b, f32, &kt, false, 0, pp_) &&
-           kt.tail_bytes + (rt ? 2 : 1) * kt.out_stage_bytes + 2 * (2 * tile_m * b * 2 + 2 * bn * b * 2) > kSmemBudget)
-      b /= 2;
-    return b;
+  if (!have) return false;
+  // classic estimate: one 128-row box per (tap, chunk); weights resident only below 64 KB
+  int cTW, cTH, cNB;
+  choose_box(d->out.B, P.Ho, P.Wo, kTileM, &cTW, &cTH, &cNB);
+  const long long tiles_c = (long long)ceil_div(P.Wo, cTW) * ceil_div(P.Ho, cTH) * ceil_div(d->out.B, cNB) * ceil_div(cout, bn);
+  const int chunks_c = cin / bk;
+  const long long w_c = (long long)n_taps * chunks_c * 2 * bn * bk * 2;
+  const bool res_c = pin && !d->no_resident && w_c <= 64 * 1024;
+  const double fill_c = ((double)n_taps * chunks_c * kTileM * bk * 4 + (res_c ? 0.0 : (double)w_c)) / kFillBpc;
+  const double mma_c = (double)n_taps * cin / 16 * kstep_clk;
+  const double cost_c = (double)tiles_c * ((mma_c > fill_c ? mma_c : fill_c) + 300.0);
+  const double cost_h = (double)tiles_h * best.cost;
+  if (!(halo_req > 0 || cost_h < 0.95 * cost_c)) return false;
+  *out = best;
+  return true;
+}
+
+// the fp32 accumulator tile of the epilogue shares the 227 KB with the ring: halve the K chunk until two streamed stages fit
+static int fit_bk(int cin, int bn, int bk, bool f32, bool pp, bool rt) {
+  while (bk > 16 && cin % (bk / 2) == 0 && lookup_kernel(bn, bk / 2, f32, false, 0, pp)) {
+    const ConvGeom g = conv_geom(bn, bk, f32, false, pp);
+    if (smem_layout(g, 2, 2 * g.a_bytes + 2 * g.b_bytes, 0, 1, rt, false).total <= kSmemBudget) break;
+    bk /= 2;
+  }
+  return bk;
+}
+
+// ring of a plan: depth, slot bytes, resident weight slab, output staging buffers
+struct Ring {
+  int stages, resident, out_bufs, slot, weights;
+};
+
+// ring depth / resident weights / staging buffers of a classic-loader plan (geometry g, K chunk bk) that fit `budget` bytes of dynamic
+// shared memory (0 stages = no fit)
+static Ring plan_ring(const ConvProblem& P, int bn, const ConvGeom& g, int bk, bool rt, int budget) {
+  const int k_it = P.n_taps * (P.cin / bk);
+  const int a_st = 2 * g.a_bytes, b_st = 2 * g.b_bytes;
+  const bool can_res = can_pin(P.cout, bn) && !P.d.no_resident && (long long)k_it * b_st <= 64 * 1024;
+  auto fit = [&](int resident, int out_bufs) {
+    Ring r{0, resident, out_bufs, resident ? a_st : a_st + b_st, resident ? k_it * b_st : 0};
+    r.stages = stages_fitting(budget, smem_layout(g, 0, r.slot, r.weights, out_bufs, rt, false));
+    return r;
   };
-  // ring depth / resident weights / staging buffers of a classic-loader plan (kernel ke_, tile_m-pixel tiles, K chunk bk_) that fit
-  // `budget` bytes of dynamic shared memory (0 stages = no fit)
-  auto plan_smem = [&](int budget, int tile_m, int bk_, const KernelEntry& ke_, int& resident, int& out_bufs) -> int {
-    const int k_it = n_taps * (cin / bk_);
-    const int a_st = 2 * tile_m * bk_ * 2, b_st = 2 * bn * bk_ * 2;
-    const int base_ = ke_.tail_bytes + (rt ? ke_.out_stage_bytes : 0);
-    const bool can_res = can_pin && !d->no_resident && (long long)k_it * b_st <= 64 * 1024;
-    resident = 0;
-    out_bufs = 1;
-    if (can_res) {
-      // the CTA's n-tile never changes and its whole weight slab fits: keep it resident, stream only activations
-      const int st = (budget - base_ - 2 * ke_.out_stage_bytes - k_it * b_st) / a_st;
-      if (st >= 3 || (st >= 2 && k_it == 1)) {
-        resident = 1;
-        out_bufs = 2;
-        return st;
-      }
-    }
-    const int st2 = (budget - base_ - 2 * ke_.out_stage_bytes) / (a_st + b_st);
-    if (st2 >= 3) {
-      out_bufs = 2;
-      return st2;
-    }
-    if (can_res) {
-      const int st = (budget - base_ - ke_.out_stage_bytes - k_it * b_st) / a_st;
-      if (st >= 3) {
-        resident = 1;
-        return st;
-      }
-    }
-    return (budget - base_ - ke_.out_stage_bytes) / (a_st + b_st);
-  };
+  if (can_res) {
+    // the CTA's n-tile never changes and its whole weight slab fits: keep it resident, stream only activations
+    const Ring r = fit(1, 2);
+    if (r.stages >= 3 || (r.stages >= 2 && k_it == 1)) return r;
+  }
+  const Ring r2 = fit(0, 2);
+  if (r2.stages >= 3) return r2;
+  if (can_res) {
+    const Ring r = fit(1, 1);
+    if (r.stages >= 3) return r;
+  }
+  return fit(0, 1);
+}
+
+// K chunk, schedule, CTAs per SM and shared-memory plan of the layer
+struct SchedPlan {
+  int bk;
+  bool pp;
+  int ctas;  // CTAs per SM
+  bool resid_tma;
+  Ring ring;
+  SmemLayout sm;
+};
+
+static int plan_schedule(const ConvProblem& P, int bn, int bk, const HaloCfg* hc, SchedPlan* S) {
+  const CvbConvDesc* d = &P.d;
+  const bool use_halo = hc != nullptr;
+  const bool rt_on = resid_tma_on(), two_on = two_ctas_on();
+  const bool rt = use_halo ? hc->resid_tma != 0 : (P.has_resid && !P.f32 && rt_on);  // the residual tile arrives by TMA
+  if (use_halo) bk = hc->bk;
   // ---- CTAs per SM of the cooperative plan.  Narrow tiles whose ring, staging and accumulator tiles fit in half the shared memory
   // run two CTAs per SM, so one CTA's epilogue overlaps the other's main loop.  On the H100 every CTA also holds the fp32
   // accumulator tile, so most block_n = 64 plans do not fit and run one CTA per SM.
-  int st_two = 0, res_two = 0, ob_two = 1;
-  bool two_ctas = use_halo && hc.ctas == 2;
-  if (!use_halo && !yolo) {
-    bk = fit_bk(bk, false);
-    KernelEntry kc;
-    if (bn <= 64 && two_ctas_on && lookup_kernel(bn, bk, f32, &kc)) {
-      st_two = plan_smem(kSmemBudget2, kTileM, bk, kc, res_two, ob_two);
-      two_ctas = st_two >= 3 || (st_two >= 2 && ob_two == 2);
+  Ring two{};
+  bool two_ctas = use_halo && hc->ctas == 2;
+  if (!use_halo && !P.yolo) {
+    bk = fit_bk(P.cin, bn, bk, P.f32, false, rt);
+    if (bn <= 64 && two_on && lookup_kernel(bn, bk, P.f32)) {
+      two = plan_ring(P, bn, conv_geom(bn, bk, P.f32, false, false), bk, rt, kSmemBudget2);
+      two_ctas = two.stages >= 3 || (two.stages >= 2 && two.out_bufs == 2);
     }
   }
   // ---- schedule.  Cooperative: both warpgroups share each 128-pixel tile and run its epilogue together, so the tensor pipe idles
@@ -1525,46 +1637,80 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
   // the other way round.  Ping-pong re-streams the whole weight slab per 64 pixels, and the 3x3 layers without a residual measured
   // 11-19 % slower.  With a residual, the cooperative ring is only two stages deep, and ping-pong measured 28 % faster.
   CVB_REQUIRE(d->schedule >= CVB_SCHED_AUTO && d->schedule <= CVB_SCHED_PINGPONG, "conv: schedule %d unsupported", d->schedule);
-  const bool narrow_wide = bn < 128 && cout > 128;  // a layer of more than 128 channels in narrow n-tiles
-  const bool pp_ok = !yolo && !use_halo && bn <= 128 && !narrow_wide && !two_ctas;
+  const bool narrow_wide = bn < 128 && P.cout > 128;  // a layer of more than 128 channels in narrow n-tiles
+  const bool pp_ok = !P.yolo && !use_halo && bn <= 128 && !narrow_wide && !two_ctas;
   CVB_REQUIRE(d->schedule != CVB_SCHED_PINGPONG || pp_ok,
               "conv: the ping-pong schedule needs a one-CTA-per-SM plan on the classic loader with block_n = 128, or block_n <= 64 on a "
               "layer of at most 128 channels (this plan %s)",
-              yolo ? "runs the fused decode" : (use_halo ? "uses the halo loader" : (bn > 128 ? "has block_n = 256"
+              P.yolo ? "runs the fused decode" : (use_halo ? "uses the halo loader" : (bn > 128 ? "has block_n = 256"
               : (narrow_wide ? "has narrow n-tiles on a layer of more than 128 channels"
               : "runs two CTAs per SM, which already overlap one CTA's epilogue with the other's MMAs"))));
-  const bool pp_auto = n_taps == 1 || (bn == 128 ? !has_resid : has_resid);
+  const bool pp_auto = P.n_taps == 1 || (bn == 128 ? !P.has_resid : P.has_resid);
   const bool pp = pp_ok && (d->schedule == CVB_SCHED_PINGPONG || (d->schedule == CVB_SCHED_AUTO && pp_auto));
   // a ping-pong plan runs one CTA per SM: no reason for the half-size K chunks of the narrow cooperative plans
-  if (pp) bk = fit_bk(bk_full, true);
-  KernelEntry ke;
-  CVB_REQUIRE(lookup_kernel(bn, bk, f32, &ke, yolo, 0, pp), "conv: no kernel for block_n=%d block_k=%d yolo=%d", bn, bk, (int)yolo);
+  if (pp) bk = fit_bk(P.cin, bn, full_bk(P.cin), P.f32, true, rt);
+  CVB_REQUIRE(lookup_kernel(bn, bk, P.f32, P.yolo, 0, pp), "conv: no kernel for block_n=%d block_k=%d yolo=%d", bn, bk, (int)P.yolo);
 
-  CvbConvPlan* p = new (std::nothrow) CvbConvPlan();
-  CVB_REQUIRE(p != nullptr, "out of host memory");
-  ConvKArgs& a = p->args;
-  memset(&a, 0, sizeof(a));
+  // ---- shared-memory plan: ring depth, resident weights, output staging
+  const ConvGeom g = conv_geom(bn, bk, P.f32, P.yolo, pp);
+  int ctas = 1;
+  Ring ring;
+  if (P.yolo) {
+    ring = Ring{0, 0, 1, 2 * g.a_bytes + 2 * g.b_bytes, 0};
+    ring.stages = stages_fitting(kSmemBudget, smem_layout(g, 0, ring.slot, 0, 1, false, true));
+    if (ring.stages > 4) ring.stages = 4;
+  } else if (use_halo) {
+    const int w_stage = 2 * g.b_bytes;
+    ring = Ring{hc->sa, hc->resident, hc->out_bufs, (int)hc->slot, hc->resident ? P.n_taps * (P.cin / bk) * w_stage : hc->sb * w_stage};
+    ctas = hc->ctas;
+  } else if (two_ctas) {
+    // the cooperative narrow plan that fits half the SM's shared memory (decided with the schedule above)
+    ring = two;
+    ctas = 2;
+  } else {
+    ring = plan_ring(P, bn, g, bk, rt, kSmemBudget);
+  }
+  if (ring.stages > 8) ring.stages = 8;
+  CVB_REQUIRE(ring.stages >= 2, "conv: tile does not fit in shared memory (block_n=%d block_k=%d)", bn, bk);
+  S->bk = bk;
+  S->pp = pp;
+  S->ctas = ctas;
+  S->resid_tma = rt;
+  S->ring = ring;
+  S->sm = smem_layout(g, ring.stages, ring.slot, ring.weights, ring.out_bufs, rt, P.yolo);
+  // the layout must fit the budget it was sized for, start its ring slots on the swizzle atom, and leave room for every mbarrier (full /
+  // empty per ring slot and per halo weight slot, resident weights, two residual tiles)
+  const int budget = ctas == 2 ? kSmemBudget2 : kSmemBudget;
+  CVB_REQUIRE(S->sm.total <= budget && S->sm.slot % 1024 == 0,
+              "conv: internal error (shared-memory layout of %d bytes, ring slot %d, for a budget of %d)", S->sm.total, S->sm.slot, budget);
+  const int bars = 2 * ring.stages + 2 * (use_halo ? hc->sb : 0) + 3;
+  CVB_REQUIRE(bars <= kMaxBars, "conv: internal error (%d mbarriers, room for %d)", bars, kMaxBars);
+  return CVB_OK;
+}
 
-  const int tile_m = pp ? kTileM / 2 : kTileM;  // output pixels of one tile
+// ---- tile box, tile counts and loader arguments
+static void fill_tiles(const ConvProblem& P, const TapTable& T, int bn, const SchedPlan& S, const HaloCfg* hc, ConvKArgs& a) {
+  const int bk = S.bk;
+  const int tile_m = S.pp ? kTileM / 2 : kTileM;  // output pixels of one tile
   int TW, TH, NB;
-  choose_box(out.B, Ho, Wo, tile_m, &TW, &TH, &NB);
-  if (yolo) {  // one image per tile (the epilogue keeps a per-image histogram), 128 consecutive pixels of the flattened level
-    TW = Wo < kTileM ? Wo : kTileM;
+  choose_box(P.d.out.B, P.Ho, P.Wo, tile_m, &TW, &TH, &NB);
+  if (P.yolo) {  // one image per tile (the epilogue keeps a per-image histogram), 128 consecutive pixels of the flattened level
+    TW = P.Wo < kTileM ? P.Wo : kTileM;
     TH = 1;
     NB = 1;
   }
-  if (use_halo) {
-    TW = HTW;
-    TH = HTH;
+  if (hc) {
+    TW = kHaloTW;
+    TH = kHaloTH;
     NB = 1;
   }
   a.TW = TW;
   a.TH = TH;
   a.NB = NB;
-  a.tiles_w = ceil_div(Wo, TW);
-  a.tiles_h = ceil_div(Ho, TH);
-  a.tiles_b = ceil_div(out.B, NB);
-  a.tiles_n = ceil_div(cout, bn);
+  a.tiles_w = ceil_div(P.Wo, TW);
+  a.tiles_h = ceil_div(P.Ho, TH);
+  a.tiles_b = ceil_div(P.d.out.B, NB);
+  a.tiles_n = ceil_div(P.cout, bn);
   {
     const unsigned long long total_t = (unsigned long long)a.tiles_w * a.tiles_h * a.tiles_b * a.tiles_n;
     auto magic = [&](int dv) -> uint32_t {  // exact for 0 <= x <= total_t when x * dv < 2^32
@@ -1576,214 +1722,156 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     a.mg_w = magic(a.tiles_w);
     a.mg_h = magic(a.tiles_h);
   }
-  a.Ho = Ho;
-  a.Wo = Wo;
-  a.Bn = out.B;
-  a.cout = cout;
-  a.taps = win > 0 ? d->kh : d->kh * d->kw;
-  a.chunks = cin / bk;
-  a.cin = cin;
-  a.act = d->act;
+  a.Ho = P.Ho;
+  a.Wo = P.Wo;
+  a.Bn = P.d.out.B;
+  a.cout = P.cout;
+  a.taps = P.n_taps;
+  a.chunks = P.cin / bk;
+  a.cin = P.cin;
+  a.act = P.d.act;
   a.rows_valid = TW * TH * NB;
   a.a_box_bytes = (uint32_t)(TW * TH * NB * bk * 2);
   a.a_fused = (a.rows_valid % 8 == 0) ? 1 : 0;  // the lo plane must start on a swizzle-atom boundary (8 rows)
   a.a_lo_off = a.a_fused ? a.a_box_bytes : (uint32_t)(tile_m * bk * 2);
-  a.bias = d->bias;
-  a.bias_len = d->cout_pad;
-
-  for (int t = 0; t < n_taps; ++t) {
-    a.tap_map[t] = t_map[t];
-    a.tap_dh[t] = t_dh[t];
-    a.tap_dw[t] = t_dw[t];
+  a.bias = P.d.bias;
+  a.bias_len = P.d.cout_pad;
+  a.stages = S.ring.stages;
+  a.b_resident = S.ring.resident;
+  a.out_bufs = S.ring.out_bufs;
+  a.sm = S.sm;
+  for (int t = 0; t < P.n_taps; ++t) {
+    a.tap_map[t] = T.map[t];
+    a.tap_dh[t] = T.dh[t];
+    a.tap_dw[t] = T.dw[t];
   }
-  if (use_halo) {
-    a.halo = hc.mode;
-    a.n_copies = hc.n_copies;
-    a.sb_stages = hc.sb;
-    a.kskip = hc.kskip;
-    a.a_slot_bytes = hc.slot;
-    a.a_fused = hc.fused;
-    for (int c = 0; c < hc.n_copies; ++c) {
-      a.cp_map[c] = (int8_t)hc.cp_map[c];
-      a.cp_dw[c] = (int8_t)hc.cp_dw[c];
-      a.cp_dh[c] = (int8_t)hc.cp_dh[c];
-      a.cp_ntaps[c] = (int8_t)hc.cp_ntaps[c];
-      a.cp_bytes[c] = hc.cp_bytes[c];
-      a.cp_lo_off[c] = hc.fused ? hc.cp_bytes[c] : hc.cp_lo_off[c];
-      a.cp_sbo[c] = (uint32_t)(hc.cp_boxw[c] * bk * 2);  // 8 consecutive accumulator rows = 8 horizontally adjacent pixels (TW == 8)
+  if (hc) {
+    a.halo = hc->mode;
+    a.n_copies = hc->n_copies;
+    a.sb_stages = hc->sb;
+    a.kskip = hc->kskip;
+    a.a_fused = hc->fused;
+    for (int c = 0; c < hc->n_copies; ++c) {
+      a.cp_map[c] = (int8_t)hc->cp_map[c];
+      a.cp_dw[c] = (int8_t)hc->cp_dw[c];
+      a.cp_dh[c] = (int8_t)hc->cp_dh[c];
+      a.cp_ntaps[c] = (int8_t)hc->cp_ntaps[c];
+      a.cp_bytes[c] = hc->cp_bytes[c];
+      a.cp_lo_off[c] = hc->fused ? hc->cp_bytes[c] : hc->cp_lo_off[c];
+      a.cp_sbo[c] = (uint32_t)(hc->cp_boxw[c] * bk * 2);  // 8 consecutive accumulator rows = 8 horizontally adjacent pixels (TW == 8)
+      a.cp_ny[c] = (int8_t)hc->cp_ny[c];
+      a.cp_nx[c] = (int8_t)hc->cp_nx[c];
+      a.cp_w0[c] = (int8_t)hc->cp_w0[c];
+      a.cp_wy[c] = (int8_t)hc->cp_wy[c];
+      a.cp_wx[c] = (int8_t)hc->cp_wx[c];
+      a.cp_row16[c] = (uint32_t)(hc->cp_boxw[c] * bk * 2) >> 4;
     }
-    for (int t = 0; t < n_taps; ++t) {
-      a.tap_w[t] = (int8_t)hc.tap_w[t];
-      a.tap_off[t] = (uint16_t)hc.tap_off[t];
-    }
-    for (int c = 0; c < hc.n_copies; ++c) {
-      a.cp_ny[c] = (int8_t)hc.cp_ny[c];
-      a.cp_nx[c] = (int8_t)hc.cp_nx[c];
-      a.cp_w0[c] = (int8_t)hc.cp_w0[c];
-      a.cp_wy[c] = (int8_t)hc.cp_wy[c];
-      a.cp_wx[c] = (int8_t)hc.cp_wx[c];
-      a.cp_row16[c] = (uint32_t)(hc.cp_boxw[c] * bk * 2) >> 4;
+    for (int t = 0; t < P.n_taps; ++t) {
+      a.tap_w[t] = (int8_t)hc->tap_w[t];
+      a.tap_off[t] = (uint16_t)hc->tap_off[t];
     }
   }
+}
 
+// ---- tensor maps: input (5D: C, W, H, B, plane), weights (3D: K, cout_pad, plane), output and residual (5D)
+static int encode_maps(const ConvProblem& P, int bn, const SchedPlan& S, const HaloCfg* hc, ConvKArgs& a) {
+  const CvbConvDesc* d = &P.d;
+  const CvbView& in = d->in;
+  const CvbView& out = d->out;
+  const int bk = S.bk, cin = P.cin, Wo = P.Wo, Ho = P.Ho;
+  const CUtensorMapDataType f16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  int box[5] = {bk, a.TW, a.TH, a.NB, a.a_fused ? 2 : 1};
+  if (hc) {
+    box[1] = hc->map_boxw[0];
+    box[2] = hc->map_boxh[0];
+  }
+  const long long pix = (long long)in.c_pitch * 2;  // bytes per pixel
   int rc = CVB_OK;
-  // ---- input maps: 5D (C, W, H, B, plane)
-  {
-    cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB, (cuuint32_t)(a.a_fused ? 2 : 1)};
-    if (use_halo) {
-      box[1] = (cuuint32_t)hc.map_boxw[0];
-      box[2] = (cuuint32_t)hc.map_boxh[0];
-    }
-    const long long pix = (long long)in.c_pitch * 2;  // bytes per pixel
-    if (win > 0) {
-      // overlapping-window view: element (k, w, h, b, p) = padded_input[p][b][h][w + k / C][k % C]; consecutive w overlap
-      const cuuint64_t dims[5] = {(cuuint64_t)cin, (cuuint64_t)Wo, (cuuint64_t)in.H, (cuuint64_t)in.B, 2};
-      const cuuint64_t str[4] = {(cuuint64_t)pix, (cuuint64_t)(pix * in.W), (cuuint64_t)(pix * in.W * in.H), (cuuint64_t)in.plane_stride};
-      rc = encode_map(&a.tmA[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, in.base, dims, str, box, swizzle_for_bytes(bk * 2));
-    } else if (s == 1) {
-      const cuuint64_t dims[5] = {(cuuint64_t)cin, (cuuint64_t)in.W, (cuuint64_t)in.H, (cuuint64_t)in.B, 2};
-      const cuuint64_t str[4] = {(cuuint64_t)pix, (cuuint64_t)(pix * in.W), (cuuint64_t)(pix * in.W * in.H), (cuuint64_t)in.plane_stride};
-      rc = encode_map(&a.tmA[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, in.base, dims, str, box, swizzle_for_bytes(bk * 2));
-    } else {
-      for (int py = 0; py < 2 && rc == CVB_OK; ++py)
-        for (int px = 0; px < 2 && rc == CVB_OK; ++px) {
-          const int Wp = (in.W - px + 1) / 2, Hp = (in.H - py + 1) / 2;  // number of columns/rows with this parity
-          if (Wp <= 0 || Hp <= 0) {
-            a.tmA[py * 2 + px] = a.tmA[0];
-            continue;
-          }
-          if (use_halo && hc.map_boxw[py * 2 + px] > 0) {
-            box[1] = (cuuint32_t)hc.map_boxw[py * 2 + px];
-            box[2] = (cuuint32_t)hc.map_boxh[py * 2 + px];
-          }
-          const cuuint64_t dims[5] = {(cuuint64_t)cin, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)in.B, 2};
-          const cuuint64_t str[4] = {(cuuint64_t)(pix * 2), (cuuint64_t)(pix * in.W * 2), (cuuint64_t)(pix * in.W * in.H),
-                                     (cuuint64_t)in.plane_stride};
-          uint8_t* base = static_cast<uint8_t*>(in.base) + ((long long)py * in.W + px) * pix;
-          rc = encode_map(&a.tmA[py * 2 + px], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, base, dims, str, box, swizzle_for_bytes(bk * 2));
+  if (d->stride == 1) {
+    // window mode (win > 0): overlapping-window view, element (k, w, h, b, p) = padded_input[p][b][h][w + k / C][k % C];
+    // consecutive w overlap
+    rc = encode_5d(&a.tmA[0], f16, in.base, cin, P.win > 0 ? Wo : in.W, in.H, in.B, 2, pix, pix * in.W, pix * in.W * in.H,
+                   in.plane_stride, box, swizzle_for_bytes(bk * 2));
+  } else {
+    for (int py = 0; py < 2 && rc == CVB_OK; ++py)
+      for (int px = 0; px < 2 && rc == CVB_OK; ++px) {
+        const int Wp = (in.W - px + 1) / 2, Hp = (in.H - py + 1) / 2;  // number of columns/rows with this parity
+        if (Wp <= 0 || Hp <= 0) {
+          a.tmA[py * 2 + px] = a.tmA[0];
+          continue;
         }
-    }
+        if (hc && hc->map_boxw[py * 2 + px] > 0) {
+          box[1] = hc->map_boxw[py * 2 + px];
+          box[2] = hc->map_boxh[py * 2 + px];
+        }
+        const uint8_t* base = static_cast<const uint8_t*>(in.base) + ((long long)py * in.W + px) * pix;
+        rc = encode_5d(&a.tmA[py * 2 + px], f16, base, cin, Wp, Hp, in.B, 2, pix * 2, pix * in.W * 2, pix * in.W * in.H, in.plane_stride,
+                       box, swizzle_for_bytes(bk * 2));
+      }
   }
-  // ---- weight map: 3D (K, cout_pad, plane)
   if (rc == CVB_OK) {
     const long long K = (long long)a.taps * cin;
     const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)d->cout_pad, 2};
     const cuuint64_t str[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(K * 2 * d->cout_pad)};
-    const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)bn, 2};
-    rc = encode_map(&a.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(d->weights), dims, str, box, swizzle_for_bytes(bk * 2));
+    const cuuint32_t wbox[3] = {(cuuint32_t)bk, (cuuint32_t)bn, 2};
+    rc = encode_map(&a.tmB, f16, 3, const_cast<void*>(d->weights), dims, str, wbox, swizzle_for_bytes(bk * 2));
   }
-  // ---- output map: 5D (C, W, H, B, plane)
-  if (rc == CVB_OK && !yolo) {
-    if (f32) {
-      const long long pix = (long long)out.c_pitch * 4;
-      const cuuint64_t dims[5] = {(cuuint64_t)cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)out.B, 1};
-      const cuuint64_t str[4] = {(cuuint64_t)pix, (cuuint64_t)(pix * Wo), (cuuint64_t)(pix * Wo * Ho), (cuuint64_t)(pix * Wo * Ho * out.B)};
-      const cuuint32_t box[5] = {32, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB, 1};
-      rc = encode_map(&a.tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, out.base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    } else {
-      const int gch = bn >= 64 ? 64 : 32;
-      const long long pix = (long long)out.c_pitch * 2;
-      const cuuint64_t dims[5] = {(cuuint64_t)cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)out.B, 2};
-      const cuuint64_t str[4] = {(cuuint64_t)pix, (cuuint64_t)(pix * Wo), (cuuint64_t)(pix * Wo * Ho), (cuuint64_t)out.plane_stride};
-      const cuuint32_t box[5] = {(cuuint32_t)gch, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB, 1};
-      rc = encode_map(&a.tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, out.base, dims, str, box, swizzle_for_bytes(gch * 2));
-    }
+  // output and residual tiles: one output group of the tile box (fp32: one plane)
+  const ConvGeom g = conv_geom(bn, bk, P.f32, P.yolo, S.pp);
+  const int obox[5] = {g.out_group_ch, a.TW, a.TH, a.NB, 1};
+  if (rc == CVB_OK && !P.yolo) {
+    const long long opix = (long long)out.c_pitch * (P.f32 ? 4 : 2);
+    rc = encode_5d(&a.tmO, P.f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : f16, out.base, P.cout, Wo, Ho, out.B, P.f32 ? 1 : 2, opix, opix * Wo,
+                   opix * Wo * Ho, P.f32 ? opix * Wo * Ho * out.B : out.plane_stride, obox, swizzle_for_bytes(g.out_row_bytes));
   }
-  if (rc != CVB_OK) {
-    delete p;
-    return rc;
+  if (rc == CVB_OK && S.resid_tma) {  // the residual tile: same box / swizzle as the output tile
+    const CvbView& r = d->residual;
+    const long long rpix = (long long)r.c_pitch * 2;
+    rc = encode_5d(&a.tmR, f16, r.base, P.cout, Wo, Ho, out.B, 2, rpix, rpix * Wo, rpix * Wo * Ho, r.plane_stride, obox,
+                   swizzle_for_bytes(g.out_row_bytes));
   }
-  // ---- epilogue extras
+  return rc;
+}
+
+// ---- epilogue operands, fused-decode arguments, accumulation gain; returns the kernel (compile-time epilogue specialisation)
+static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& S, ConvKArgs& a) {
+  const CvbConvDesc* d = &P.d;
   if (d->residual.base) {
     const CvbView& r = d->residual;
-    if (!(r.B == out.B && r.H == Ho && r.W == Wo && r.C == cout && r.c_pitch % 8 == 0 && cout % 32 == 0 &&
-          (reinterpret_cast<uintptr_t>(r.base) & 15) == 0 && r.plane_stride % 16 == 0)) {
-      delete p;
-      return set_error(CVB_ERR_INVALID, "conv: residual view mismatch");
-    }
     a.resid = static_cast<const __half*>(r.base);
     a.resid_plane = r.plane_stride / 2;
     a.resid_pitch = r.c_pitch;
-    if (!f32 && resid_tma_on && (!use_halo || hc.resid_tma)) {  // residual tile through TMA (same box / swizzle as the output tile)
-      const int gch = bn >= 64 ? 64 : 32;
-      const long long pixr = (long long)r.c_pitch * 2;
-      const cuuint64_t dims[5] = {(cuuint64_t)cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)out.B, 2};
-      const cuuint64_t str[4] = {(cuuint64_t)pixr, (cuuint64_t)(pixr * Wo), (cuuint64_t)(pixr * Wo * Ho), (cuuint64_t)r.plane_stride};
-      const cuuint32_t box[5] = {(cuuint32_t)gch, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB, 1};
-      rc = encode_map(&a.tmR, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, r.base, dims, str, box, swizzle_for_bytes(gch * 2));
-      if (rc != CVB_OK) {
-        delete p;
-        return rc;
-      }
-      a.resid_tma = 1;
-    }
+    a.resid_tma = S.resid_tma ? 1 : 0;
     a.resid_first = d->residual_before_act ? 1 : 0;
     a.resid_scale = d->residual_scale != 0.0f ? d->residual_scale : 1.0f;
   }
   if (d->up_partial.base) {
     const CvbView& u = d->up_partial;
-    if (!(u.B == out.B && u.H == (Ho + 1) / 2 && u.W == (Wo + 1) / 2 && u.C == cout && u.c_pitch % 4 == 0 && cout % 32 == 0 &&
-          (reinterpret_cast<uintptr_t>(u.base) & 15) == 0)) {
-      delete p;
-      return set_error(CVB_ERR_INVALID, "conv: up_partial view mismatch");
-    }
     a.up = static_cast<const float*>(u.base);
     a.up_pitch = u.c_pitch;
     a.up_H = u.H;
     a.up_W = u.W;
   }
-  // ---- shared-memory plan: ring depth, resident weights, output staging
-  const int k_iters = a.taps * a.chunks;
-  const int a_stage = 2 * tile_m * bk * 2;   // hi + lo activation tiles of one K chunk
-  const int b_stage = 2 * bn * bk * 2;       // hi + lo weight tiles of one K chunk
-  const int base = ke.tail_bytes + (a.resid_tma ? ke.out_stage_bytes : 0);
-  int stages = 0, ctas_per_sm = 1;
-  if (yolo) {
+  if (P.yolo) {
     const CvbYoloDecode& y = *d->yolo;
-    stages = (kSmemBudget - ke.tail_bytes - kYoloStageBytes - kNmsBins * 4 - kYoloBiasBytes) / (a_stage + b_stage);
-    if (stages > 4) stages = 4;
-    a.b_resident = 0;
-    a.out_bufs = 1;
     a.tile_contig = 1;
     a.yz = y.z;
     a.y_zrows = y.z_rows;
     a.y_zoff = y.z_off;
     a.y_no = y.no;
-    a.y_nx = yolo_nx;
-    a.y_nx_magic = (uint32_t)((0x100000000ULL + (unsigned long long)yolo_nx - 1) / (unsigned long long)yolo_nx);
+    a.y_nx = P.yolo_nx;
+    a.y_nx_magic = (uint32_t)((0x100000000ULL + (unsigned long long)P.yolo_nx - 1) / (unsigned long long)P.yolo_nx);
     a.y_multi = y.multi_label ? 1 : 0;
     a.y_stride = y.stride;
     a.y_conf = y.conf_thres;
     for (int i = 0; i < 8; ++i) a.y_anchor[i] = y.anchors_px[i];
     a.y_hist = static_cast<unsigned int*>(y.nms_workspace);
-    a.y_rowmax = y.nms_workspace ? reinterpret_cast<float*>(static_cast<uint8_t*>(y.nms_workspace) + nms_ws_rowmax_offset(out.B)) : nullptr;
-  } else if (use_halo) {
-    stages = hc.sa;
-    a.b_resident = hc.resident;
-    a.out_bufs = hc.out_bufs;
-    ctas_per_sm = hc.ctas;
-  } else if (two_ctas) {
-    // the cooperative narrow plan that fits half the SM's shared memory (decided with the schedule above)
-    stages = st_two;
-    a.b_resident = res_two;
-    a.out_bufs = ob_two;
-    ctas_per_sm = 2;
+    a.y_rowmax = y.nms_workspace ? reinterpret_cast<float*>(static_cast<uint8_t*>(y.nms_workspace) + nms_ws_rowmax_offset(d->out.B)) : nullptr;
   }
-  if (stages == 0) stages = plan_smem(kSmemBudget, tile_m, bk, ke, a.b_resident, a.out_bufs);
-  if (stages > 8) stages = 8;
-  if (use_halo && (a.resid_tma != hc.resid_tma)) {
-    delete p;
-    return set_error(CVB_ERR_INVALID, "conv: internal error (halo plan / residual staging mismatch)");
-  }
-  if (stages < 2) {
-    delete p;
-    return set_error(CVB_ERR_INVALID, "conv: tile does not fit in shared memory (block_n=%d block_k=%d)", bn, bk);
-  }
-  a.stages = stages;
   {
     // one accumulation chain per tile: the hi*hi products (and, at block_n = 256, the cross terms too: one register accumulator) of
     // every K step; rz_gain undoes the mean round-toward-zero shrink of the chain
-    const int chain = (bn <= 128 ? 1 : 3) * a.taps * cin / 16;
+    const int chain = (bn <= 128 ? 1 : 3) * a.taps * P.cin / 16;
     static const double rz_c = [] {
       // mean |sum| shrink per chained MMA of the tensor core's round-toward-zero fp32 accumulation (tools/precision_probe.py);
       // CVB_RZ_COMP overrides it
@@ -1792,30 +1880,25 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     }();
     a.rz_gain = (float)(1.0 + rz_c * (double)chain);
   }
-  p->smem = base + stages * (a_stage + (a.b_resident ? 0 : b_stage)) + (a.b_resident ? k_iters * b_stage : 0) + a.out_bufs * ke.out_stage_bytes;
-  if (use_halo) p->smem = hc.smem;
-  if (yolo) p->smem = ke.tail_bytes + kYoloStageBytes + kNmsBins * 4 + kYoloBiasBytes + stages * (a_stage + b_stage);
-  p->fn = ke.fn;
-  {
-    // compile-time specialised epilogues for the two hot modes (same tile / smem geometry as the generic kernel picked above)
-    static const bool spec_on = [] { const char* e = getenv("CVB_EPI_SPEC"); return !(e && atoi(e) == 0); }();  // A/B knob
-    int epi = 0;
-    if (spec_on && !f32 && !yolo && !d->up_partial.base) {
-      if (d->act == CVB_ACT_SILU) {
-        if (!d->residual.base) epi = 1;
-        else if (a.resid_tma && !a.resid_first && a.resid_scale == 1.0f) epi = 2;
-      } else if (d->act == CVB_ACT_RELU) {
-        if (!d->residual.base) epi = 3;
-        else if (a.resid_tma && a.resid_first && a.resid_scale == 1.0f) epi = 4;
-      }
-    }
-    if (epi) {
-      KernelEntry k2;
-      if (lookup_kernel(bn, bk, f32, &k2, false, epi, pp)) p->fn = k2.fn;
+  // compile-time specialised epilogues for the two hot modes (same tile / smem geometry as the generic kernel)
+  static const bool spec_on = [] { const char* e = getenv("CVB_EPI_SPEC"); return !(e && atoi(e) == 0); }();  // A/B knob
+  int epi = 0;
+  if (spec_on && !P.f32 && !P.yolo && !d->up_partial.base) {
+    if (d->act == CVB_ACT_SILU) {
+      if (!d->residual.base) epi = 1;
+      else if (a.resid_tma && !a.resid_first && a.resid_scale == 1.0f) epi = 2;
+    } else if (d->act == CVB_ACT_RELU) {
+      if (!d->residual.base) epi = 3;
+      else if (a.resid_tma && a.resid_first && a.resid_scale == 1.0f) epi = 4;
     }
   }
-  p->threads = kThreads;
-  p->schedule = pp ? CVB_SCHED_PINGPONG : CVB_SCHED_COOPERATIVE;
+  const void* fn = epi ? lookup_kernel(bn, S.bk, P.f32, false, epi, S.pp) : nullptr;
+  return fn ? fn : lookup_kernel(bn, S.bk, P.f32, P.yolo, 0, S.pp);
+}
+
+// ---- diagnostics switches and the persistent launch grid
+static int set_launch(const ConvProblem& P, int bn, const SchedPlan& S, CvbConvPlan* p) {
+  ConvKArgs& a = p->args;
   {
     const char* e = getenv("CVB_DBG");  // diagnostics only (tools/conv_pipeline_profile.py): results are wrong when set
     a.dbg = e ? atoi(e) : 0;
@@ -1825,7 +1908,9 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
     }();
     a.wait_hint = (uint32_t)(hint > 0 ? hint : 0);
   }
-
+  p->smem = S.sm.total;
+  p->threads = kThreads;
+  p->schedule = S.pp ? CVB_SCHED_PINGPONG : CVB_SCHED_COOPERATIVE;
   static std::mutex mu;
   {
     std::lock_guard<std::mutex> lk(mu);
@@ -1835,34 +1920,57 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* d, CvbConvPlan** out_plan
       if (e == cudaSuccess) e = cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
       if (e != cudaSuccess || g_num_sms <= 0) {
         g_num_sms = 0;
-        delete p;
         return set_error(CVB_ERR_NO_DEVICE, "no CUDA device: %s", cudaGetErrorString(e));
       }
     }
     cudaError_t e = cudaFuncSetAttribute(p->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-    if (e != cudaSuccess) {
-      delete p;
-      return set_error(CVB_ERR_CUDA, "cudaFuncSetAttribute(smem) failed: %s", cudaGetErrorString(e));
-    }
+    if (e != cudaSuccess) return set_error(CVB_ERR_CUDA, "cudaFuncSetAttribute(smem) failed: %s", cudaGetErrorString(e));
   }
   const long long total = (long long)a.tiles_w * a.tiles_h * a.tiles_b * a.tiles_n;
   int sms = g_num_sms;
-  if (d->sm_limit > 0 && d->sm_limit < sms) sms = d->sm_limit;
-  sms *= ctas_per_sm;
+  if (P.d.sm_limit > 0 && P.d.sm_limit < sms) sms = P.d.sm_limit;
+  sms *= S.ctas;
   p->grid = (int)(total < sms ? total : sms);
   if (a.b_resident && a.tiles_n > 1) {
     p->grid -= p->grid % a.tiles_n;  // every CTA keeps one n-tile (tile % tiles_n constant along its stride)
     if (p->grid < a.tiles_n) p->grid = a.tiles_n;
   }
-  {
-    static const bool dbg = [] { const char* e = getenv("CVB_PLAN_DEBUG"); return e && atoi(e) != 0; }();
-    if (dbg)
-      fprintf(stderr, "[cvb plan] cin=%d cout=%d k=%dx%d s=%d out=%dx%dx%d bn=%d bk=%d stages=%d resident=%d out_bufs=%d ctas/sm=%d "
-              "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s\n", cin, cout, d->kh, d->kw, d->stride, out.B, Ho, Wo, bn, bk,
-              stages, a.b_resident, a.out_bufs, ctas_per_sm, p->smem, p->grid, total, a.resid_tma, a.halo,
-              a.n_copies, a.sb_stages, a.a_slot_bytes, a.kskip, pp ? "pingpong" : "cooperative");
-  }
-  *out_plan = p;
+  static const bool dbg = [] { const char* e = getenv("CVB_PLAN_DEBUG"); return e && atoi(e) != 0; }();
+  if (dbg)
+    fprintf(stderr, "[cvb plan] cin=%d cout=%d k=%dx%d s=%d out=%dx%dx%d bn=%d bk=%d stages=%d resident=%d out_bufs=%d ctas/sm=%d "
+            "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s\n", P.cin, P.cout, P.d.kh, P.d.kw,
+            P.d.stride, P.d.out.B, P.Ho, P.Wo, bn, S.bk, a.stages, a.b_resident, a.out_bufs, S.ctas, p->smem, p->grid, total, a.resid_tma,
+            a.halo, a.n_copies, a.sb_stages, a.halo ? (unsigned)a.sm.slot : 0u, a.kskip, S.pp ? "pingpong" : "cooperative");
+  return CVB_OK;
+}
+
+}  // namespace cvb
+
+extern "C" int cvb_conv_plan_create(const CvbConvDesc* desc, CvbConvPlan** out_plan) {
+  using namespace cvb;
+  CVB_REQUIRE(desc != nullptr && out_plan != nullptr, "null argument");
+  *out_plan = nullptr;
+  ConvProblem P;
+  int rc = validate_desc(*desc, &P);
+  if (rc != CVB_OK) return rc;
+  int bn, bk;
+  if ((rc = choose_block(P, &bn, &bk)) != CVB_OK) return rc;
+  TapTable taps;
+  if ((rc = build_taps(P, &taps)) != CVB_OK) return rc;
+  HaloCfg hc;
+  const HaloCfg* halo = plan_halo(P, taps, bn, bk, &hc) ? &hc : nullptr;
+  SchedPlan S;
+  if ((rc = plan_schedule(P, bn, bk, halo, &S)) != CVB_OK) return rc;
+  std::unique_ptr<CvbConvPlan> p(new (std::nothrow) CvbConvPlan());
+  CVB_REQUIRE(p != nullptr, "out of host memory");
+  memset(&p->args, 0, sizeof(p->args));
+  fill_tiles(P, taps, bn, S, halo, p->args);
+  rc = encode_maps(P, bn, S, halo, p->args);
+  if (rc != CVB_OK) return rc;
+  p->fn = fill_epilogue(P, bn, S, p->args);
+  rc = set_launch(P, bn, S, p.get());
+  if (rc != CVB_OK) return rc;
+  *out_plan = p.release();
   return CVB_OK;
 }
 
