@@ -68,13 +68,19 @@ struct alignas(64) TConvArgs {
   const __nv_bfloat16* y_prev;  // SiLU' epilogue: conv output of the layer that produced this conv's input, and its BN scale / shift
   const float* s_prev;
   const float* t_prev;
+  // PRED epilogue: fp32 NCHW [B, c_tot, out_H, out_W], GEMM column c -> channel c_off + c, columns >= n_store (zero weight rows) dropped
+  float* out_f32;
+  const float* bias;
+  int c_tot, c_off, n_store;
 };
 
 // D[128 pixels, BN couts] = sum over (tap, 64-channel chunk) of A[pixels, 64] * W[couts, 64]^T, bf16 x bf16 -> fp32 in registers
 // (warpgroup w: pixel rows 64w..64w+63).
 // SILU_BWD: the result is d(loss)/d(a_prev) with a_prev = silu(z_prev), z_prev = y_prev * s + t: the epilogue multiplies by silu'(z_prev),
 // so the producer's activation gradient never makes a round trip through HBM.
-template <int BN, bool SILU_BWD>
+// PRED: the head's prediction convs (nn.Conv2d with bias, no BatchNorm / activation): out_f32 = D + bias in fp32, stored NCHW because the
+// loss reads the reference's [B, 5 + num_classes, h, w] tensor.
+template <int BN, bool SILU_BWD, bool PRED = false>
 __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_constant__ TConvArgs a) {
   constexpr int A_BYTES = 128 * 128;
   constexpr int B_BYTES = BN * 128;
@@ -174,6 +180,17 @@ __global__ void __launch_bounds__(kTThreads, 1) tconv_kernel(const __grid_consta
       const int th = r2 % a.TH, nb = r2 / a.TH;
       const int ow = w0 + tw, oh = h0 + th, ob = b0 + nb;
       if (!(ow < a.W && oh < a.H && ob < a.B)) continue;
+      if (PRED) {
+        const size_t plane = (size_t)a.out_H * a.out_W;
+        float* ocol = a.out_f32 + ((size_t)ob * a.c_tot + a.c_off + n0) * plane + (size_t)oh * a.out_W + ow;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + cq;
+          if (n0 + c < a.n_store) ocol[c * plane] = d[4 * j + 2 * h] + __ldg(a.bias + n0 + c);
+          if (n0 + c + 1 < a.n_store) ocol[(c + 1) * plane] = d[4 * j + 2 * h + 1] + __ldg(a.bias + n0 + c + 1);
+        }
+        continue;
+      }
       const size_t pix = ((size_t)ob * a.out_H + (oh * a.os + a.ooh)) * a.out_W + (ow * a.os + a.oow);
       __nv_bfloat16* orow = a.out + pix * a.cout + n0;
 #pragma unroll
@@ -680,6 +697,102 @@ __global__ void __launch_bounds__(kEwThreads) spp_pool_bwd_kernel(const __nv_bfl
   }
 }
 
+// ------------------------------------------------------------------------------------------------ YOLOX neck and head
+// Neck top-down path (src/models/necks/yolox_neck.py:52-62): cat [B,2h,2w,Ca+Cb] = [nearest_up2(a) | b].  Thread = one 16-byte vector of cat.
+__global__ void __launch_bounds__(kEwThreads) upsample_cat_fwd_kernel(const __nv_bfloat16* __restrict__ a, int B, int h, int w, int Ca,
+                                                                      const __nv_bfloat16* __restrict__ b, int Cb, __nv_bfloat16* __restrict__ cat) {
+  const int cva = Ca / 8, cvb = Cb / 8, cv = cva + cvb, W2 = 2 * w;
+  const long long n = (long long)B * 4 * h * w * cv;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int v = (int)(i % cv);
+    const long long p = i / cv;
+    const int x = (int)(p % W2);
+    const long long t = p / W2;
+    const int y = (int)(t % (2 * h));
+    const long long img = t / (2 * h);
+    reinterpret_cast<uint4*>(cat)[i] = v < cva ? __ldg(reinterpret_cast<const uint4*>(a + ((img * h + y / 2) * w + x / 2) * Ca) + v)
+                                               : __ldg(reinterpret_cast<const uint4*>(b + p * Cb) + (v - cva));
+  }
+}
+
+// g = d(loss)/d(cat) -> da [B,h,w,Ca] = the 2x2 sum of g[..., :Ca] (fp32, in the fixed order (0,0), (0,1), (1,0), (1,1), one bf16 rounding)
+// and db [B,2h,2w,Cb] = g[..., Ca:].  Items [0, na) are da vectors, the rest db vectors; no atomics, so bitwise reproducible.
+__global__ void __launch_bounds__(kEwThreads) upsample_cat_bwd_kernel(const __nv_bfloat16* __restrict__ g, int B, int h, int w, int Ca, int Cb,
+                                                                      __nv_bfloat16* __restrict__ da, __nv_bfloat16* __restrict__ db) {
+  const int cva = Ca / 8, cvb = Cb / 8, cv = cva + cvb, W2 = 2 * w;
+  const long long na = (long long)B * h * w * cva, n = na + (long long)B * 4 * h * w * cvb;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    if (i < na) {
+      const int v = (int)(i % cva);
+      const long long p = i / cva;
+      const int x = (int)(p % w);
+      const long long t = p / w;
+      const int y = (int)(t % h);
+      const long long img = t / h;
+      float acc[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = 0.0f;
+#pragma unroll
+      for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 2; ++dx) {
+          const long long q = (img * 2 * h + 2 * y + dy) * W2 + 2 * x + dx;
+          float f[8];
+          bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(g + q * 8 * cv) + v), f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) acc[j] += f[j];
+        }
+      reinterpret_cast<uint4*>(da)[i] = float_to_bf16x8(acc);
+    } else {
+      const long long k = i - na;
+      const int v = (int)(k % cvb);
+      const long long p = k / cvb;
+      reinterpret_cast<uint4*>(db)[k] = __ldg(reinterpret_cast<const uint4*>(g + p * 8 * cv) + cva + v);
+    }
+  }
+}
+
+// Prediction-conv backward, the gradient half: the loss's fp32 NCHW gradient of output channels [c_off, c_off + cout) -> the bf16 NHWC operand
+// dy [B,h,w,cout_pad] of backward-data / backward-weight, channels past cout zero.  Item i = v * npix + p (vector-major), so a warp reads 32
+// consecutive pixels of one channel plane.
+__global__ void __launch_bounds__(kEwThreads) pred_grad_nhwc_kernel(const float* __restrict__ g, int B, int c_tot, long long hw, int c_off, int cout, int cout_pad,
+                                                                    __nv_bfloat16* __restrict__ dy) {
+  const int cv = cout_pad / 8;
+  const long long npix = (long long)B * hw, n = npix * cv;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int v = (int)(i / npix);
+    const long long p = i % npix;
+    const long long b = p / hw, q = p % hw;
+    const float* col = g + (b * c_tot + c_off) * hw + q;
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = 8 * v + j;
+      f[j] = c < cout ? __ldg(col + c * hw) : 0.0f;
+    }
+    reinterpret_cast<uint4*>(dy + p * cout_pad)[v] = float_to_bf16x8(f);
+  }
+}
+
+// ... and the bias half: dbias[c] = sum over images and pixels of g[:, c_off + c], one CTA per channel, thread partial sums combined by a
+// fixed shared-memory tree (deterministic, no atomics).
+__global__ void __launch_bounds__(kEwThreads) pred_bias_grad_kernel(const float* __restrict__ g, int B, int c_tot, long long hw, int c_off, float* __restrict__ dbias) {
+  __shared__ float part[kEwThreads];
+  const int c = blockIdx.x;
+  float acc = 0.0f;
+  for (int b = 0; b < B; ++b) {
+    const float* plane = g + ((long long)b * c_tot + c_off + c) * hw;
+    for (long long q = threadIdx.x; q < hw; q += kEwThreads) acc += __ldg(plane + q);
+  }
+  part[threadIdx.x] = acc;
+  __syncthreads();
+  for (int s = kEwThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) part[threadIdx.x] += part[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) dbias[c] = part[0];
+}
+
 // fp32 master weights [cout][cin][kh][kw] (nn.Conv2d) -> bf16 [cout][kh*kw][cin] (forward / wgrad layout) and the backward-data operand
 // bf16 [cin][kh*kw][cout] with the taps rotated by 180 degrees.  The K rows are kin_pad = kpad(cin) / kout_pad = kpad(cout) long (16 and 32
 // channels: one zero-padded 64-channel chunk; the padding is zeroed by the caller)
@@ -809,7 +922,9 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
     if (rc != CVB_OK) return rc;
   }
   const void* fn;
-  if (bn == 128) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<128, true>) : reinterpret_cast<const void*>(&tconv_kernel<128, false>);
+  if (a.out_f32) fn = bn == 128 ? reinterpret_cast<const void*>(&tconv_kernel<128, false, true>)
+                               : (bn == 64 ? reinterpret_cast<const void*>(&tconv_kernel<64, false, true>) : reinterpret_cast<const void*>(&tconv_kernel<32, false, true>));
+  else if (bn == 128) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<128, true>) : reinterpret_cast<const void*>(&tconv_kernel<128, false>);
   else if (bn == 64) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<64, true>) : reinterpret_cast<const void*>(&tconv_kernel<64, false>);
   else fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<32, true>) : reinterpret_cast<const void*>(&tconv_kernel<32, false>);
   const int k_iters = a.taps * (kpad64(a.cin) / 64);
@@ -823,44 +938,100 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
   return CVB_OK;
 }
 
-extern "C" int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t stride, void* out,
-                              const void* y_prev, const float* bn_stat_prev, void* stream) {
-  CVB_REQUIRE(x && w_packed && out, "train_conv: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout) && B > 0 && H > 0 && W > 0,
-              "train_conv: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", cin, cout, k);
-  CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv: stride 1, or stride 2 with k = 3");
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, "train_conv: pointers must be 16-byte aligned");
-  CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv: the SiLU' epilogue needs both y_prev and its BN statistics");
-  TConvArgs a;
+// Stride-1 geometry with padding `pad`: the output is (H + 2 pad - k + 1) x (W + 2 pad - k + 1) and tap t reads input pixel
+// (h + t / k - pad, w + t % k - pad).  TMA zero-fills the pixels outside the map (pad > 0); a negative pad crops the border instead.
+static int conv_s1_setup(TConvArgs& a, const void* x, int B, int H, int W, int cin, int cout, int k, int pad) {
   memset(&a, 0, sizeof(a));
-  const int Ho = (H + 2 * (k / 2) - k) / stride + 1, Wo = (W + 2 * (k / 2) - k) / stride + 1;
+  const int Ho = H + 2 * pad - k + 1, Wo = W + 2 * pad - k + 1;
   a.H = Ho;
   a.W = Wo;
   a.B = B;
   a.cin = cin;
   a.cout = cout;
   a.taps = k * k;
-  a.out = static_cast<__nv_bfloat16*>(out);
   a.out_H = Ho;
   a.out_W = Wo;
   a.os = 1;
   choose_box128(B, Ho, Wo, &a.TW, &a.TH, &a.NB);
+  for (int t = 0; t < k * k; ++t) {
+    a.tap_dh[t] = (int8_t)(t / k - pad);
+    a.tap_dw[t] = (int8_t)(t % k - pad);
+    a.tap_map[t] = 0;
+    a.tap_wblk[t] = (int8_t)t;
+  }
+  return act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
+}
+
+// paddings of the stride-1 training convolutions: k // 2 (BaseConv), 1 on a 1x1 conv (the YOLOX head stems, heads/yolox_head.py:35) and
+// k - 1 - 1 = -1, the backward-data of that stem
+static bool train_pad_ok(int k, int pad) { return k == 1 ? (pad >= -1 && pad <= 1) : (k == 3 && pad == 1); }
+
+static int train_conv(const void* x, int B, int H, int W, int cin, const void* w_packed, int cout, int k, int stride, int pad, void* out, const void* y_prev,
+                      const float* bn_stat_prev, void* stream) {
+  CVB_REQUIRE(x && w_packed && out, "train_conv: null tensor");
+  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout) && B > 0 && H > 0 && W > 0,
+              "train_conv: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", cin, cout, k);
+  CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv: stride 1, or stride 2 with k = 3");
+  CVB_REQUIRE(train_pad_ok(k, pad), "train_conv: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", k, pad);
+  CVB_REQUIRE(H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "train_conv: empty output (H=%d W=%d k=%d pad=%d)", H, W, k, pad);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, "train_conv: pointers must be 16-byte aligned");
+  CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv: the SiLU' epilogue needs both y_prev and its BN statistics");
+  TConvArgs a;
   int rc = CVB_OK;
   if (stride == 1) {
-    for (int t = 0; t < k * k; ++t) {
-      a.tap_dh[t] = (int8_t)(t / k - k / 2);
-      a.tap_dw[t] = (int8_t)(t % k - k / 2);
-      a.tap_map[t] = 0;
-      a.tap_wblk[t] = (int8_t)t;
-    }
-    rc = act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
+    rc = conv_s1_setup(a, x, B, H, W, cin, cout, k, pad);
   } else {
+    memset(&a, 0, sizeof(a));
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    a.H = Ho;
+    a.W = Wo;
+    a.B = B;
+    a.cin = cin;
+    a.cout = cout;
+    a.out_H = Ho;
+    a.out_W = Wo;
+    a.os = 1;
+    choose_box128(B, Ho, Wo, &a.TW, &a.TH, &a.NB);
     a.taps = s2_taps(H, W, a.tap_dh, a.tap_dw, a.tap_map, a.tap_wblk);
     for (int py = 0; py < 2 && rc == CVB_OK; ++py)
       for (int px = 0; px < 2 && rc == CVB_OK; ++px) rc = act_map_strided(&a.tmA[py * 2 + px], x, B, H, W, cin, 2, py, px, a.TW, a.TH, a.NB);
   }
   if (rc != CVB_OK) return rc;
+  a.out = static_cast<__nv_bfloat16*>(out);
   return launch_tconv(a, w_packed, k * k, y_prev, bn_stat_prev, stream);
+}
+
+extern "C" int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t stride, void* out,
+                              const void* y_prev, const float* bn_stat_prev, void* stream) {
+  return train_conv(x, B, H, W, cin, w_packed, cout, k, stride, k / 2, out, y_prev, bn_stat_prev, stream);
+}
+
+extern "C" int cvb_train_conv_pad(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t pad, void* out,
+                                  const void* y_prev, const float* bn_stat_prev, void* stream) {
+  return train_conv(x, B, H, W, cin, w_packed, cout, k, 1, pad, out, y_prev, bn_stat_prev, stream);
+}
+
+// training width of a prediction conv's GEMM: the channels rounded up to 16, 32 or a multiple of 64
+static int pred_cout_pad(int c) { return c <= 16 ? 16 : (c <= 32 ? 32 : kpad64(c)); }
+
+extern "C" int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t cout_pad,
+                                   const float* bias, float* out, int32_t c_tot, int32_t c_off, void* stream) {
+  CVB_REQUIRE(x && w_packed && bias && out, "train_pred_conv: null tensor");
+  CVB_REQUIRE(train_channels_ok(cin) && B > 0 && H > 0 && W > 0, "train_pred_conv: cin must be 16, 32 or a multiple of 64 (cin=%d)", cin);
+  CVB_REQUIRE(cout > 0 && cout_pad == pred_cout_pad(cout), "train_pred_conv: cout_pad must be the next training width of cout (cout=%d cout_pad=%d)", cout, cout_pad);
+  CVB_REQUIRE(c_off >= 0 && c_off + cout <= c_tot, "train_pred_conv: channels [%d, %d) outside the %d-channel output", c_off, c_off + cout, c_tot);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed)) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0 &&
+                  (reinterpret_cast<uintptr_t>(bias) & 3) == 0,
+              "train_pred_conv: x / w_packed must be 16-byte, out / bias 4-byte aligned");
+  TConvArgs a;
+  const int rc = conv_s1_setup(a, x, B, H, W, cin, cout_pad, 1, 0);
+  if (rc != CVB_OK) return rc;
+  a.out_f32 = out;
+  a.bias = bias;
+  a.c_tot = c_tot;
+  a.c_off = c_off;
+  a.n_store = cout;
+  return launch_tconv(a, w_packed, 1, nullptr, nullptr, stream);
 }
 
 // Backward-data of the 3x3 / stride 2 / pad 1 convolution: dx[2a + pi, 2b + pj] gets dy[a + dh, b + dw] through the taps whose parity matches
@@ -911,16 +1082,17 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
   return CVB_OK;
 }
 
-extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t stride, float* dw,
-                                    void* stream) {
+static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int cin, int cout, int k, int stride, int pad, float* dw, void* stream) {
   CVB_REQUIRE(x && dy && dw, "train_conv_wgrad: null tensor");
   CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout),
               "train_conv_wgrad: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d)", cin, cout);
   CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv_wgrad: stride 1, or stride 2 with k = 3");
+  CVB_REQUIRE(train_pad_ok(k, pad), "train_conv_wgrad: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", k, pad);
+  CVB_REQUIRE(B > 0 && H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "train_conv_wgrad: empty output (H=%d W=%d k=%d pad=%d)", H, W, k, pad);
   CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15) == 0, "train_conv_wgrad: pointers must be 16-byte aligned");
   TWgradArgs a;
   memset(&a, 0, sizeof(a));
-  const int Ho = (H + 2 * (k / 2) - k) / stride + 1, Wo = (W + 2 * (k / 2) - k) / stride + 1;
+  const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   choose_box128(B, Ho, Wo, &a.TW, &a.TH, &a.NB);
   a.tiles_w = ceil_div(Wo, a.TW);
   a.tiles_h = ceil_div(Ho, a.TH);
@@ -943,8 +1115,8 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   int rc = CVB_OK, ntaps = k * k;
   if (stride == 1) {
     for (int t = 0; t < k * k; ++t) {
-      a.tap_dh[t] = (int8_t)(t / k - k / 2);
-      a.tap_dw[t] = (int8_t)(t % k - k / 2);
+      a.tap_dh[t] = (int8_t)(t / k - pad);
+      a.tap_dw[t] = (int8_t)(t % k - pad);
       a.tap_map[t] = 0;
       a.tap_idx[t] = (int8_t)t;
     }
@@ -968,6 +1140,16 @@ extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, in
   CVB_CHECK_CUDA(cudaLaunchKernel(fn, grid, dim3(kTThreads), kargs, (size_t)smem, as_stream(stream)));
   count_launch();
   return CVB_OK;
+}
+
+extern "C" int cvb_train_conv_wgrad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t stride, float* dw,
+                                    void* stream) {
+  return train_conv_wgrad(x, dy, B, H, W, cin, cout, k, stride, k / 2, dw, stream);
+}
+
+extern "C" int cvb_train_conv_wgrad_pad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t pad, float* dw,
+                                        void* stream) {
+  return train_conv_wgrad(x, dy, B, H, W, cin, cout, k, 1, pad, dw, stream);
 }
 
 // reduction kernels: `np` pixel lanes per CTA, at least ~4 pixels per thread, at most four CTAs per SM (2C global atomics per CTA)
@@ -1056,5 +1238,47 @@ extern "C" int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B,
                                                                          static_cast<__nv_bfloat16*>(da));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_upsample_cat_fwd(const void* a, int32_t B, int32_t h, int32_t w, int32_t Ca, const void* b, int32_t Cb, void* cat, void* stream) {
+  CVB_REQUIRE(a && b && cat && B > 0 && h > 0 && w > 0 && Ca > 0 && Cb > 0, "train_upsample_cat_fwd: bad argument");
+  CVB_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "train_upsample_cat_fwd: channels must be multiples of 8 (Ca=%d Cb=%d)", Ca, Cb);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0,
+              "train_upsample_cat_fwd: pointers must be 16-byte aligned");
+  const long long n = (long long)B * 4 * h * w * ((Ca + Cb) / 8);
+  upsample_cat_fwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, h, w, Ca, static_cast<const __nv_bfloat16*>(b),
+                                                                             Cb, static_cast<__nv_bfloat16*>(cat));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_upsample_cat_bwd(const void* g, int32_t B, int32_t h, int32_t w, int32_t Ca, int32_t Cb, void* da, void* db, void* stream) {
+  CVB_REQUIRE(g && da && db && B > 0 && h > 0 && w > 0 && Ca > 0 && Cb > 0, "train_upsample_cat_bwd: bad argument");
+  CVB_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "train_upsample_cat_bwd: channels must be multiples of 8 (Ca=%d Cb=%d)", Ca, Cb);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da) | reinterpret_cast<uintptr_t>(db)) & 15) == 0,
+              "train_upsample_cat_bwd: pointers must be 16-byte aligned");
+  const long long n = (long long)B * h * w * (Ca / 8) + (long long)B * 4 * h * w * (Cb / 8);
+  upsample_cat_bwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), B, h, w, Ca, Cb, static_cast<__nv_bfloat16*>(da),
+                                                                             static_cast<__nv_bfloat16*>(db));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int32_t h, int32_t w, int32_t c_off, int32_t cout, int32_t cout_pad, void* dy, float* dbias,
+                                   void* stream) {
+  CVB_REQUIRE(g && dy && dbias && B > 0 && h > 0 && w > 0, "train_pred_grad: bad argument");
+  CVB_REQUIRE(cout > 0 && cout_pad == pred_cout_pad(cout), "train_pred_grad: cout_pad must be the next training width of cout (cout=%d cout_pad=%d)", cout, cout_pad);
+  CVB_REQUIRE(c_off >= 0 && c_off + cout <= c_tot, "train_pred_grad: channels [%d, %d) outside the %d-channel gradient", c_off, c_off + cout, c_tot);
+  CVB_REQUIRE((reinterpret_cast<uintptr_t>(dy) & 15) == 0 && ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dbias)) & 3) == 0,
+              "train_pred_grad: dy must be 16-byte, g / dbias 4-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  const long long hw = (long long)h * w;
+  pred_grad_nhwc_kernel<<<ew_grid((long long)B * hw * (cout_pad / 8)), kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, cout, cout_pad, static_cast<__nv_bfloat16*>(dy));
+  pred_bias_grad_kernel<<<cout, kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, dbias);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(2);
   return CVB_OK;
 }

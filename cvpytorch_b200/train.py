@@ -7,8 +7,12 @@ Mirrors (paths relative to the reference checkout), with the same constructor ar
   Focus        src/models/modules/yolo_modules.py:19-37     2x2 space-to-depth (patches tl, bl, tr, br) -> 3x3 conv 12 -> cout
   SPPF         src/models/modules/yolo_modules.py:165-194   conv1 -> cat[x, maxpool5, maxpool9, maxpool13] (parallel pools) -> conv2
   CSPDarknet   src/models/backbones/det/csp_darknet.py:25-129   stem, four stages, SPPF in stage4
+  YOLOXNeck    src/models/necks/yolox_neck.py:13-74           top-down (upsample + concat) and bottom-up (stride-2 conv + concat) CSP path
+  ConvModule   src/models/modules/convs.py                     conv -> BN -> SiLU as the YOLOX head builds it (1x1 stems with padding 1)
+  YOLOXHead    src/models/heads/yolox_head.py:14-88            stems, cls / reg branches, prediction convs with bias -> fp32 NCHW outputs
 
-Channel counts of every convolution: 16, 32 or multiples of 64 (YOLOX-n, -s and -l; the 24 / 48 / 80-wide -t, -m and -x raise).
+Channel counts of every convolution: 16, 32 or multiples of 64 (YOLOX-n, -s and -l; the 24 / 48 / 80-wide -t, -m and -x raise).  The
+prediction convs (num_classes, 4 and 1 outputs) run as GEMMs zero-padded to the next such width.
 
 What runs where: every convolution (forward, backward-data, backward-weight) is a bf16 wgmma implicit GEMM and every BatchNorm / SiLU pass
 (statistics, apply, backward reductions, backward apply) is a kernel of libcvb200.so (csrc/train_kernels.cu).  torch.autograd only chains the
@@ -19,6 +23,7 @@ weight gradients (BASELINE.json configs[3] asks for a bf16 step).  No CPU fallba
 Inside a block activations are NHWC bf16; `CSPLayer.forward` accepts / returns the reference's NCHW tensors (layout change at the boundary).
 """
 import ctypes
+import math
 
 import torch
 import torch.nn as nn
@@ -57,12 +62,20 @@ def pack_weights(w):
     return wf, wb
 
 
-def conv(x, w_packed, cout, k, y_prev=None, stat_prev=None, stride=1):
-    """x NHWC bf16 [B,H,W,cin] -> [B,Ho,Wo,cout] (pad k//2).  (y_prev, stat_prev): SiLU' epilogue of the producing layer (backward-data only)."""
+def conv(x, w_packed, cout, k, y_prev=None, stat_prev=None, stride=1, pad=None):
+    """x NHWC bf16 [B,H,W,cin] -> [B,Ho,Wo,cout] (pad k//2, or `pad` at stride 1: -1, 0 or 1 with k = 1).  (y_prev, stat_prev): SiLU' epilogue
+    of the producing layer (backward-data only)."""
     B, H, W, cin = x.shape
-    Ho, Wo = (H + 2 * (k // 2) - k) // stride + 1, (W + 2 * (k // 2) - k) // stride + 1
+    p = k // 2 if pad is None else pad
+    Ho, Wo = (H + 2 * p - k) // stride + 1, (W + 2 * p - k) // stride + 1
     out = torch.empty((B, Ho, Wo, cout), dtype=torch.bfloat16, device=x.device)
-    _lib.check(_lib.lib().cvb_train_conv(_p(x), B, H, W, cin, _p(w_packed), cout, k, stride, _p(out), _p(y_prev), _p(stat_prev), _stream()), 'cvb_train_conv')
+    if pad is None:
+        _lib.check(_lib.lib().cvb_train_conv(_p(x), B, H, W, cin, _p(w_packed), cout, k, stride, _p(out), _p(y_prev), _p(stat_prev), _stream()), 'cvb_train_conv')
+    else:
+        if stride != 1:
+            raise ValueError('train.conv: an explicit padding is for stride-1 convolutions')
+        _lib.check(_lib.lib().cvb_train_conv_pad(_p(x), B, H, W, cin, _p(w_packed), cout, k, pad, _p(out), _p(y_prev), _p(stat_prev), _stream()),
+                   'cvb_train_conv_pad')
     return out
 
 
@@ -75,12 +88,17 @@ def conv_dgrad_s2(dy, w_bwd, cin, H, W, y_prev=None, stat_prev=None):
     return dx
 
 
-def conv_wgrad(x, dy, k, stride=1):
-    """-> fp32 [cout, cin, k, k] (the nn.Conv2d layout)."""
+def conv_wgrad(x, dy, k, stride=1, pad=None):
+    """-> fp32 [cout, cin, k, k] (the nn.Conv2d layout).  `pad`: as in conv (stride 1)."""
     B, H, W, cin = x.shape
     cout = dy.shape[3]
     dw = torch.zeros((cout, k * k, cin), dtype=torch.float32, device=x.device)
-    _lib.check(_lib.lib().cvb_train_conv_wgrad(_p(x), _p(dy), B, H, W, cin, cout, k, stride, _p(dw), _stream()), 'cvb_train_conv_wgrad')
+    if pad is None:
+        _lib.check(_lib.lib().cvb_train_conv_wgrad(_p(x), _p(dy), B, H, W, cin, cout, k, stride, _p(dw), _stream()), 'cvb_train_conv_wgrad')
+    else:
+        if stride != 1:
+            raise ValueError('train.conv_wgrad: an explicit padding is for stride-1 convolutions')
+        _lib.check(_lib.lib().cvb_train_conv_wgrad_pad(_p(x), _p(dy), B, H, W, cin, cout, k, pad, _p(dw), _stream()), 'cvb_train_conv_wgrad_pad')
     return dw.view(cout, k, k, cin).permute(0, 3, 1, 2)
 
 
@@ -88,13 +106,13 @@ class _ConvBnSiLU(torch.autograd.Function):
     """a = silu(bn_train(conv(x, W))) with the backward the reference obtains from torch.autograd, on the H100 kernels."""
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1, pad=None):
         _check_cuda(x, 'BaseConv (H100 training)')
         B, H, W, cin = x.shape
         cout = weight.shape[0]
         L = _lib.lib()
         wf, wb = pack_weights(weight)
-        y = conv(x, wf, cout, k, stride=stride)
+        y = conv(x, wf, cout, k, stride=stride, pad=pad)
         npix = B * y.shape[1] * y.shape[2]
         stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
         scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
@@ -106,6 +124,7 @@ class _ConvBnSiLU(torch.autograd.Function):
         ctx.save_for_backward(x, y, stat, g32, wb)
         ctx.k = k
         ctx.stride = stride
+        ctx.pad = pad
         ctx.need_dx = x.requires_grad
         return a
 
@@ -121,11 +140,14 @@ class _ConvBnSiLU(torch.autograd.Function):
         dy = torch.empty_like(y)
         _lib.check(L.cvb_train_bn_silu_bwd(_p(da), 0, _p(y), B * y.shape[1] * y.shape[2], cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()),
                    'cvb_train_bn_silu_bwd')
-        dw = conv_wgrad(x, dy, k, ctx.stride)
+        dw = conv_wgrad(x, dy, k, ctx.stride, ctx.pad)
         dx = None
         if ctx.need_dx:
-            dx = conv(dy, wb, cin, k) if ctx.stride == 1 else conv_dgrad_s2(dy, wb, cin, H, W)
-        return dx, dw, sums[1].clone(), sums[0].clone(), None, None, None, None, None, None
+            if ctx.stride == 2:
+                dx = conv_dgrad_s2(dy, wb, cin, H, W)
+            else:  # backward-data of a padding-p conv: the same conv over dy with the rotated weights and padding k - 1 - p
+                dx = conv(dy, wb, cin, k, pad=None if ctx.pad is None else k - 1 - ctx.pad)
+        return dx, dw, sums[1].clone(), sums[0].clone(), None, None, None, None, None, None, None
 
 
 class _BottleneckChain(torch.autograd.Function):
@@ -432,3 +454,223 @@ class CSPDarknet(nn.Module):
     def forward(self, x):
         outs = [o.permute(0, 3, 1, 2).to(x.dtype) for o in self.forward_nhwc(x)]
         return outs if len(self.out_stages) > 1 else outs[0]
+
+
+# ------------------------------------------------------------------------------------------------ YOLOX neck and head
+def upsample_cat(a, b):
+    """a NHWC bf16 [B,h,w,Ca], b [B,2h,2w,Cb] -> [B,2h,2w,Ca+Cb] = [nearest_up2(a) | b] (the neck's nn.Upsample + torch.cat, upsampled map first)."""
+    B, h, w, Ca = a.shape
+    Cb = b.shape[3]
+    if tuple(b.shape[:3]) != (B, 2 * h, 2 * w):
+        raise ValueError(f'upsample_cat: b must be [B, 2h, 2w, Cb] for a [B, h, w, Ca] (got a {tuple(a.shape)}, b {tuple(b.shape)})')
+    cat = torch.empty((B, 2 * h, 2 * w, Ca + Cb), dtype=torch.bfloat16, device=a.device)
+    _lib.check(_lib.lib().cvb_train_upsample_cat_fwd(_p(a), B, h, w, Ca, _p(b), Cb, _p(cat), _stream()), 'cvb_train_upsample_cat_fwd')
+    return cat
+
+
+def upsample_cat_backward(g, Ca):
+    """g = d(loss)/d(cat) [B,2h,2w,Ca+Cb] -> (da [B,h,w,Ca] = the 2x2 sums of g[..., :Ca], db = g[..., Ca:]); deterministic, fp32 sums."""
+    B, H2, W2, C = g.shape
+    da = torch.empty((B, H2 // 2, W2 // 2, Ca), dtype=torch.bfloat16, device=g.device)
+    db = torch.empty((B, H2, W2, C - Ca), dtype=torch.bfloat16, device=g.device)
+    _lib.check(_lib.lib().cvb_train_upsample_cat_bwd(_p(g), B, H2 // 2, W2 // 2, Ca, C - Ca, _p(da), _p(db), _stream()), 'cvb_train_upsample_cat_bwd')
+    return da, db
+
+
+class _UpsampleCat(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, a, b):
+        _check_cuda(a, 'YOLOXNeck (H100 training)')
+        ctx.ca = a.shape[3]
+        return upsample_cat(a.contiguous(), b.contiguous())
+
+    @staticmethod
+    def backward(ctx, g):
+        return upsample_cat_backward(g.contiguous(), ctx.ca)
+
+
+def pred_cout_pad(c):
+    """GEMM width of a prediction conv with c outputs: the next training width (16, 32 or a multiple of 64)."""
+    return 16 if c <= 16 else (32 if c <= 32 else kpad(c))
+
+
+def pred_conv(x, w_packed, cout, bias, out, c_off):
+    """1x1 prediction conv with bias: x NHWC bf16 [B,h,w,cin], w_packed = pack_weights(weight zero-padded to pred_cout_pad(cout) rows)[0]
+    -> out fp32 NCHW [B,Ctot,h,w] channels [c_off, c_off + cout) = conv + bias."""
+    B, h, w, cin = x.shape
+    _lib.check(_lib.lib().cvb_train_pred_conv(_p(x), B, h, w, cin, _p(w_packed), cout, pred_cout_pad(cout), _p(bias), _p(out), out.shape[1], c_off, _stream()),
+               'cvb_train_pred_conv')
+
+
+def pred_grad(g, c_off, cout):
+    """g fp32 NCHW [B,Ctot,h,w] -> (dy bf16 NHWC [B,h,w,pred_cout_pad(cout)] = channels [c_off, c_off + cout) of g, zero-padded; dbias [cout])."""
+    B, Ctot, h, w = g.shape
+    cp = pred_cout_pad(cout)
+    dy = torch.empty((B, h, w, cp), dtype=torch.bfloat16, device=g.device)
+    db = torch.empty((cout,), dtype=torch.float32, device=g.device)
+    _lib.check(_lib.lib().cvb_train_pred_grad(_p(g), B, Ctot, h, w, c_off, cout, cp, _p(dy), _p(db), _stream()), 'cvb_train_pred_grad')
+    return dy, db
+
+
+class _HeadPred(torch.autograd.Function):
+    """One level's output [B, 5 + num_classes, h, w] fp32 NCHW = cat(reg_obj_preds(reg_feat), cls_preds(cls_feat)) (heads/yolox_head.py:75-85):
+    reg (4) + obj (1) are one GEMM over reg_feat at channel 0, cls a second GEMM over cls_feat at channel 5, both writing the output in place."""
+
+    @staticmethod
+    def forward(ctx, reg_feat, cls_feat, w_ro, b_ro, w_cls, b_cls):
+        _check_cuda(reg_feat, 'YOLOXHead (H100 training)')
+        B, h, w, _ = reg_feat.shape
+        out = torch.empty((B, w_ro.shape[0] + w_cls.shape[0], h, w), dtype=torch.float32, device=reg_feat.device)
+        wbs = []
+        for x, wt, b, c_off in ((reg_feat, w_ro, b_ro, 0), (cls_feat, w_cls, b_cls, w_ro.shape[0])):
+            cout = wt.shape[0]
+            wf, wb = pack_weights(nn.functional.pad(wt.detach().float(), (0, 0, 0, 0, 0, 0, 0, pred_cout_pad(cout) - cout)))
+            pred_conv(x.contiguous(), wf, cout, b.detach().float().contiguous(), out, c_off)
+            wbs.append(wb)
+        ctx.save_for_backward(reg_feat, cls_feat, *wbs)
+        ctx.couts = (w_ro.shape[0], w_cls.shape[0])
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        reg_feat, cls_feat, wb_ro, wb_cls = ctx.saved_tensors
+        g = g.contiguous()
+        res = []
+        for x, wb, c_off, cout, need in ((reg_feat, wb_ro, 0, ctx.couts[0], ctx.needs_input_grad[0]), (cls_feat, wb_cls, ctx.couts[0], ctx.couts[1], ctx.needs_input_grad[1])):
+            dy, db = pred_grad(g, c_off, cout)
+            dw = conv_wgrad(x, dy, 1)[:cout]
+            dx = conv(dy, wb, x.shape[3], 1) if need else None
+            res.append((dx, dw, db))
+        (dx_ro, dw_ro, db_ro), (dx_cls, dw_cls, db_cls) = res
+        return dx_ro, dx_cls, dw_ro, db_ro, dw_cls, db_cls
+
+
+class ConvModule(nn.Module):
+    """src/models/modules/convs.py ConvModule as heads/yolox_head.py:33-49 builds it: conv (no bias) -> BatchNorm -> SiLU, training mode.
+    kernel_size 1 or 3, stride 1, padding kernel_size // 2 or 1 (the head stems are 1x1 convs with padding 1).  forward: NHWC bf16 in / out."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, activation='SiLU'):
+        super().__init__()
+        if kernel_size not in (1, 3) or stride != 1 or padding not in (kernel_size // 2, 1) or activation != 'SiLU':
+            raise NotImplementedError('H100 training ConvModule: kernel_size 1 or 3, stride 1, padding kernel_size // 2 or 1, SiLU')
+        if not (channels_ok(in_channels) and channels_ok(out_channels)):
+            raise NotImplementedError(f'H100 training ConvModule: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
+        self.conv = nn.Conv2d(in_channels, out_channels, kernel_size, stride, padding, bias=False)
+        self.bn = nn.BatchNorm2d(out_channels)
+        self.act = nn.SiLU(inplace=True)  # (parameter-free; module-tree parity)
+        self.ksize, self.padding = kernel_size, padding
+
+    def forward(self, x):
+        if not self.training:
+            raise RuntimeError('cvpytorch_b200.train.ConvModule is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
+        bn = self.bn
+        mom = _bn_momentum(bn)
+        return _ConvBnSiLU.apply(x, self.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, mom, self.ksize, 1, self.padding)
+
+
+def _set_bn(m):
+    for mod in m.modules():
+        if isinstance(mod, nn.BatchNorm2d):
+            mod.eps, mod.momentum = 1e-3, 0.03
+
+
+def _to_nhwc(xs):
+    for x in xs:
+        _check_cuda(x, 'YOLOX neck / head (H100 training)')
+    return [x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16) for x in xs]
+
+
+class YOLOXNeck(nn.Module):
+    """src/models/necks/yolox_neck.py:13-74, training mode, same constructor and state_dict keys; BatchNorm eps 1e-3, momentum 0.03.
+    forward_nhwc([x2, x1, x0] NHWC bf16) -> [pan_out2, pan_out1, pan_out0] NHWC bf16; forward takes and returns NCHW.  The top-down
+    upsample + concat is one kernel each way (cvb_train_upsample_cat_*); the bottom-up concats are torch.cat, as in CSPLayer.  The maps must
+    halve exactly (x2 = 2 x1 = 4 x0 in height and width).  Evaluation: load the state_dict into cvpytorch_b200.yolox_models.YOLOXNeck."""
+
+    def __init__(self, subtype='yolox_s', channels=[256, 512, 1024], depth_mul=1.0, width_mul=1.0):
+        super().__init__()
+        assert isinstance(channels, list)
+        self.subtype, self.channels, self.num_ins = subtype, channels, len(channels)
+        c = list(map(lambda x: max(round(x * width_mul), 1), channels))
+        n = list(map(lambda x: max(round(x * depth_mul), 1), [3, 3, 3, 3]))
+        bad = sorted({v for v in c + [int(v * 0.5) for v in c] if not channels_ok(v)})
+        if bad:
+            raise NotImplementedError(f'H100 training YOLOXNeck: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        self.upsample = nn.Upsample(scale_factor=2, mode='nearest')  # (parameter-free; module-tree parity)
+        self.lateral_conv0 = BaseConv(c[2], c[1], 1, 1)
+        self.C3_p4 = CSPLayer(2 * c[1], c[1], n[0], False)
+        self.reduce_conv1 = BaseConv(c[1], c[0], 1, 1)
+        self.C3_p3 = CSPLayer(2 * c[0], c[0], n[1], False)
+        self.bu_conv2 = BaseConv(c[0], c[0], 3, 2)
+        self.C3_n3 = CSPLayer(2 * c[0], c[1], n[2], False)
+        self.bu_conv1 = BaseConv(c[1], c[1], 3, 2)
+        self.C3_n4 = CSPLayer(2 * c[1], c[2], n[3], False)
+        _set_bn(self)
+
+    def forward_nhwc(self, x):
+        if not self.training:
+            raise RuntimeError('cvpytorch_b200.train.YOLOXNeck is the TRAINING drop-in (batch statistics); load its state_dict into '
+                               'cvpytorch_b200.yolox_models.YOLOXNeck for eval()')
+        if len(x) != self.num_ins:
+            raise ValueError(f'YOLOXNeck: {self.num_ins} feature maps expected, got {len(x)}')
+        x2, x1, x0 = x
+        for big, small in ((x1, x0), (x2, x1)):
+            if big.shape[0] != small.shape[0] or big.shape[1] != 2 * small.shape[1] or big.shape[2] != 2 * small.shape[2]:
+                raise ValueError(f'YOLOXNeck: each feature map must be exactly twice the next one in height and width (got {[tuple(t.shape) for t in x]}, NHWC)')
+        fpn_out0 = self.lateral_conv0(x0)
+        f_out0 = self.C3_p4.forward_nhwc(_UpsampleCat.apply(fpn_out0, x1))
+        fpn_out1 = self.reduce_conv1(f_out0)
+        pan_out2 = self.C3_p3.forward_nhwc(_UpsampleCat.apply(fpn_out1, x2))
+        pan_out1 = self.C3_n3.forward_nhwc(torch.cat((self.bu_conv2(pan_out2), fpn_out1), dim=3))
+        pan_out0 = self.C3_n4.forward_nhwc(torch.cat((self.bu_conv1(pan_out1), fpn_out0), dim=3))
+        return [pan_out2, pan_out1, pan_out0]
+
+    def forward(self, x):
+        return [o.permute(0, 3, 1, 2).to(x[0].dtype) for o in self.forward_nhwc(_to_nhwc(x))]
+
+
+class YOLOXHead(nn.Module):
+    """src/models/heads/yolox_head.py:14-88, training mode, same constructor and state_dict keys (stems, cls_convs, reg_convs, cls_preds,
+    reg_preds, obj_preds), the prior-probability bias of cls_preds / obj_preds, BatchNorm eps 1e-3, momentum 0.03.  forward (NCHW maps) and
+    forward_nhwc (NHWC bf16 maps, e.g. YOLOXNeck.forward_nhwc's) both return the reference's list of fp32 NCHW [B, 5 + num_classes, h + 2, w + 2]
+    outputs (reg, obj, cls), contiguous, for the reference YOLOXLoss.  Widths: int(256 * width_mul) and the inputs must be 16, 32 or multiples of
+    64.  Evaluation: load the state_dict into cvpytorch_b200.yolox_models.YOLOXHead."""
+
+    def __init__(self, num_classes=80, subtype='yolox_s', in_channels=[256, 512, 1024], strides=[8, 16, 32], depth_mul=1.0, width_mul=1.0):
+        super().__init__()
+        self.num_classes, self.subtype, self.strides, self.n_anchors = num_classes, subtype, strides, 1
+        ic = list(map(lambda x: max(round(x * width_mul), 1), in_channels))
+        p = int(256 * width_mul)
+        bad = sorted({v for v in ic + [p] if not channels_ok(v)})
+        if bad:
+            raise NotImplementedError(f'H100 training YOLOXHead: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        self.stems, self.cls_convs, self.reg_convs = nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
+        self.cls_preds, self.reg_preds, self.obj_preds = nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
+        for c in ic:
+            self.stems.append(ConvModule(c, p, 1, 1, padding=1))  # padding=1 on a 1x1 conv: every head map is 2 pixels larger
+            self.cls_convs.append(nn.Sequential(ConvModule(p, p, 3, 1, 1), ConvModule(p, p, 3, 1, 1)))
+            self.reg_convs.append(nn.Sequential(ConvModule(p, p, 3, 1, 1), ConvModule(p, p, 3, 1, 1)))
+            self.cls_preds.append(nn.Conv2d(p, self.n_anchors * num_classes, 1, 1, 0))
+            self.reg_preds.append(nn.Conv2d(p, 4, 1, 1, 0))
+            self.obj_preds.append(nn.Conv2d(p, self.n_anchors * 1, 1, 1, 0))
+        _set_bn(self)
+        prior = -math.log((1 - 1e-2) / 1e-2)  # heads/yolox_head.py:54-72
+        with torch.no_grad():
+            for conv in list(self.cls_preds) + list(self.obj_preds):
+                conv.bias.fill_(prior)
+
+    def forward_nhwc(self, x):
+        if not self.training:
+            raise RuntimeError('cvpytorch_b200.train.YOLOXHead is the TRAINING drop-in (batch statistics); load its state_dict into '
+                               'cvpytorch_b200.yolox_models.YOLOXHead for eval()')
+        outputs = []
+        for k, xx in enumerate(x):
+            xx = self.stems[k](xx)  # (the stem's output fans out to both branches: autograd adds the two gradients)
+            cls_feat = self.cls_convs[k](xx)
+            reg_feat = self.reg_convs[k](xx)
+            w_ro = torch.cat((self.reg_preds[k].weight, self.obj_preds[k].weight), 0)
+            b_ro = torch.cat((self.reg_preds[k].bias, self.obj_preds[k].bias), 0)
+            outputs.append(_HeadPred.apply(reg_feat, cls_feat, w_ro, b_ro, self.cls_preds[k].weight, self.cls_preds[k].bias))
+        return outputs
+
+    def forward(self, x):
+        return self.forward_nhwc(_to_nhwc(x))

@@ -372,6 +372,23 @@ int cvb_coco_pack(const float* rows, int32_t B, int32_t M, int32_t row_stride, c
  *   (ties: the first maximal element, as torch's max_pool2d).
  * cvb_train_spp_pool_bwd: g = d(loss)/d(cat) [B,H,W,4C], idx of the forward -> da [B,H,W,C] = g[..., :C] + the pooled gradients routed to
  *   their winners; a gather summed in fp32 in a fixed order (bitwise reproducible).
+ *
+ * YOLOX neck and head training (src/models/necks/yolox_neck.py:13-74, src/models/heads/yolox_head.py:14-88) adds:
+ * cvb_train_upsample_cat_fwd: cat [B,2h,2w,Ca+Cb] = [nearest_up2(a [B,h,w,Ca]) | b [B,2h,2w,Cb]] (the neck's top-down upsample + concat,
+ *   the upsampled map first).  Ca, Cb multiples of 8; a plain copy, bit-exact.
+ * cvb_train_upsample_cat_bwd: g = d(loss)/d(cat) -> da [B,h,w,Ca] = 2x2 sum of g[..., :Ca] (fp32 in a fixed order, rounded to bf16 once)
+ *   and db = g[..., Ca:]; no atomics, bitwise reproducible.
+ * cvb_train_conv_pad / cvb_train_conv_wgrad_pad: cvb_train_conv / cvb_train_conv_wgrad at stride 1 with padding `pad`: the output is
+ *   (H + 2 pad - k + 1) x (W + 2 pad - k + 1), tap t reads (h + t / k - pad, w + t % k - pad).  k = 1 with pad -1, 0 or 1; k = 3 with pad 1.
+ *   The head stems are 1x1 convs with pad 1 (every head map is 2 pixels larger than its feature map); their backward-data is the pad
+ *   k - 1 - 1 = -1 conv of dy with w_bwd (the border is cropped).  cvb_train_conv / cvb_train_conv_wgrad are these with pad = k / 2.
+ * cvb_train_pred_conv: the head's prediction convs (1x1, bias, no BatchNorm or activation).  A cout_pad-wide GEMM over x [B,H,W,cin] with
+ *   w_packed = cvb_train_pack_weights of the weight zero-padded to cout_pad rows; out fp32 NCHW [B,c_tot,H,W] channels
+ *   [c_off, c_off + cout) = GEMM columns [0, cout) + bias (the other channels are not written).  cout_pad = cout rounded up to 16, 32 or a
+ *   multiple of 64.
+ * cvb_train_pred_grad: g fp32 NCHW [B,c_tot,h,w] (the loss's gradient of the head output) -> dy bf16 NHWC [B,h,w,cout_pad] = channels
+ *   [c_off, c_off + cout) of g, zero past cout (the operand of backward-data / backward-weight), and dbias [cout] = the sum of those
+ *   channels over images and pixels (fp32, fixed order).
  */
 int cvb_train_pack_weights(const float* w, int32_t cout, int32_t cin, int32_t k, void* w_fwd, void* w_bwd, void* stream);
 int cvb_train_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t stride, void* out,
@@ -388,6 +405,16 @@ int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void* y, int64_t
 int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream);
 int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream);
 int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, void* da, void* stream);
+int cvb_train_upsample_cat_fwd(const void* a, int32_t B, int32_t h, int32_t w, int32_t Ca, const void* b, int32_t Cb, void* cat, void* stream);
+int cvb_train_upsample_cat_bwd(const void* g, int32_t B, int32_t h, int32_t w, int32_t Ca, int32_t Cb, void* da, void* db, void* stream);
+int cvb_train_conv_pad(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t pad, void* out,
+                       const void* y_prev, const float* bn_stat_prev, void* stream);
+int cvb_train_conv_wgrad_pad(const void* x, const void* dy, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t k, int32_t pad, float* dw,
+                             void* stream);
+int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t cout_pad, const float* bias,
+                        float* out, int32_t c_tot, int32_t c_off, void* stream);
+int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int32_t h, int32_t w, int32_t c_off, int32_t cout, int32_t cout_pad, void* dy, float* dbias,
+                        void* stream);
 
 /* Library info / errors */
 const char* cvb_last_error_string(void);
