@@ -1,5 +1,6 @@
-// Training-step kernels for the YOLOX C3 block (SURVEY.md 8 f-3): conv forward / backward-data / backward-weight as bf16 implicit
-// GEMMs on wgmma + TMA, and the BatchNorm(batch statistics) + SiLU forward / backward element-wise passes around them.
+// Training-step kernels for the whole YOLOX network, backbone, neck and head (SURVEY.md 8 f-3): conv forward / backward-data /
+// backward-weight as bf16 implicit GEMMs on wgmma + TMA, the BatchNorm(batch statistics) + SiLU forward / backward element-wise passes
+// around them, and the Focus space-to-depth, SPPF pooling, neck upsample-concat and head prediction-conv passes.
 //
 // Replaces, for one  BaseConv = nn.Conv2d -> nn.BatchNorm2d -> SiLU  in training mode (src/models/modules/yolox_modules.py:35-55) and
 // its autograd backward (what trainer.py:177-207 runs through cuDNN / ATen):
@@ -11,8 +12,9 @@
 //             dx = conv(dy, W rotated by 180 degrees, in/out swapped)   tconv_kernel again (optionally with the PRODUCER's SiLU' in the epilogue)
 //             dW[co][tap][ci] = sum_pixels dy[p][co] * x[p + tap][ci]    twgrad_kernel   (K = pixels: both operands MN-major in shared memory)
 //
-// Layout: activations and gradients are NHWC bf16, dense (pitch == C, C a multiple of 64); weights bf16 [cout][kh*kw][cin] (K-major rows),
-// fp32 master weights / fp32 weight gradients outside.  One TMA box {64 channels, TW, TH, NB} with TW*TH*NB == 128 pixels is at the same
+// Layout: activations and gradients are NHWC bf16, dense (pitch == C; C = 16, 32 or a multiple of 64, and TMA zero-fills a box's channels
+// past a 16- or 32-channel C); weights bf16 [cout][kh*kw][kpad(cin)] (K-major rows, zero-padded to 64 channels), fp32 master weights / fp32
+// weight gradients outside.  One TMA box {64 channels, TW, TH, NB} with TW*TH*NB == 128 pixels is at the same
 // time a K-major A tile of the forward GEMM (row = pixel, 128 bytes of channels) and an MN-major operand of the weight-gradient GEMM
 // (K = pixel rows); out-of-bounds pixels are zero-filled by TMA = the convolution padding, and contribute nothing to dW.
 #include <cuda_bf16.h>
@@ -876,14 +878,30 @@ extern "C" int cvb_train_pack_weights(const float* w, int32_t cout, int32_t cin,
   return CVB_OK;
 }
 
-// tensor map of one parity class (py, px) of an NHWC tensor: pixels (2i + py, 2j + px); (0, 0) with step 1 is the plain map
-static int act_map_strided(CUtensorMap* m, const void* base, int B, int H, int W, int C, int step, int py, int px, int TW, int TH, int NB) {
-  const int Wp = (W - px + step - 1) / step, Hp = (H - py + step - 1) / step;
-  if (Wp <= 0 || Hp <= 0) return act_map(m, base, B, H, W, C, TW, TH, NB);  // no pixel of this parity, no tap reads it (s2_taps): any valid map
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
-  const cuuint64_t str[3] = {(cuuint64_t)C * 2 * step, (cuuint64_t)C * 2 * W * step, (cuuint64_t)C * 2 * W * H};
+// m[py * 2 + px]: tensor map of the parity class (py, px) of an NHWC tensor, pixels (2i + py, 2j + px), the inputs of s2_taps' tap_map
+static int parity_maps(CUtensorMap* m, const void* base, int B, int H, int W, int C, int TW, int TH, int NB) {
   const cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB};
-  return encode_tiled(m, 4, static_cast<const uint8_t*>(base) + ((size_t)py * W + px) * C * 2, dims, str, box);
+  int rc = CVB_OK;
+  for (int p = 0; p < 4 && rc == CVB_OK; ++p) {
+    const int py = p >> 1, px = p & 1;
+    const int Wp = (W - px + 1) / 2, Hp = (H - py + 1) / 2;
+    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
+    const cuuint64_t str[3] = {(cuuint64_t)C * 2 * 2, (cuuint64_t)C * 2 * W * 2, (cuuint64_t)C * 2 * W * H};
+    if (Wp <= 0 || Hp <= 0) rc = act_map(&m[p], base, B, H, W, C, TW, TH, NB);  // no pixel of this parity, no tap reads it (s2_taps): any valid map
+    else rc = encode_tiled(&m[p], 4, static_cast<const uint8_t*>(base) + ((size_t)py * W + px) * C * 2, dims, str, box);
+  }
+  return rc;
+}
+
+// stride 1, padding pad: tap t reads input pixel (h + t / k - pad, w + t % k - pad) of the one input map and weight K block t.  -> k * k
+static int s1_taps(int k, int pad, int8_t* dh, int8_t* dw, int8_t* map, int8_t* tap) {
+  for (int t = 0; t < k * k; ++t) {
+    dh[t] = (int8_t)(t / k - pad);
+    dw[t] = (int8_t)(t % k - pad);
+    map[t] = 0;
+    tap[t] = (int8_t)t;
+  }
+  return k * k;
 }
 
 // stride-2 3x3 / pad 1: tap (ky, kx) reads input pixel (2h + ky - 1, 2w + kx - 1) = parity class ((ky + 1) & 1, (kx + 1) & 1) at index
@@ -904,11 +922,28 @@ static int s2_taps(int H, int W, int8_t* dh, int8_t* dw, int8_t* map, int8_t* ta
   return n;
 }
 
+// Zeroed launch arguments for an H x W x B tile grid whose point (h, w) writes pixel (h * os + ooh, w * os + oow) of the out_H x out_W
+// tensor `out`, with the grid's 128-pixel box and tile counts.  The caller adds the taps and their input maps.
+static void tconv_geometry(TConvArgs& a, int B, int H, int W, int cin, int cout, void* out, int out_H, int out_W, int os, int ooh, int oow) {
+  memset(&a, 0, sizeof(a));
+  a.B = B;
+  a.H = H;
+  a.W = W;
+  a.cin = cin;
+  a.cout = cout;
+  a.out = static_cast<__nv_bfloat16*>(out);
+  a.out_H = out_H;
+  a.out_W = out_W;
+  a.os = os;
+  a.ooh = ooh;
+  a.oow = oow;
+  choose_box128(B, H, W, &a.TW, &a.TH, &a.NB);
+  a.tiles_w = ceil_div(W, a.TW);
+  a.tiles_h = ceil_div(H, a.TH);
+  a.tiles_b = ceil_div(B, a.NB);
+}
+
 static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const void* y_prev, const float* bn_stat_prev, void* stream) {
-  choose_box128(a.B, a.H, a.W, &a.TW, &a.TH, &a.NB);
-  a.tiles_w = ceil_div(a.W, a.TW);
-  a.tiles_h = ceil_div(a.H, a.TH);
-  a.tiles_b = ceil_div(a.B, a.NB);
   a.y_prev = static_cast<const __nv_bfloat16*>(y_prev);
   a.s_prev = bn_stat_prev ? bn_stat_prev + 2 * (size_t)a.cout : nullptr;
   a.t_prev = bn_stat_prev ? bn_stat_prev + 3 * (size_t)a.cout : nullptr;
@@ -921,12 +956,12 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
     const int rc = encode_tiled(&a.tmB, 2, w_packed, dims, str, box);
     if (rc != CVB_OK) return rc;
   }
-  const void* fn;
-  if (a.out_f32) fn = bn == 128 ? reinterpret_cast<const void*>(&tconv_kernel<128, false, true>)
-                               : (bn == 64 ? reinterpret_cast<const void*>(&tconv_kernel<64, false, true>) : reinterpret_cast<const void*>(&tconv_kernel<32, false, true>));
-  else if (bn == 128) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<128, true>) : reinterpret_cast<const void*>(&tconv_kernel<128, false>);
-  else if (bn == 64) fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<64, true>) : reinterpret_cast<const void*>(&tconv_kernel<64, false>);
-  else fn = y_prev ? reinterpret_cast<const void*>(&tconv_kernel<32, true>) : reinterpret_cast<const void*>(&tconv_kernel<32, false>);
+  // tconv_kernel<BN, SILU_BWD, PRED> by [BN = 32, 64, 128][plain, SiLU' epilogue, PRED]
+  const void* const fns[3][3] = {
+      {reinterpret_cast<const void*>(&tconv_kernel<32, false>), reinterpret_cast<const void*>(&tconv_kernel<32, true>), reinterpret_cast<const void*>(&tconv_kernel<32, false, true>)},
+      {reinterpret_cast<const void*>(&tconv_kernel<64, false>), reinterpret_cast<const void*>(&tconv_kernel<64, true>), reinterpret_cast<const void*>(&tconv_kernel<64, false, true>)},
+      {reinterpret_cast<const void*>(&tconv_kernel<128, false>), reinterpret_cast<const void*>(&tconv_kernel<128, true>), reinterpret_cast<const void*>(&tconv_kernel<128, false, true>)}};
+  const void* fn = fns[bn / 64][a.out_f32 ? 2 : (y_prev ? 1 : 0)];
   const int k_iters = a.taps * (kpad64(a.cin) / 64);
   a.stages = k_iters < kTStagesFwd ? k_iters : kTStagesFwd;
   const int smem = a.stages * (128 * 128 + bn * 128) + 256 + 2 * bn * 4;
@@ -938,66 +973,42 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
   return CVB_OK;
 }
 
-// Stride-1 geometry with padding `pad`: the output is (H + 2 pad - k + 1) x (W + 2 pad - k + 1) and tap t reads input pixel
-// (h + t / k - pad, w + t % k - pad).  TMA zero-fills the pixels outside the map (pad > 0); a negative pad crops the border instead.
-static int conv_s1_setup(TConvArgs& a, const void* x, int B, int H, int W, int cin, int cout, int k, int pad) {
-  memset(&a, 0, sizeof(a));
-  const int Ho = H + 2 * pad - k + 1, Wo = W + 2 * pad - k + 1;
-  a.H = Ho;
-  a.W = Wo;
-  a.B = B;
-  a.cin = cin;
-  a.cout = cout;
-  a.taps = k * k;
-  a.out_H = Ho;
-  a.out_W = Wo;
-  a.os = 1;
-  choose_box128(B, Ho, Wo, &a.TW, &a.TH, &a.NB);
-  for (int t = 0; t < k * k; ++t) {
-    a.tap_dh[t] = (int8_t)(t / k - pad);
-    a.tap_dw[t] = (int8_t)(t % k - pad);
-    a.tap_map[t] = 0;
-    a.tap_wblk[t] = (int8_t)t;
-  }
-  return act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
-}
-
 // paddings of the stride-1 training convolutions: k // 2 (BaseConv), 1 on a 1x1 conv (the YOLOX head stems, heads/yolox_head.py:35) and
 // k - 1 - 1 = -1, the backward-data of that stem
 static bool train_pad_ok(int k, int pad) { return k == 1 ? (pad >= -1 && pad <= 1) : (k == 3 && pad == 1); }
 
+// Shape rules of a training convolution (forward / backward-data and backward-weight alike).  aligned: the OR of the addresses that must
+// be 16-byte aligned.  A stride-1 output is (H + 2 pad - k + 1) x (W + 2 pad - k + 1): TMA zero-fills the pixels outside the input
+// (pad > 0), a negative pad crops its border instead.
+static int check_conv_shape(const char* fn, int B, int H, int W, int cin, int cout, int k, int stride, int pad, uintptr_t aligned) {
+  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout),
+              "%s: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", fn, cin, cout, k);
+  CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "%s: stride 1, or stride 2 with k = 3", fn);
+  CVB_REQUIRE(train_pad_ok(k, pad), "%s: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", fn, k, pad);
+  CVB_REQUIRE(B > 0 && H > 0 && W > 0 && H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "%s: empty output (B=%d H=%d W=%d k=%d pad=%d)", fn, B, H, W,
+              k, pad);
+  CVB_REQUIRE((aligned & 15) == 0, "%s: pointers must be 16-byte aligned", fn);
+  return CVB_OK;
+}
+
 static int train_conv(const void* x, int B, int H, int W, int cin, const void* w_packed, int cout, int k, int stride, int pad, void* out, const void* y_prev,
                       const float* bn_stat_prev, void* stream) {
   CVB_REQUIRE(x && w_packed && out, "train_conv: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout) && B > 0 && H > 0 && W > 0,
-              "train_conv: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", cin, cout, k);
-  CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv: stride 1, or stride 2 with k = 3");
-  CVB_REQUIRE(train_pad_ok(k, pad), "train_conv: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", k, pad);
-  CVB_REQUIRE(H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "train_conv: empty output (H=%d W=%d k=%d pad=%d)", H, W, k, pad);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, "train_conv: pointers must be 16-byte aligned");
+  int rc = check_conv_shape("train_conv", B, H, W, cin, cout, k, stride, pad,
+                            reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out));
+  if (rc != CVB_OK) return rc;
   CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv: the SiLU' epilogue needs both y_prev and its BN statistics");
   TConvArgs a;
-  int rc = CVB_OK;
+  const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
+  tconv_geometry(a, B, Ho, Wo, cin, cout, out, Ho, Wo, 1, 0, 0);
   if (stride == 1) {
-    rc = conv_s1_setup(a, x, B, H, W, cin, cout, k, pad);
+    a.taps = s1_taps(k, pad, a.tap_dh, a.tap_dw, a.tap_map, a.tap_wblk);
+    rc = act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
   } else {
-    memset(&a, 0, sizeof(a));
-    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-    a.H = Ho;
-    a.W = Wo;
-    a.B = B;
-    a.cin = cin;
-    a.cout = cout;
-    a.out_H = Ho;
-    a.out_W = Wo;
-    a.os = 1;
-    choose_box128(B, Ho, Wo, &a.TW, &a.TH, &a.NB);
     a.taps = s2_taps(H, W, a.tap_dh, a.tap_dw, a.tap_map, a.tap_wblk);
-    for (int py = 0; py < 2 && rc == CVB_OK; ++py)
-      for (int px = 0; px < 2 && rc == CVB_OK; ++px) rc = act_map_strided(&a.tmA[py * 2 + px], x, B, H, W, cin, 2, py, px, a.TW, a.TH, a.NB);
+    rc = parity_maps(a.tmA, x, B, H, W, cin, a.TW, a.TH, a.NB);
   }
   if (rc != CVB_OK) return rc;
-  a.out = static_cast<__nv_bfloat16*>(out);
   return launch_tconv(a, w_packed, k * k, y_prev, bn_stat_prev, stream);
 }
 
@@ -1024,7 +1035,9 @@ extern "C" int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t 
                   (reinterpret_cast<uintptr_t>(bias) & 3) == 0,
               "train_pred_conv: x / w_packed must be 16-byte, out / bias 4-byte aligned");
   TConvArgs a;
-  const int rc = conv_s1_setup(a, x, B, H, W, cin, cout_pad, 1, 0);
+  tconv_geometry(a, B, H, W, cin, cout_pad, nullptr, H, W, 1, 0, 0);
+  a.taps = s1_taps(1, 0, a.tap_dh, a.tap_dw, a.tap_map, a.tap_wblk);
+  const int rc = act_map(&a.tmA[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
   if (rc != CVB_OK) return rc;
   a.out_f32 = out;
   a.bias = bias;
@@ -1048,18 +1061,7 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
       const int Hs = (H - pi + 1) / 2, Ws = (W - pj + 1) / 2;  // pixels of this parity class
       if (Hs <= 0 || Ws <= 0) continue;
       TConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.H = Hs;
-      a.W = Ws;
-      a.B = B;
-      a.cin = cout;  // the GEMM's K: dy channels
-      a.cout = cin;  // the GEMM's N: dx channels
-      a.out = static_cast<__nv_bfloat16*>(dx);
-      a.out_H = H;
-      a.out_W = W;
-      a.os = 2;
-      a.ooh = pi;
-      a.oow = pj;
+      tconv_geometry(a, B, Hs, Ws, cout, cin, dx, H, W, 2, pi, pj);  // the GEMM's K: dy channels, its N: dx channels
       int nt = 0;
       for (int ky = 0; ky < 3; ++ky) {
         if (((ky + 1) & 1) != pi) continue;  // rows of parity pi are reached by ky with 2*oh + ky - 1 = ih
@@ -1073,7 +1075,6 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
         }
       }
       a.taps = nt;
-      choose_box128(B, Hs, Ws, &a.TW, &a.TH, &a.NB);
       int rc = act_map(&a.tmA[0], dy, B, Ho, Wo, cout, a.TW, a.TH, a.NB);
       if (rc != CVB_OK) return rc;
       rc = launch_tconv(a, w_bwd, 9, y_prev, bn_stat_prev, stream);
@@ -1084,12 +1085,8 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
 
 static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int cin, int cout, int k, int stride, int pad, float* dw, void* stream) {
   CVB_REQUIRE(x && dy && dw, "train_conv_wgrad: null tensor");
-  CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout),
-              "train_conv_wgrad: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d)", cin, cout);
-  CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "train_conv_wgrad: stride 1, or stride 2 with k = 3");
-  CVB_REQUIRE(train_pad_ok(k, pad), "train_conv_wgrad: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", k, pad);
-  CVB_REQUIRE(B > 0 && H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "train_conv_wgrad: empty output (H=%d W=%d k=%d pad=%d)", H, W, k, pad);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy)) & 15) == 0, "train_conv_wgrad: pointers must be 16-byte aligned");
+  int rc = check_conv_shape("train_conv_wgrad", B, H, W, cin, cout, k, stride, pad, reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy));
+  if (rc != CVB_OK) return rc;
   TWgradArgs a;
   memset(&a, 0, sizeof(a));
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
@@ -1112,25 +1109,20 @@ static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, 
   if (splits < 1) splits = 1;
   if (splits > m_tiles) splits = m_tiles;
   a.splits = splits;
-  int rc = CVB_OK, ntaps = k * k;
+  int ntaps;
   if (stride == 1) {
-    for (int t = 0; t < k * k; ++t) {
-      a.tap_dh[t] = (int8_t)(t / k - pad);
-      a.tap_dw[t] = (int8_t)(t % k - pad);
-      a.tap_map[t] = 0;
-      a.tap_idx[t] = (int8_t)t;
-    }
+    ntaps = s1_taps(k, pad, a.tap_dh, a.tap_dw, a.tap_map, a.tap_idx);
     rc = act_map(&a.tmX[0], x, B, H, W, cin, a.TW, a.TH, a.NB);
   } else {
     ntaps = s2_taps(H, W, a.tap_dh, a.tap_dw, a.tap_map, a.tap_idx);  // the taps left out keep dw = 0
-    for (int py = 0; py < 2 && rc == CVB_OK; ++py)
-      for (int px = 0; px < 2 && rc == CVB_OK; ++px) rc = act_map_strided(&a.tmX[py * 2 + px], x, B, H, W, cin, 2, py, px, a.TW, a.TH, a.NB);
+    rc = parity_maps(a.tmX, x, B, H, W, cin, a.TW, a.TH, a.NB);
   }
   if (rc == CVB_OK) rc = act_map(&a.tmD, dy, B, Ho, Wo, cout, a.TW, a.TH, a.NB);
   if (rc != CVB_OK) return rc;
-  const void* fn = narrow ? reinterpret_cast<const void*>(&twgrad_kernel<1, true>)
-                          : (npan == 1 ? reinterpret_cast<const void*>(&twgrad_kernel<1>)
-                                       : (npan == 2 ? reinterpret_cast<const void*>(&twgrad_kernel<2>) : reinterpret_cast<const void*>(&twgrad_kernel<4>)));
+  // twgrad_kernel<NPAN> for NPAN = 1, 2, 4 (index npan / 2); twgrad_kernel<1, true> for cout = 16 or 32
+  const void* const fns[3] = {reinterpret_cast<const void*>(&twgrad_kernel<1>), reinterpret_cast<const void*>(&twgrad_kernel<2>),
+                              reinterpret_cast<const void*>(&twgrad_kernel<4>)};
+  const void* fn = narrow ? reinterpret_cast<const void*>(&twgrad_kernel<1, true>) : fns[npan / 2];
   const int stages = npan == 4 ? 2 : kTStagesWg;
   const int smem = stages * ((2 + npan) * 128 * 128) + 256;
   CVB_REQUIRE(smem <= 232448, "train_conv_wgrad: cout=%d needs %d bytes of shared memory", cout, smem);

@@ -102,29 +102,82 @@ def conv_wgrad(x, dy, k, stride=1, pad=None):
     return dw.view(cout, k, k, cin).permute(0, 3, 1, 2)
 
 
+def _to_nhwc(x, what):
+    """A drop-in's NCHW input -> the NHWC bf16 layout of the training layers (CUDA only)."""
+    _check_cuda(x, what)
+    return x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)
+
+
+def _to_nchw(x, dtype):
+    """An NHWC bf16 layer output -> the reference's NCHW layout in `dtype` (a permuted view, converted only when dtype is not bf16)."""
+    return x.permute(0, 3, 1, 2).to(dtype)
+
+
+def _require_training(m, message):
+    """The drop-ins use batch statistics only: eval() goes through the inference modules."""
+    if not m.training:
+        raise RuntimeError(message)
+
+
+def _require_widths(widths, message):
+    """NotImplementedError(message(bad widths)) unless every channel count is 16, 32 or a multiple of 64."""
+    bad = sorted({c for c in widths if not channels_ok(c)})
+    if bad:
+        raise NotImplementedError(message(bad))
+
+
+def _bn_momentum(bn):
+    """Counts the step and returns the running-statistics momentum nn.BatchNorm2d would use (momentum None: cumulative average)."""
+    bn.num_batches_tracked += 1
+    return bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
+
+
+def _set_bn(m):
+    """Every BatchNorm of `m` gets the reference YOLOX's eps 1e-3 and momentum 0.03."""
+    for mod in m.modules():
+        if isinstance(mod, nn.BatchNorm2d):
+            mod.eps, mod.momentum = 1e-3, 0.03
+
+
+def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1, pad=None):
+    """a = silu(bn_train(conv(x, weight))) -> (a, (y, stat, g32, wb)): what _bn_silu_backward and the backward convolutions need (the conv
+    output, the BN statistics, fp32 gamma and the backward-data weights).  Updates the running statistics."""
+    cout = weight.shape[0]
+    L = _lib.lib()
+    wf, wb = pack_weights(weight)
+    y = conv(x, wf, cout, k, stride=stride, pad=pad)
+    npix = y.shape[0] * y.shape[1] * y.shape[2]
+    stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
+    scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
+    g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
+    _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                    _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
+    a = torch.empty_like(y)
+    _lib.check(L.cvb_train_bn_silu_fwd(_p(y), npix, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_silu_fwd')
+    return a, (y, stat, g32, wb)
+
+
+def _bn_silu_backward(g, g_is_dz, y, stat, g32):
+    """g = d(loss)/d(a), or d(loss)/d(z) with z the BN output when g_is_dz (a SiLU' epilogue already applied) -> (dy = d(loss)/d(y),
+    dgamma, dbeta)."""
+    g = g.contiguous()
+    cout = y.shape[3]
+    sums = torch.empty((2, cout), dtype=torch.float32, device=y.device)
+    dy = torch.empty_like(y)
+    _lib.check(_lib.lib().cvb_train_bn_silu_bwd(_p(g), int(g_is_dz), _p(y), y.shape[0] * y.shape[1] * y.shape[2], cout, _p(stat), _p(g32), _p(sums), _p(dy),
+                                                _stream()), 'cvb_train_bn_silu_bwd')
+    return dy, sums[1].clone(), sums[0].clone()
+
+
 class _ConvBnSiLU(torch.autograd.Function):
     """a = silu(bn_train(conv(x, W))) with the backward the reference obtains from torch.autograd, on the H100 kernels."""
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1, pad=None):
         _check_cuda(x, 'BaseConv (H100 training)')
-        B, H, W, cin = x.shape
-        cout = weight.shape[0]
-        L = _lib.lib()
-        wf, wb = pack_weights(weight)
-        y = conv(x, wf, cout, k, stride=stride, pad=pad)
-        npix = B * y.shape[1] * y.shape[2]
-        stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
-        scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
-        g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-        _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
-                                        _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
-        a = torch.empty_like(y)
-        _lib.check(L.cvb_train_bn_silu_fwd(_p(y), npix, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_silu_fwd')
-        ctx.save_for_backward(x, y, stat, g32, wb)
-        ctx.k = k
-        ctx.stride = stride
-        ctx.pad = pad
+        a, saved = _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride, pad)
+        ctx.save_for_backward(x, *saved)
+        ctx.k, ctx.stride, ctx.pad = k, stride, pad
         ctx.need_dx = x.requires_grad
         return a
 
@@ -133,13 +186,7 @@ class _ConvBnSiLU(torch.autograd.Function):
         x, y, stat, g32, wb = ctx.saved_tensors
         k = ctx.k
         B, H, W, cin = x.shape
-        cout = y.shape[3]
-        L = _lib.lib()
-        da = da.contiguous()
-        sums = torch.empty((2, cout), dtype=torch.float32, device=x.device)
-        dy = torch.empty_like(y)
-        _lib.check(L.cvb_train_bn_silu_bwd(_p(da), 0, _p(y), B * y.shape[1] * y.shape[2], cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()),
-                   'cvb_train_bn_silu_bwd')
+        dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32)
         dw = conv_wgrad(x, dy, k, ctx.stride, ctx.pad)
         dx = None
         if ctx.need_dx:
@@ -147,7 +194,7 @@ class _ConvBnSiLU(torch.autograd.Function):
                 dx = conv_dgrad_s2(dy, wb, cin, H, W)
             else:  # backward-data of a padding-p conv: the same conv over dy with the rotated weights and padding k - 1 - p
                 dx = conv(dy, wb, cin, k, pad=None if ctx.pad is None else k - 1 - ctx.pad)
-        return dx, dw, sums[1].clone(), sums[0].clone(), None, None, None, None, None, None, None
+        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None
 
 
 class _BottleneckChain(torch.autograd.Function):
@@ -155,80 +202,66 @@ class _BottleneckChain(torch.autograd.Function):
     the 1x1 layer's SiLU' in its epilogue (dz_t leaves the tensor core already multiplied; d(loss)/dt is never written)."""
 
     @staticmethod
-    def forward(ctx, x, w1, g1, b1, rm1, rv1, w2, g2, b2, rm2, rv2, eps, momentum):
+    def forward(ctx, x, w1, g1, b1, rm1, rv1, eps1, mom1, w2, g2, b2, rm2, rv2, eps2, mom2):
         _check_cuda(x, 'Bottleneck (H100 training)')
-        B, H, W, cin = x.shape
-        L = _lib.lib()
-        npix = B * H * W
-
-        def layer(inp, w, g, b, rm, rv, k):
-            cout = w.shape[0]
-            wf, wb = pack_weights(w)
-            y = conv(inp, wf, cout, k)
-            stat = torch.empty((4, cout), dtype=torch.float32, device=inp.device)
-            scratch = torch.empty((2, cout), dtype=torch.float32, device=inp.device)
-            g32, b32 = g.detach().float().contiguous(), b.detach().float().contiguous()
-            _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(rm), _p(rv), _p(scratch), _p(stat), _stream()),
-                       'cvb_train_bn_stats')
-            a = torch.empty_like(y)
-            _lib.check(L.cvb_train_bn_silu_fwd(_p(y), npix, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_silu_fwd')
-            return y, stat, g32, wb, a
-
-        y1, st1, g1f, wb1, t = layer(x, w1, g1, b1, rm1, rv1, 1)
-        y2, st2, g2f, wb2, u = layer(t, w2, g2, b2, rm2, rv2, 3)
-        ctx.save_for_backward(x, y1, st1, g1f, wb1, t, y2, st2, g2f, wb2)
+        t, saved1 = _conv_bn_silu(x, w1, g1, b1, rm1, rv1, eps1, mom1, 1)
+        u, saved2 = _conv_bn_silu(t, w2, g2, b2, rm2, rv2, eps2, mom2, 3)
+        ctx.save_for_backward(x, t, *saved1, *saved2)
         ctx.need_dx = x.requires_grad
         return u
 
     @staticmethod
     def backward(ctx, du):
-        x, y1, st1, g1f, wb1, t, y2, st2, g2f, wb2 = ctx.saved_tensors
-        B, H, W, cin = x.shape
-        c1, c2 = y1.shape[3], y2.shape[3]
-        npix = B * H * W
-        L = _lib.lib()
-        du = du.contiguous()
-        sums2 = torch.empty((2, c2), dtype=torch.float32, device=x.device)
-        dy2 = torch.empty_like(y2)
-        _lib.check(L.cvb_train_bn_silu_bwd(_p(du), 0, _p(y2), npix, c2, _p(st2), _p(g2f), _p(sums2), _p(dy2), _stream()), 'cvb_train_bn_silu_bwd')
+        x, t, y1, st1, g1f, wb1, y2, st2, g2f, wb2 = ctx.saved_tensors
+        dy2, dg2, db2 = _bn_silu_backward(du, False, y2, st2, g2f)
         dw2 = conv_wgrad(t, dy2, 3)
-        dz1 = conv(dy2, wb2, c1, 3, y_prev=y1, stat_prev=st1)  # backward-data of the 3x3 with the 1x1 layer's SiLU' in the epilogue
-        sums1 = torch.empty((2, c1), dtype=torch.float32, device=x.device)
-        dy1 = torch.empty_like(y1)
-        _lib.check(L.cvb_train_bn_silu_bwd(_p(dz1), 1, _p(y1), npix, c1, _p(st1), _p(g1f), _p(sums1), _p(dy1), _stream()), 'cvb_train_bn_silu_bwd')
+        dz1 = conv(dy2, wb2, y1.shape[3], 3, y_prev=y1, stat_prev=st1)  # backward-data of the 3x3 with the 1x1 layer's SiLU' in the epilogue
+        dy1, dg1, db1 = _bn_silu_backward(dz1, True, y1, st1, g1f)
         dw1 = conv_wgrad(x, dy1, 1)
-        dx = conv(dy1, wb1, cin, 1) if ctx.need_dx else None
-        return (dx, dw1, sums1[1].clone(), sums1[0].clone(), None, None, dw2, sums2[1].clone(), sums2[0].clone(), None, None, None, None)
+        dx = conv(dy1, wb1, x.shape[3], 1) if ctx.need_dx else None
+        return dx, dw1, dg1, db1, None, None, None, None, dw2, dg2, db2, None, None, None, None
 
 
-class BaseConv(nn.Module):
-    """src/models/modules/yolox_modules.py:35-55 (act='silu', groups=1; stride 1, or stride 2 with ksize 3 = the downsampling conv in front of
-    every CSPLayer of the YOLOX backbone).  forward: NHWC bf16 in -> NHWC bf16 out."""
+class _ConvBnSiLULayer(nn.Module):
+    """conv (no bias) -> BatchNorm (batch statistics) -> SiLU as one _ConvBnSiLU, with the reference's conv / bn / act children.
+    forward: NHWC bf16 in -> NHWC bf16 out.  `padding` None: k // 2 through cvb_train_conv (stride 1 or 2); otherwise cvb_train_conv_pad."""
+    drop_in = None  # the public module named in the eval() refusal
 
-    def __init__(self, in_channels, out_channels, ksize, stride, groups=1, bias=False, act='silu'):
+    def __init__(self, in_channels, out_channels, ksize, stride=1, padding=None):
         super().__init__()
-        if not (stride == 1 or (stride == 2 and ksize == 3)) or groups != 1 or bias or act != 'silu' or ksize not in (1, 3):
-            raise NotImplementedError('H100 training BaseConv: ksize in {1,3}, stride 1 (or 2 with ksize 3), groups 1, no bias, SiLU')
-        if not (channels_ok(in_channels) and channels_ok(out_channels)):
-            raise NotImplementedError(f'H100 training BaseConv: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
-        self.conv = nn.Conv2d(in_channels, out_channels, kernel_size=ksize, stride=stride, padding=(ksize - 1) // 2, groups=groups, bias=bias)
+        self.conv = nn.Conv2d(in_channels, out_channels, ksize, stride, ksize // 2 if padding is None else padding, bias=False)
         self.bn = nn.BatchNorm2d(out_channels)
         self.act = nn.SiLU(inplace=True)  # (parameter-free; kept for module-tree parity with the reference)
-        self.ksize = ksize
-        self.stride = stride
+        self.ksize, self.stride, self.padding = ksize, stride, padding
+
+    def _bn_inputs(self):
+        """Counts the step -> the _ConvBnSiLU / _BottleneckChain arguments of this layer's BatchNorm."""
+        bn = self.bn
+        return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, _bn_momentum(bn)
 
     def forward(self, x):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.BaseConv is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
-        bn = self.bn
-        bn.num_batches_tracked += 1
-        mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-        return _ConvBnSiLU.apply(x, self.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, mom, self.ksize, self.stride)
+        return self._layer(x, self.conv.weight)
+
+    def _layer(self, x, weight):
+        _require_training(self, f'cvpytorch_b200.train.{self.drop_in} is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
+        return _ConvBnSiLU.apply(x, weight, *self._bn_inputs(), self.ksize, self.stride, self.padding)
+
+
+class BaseConv(_ConvBnSiLULayer):
+    """src/models/modules/yolox_modules.py:35-55 (act='silu', groups=1; stride 1, or stride 2 with ksize 3 = the downsampling conv in front of
+    every CSPLayer of the YOLOX backbone).  forward: NHWC bf16 in -> NHWC bf16 out."""
+    drop_in = 'BaseConv'
+
+    def __init__(self, in_channels, out_channels, ksize, stride, groups=1, bias=False, act='silu'):
+        if not (stride == 1 or (stride == 2 and ksize == 3)) or groups != 1 or bias or act != 'silu' or ksize not in (1, 3):
+            raise NotImplementedError('H100 training BaseConv: ksize in {1,3}, stride 1 (or 2 with ksize 3), groups 1, no bias, SiLU')
+        _require_widths((in_channels, out_channels),
+                        lambda bad: f'H100 training BaseConv: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
+        super().__init__(in_channels, out_channels, ksize, stride)
 
     def forward_nchw(self, x):
         """Reference interface (NCHW in / out) for a stand-alone BaseConv, e.g. the stride-2 conv of a `dark` stage."""
-        _check_cuda(x, 'BaseConv (H100 training)')
-        return self.forward(x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)).permute(0, 3, 1, 2).to(x.dtype)
+        return _to_nchw(self.forward(_to_nhwc(x, 'BaseConv (H100 training)')), x.dtype)
 
 
 class Bottleneck(nn.Module):
@@ -244,14 +277,9 @@ class Bottleneck(nn.Module):
         self.use_add = shortcut and in_channels == out_channels
 
     def forward(self, x):
-        if not self.training:
-            raise RuntimeError('training drop-in: call .train()')
+        _require_training(self, 'training drop-in: call .train()')
         c1, c2 = self.conv1, self.conv2
-        for bn in (c1.bn, c2.bn):
-            bn.num_batches_tracked += 1
-        mom = c1.bn.momentum if c1.bn.momentum is not None else 1.0 / float(c1.bn.num_batches_tracked)
-        y = _BottleneckChain.apply(x, c1.conv.weight, c1.bn.weight, c1.bn.bias, c1.bn.running_mean, c1.bn.running_var,
-                                   c2.conv.weight, c2.bn.weight, c2.bn.bias, c2.bn.running_mean, c2.bn.running_var, c1.bn.eps, mom)
+        y = _BottleneckChain.apply(x, c1.conv.weight, *c1._bn_inputs(), c2.conv.weight, *c2._bn_inputs())
         if self.use_add:
             y = y + x
         return y
@@ -275,9 +303,7 @@ class CSPLayer(nn.Module):
         return self.conv3(torch.cat((x_1, x_2), dim=3))
 
     def forward(self, x):
-        _check_cuda(x, 'CSPLayer (H100 training)')
-        xh = x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)
-        return self.forward_nhwc(xh).permute(0, 3, 1, 2).to(x.dtype)
+        return _to_nchw(self.forward_nhwc(_to_nhwc(x, 'CSPLayer (H100 training)')), x.dtype)
 
 
 # ------------------------------------------------------------------------------------------------ whole backbone: Focus stem, SPPF, CSPDarknet
@@ -325,28 +351,16 @@ class _SppPool(torch.autograd.Function):
         return spp_pool_backward(g.contiguous(), idx)
 
 
-def _bn_momentum(bn):
-    bn.num_batches_tracked += 1
-    return bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-
-
-class _StemConv(nn.Module):
+class _StemConv(_ConvBnSiLULayer):
     """The Focus stem's ConvModule (keys conv.weight [cout,12,3,3], bn.*): on the kernels a 16 -> cout BaseConv over cvb_train_focus_s2d's
     output, with the weight zero-padded to 16 input channels (its gradient is the first 12).  Computes no input gradient."""
+    drop_in = 'Focus'
 
     def __init__(self, in_channels, out_channels):
-        super().__init__()
-        self.conv = nn.Conv2d(in_channels, out_channels, kernel_size=3, stride=1, padding=1, bias=False)
-        self.bn = nn.BatchNorm2d(out_channels)
-        self.act = nn.SiLU(inplace=True)  # (parameter-free; module-tree parity)
+        super().__init__(in_channels, out_channels, 3)
 
     def forward(self, s2d):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.Focus is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
-        bn = self.bn
-        mom = _bn_momentum(bn)
-        w16 = nn.functional.pad(self.conv.weight, (0, 0, 0, 0, 0, s2d.shape[3] - self.conv.weight.shape[1]))
-        return _ConvBnSiLU.apply(s2d, w16, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, mom, 3, 1)
+        return self._layer(s2d, nn.functional.pad(self.conv.weight, (0, 0, 0, 0, 0, s2d.shape[3] - self.conv.weight.shape[1])))
 
 
 class Focus(nn.Module):
@@ -357,8 +371,7 @@ class Focus(nn.Module):
         super().__init__()
         if in_channels != 3 or kernel_sizes != 3 or stride != 1:
             raise NotImplementedError('H100 training Focus: the 3-channel image, 3x3 conv, stride 1 (the YOLOX stem)')
-        if not channels_ok(out_channels):
-            raise NotImplementedError(f'H100 training Focus: out_channels must be 16, 32 or a multiple of 64 (got {out_channels})')
+        _require_widths((out_channels,), lambda bad: f'H100 training Focus: out_channels must be 16, 32 or a multiple of 64 (got {out_channels})')
         self.conv = _StemConv(in_channels * 4, out_channels)
 
     def forward_nhwc(self, x):
@@ -367,7 +380,7 @@ class Focus(nn.Module):
         return self.conv(focus_s2d(x))
 
     def forward(self, x):
-        return self.forward_nhwc(x).permute(0, 3, 1, 2).to(x.dtype)
+        return _to_nchw(self.forward_nhwc(x), x.dtype)
 
 
 class SPPF(nn.Module):
@@ -389,8 +402,7 @@ class SPPF(nn.Module):
         return self.conv2(_SppPool.apply(self.conv1(x)))
 
     def forward(self, x):
-        _check_cuda(x, 'SPPF (H100 training)')
-        return self.forward_nhwc(x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)).permute(0, 3, 1, 2).to(x.dtype)
+        return _to_nchw(self.forward_nhwc(_to_nhwc(x, 'SPPF (H100 training)')), x.dtype)
 
 
 def _nhwc(m, x):
@@ -424,23 +436,19 @@ class CSPDarknet(nn.Module):
         ch = list(map(lambda x: int(x * width_mul), out_channels))
         nl = list(map(lambda x: max(round(x * depth_mul), 1), layers))
         self.layers = nl
-        bad = sorted({c for c in ch + [c // 2 for c in ch[1:]] if not channels_ok(c)})
-        if bad:
-            raise NotImplementedError(f'H100 training CSPDarknet {subtype}: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        _require_widths(ch + [c // 2 for c in ch[1:]],
+                        lambda bad: f'H100 training CSPDarknet {subtype}: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
         self.stem = Focus(3, ch[0], kernel_sizes=3)
         self.stage1 = nn.Sequential(BaseConv(ch[0], ch[1], 3, 2), CSPLayer(ch[1], ch[1], n=nl[0], shortcut=True))
         self.stage2 = nn.Sequential(BaseConv(ch[1], ch[2], 3, 2), CSPLayer(ch[2], ch[2], n=nl[1], shortcut=True))
         self.stage3 = nn.Sequential(BaseConv(ch[2], ch[3], 3, 2), CSPLayer(ch[3], ch[3], n=nl[2], shortcut=True))
         self.stage4 = nn.Sequential(BaseConv(ch[3], ch[4], 3, 2), SPPF(ch[4], ch[4], kernel_sizes=spp_ksizes), CSPLayer(ch[4], ch[4], n=nl[3], shortcut=False))
         self.out_channels = ch[out_stages[0]:out_stages[-1] + 1]
-        for m in self.modules():
-            if isinstance(m, nn.BatchNorm2d):
-                m.eps, m.momentum = 1e-3, 0.03
+        _set_bn(self)
 
     def forward_nhwc(self, x):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.CSPDarknet is the TRAINING drop-in (batch statistics); load its state_dict into '
-                               'cvpytorch_b200.yolox_models.CSPDarknet for eval()')
+        _require_training(self, 'cvpytorch_b200.train.CSPDarknet is the TRAINING drop-in (batch statistics); load its state_dict into '
+                                'cvpytorch_b200.yolox_models.CSPDarknet for eval()')
         _check_cuda(x, 'CSPDarknet (H100 training)')
         h = self.stem.forward_nhwc(x)
         outs = []
@@ -452,7 +460,7 @@ class CSPDarknet(nn.Module):
         return outs
 
     def forward(self, x):
-        outs = [o.permute(0, 3, 1, 2).to(x.dtype) for o in self.forward_nhwc(x)]
+        outs = [_to_nchw(o, x.dtype) for o in self.forward_nhwc(x)]
         return outs if len(self.out_stages) > 1 else outs[0]
 
 
@@ -545,39 +553,17 @@ class _HeadPred(torch.autograd.Function):
         return dx_ro, dx_cls, dw_ro, db_ro, dw_cls, db_cls
 
 
-class ConvModule(nn.Module):
+class ConvModule(_ConvBnSiLULayer):
     """src/models/modules/convs.py ConvModule as heads/yolox_head.py:33-49 builds it: conv (no bias) -> BatchNorm -> SiLU, training mode.
     kernel_size 1 or 3, stride 1, padding kernel_size // 2 or 1 (the head stems are 1x1 convs with padding 1).  forward: NHWC bf16 in / out."""
+    drop_in = 'ConvModule'
 
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, activation='SiLU'):
-        super().__init__()
         if kernel_size not in (1, 3) or stride != 1 or padding not in (kernel_size // 2, 1) or activation != 'SiLU':
             raise NotImplementedError('H100 training ConvModule: kernel_size 1 or 3, stride 1, padding kernel_size // 2 or 1, SiLU')
-        if not (channels_ok(in_channels) and channels_ok(out_channels)):
-            raise NotImplementedError(f'H100 training ConvModule: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
-        self.conv = nn.Conv2d(in_channels, out_channels, kernel_size, stride, padding, bias=False)
-        self.bn = nn.BatchNorm2d(out_channels)
-        self.act = nn.SiLU(inplace=True)  # (parameter-free; module-tree parity)
-        self.ksize, self.padding = kernel_size, padding
-
-    def forward(self, x):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.ConvModule is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
-        bn = self.bn
-        mom = _bn_momentum(bn)
-        return _ConvBnSiLU.apply(x, self.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, mom, self.ksize, 1, self.padding)
-
-
-def _set_bn(m):
-    for mod in m.modules():
-        if isinstance(mod, nn.BatchNorm2d):
-            mod.eps, mod.momentum = 1e-3, 0.03
-
-
-def _to_nhwc(xs):
-    for x in xs:
-        _check_cuda(x, 'YOLOX neck / head (H100 training)')
-    return [x.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16) for x in xs]
+        _require_widths((in_channels, out_channels),
+                        lambda bad: f'H100 training ConvModule: channel counts must be 16, 32 or multiples of 64 (got {in_channels} -> {out_channels})')
+        super().__init__(in_channels, out_channels, kernel_size, stride, padding)
 
 
 class YOLOXNeck(nn.Module):
@@ -592,9 +578,8 @@ class YOLOXNeck(nn.Module):
         self.subtype, self.channels, self.num_ins = subtype, channels, len(channels)
         c = list(map(lambda x: max(round(x * width_mul), 1), channels))
         n = list(map(lambda x: max(round(x * depth_mul), 1), [3, 3, 3, 3]))
-        bad = sorted({v for v in c + [int(v * 0.5) for v in c] if not channels_ok(v)})
-        if bad:
-            raise NotImplementedError(f'H100 training YOLOXNeck: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        _require_widths(c + [int(v * 0.5) for v in c],
+                        lambda bad: f'H100 training YOLOXNeck: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
         self.upsample = nn.Upsample(scale_factor=2, mode='nearest')  # (parameter-free; module-tree parity)
         self.lateral_conv0 = BaseConv(c[2], c[1], 1, 1)
         self.C3_p4 = CSPLayer(2 * c[1], c[1], n[0], False)
@@ -607,9 +592,8 @@ class YOLOXNeck(nn.Module):
         _set_bn(self)
 
     def forward_nhwc(self, x):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.YOLOXNeck is the TRAINING drop-in (batch statistics); load its state_dict into '
-                               'cvpytorch_b200.yolox_models.YOLOXNeck for eval()')
+        _require_training(self, 'cvpytorch_b200.train.YOLOXNeck is the TRAINING drop-in (batch statistics); load its state_dict into '
+                                'cvpytorch_b200.yolox_models.YOLOXNeck for eval()')
         if len(x) != self.num_ins:
             raise ValueError(f'YOLOXNeck: {self.num_ins} feature maps expected, got {len(x)}')
         x2, x1, x0 = x
@@ -625,7 +609,7 @@ class YOLOXNeck(nn.Module):
         return [pan_out2, pan_out1, pan_out0]
 
     def forward(self, x):
-        return [o.permute(0, 3, 1, 2).to(x[0].dtype) for o in self.forward_nhwc(_to_nhwc(x))]
+        return [_to_nchw(o, x[0].dtype) for o in self.forward_nhwc([_to_nhwc(t, 'YOLOX neck / head (H100 training)') for t in x])]
 
 
 class YOLOXHead(nn.Module):
@@ -640,9 +624,8 @@ class YOLOXHead(nn.Module):
         self.num_classes, self.subtype, self.strides, self.n_anchors = num_classes, subtype, strides, 1
         ic = list(map(lambda x: max(round(x * width_mul), 1), in_channels))
         p = int(256 * width_mul)
-        bad = sorted({v for v in ic + [p] if not channels_ok(v)})
-        if bad:
-            raise NotImplementedError(f'H100 training YOLOXHead: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
+        _require_widths(ic + [p],
+                        lambda bad: f'H100 training YOLOXHead: widths {bad} are not on the training path (channels must be 16, 32 or multiples of 64)')
         self.stems, self.cls_convs, self.reg_convs = nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
         self.cls_preds, self.reg_preds, self.obj_preds = nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
         for c in ic:
@@ -659,9 +642,8 @@ class YOLOXHead(nn.Module):
                 conv.bias.fill_(prior)
 
     def forward_nhwc(self, x):
-        if not self.training:
-            raise RuntimeError('cvpytorch_b200.train.YOLOXHead is the TRAINING drop-in (batch statistics); load its state_dict into '
-                               'cvpytorch_b200.yolox_models.YOLOXHead for eval()')
+        _require_training(self, 'cvpytorch_b200.train.YOLOXHead is the TRAINING drop-in (batch statistics); load its state_dict into '
+                                'cvpytorch_b200.yolox_models.YOLOXHead for eval()')
         outputs = []
         for k, xx in enumerate(x):
             xx = self.stems[k](xx)  # (the stem's output fans out to both branches: autograd adds the two gradients)
@@ -673,4 +655,4 @@ class YOLOXHead(nn.Module):
         return outputs
 
     def forward(self, x):
-        return self.forward_nhwc(_to_nhwc(x))
+        return self.forward_nhwc([_to_nhwc(t, 'YOLOX neck / head (H100 training)') for t in x])
