@@ -368,7 +368,7 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
             const float sc = __fmul_rn(o, obj);  // same fp32 product the NMS kernels recompute from z (yolov5.py:106)
             if (multi_label) {
               if (sc > conf) {
-                atomicAdd(&s_hist[min(__float_as_uint(sc) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
+                atomicAdd(&s_hist[nms_score_bin(sc)], 1u);
                 rbest = fmaxf(rbest, sc);
               }
             } else {
@@ -383,7 +383,7 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
         for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
         if (lane == 0) {
           rowmax[(size_t)b * z_rows + z_off + orow] = rbest;
-          if (!multi_label && rbest > conf) atomicAdd(&s_hist[min(__float_as_uint(rbest) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
+          if (!multi_label && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
         }
       }
     }
@@ -466,15 +466,15 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_fast_kernel(const 
           const float s1 = __fmul_rn(y1, obj);
           const float s2 = v2 ? __fmul_rn(y2, obj) : 0.0f;
           if (MULTI) {
-            if (s0 > conf) atomicAdd(&s_hist[min(__float_as_uint(s0) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
-            if (s1 > conf) atomicAdd(&s_hist[min(__float_as_uint(s1) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
-            if (s2 > conf) atomicAdd(&s_hist[min(__float_as_uint(s2) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
+            if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
+            if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
+            if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
           }
           rbest = fmaxf(fmaxf(s0, s1), s2);
           if (!(rbest > conf)) rbest = 0.0f;
 #pragma unroll
           for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
-          if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[min(__float_as_uint(rbest) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
+          if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
         }
         if (ok && lane == 0) rmb[orow] = rbest;
       }

@@ -204,7 +204,7 @@ __device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uin
     }                                          \
   } while (0)
 
-// NMS score histogram in shared memory: ++hist[min(bits(sc) >> 17, kNmsBins - 1)] iff `on` -- one predicated red.shared, no branch
+// NMS score histogram in shared memory: ++hist[nms_score_bin(sc)] iff `on` (must match that definition in internal.h) -- one predicated red.shared, no branch
 // (a C++ `if (on) atomicAdd(...)` compiles to a ~14-instruction divergent region per score, which dominated the fused-decode epilogue)
 __device__ __forceinline__ void hist_inc_if(uint32_t hist_smem_addr, float sc, bool on) {
   asm volatile(
@@ -815,7 +815,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
             float rm = fmaxf(y_part[row], y_part[kTileM + row]);
             if (!(rm > conf)) rm = 0.0f;
             a.y_rowmax[lvl_row0 + (size_t)ow] = rm;
-            if (!a.y_multi && rm > conf) atomicAdd(&hist_s[min(__float_as_uint(rm) >> 17, (uint32_t)(kNmsBins - 1))], 1u);
+            if (!a.y_multi && rm > conf) atomicAdd(&hist_s[nms_score_bin(rm)], 1u);
           }
         }
         if (prof_on) prof_acc[4] += clock64() - pt0;  // copy-out issue + rowmax

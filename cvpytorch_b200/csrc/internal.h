@@ -38,8 +38,12 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// NMS score histogram (shared by nms.cu and the decode kernel): bin = float_bits(score) >> 17, per image
+// NMS score histogram (shared by nms.cu, the decode kernels and the fused-decode conv epilogue): kNmsBins bins per image
 constexpr int kNmsBins = 16384;
+#ifdef __CUDACC__
+// Histogram bin of a score: its fp32 bits >> 17, monotone in non-negative scores; sign-bit patterns clamp to the last bin.
+__device__ __forceinline__ uint32_t nms_score_bin(float score) { return min(__float_as_uint(score) >> 17, (uint32_t)(kNmsBins - 1)); }
+#endif
 constexpr int kNmsCap = 65536;   // candidate key capacity per image (phase B)
 constexpr int kNmsCapA = 4096;   // phase-A candidate capacity = one shared-memory sort chunk
 

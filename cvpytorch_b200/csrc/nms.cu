@@ -23,7 +23,7 @@
 
 namespace cvb {
 
-constexpr int kBins = kNmsBins;  // score_bits >> 17 for positive floats
+constexpr int kBins = kNmsBins;  // nms_score_bin (internal.h)
 constexpr int kCap = kNmsCap;  // candidate key capacity per image
 constexpr int kChunk = 4096;   // keys sorted per CTA in shared memory
 constexpr int kGreedyThreads = 512;
@@ -46,16 +46,12 @@ struct NmsWs {
   int phase;        // 0 = A, 1 = B
 };
 
-__host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-static size_t ws_head_bytes(int B) { return nms_ws_head_bytes(B); }
-
 static NmsWs carve_ws(void* ws, int B, int phase) {
   NmsWs w;
   uint8_t* p = static_cast<uint8_t*>(ws);
-  const size_t slot = align_up((size_t)B * 4, 256);
+  const size_t slot = nms_align_up((size_t)B * 4, 256);
   w.hist = reinterpret_cast<uint32_t*>(p);
-  p += align_up((size_t)B * kBins * 4, 256);
+  p += nms_align_up((size_t)B * kBins * 4, 256);
   uint32_t* cntB = reinterpret_cast<uint32_t*>(p);
   uint32_t* tbinB = reinterpret_cast<uint32_t*>(p + slot);
   uint32_t* cntA = reinterpret_cast<uint32_t*>(p + 2 * slot);
@@ -81,13 +77,229 @@ static NmsWs carve_ws(void* ws, int B, int phase) {
   return w;
 }
 
+// ------------------------------------------------------------------ building blocks of the YOLOv5, YOLOX and FCOS pipelines
+// Sort key of a candidate: score bits above, ~id below.  Scores are non-negative, so descending key order is descending score
+// with ties broken by the lower id (torchvision's stable order), and no two keys are equal.
+__device__ __forceinline__ uint64_t make_key(uint32_t score_bits, uint32_t id) {
+  return ((uint64_t)score_bits << 32) | (uint64_t)(0xFFFFFFFFu - id);
+}
+__device__ __forceinline__ uint32_t key_id(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull); }
+__device__ __forceinline__ float key_score(uint64_t key) { return __uint_as_float((uint32_t)(key >> 32)); }
+
+// Largest score(c), c in [0, nc), over the warp, returned in `best`, and its class: the first maximum wins, like torch.max.
+template <class Score>
+__device__ __forceinline__ int warp_argmax_first(int nc, Score score, float& best) {
+  const int lane = threadIdx.x & 31;
+  best = -1.0f;
+  int bi = 0x7fffffff;
+  for (int c = lane; c < nc; c += 32) {
+    const float s = score(c);
+    if (s > best) {
+      best = s;
+      bi = c;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) {
+      best = ob;
+      bi = oi;
+    }
+  }
+  return bi;
+}
+
+// Warp-aggregated append: the lanes with `pass` take consecutive slots, in lane order, from one atomicAdd on *counter.
+// Returns the lane's slot (meaningless where !pass).  The whole warp calls it.
+__device__ __forceinline__ uint32_t warp_append(uint32_t* counter, bool pass) {
+  const int lane = threadIdx.x & 31;
+  const uint32_t m = __ballot_sync(0xffffffffu, pass);
+  if (m == 0) return 0;
+  uint32_t base = 0;
+  if (lane == 0) base = atomicAdd(counter, (uint32_t)__popc(m));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  return base + __popc(m & ((1u << lane) - 1));
+}
+
+// Max of v over the block, returned to every thread.  The whole block calls it; red holds one float per warp.
+template <int kThreads>
+__device__ __forceinline__ float block_max(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float m = red[0];
+  for (int w = 1; w < kThreads / 32; ++w) m = fmaxf(m, red[w]);
+  return m;
+}
+
+// Top-k threshold of a score histogram (global or shared): the highest bin t whose bins [t, kBins) hold >= target candidates,
+// 0 when the whole histogram holds fewer.  Warp 0 writes it to *tbin and the histogram's total to *total (when given).  The
+// whole block of kThreads calls it; seg is kBins / 32 words of shared memory.
+template <int kThreads>
+__device__ __forceinline__ void top_bin_search(const uint32_t* hist, uint32_t target, uint32_t* seg, uint32_t* tbin, uint32_t* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int sgi = warp; sgi < kBins / 32; sgi += kThreads / 32) {  // sums of 32-bin segments (coalesced reads, one warp reduction each)
+    uint32_t v = hist[sgi * 32 + lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) seg[sgi] = v;
+  }
+  __syncthreads();
+  if (warp != 0) return;
+  // top-down scan: lane l owns the kPer consecutive segments just below those of lane l-1
+  constexpr int kPer = kBins / 32 / 32;
+  const int top = kBins / 32 - 1 - lane * kPer;
+  uint32_t part = 0;
+  for (int i = 0; i < kPer; ++i) part += seg[top - i];
+  uint32_t incl = part;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  const uint32_t sum = __shfl_sync(0xffffffffu, incl, 31);
+  if (lane == 0) {
+    *tbin = 0;  // default: everything
+    if (total) *total = sum;
+  }
+  __syncwarp();
+  uint32_t run = incl - part;  // candidates in all higher segments
+  if (run < target && incl >= target) {  // exactly one lane crosses the target
+    for (int i = 0; i < kPer; ++i) {
+      const int sgi = top - i;
+      if (run + seg[sgi] >= target) {
+        for (int j = 31; j >= 0; --j) {
+          run += hist[sgi * 32 + j];
+          if (run >= target) {
+            *tbin = (uint32_t)(sgi * 32 + j);
+            break;
+          }
+        }
+        break;
+      }
+      run += seg[sgi];
+    }
+  }
+}
+
+__device__ __forceinline__ void cmpswap(uint64_t* s, int i, int l, bool desc) {
+  const uint64_t x = s[i], y = s[l];
+  if (desc ? (x < y) : (x > y)) {
+    s[i] = y;
+    s[l] = x;
+  }
+}
+
+// Stages k = k_lo .. k_hi (powers of two) of a bitonic sort, run on the n keys s = keys[start, start + n) of the sequence held in
+// shared memory (n a power of two), steps j < n only: steps j >= n pair keys of different tiles and run elsewhere.  The pair
+// (i, i + j) is put in descending order where ((start + i) & k) == 0, ascending elsewhere.  The caller syncs before it reads s.
+__device__ __forceinline__ void bitonic_tile(uint64_t* s, int n, uint32_t start, int k_lo, int k_hi) {
+  for (int k = k_lo; k <= k_hi; k <<= 1)
+    for (int j = min(k, n) >> 1; j > 0; j >>= 1) {
+      __syncthreads();
+      for (int t = threadIdx.x; t < n / 2; t += blockDim.x) {
+        const int i = 2 * j * (t / j) + (t % j);
+        cmpswap(s, i, i + j, ((start + i) & k) == 0);
+      }
+    }
+}
+
+// Torchvision's IoU test: fp32 IoU, areas without +1, compared in double against the threshold
+__device__ __forceinline__ bool iou_gt(const float4& a, float aa, const float4& b, float ab, double thr) {
+  const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
+  const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
+  const float w = fmaxf(0.0f, __fsub_rn(xx2, xx1));
+  const float h = fmaxf(0.0f, __fsub_rn(yy2, yy1));
+  const float inter = __fmul_rn(w, h);
+  const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter));
+  return (double)ovr > thr;
+}
+
+// Greedy NMS over candidates in score order, one chunk of kChunk at a time.
+template <int kChunk>
+struct GreedyChunk {
+  float4 box[kChunk];  // the chunk's survivors, compacted in score order: boxes as the suppression rule sees them
+  float area[kChunk];
+  int cls[kChunk];
+  uint32_t payload[kChunk];            // the caller's handle of the candidate
+  uint32_t mask[kChunk][kChunk / 32];  // bit c of row r: survivor r suppresses survivor c > r
+  uint32_t keep[kChunk];               // rows kept by the resolve, in order
+  uint32_t warp_cnt[32];
+  uint32_t m, nk;
+};
+
+// Thread t < kChunk holds the chunk's candidate t; it is not `alive` past the end of the list or when a box kept in an earlier
+// chunk suppresses it.  The survivors are compacted in order, suppress(r, c) (survivor r < c of G suppresses c) fills the bit mask,
+// and one warp resolves it in order, keeping at most `limit` rows.  Returns the number kept; G.keep lists their rows.  The caller syncs before G is reused.
+template <int kThreads, int kChunk, class Suppress>
+__device__ __forceinline__ int greedy_chunk(GreedyChunk<kChunk>& G, bool alive, const float4& box, float area, int cls, uint32_t payload,
+                                            int limit, Suppress suppress) {
+  static_assert(kThreads >= kChunk && kThreads <= 1024, "one thread per candidate of the chunk");
+  constexpr int kWarps = kThreads / 32;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // order-preserving compaction of the survivors
+  const uint32_t bal = __ballot_sync(0xffffffffu, alive);
+  if (lane == 0) G.warp_cnt[warp] = __popc(bal);
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t v = (lane < kWarps) ? G.warp_cnt[lane] : 0;
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += u;
+    }
+    if (lane < kWarps) G.warp_cnt[lane] = inc - v;
+    if (lane == 31) G.m = inc;
+  }
+  __syncthreads();
+  const int m = (int)G.m;
+  if (alive) {
+    const int pos = (int)G.warp_cnt[warp] + __popc(bal & ((1u << lane) - 1));
+    G.box[pos] = box;
+    G.area[pos] = area;
+    G.cls[pos] = cls;
+    G.payload[pos] = payload;
+  }
+  __syncthreads();
+  // suppression bit mask among the m survivors (row r suppresses column c > r)
+  const int words = (m + 31) >> 5;
+  if (tid < m) {
+    for (int wd = 0; wd < words; ++wd) {
+      uint32_t bits = 0;
+      const int c0 = wd << 5, c1 = min(m, c0 + 32);
+      for (int c = max(c0, tid + 1); c < c1; ++c)
+        if (suppress(tid, c)) bits |= 1u << (c & 31);
+      G.mask[tid][wd] = bits;
+    }
+  }
+  __syncthreads();
+  // sequential greedy resolve by one warp; lane l owns word l of the "removed" bitset
+  if (warp == 0) {
+    uint32_t removed = 0;
+    int nk = 0;
+    for (int r = 0; r < m && nk < limit; ++r) {
+      const uint32_t rw = __shfl_sync(0xffffffffu, removed, r >> 5);
+      if (!((rw >> (r & 31)) & 1u)) {
+        if (lane == 0) G.keep[nk] = (uint32_t)r;
+        ++nk;
+        if (lane < words) removed |= G.mask[r][lane];
+      }
+    }
+    if (lane == 0) G.nk = (uint32_t)nk;
+  }
+  __syncthreads();
+  return (int)G.nk;
+}
+
 // ------------------------------------------------------------------ counting pass (only when the decode kernel did not build the histogram)
 // Grid (ceil(A / kRowsPerCta), B); each warp walks rows of ONE image: histogram of score bits (spread global atomics) and the
 // per-row best score (rowmax) that lets the emit passes skip rows.
 constexpr int kRowsPerCta = 64;
 constexpr int kScanThreads = 256;
-
-__device__ __forceinline__ uint32_t score_bin(uint32_t bits) { return min(bits >> 17, (uint32_t)(kBins - 1)); }
 
 __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __restrict__ pred, int A, int nc, float conf, int multi_label,
                                                                  NmsWs ws) {
@@ -120,7 +332,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __
         for (int c = lane; c < nc; c += 32) {
           const float sc = __fmul_rn(__ldg(r + 5 + c), ob);
           if (sc > conf) {
-            atomicAdd(&hist[score_bin(__float_as_uint(sc))], 1u);
+            atomicAdd(&hist[nms_score_bin(sc)], 1u);
             rbest = fmaxf(rbest, sc);
           }
         }
@@ -133,7 +345,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __
       if (!(rbest > conf)) rbest = 0.0f;
       if (lane == 0) {
         rowmax[anchor] = rbest;
-        if (!multi_label && rbest > conf) atomicAdd(&hist[score_bin(__float_as_uint(rbest))], 1u);
+        if (!multi_label && rbest > conf) atomicAdd(&hist[nms_score_bin(rbest)], 1u);
       }
     }
   }
@@ -164,8 +376,8 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
   for (int r = threadIdx.x; r < kEmitRows; r += kScanThreads) {
     const int row = row0 + r;
     if (row < A) {
-      const uint32_t rb = __float_as_uint(__ldg(rowmax + row));
-      if (rb != 0u && score_bin(rb) >= tb) s_live[atomicAdd(&s_nlive, 1u)] = row;
+      const float rm = __ldg(rowmax + row);
+      if (__float_as_uint(rm) != 0u && nms_score_bin(rm) >= tb) s_live[atomicAdd(&s_nlive, 1u)] = row;
     }
   }
   __syncthreads();
@@ -199,25 +411,10 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
 #pragma unroll
           for (int k = 0; k < 3; ++k) {
             const int c = k * 32 + lane;
-            bool pass = false;
-            uint32_t bits = 0;
-            if (c < nc) {
-              const float sc = __fmul_rn(v[i][k], ob[i]);
-              if (sc > conf) {
-                bits = __float_as_uint(sc);
-                pass = score_bin(bits) >= tb;
-              }
-            }
-            const uint32_t m = __ballot_sync(0xffffffffu, pass);
-            if (m) {
-              uint32_t sb = 0;
-              if (lane == 0) sb = atomicAdd(&s_cnt, (uint32_t)__popc(m));
-              sb = __shfl_sync(0xffffffffu, sb, 0);
-              if (pass) {
-                const uint32_t id = (uint32_t)an[i] * (uint32_t)nc + (uint32_t)c;
-                stage[sb + __popc(m & ((1u << lane) - 1))] = ((uint64_t)bits << 32) | (uint64_t)(0xFFFFFFFFu - id);
-              }
-            }
+            const float sc = (c < nc) ? __fmul_rn(v[i][k], ob[i]) : 0.0f;
+            const bool pass = c < nc && sc > conf && nms_score_bin(sc) >= tb;
+            const uint32_t slot = warp_append(&s_cnt, pass);
+            if (pass) stage[slot] = make_key(__float_as_uint(sc), (uint32_t)an[i] * (uint32_t)nc + (uint32_t)c);
           }
         }
       }
@@ -230,53 +427,17 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
       if (multi_label) {
         for (int c0 = 0; c0 < nc; c0 += 32) {
           const int c = c0 + lane;
-          bool pass = false;
-          uint32_t bits = 0;
-          if (c < nc) {
-            const float sc = __fmul_rn(__ldg(r + 5 + c), ob);
-            if (sc > conf) {
-              bits = __float_as_uint(sc);
-              pass = score_bin(bits) >= tb;
-            }
-          }
-          const uint32_t m = __ballot_sync(0xffffffffu, pass);
-          if (m) {
-            uint32_t sb = 0;
-            if (lane == 0) sb = atomicAdd(&s_cnt, (uint32_t)__popc(m));
-            sb = __shfl_sync(0xffffffffu, sb, 0);
-            if (pass) {
-              const uint32_t id = (uint32_t)anchor * (uint32_t)nc + (uint32_t)c;
-              stage[sb + __popc(m & ((1u << lane) - 1))] = ((uint64_t)bits << 32) | (uint64_t)(0xFFFFFFFFu - id);
-            }
-          }
+          const float sc = (c < nc) ? __fmul_rn(__ldg(r + 5 + c), ob) : 0.0f;
+          const bool pass = c < nc && sc > conf && nms_score_bin(sc) >= tb;
+          const uint32_t slot = warp_append(&s_cnt, pass);
+          if (pass) stage[slot] = make_key(__float_as_uint(sc), (uint32_t)anchor * (uint32_t)nc + (uint32_t)c);
         }
       } else {
-        // best class only: conf, j = x[:, 5:].max(1)  (first maximum wins ties)
-        float best = -1.0f;
-        int bi = 0x7fffffff;
-        for (int c = lane; c < nc; c += 32) {
-          const float sc = __fmul_rn(__ldg(r + 5 + c), ob);
-          if (sc > best) {
-            best = sc;
-            bi = c;
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ob2 = __shfl_xor_sync(0xffffffffu, best, o);
-          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ob2 > best || (ob2 == best && oi < bi)) {
-            best = ob2;
-            bi = oi;
-          }
-        }
-        if (lane == 0 && best > conf) {
-          const uint32_t bits = __float_as_uint(best);
-          if (score_bin(bits) >= tb) {
-            const uint32_t id = (uint32_t)anchor * (uint32_t)nc + (uint32_t)bi;
-            stage[atomicAdd(&s_cnt, 1u)] = ((uint64_t)bits << 32) | (uint64_t)(0xFFFFFFFFu - id);
-          }
-        }
+        // best class only: conf, j = x[:, 5:].max(1)
+        float best;
+        const int bi = warp_argmax_first(nc, [&](int c) { return __fmul_rn(__ldg(r + 5 + c), ob); }, best);
+        if (lane == 0 && best > conf && nms_score_bin(best) >= tb)
+          stage[atomicAdd(&s_cnt, 1u)] = make_key(__float_as_uint(best), (uint32_t)anchor * (uint32_t)nc + (uint32_t)bi);
       }
     }
     __syncthreads();
@@ -296,52 +457,9 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
 
 // ------------------------------------------------------------------ threshold bin: smallest set of top bins holding >= max_nms
 __global__ void __launch_bounds__(256) nms_threshold_kernel(NmsWs ws, int target) {
-  __shared__ uint32_t seg[kBins / 32];  // sums of 32-bin segments (coalesced reads, one warp reduction each)
+  __shared__ uint32_t seg[kBins / 32];
   const int b = blockIdx.x;
-  const uint32_t* h = ws.hist + (size_t)b * kBins;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int sgi = warp; sgi < kBins / 32; sgi += 8) {
-    uint32_t v = h[sgi * 32 + lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) seg[sgi] = v;
-  }
-  __syncthreads();
-  if (warp != 0) return;
-  // top-down scan: lane l owns the kPer consecutive segments just below those of lane l-1
-  constexpr int kPer = kBins / 32 / 32;
-  const int top = kBins / 32 - 1 - lane * kPer;
-  uint32_t part = 0;
-  for (int i = 0; i < kPer; ++i) part += seg[top - i];
-  uint32_t incl = part;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += u;
-  }
-  const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-  if (lane == 0) {
-    ws.tbin[b] = 0;  // default: everything
-    ws.total[b] = total;
-  }
-  __syncwarp();
-  uint32_t run = incl - part;  // candidates in all higher segments
-  if (run < (uint32_t)target && incl >= (uint32_t)target) {  // exactly one lane crosses the target
-    for (int i = 0; i < kPer; ++i) {
-      const int sgi = top - i;
-      if (run + seg[sgi] >= (uint32_t)target) {
-        for (int j = 31; j >= 0; --j) {
-          run += h[sgi * 32 + j];
-          if (run >= (uint32_t)target) {
-            ws.tbin[b] = (uint32_t)(sgi * 32 + j);
-            break;
-          }
-        }
-        break;
-      }
-      run += seg[sgi];
-    }
-  }
+  top_bin_search<256>(ws.hist + (size_t)b * kBins, (uint32_t)target, seg, &ws.tbin[b], &ws.total[b]);
 }
 
 // ------------------------------------------------------------------ segmented bitonic sort (descending)
@@ -351,14 +469,6 @@ __device__ __forceinline__ uint32_t seg_npad(const NmsWs& ws, int b, uint32_t* n
   if (ws.phase == 1 && ws.done[b]) n = 0;  // nothing to sort: every chunk beyond the first returns immediately
   *n_out = n;
   return n <= 1 ? 1u : (1u << (32 - __clz(n - 1)));
-}
-
-__device__ __forceinline__ void cmpswap(uint64_t* s, int i, int l, bool desc) {
-  const uint64_t x = s[i], y = s[l];
-  if (desc ? (x < y) : (x > y)) {
-    s[i] = y;
-    s[l] = x;
-  }
 }
 
 // full sort of each 4096-key chunk (stages k = 2..4096)
@@ -372,73 +482,15 @@ __global__ void __launch_bounds__(1024) bitonic_local_sort_kernel(NmsWs ws) {
   if (ws.phase == 1 && ws.done[b]) return;
   uint64_t* keys = ws.keys + (size_t)b * ws.cap;
   for (int i = threadIdx.x; i < kChunk; i += blockDim.x) s[i] = (start + i < n) ? keys[start + i] : 0ull;
-  for (int k = 2; k <= kChunk; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      __syncthreads();
-      for (int t = threadIdx.x; t < kChunk / 2; t += blockDim.x) {
-        const int i = 2 * j * (t / j) + (t % j);
-        cmpswap(s, i, i + j, ((start + i) & k) == 0);
-      }
-    }
+  bitonic_tile(s, kChunk, start, 2, kChunk);
   __syncthreads();
   for (int i = threadIdx.x; i < kChunk; i += blockDim.x) keys[start + i] = s[i];
-}
-
-// one compare-exchange step with partner distance j >= kChunk
-__global__ void bitonic_global_step_kernel(NmsWs ws, uint32_t k, uint32_t j) {
-  const int b = blockIdx.y;
-  uint32_t n;
-  const uint32_t npad = seg_npad(ws, b, &n);
-  if (k > npad) return;
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t i = 2 * j * (t / j) + (t % j);
-  if (i >= npad) return;
-  uint64_t* keys = ws.keys + (size_t)b * ws.cap;
-  const uint64_t x = keys[i], y = keys[i + j];
-  const bool desc = (i & k) == 0;
-  if (desc ? (x < y) : (x > y)) {
-    keys[i] = y;
-    keys[i + j] = x;
-  }
-}
-
-// remaining steps j = kChunk/2 .. 1 of stage k, fused in shared memory
-__global__ void __launch_bounds__(1024) bitonic_local_merge_kernel(NmsWs ws, uint32_t k) {
-  __shared__ uint64_t s[kChunk];
-  const int b = blockIdx.y;
-  uint32_t n;
-  const uint32_t npad = seg_npad(ws, b, &n);
-  if (k > npad) return;
-  const uint32_t start = blockIdx.x * kChunk;
-  if (start >= npad) return;
-  uint64_t* keys = ws.keys + (size_t)b * ws.cap;
-  for (int i = threadIdx.x; i < kChunk; i += blockDim.x) s[i] = keys[start + i];
-  for (int j = kChunk >> 1; j > 0; j >>= 1) {
-    __syncthreads();
-    for (int t = threadIdx.x; t < kChunk / 2; t += blockDim.x) {
-      const int i = 2 * j * (t / j) + (t % j);
-      cmpswap(s, i, i + j, ((start + i) & k) == 0);
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < kChunk; i += blockDim.x) keys[start + i] = s[i];
-}
-
-// ------------------------------------------------------------------ greedy scan
-__device__ __forceinline__ bool iou_gt(const float4& a, float aa, const float4& b, float ab, double thr) {
-  const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-  const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-  const float w = fmaxf(0.0f, __fsub_rn(xx2, xx1));
-  const float h = fmaxf(0.0f, __fsub_rn(yy2, yy1));
-  const float inter = __fmul_rn(w, h);
-  const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter));
-  return (double)ovr > thr;
 }
 
 // Phase B in ONE cooperative launch: the whole segmented bitonic sort (local sort, global steps, local merges) with grid-wide
 // barriers between steps.  When no image needs phase B (the common case: phase A already kept max_det boxes everywhere) every
 // CTA sees that from the `done` flags and returns before the first barrier, so the idle cost is one small launch instead of
-// fifteen.  Same compare-exchange network, hence the same (unique-key) result as the separate kernels above.
+// one launch per step.
 __global__ void __launch_bounds__(1024) bitonic_full_sort_kernel(NmsWs ws, int B) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
@@ -464,14 +516,7 @@ __global__ void __launch_bounds__(1024) bitonic_full_sort_kernel(NmsWs ws, int B
     uint64_t* keys = ws.keys + (size_t)b * ws.cap;
     __syncthreads();
     for (int i = threadIdx.x; i < kChunk; i += blockDim.x) s[i] = (start + i < n) ? keys[start + i] : 0ull;
-    for (int k = 2; k <= kChunk; k <<= 1)
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        __syncthreads();
-        for (int t = threadIdx.x; t < kChunk / 2; t += blockDim.x) {
-          const int i = 2 * j * (t / j) + (t % j);
-          cmpswap(s, i, i + j, ((start + i) & k) == 0);
-        }
-      }
+    bitonic_tile(s, kChunk, start, 2, kChunk);
     __syncthreads();
     for (int i = threadIdx.x; i < kChunk; i += blockDim.x) keys[start + i] = s[i];
   }
@@ -487,13 +532,7 @@ __global__ void __launch_bounds__(1024) bitonic_full_sort_kernel(NmsWs ws, int B
         if (k > npad) continue;
         const uint32_t i = 2 * j * (t / j) + (t % j);
         if (i >= npad) continue;
-        uint64_t* keys = ws.keys + (size_t)b * ws.cap;
-        const uint64_t x = keys[i], y = keys[i + j];
-        const bool desc = (i & k) == 0;
-        if (desc ? (x < y) : (x > y)) {
-          keys[i] = y;
-          keys[i + j] = x;
-        }
+        cmpswap(ws.keys + (size_t)b * ws.cap, (int)i, (int)(i + j), (i & k) == 0);
       }
       grid.sync();
     }
@@ -506,13 +545,7 @@ __global__ void __launch_bounds__(1024) bitonic_full_sort_kernel(NmsWs ws, int B
       uint64_t* keys = ws.keys + (size_t)b * ws.cap;
       __syncthreads();
       for (int i = threadIdx.x; i < kChunk; i += blockDim.x) s[i] = keys[start + i];
-      for (int j = kChunk >> 1; j > 0; j >>= 1) {
-        __syncthreads();
-        for (int t = threadIdx.x; t < kChunk / 2; t += blockDim.x) {
-          const int i = 2 * j * (t / j) + (t % j);
-          cmpswap(s, i, i + j, ((start + i) & k) == 0);
-        }
-      }
+      bitonic_tile(s, kChunk, start, (int)k, (int)k);
       __syncthreads();
       for (int i = threadIdx.x; i < kChunk; i += blockDim.x) keys[start + i] = s[i];
     }
@@ -520,29 +553,27 @@ __global__ void __launch_bounds__(1024) bitonic_full_sort_kernel(NmsWs ws, int B
   }
 }
 
-struct GreedySmem {
-  float4 cbox[kGreedyThreads];   // class-offset boxes of the alive candidates of this chunk (compacted)
-  float4 cbox0[kGreedyThreads];  // un-offset boxes
-  float carea[kGreedyThreads];
-  float cscore[kGreedyThreads];
-  uint32_t cid[kGreedyThreads];
-  uint32_t mask[kGreedyThreads][kGreedyThreads / 32];
-  uint32_t keeplist[kGreedyThreads];
-  uint32_t warp_cnt[kGreedyThreads / 32];
-  uint32_t m_alive, new_kept;
-};
+// ------------------------------------------------------------------ greedy scan
+using GreedySmem = GreedyChunk<kGreedyThreads>;
+
+// xywh2xyxy of one prediction row in fp32 (yolov5.py:52-59)
+__device__ __forceinline__ float4 row_xyxy(const float* r) {
+  const float cx = __ldg(r), cy = __ldg(r + 1), w = __ldg(r + 2), h = __ldg(r + 3);
+  const float hw = __fmul_rn(w, 0.5f), hh = __fmul_rn(h, 0.5f);
+  return make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
+}
 
 __global__ void __launch_bounds__(kGreedyThreads) nms_greedy_kernel(const float* __restrict__ pred, int A, int nc, NmsWs ws,
                                                                      double iou_thr, int max_nms, int max_det, float max_wh,
                                                                      float* __restrict__ det, int* __restrict__ det_idx,
                                                                      int* __restrict__ det_count) {
   extern __shared__ uint8_t gs_raw[];
-  GreedySmem& S = *reinterpret_cast<GreedySmem*>(gs_raw);
+  GreedySmem& G = *reinterpret_cast<GreedySmem*>(gs_raw);
   float4* kbox = reinterpret_cast<float4*>(gs_raw + sizeof(GreedySmem));  // [max_det]
   float* karea = reinterpret_cast<float*>(kbox + max_det);                // [max_det]
 
   const int b = blockIdx.x;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int no = nc + 5;
   if (ws.phase == 1 && ws.done[b]) return;
   uint32_t n = ws.cnt[b];
@@ -553,29 +584,21 @@ __global__ void __launch_bounds__(kGreedyThreads) nms_greedy_kernel(const float*
   if (n > (uint32_t)ws.cap) n = ws.cap;
   if (n > (uint32_t)max_nms) n = max_nms;
   const uint64_t* keys = ws.keys + (size_t)b * ws.cap;
+  const float* predb = pred + (size_t)b * A * no;
   int kept_n = 0;
 
   for (uint32_t base = 0; base < n && kept_n < max_det; base += kGreedyThreads) {
     const uint32_t i = base + tid;
     bool alive = i < n;
-    float4 box = make_float4(0, 0, 0, 0), box0 = box;
-    float area = 0.0f, score = 0.0f;
-    uint32_t id = 0;
+    float4 box = make_float4(0, 0, 0, 0);
+    float area = 0.0f;
     if (alive) {
-      const uint64_t key = keys[i];
-      id = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);
-      score = __uint_as_float((uint32_t)(key >> 32));
-    }
-    if (alive) {
-      const uint32_t anchor = id / (uint32_t)nc, cls = id % (uint32_t)nc;
-      const float* r = pred + ((size_t)b * A + anchor) * no;
-      const float cx = __ldg(r), cy = __ldg(r + 1), w = __ldg(r + 2), h = __ldg(r + 3);
-      const float hw = __fmul_rn(w, 0.5f), hh = __fmul_rn(h, 0.5f);
-      box0 = make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
-      const float off = __fmul_rn((float)cls, max_wh);
-      box = make_float4(__fadd_rn(box0.x, off), __fadd_rn(box0.y, off), __fadd_rn(box0.z, off), __fadd_rn(box0.w, off));
+      const uint32_t id = key_id(keys[i]);
+      const float4 b0 = row_xyxy(predb + (size_t)(id / (uint32_t)nc) * no);
+      const float off = __fmul_rn((float)(id % (uint32_t)nc), max_wh);
+      box = make_float4(__fadd_rn(b0.x, off), __fadd_rn(b0.y, off), __fadd_rn(b0.z, off), __fadd_rn(b0.w, off));
       area = __fmul_rn(__fsub_rn(box.z, box.x), __fsub_rn(box.w, box.y));
-      // phase 1: suppressed by an already kept (higher score) box?
+      // suppressed by an already kept (higher score) box?
       for (int k = 0; k < kept_n; ++k) {
         if (iou_gt(kbox[k], karea[k], box, area, iou_thr)) {
           alive = false;
@@ -583,79 +606,25 @@ __global__ void __launch_bounds__(kGreedyThreads) nms_greedy_kernel(const float*
         }
       }
     }
-    // order-preserving compaction of the survivors
-    const uint32_t bal = __ballot_sync(0xffffffffu, alive);
-    if (lane == 0) S.warp_cnt[warp] = __popc(bal);
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t v = (lane < kGreedyThreads / 32) ? S.warp_cnt[lane] : 0;
-      uint32_t inc = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-      }
-      if (lane < kGreedyThreads / 32) S.warp_cnt[lane] = inc - v;
-      if (lane == 31) S.m_alive = inc;
-    }
-    __syncthreads();
-    const int m = (int)S.m_alive;
-    if (alive) {
-      const int pos = (int)S.warp_cnt[warp] + __popc(bal & ((1u << lane) - 1));
-      S.cbox[pos] = box;
-      S.cbox0[pos] = box0;
-      S.carea[pos] = area;
-      S.cscore[pos] = score;
-      S.cid[pos] = id;
-    }
-    __syncthreads();
-    // phase 2: suppression bit mask among the m survivors (row r suppresses column c > r)
-    const int words = (m + 31) >> 5;
-    if (tid < m) {
-      const float4 me = S.cbox[tid];
-      const float ma = S.carea[tid];
-      for (int wd = 0; wd < words; ++wd) {
-        uint32_t bits = 0;
-        const int c0 = wd << 5;
-        const int c1 = min(m, c0 + 32);
-        for (int c = max(c0, tid + 1); c < c1; ++c)
-          if (iou_gt(me, ma, S.cbox[c], S.carea[c], iou_thr)) bits |= 1u << (c & 31);
-        S.mask[tid][wd] = bits;
-      }
-    }
-    __syncthreads();
-    // phase 3: sequential greedy resolve by one warp; lane l owns word l of the "removed" bitset
-    if (warp == 0) {
-      uint32_t removed = 0;
-      int nk = 0;
-      for (int r = 0; r < m; ++r) {
-        if (kept_n + nk >= max_det) break;
-        const uint32_t rw = __shfl_sync(0xffffffffu, removed, r >> 5);
-        if (!((rw >> (r & 31)) & 1u)) {
-          if (lane == 0) S.keeplist[nk] = (uint32_t)r;
-          ++nk;
-          if (lane < words) removed |= S.mask[r][lane];
-        }
-      }
-      if (lane == 0) S.new_kept = (uint32_t)nk;
-    }
-    __syncthreads();
-    // phase 4: append to the kept list and write the detections
-    const int nk = (int)S.new_kept;
+    const int nk = greedy_chunk<kGreedyThreads>(G, alive, box, area, 0, i, max_det - kept_n,
+                                                [&](int r, int c) { return iou_gt(G.box[r], G.area[r], G.box[c], G.area[c], iou_thr); });
+    // append to the kept list and write the detections; the payload is the candidate's key position
     for (int t = tid; t < nk; t += kGreedyThreads) {
-      const int r = (int)S.keeplist[t];
+      const int r = (int)G.keep[t];
       const int o = kept_n + t;
-      kbox[o] = S.cbox[r];
-      karea[o] = S.carea[r];
-      const float4 b0 = S.cbox0[r];
+      kbox[o] = G.box[r];
+      karea[o] = G.area[r];
+      const uint64_t key = keys[G.payload[r]];
+      const uint32_t id = key_id(key);
+      const float4 b0 = row_xyxy(predb + (size_t)(id / (uint32_t)nc) * no);
       float* d = det + ((size_t)b * max_det + o) * 6;
       d[0] = b0.x;
       d[1] = b0.y;
       d[2] = b0.z;
       d[3] = b0.w;
-      d[4] = S.cscore[r];
-      d[5] = (float)(S.cid[r] % (uint32_t)nc);
-      det_idx[(size_t)b * max_det + o] = (int)S.cid[r];
+      d[4] = key_score(key);
+      d[5] = (float)(id % (uint32_t)nc);
+      det_idx[(size_t)b * max_det + o] = (int)id;
     }
     kept_n += nk;
     __syncthreads();
@@ -679,7 +648,7 @@ extern "C" size_t cvb_nms_workspace_bytes(int32_t B, int32_t A, int32_t nc) {
 
 extern "C" int cvb_nms_workspace_reset(void* workspace, size_t workspace_bytes, int32_t B, void* stream) {
   CVB_REQUIRE(workspace && B > 0 && workspace_bytes >= cvb_nms_workspace_bytes(B, 1, 1), "nms reset: bad workspace");
-  CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, ws_head_bytes(B), as_stream(stream)));
+  CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, nms_ws_head_bytes(B), as_stream(stream)));
   return CVB_OK;
 }
 
@@ -693,7 +662,7 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   CVB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "nms: workspace must be 256-byte aligned");
   cudaStream_t st = as_stream(stream);
   NmsWs wsA = carve_ws(workspace, p->B, 0), wsB = carve_ws(workspace, p->B, 1);
-  if (!p->hist_ready) CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, ws_head_bytes(p->B), st));
+  if (!p->hist_ready) CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, nms_ws_head_bytes(p->B), st));
   if (status) CVB_CHECK_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), st));
   CVB_CHECK_CUDA(cudaMemsetAsync(det, 0, (size_t)p->B * p->max_det * 6 * sizeof(float), st));
   CVB_CHECK_CUDA(cudaMemsetAsync(det_idx, 0xFF, (size_t)p->B * p->max_det * sizeof(int32_t), st));
@@ -772,24 +741,8 @@ __global__ void __launch_bounds__(256) yolox_decode_kernel(const float* __restri
   const int p = (int)(warp - (long long)b * hw);
   const int py = p / W, px = p - py * W;
   const float* c = cls + (size_t)warp * cls_pitch;
-  float best = -1.0f;
-  int bi = 0x7fffffff;
-  for (int k = lane; k < nc; k += 32) {
-    const float sc = sigmoid_fast(__ldg(c + k));
-    if (sc > best) {
-      best = sc;
-      bi = k;
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ob > best || (ob == best && oi < bi)) {
-      best = ob;
-      bi = oi;
-    }
-  }
+  float best;
+  const int bi = warp_argmax_first(nc, [&](int k) { return sigmoid_fast(__ldg(c + k)); }, best);
   if (lane == 0) {
     const float* r = ro + (size_t)warp * ro_pitch;
     const float cx = __fmul_rn(__fadd_rn(__ldg(r), (float)px), stride);
@@ -810,17 +763,10 @@ constexpr int kXChunk = 512;
 
 struct YoloxSmem {
   uint64_t keys[kXKeys];
-  float4 cbox[kXChunk];    // boxes as seen by NMS (class offset added in coordinate-trick mode)
-  float carea[kXChunk];
-  int ccls[kXChunk];
-  uint32_t cidx[kXChunk];
-  uint32_t mask[kXChunk][kXChunk / 32];
-  uint32_t keeplist[kXChunk];
-  uint32_t warp_cnt[kXThreads / 32];
+  GreedyChunk<kXChunk> g;  // boxes as seen by NMS (class offset added in coordinate-trick mode); payload = candidate index
   float red[kXThreads / 32];
   int cls_head[1024];      // per-class (hashed by class & 1023) chain of kept boxes: head index, links in knext (-1 = end)
-  uint32_t n, m_alive, new_kept;
-  float unit;
+  uint32_t n;
 };
 
 // One CTA per image: score filter (obj * class_conf >= conf_thre, :58), stable descending order (score, then lower index),
@@ -834,7 +780,7 @@ __global__ void __launch_bounds__(kXThreads) yolox_nms_kernel(const float* __res
   extern __shared__ uint8_t xs_raw[];
   YoloxSmem& S = *reinterpret_cast<YoloxSmem*>(xs_raw);
   const int b = blockIdx.x;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const float* cb = cand + (size_t)b * A * 8;
   float4* kbox = kbox_g + (size_t)b * A;
   float* karea = karea_g + (size_t)b * A;
@@ -850,19 +796,12 @@ __global__ void __launch_bounds__(kXThreads) yolox_nms_kernel(const float* __res
     if (hi.w >= conf) {
       const float4 bx = __ldg(reinterpret_cast<const float4*>(cb + (size_t)i * 8));
       cmax = fmaxf(cmax, fmaxf(fmaxf(bx.x, bx.y), fmaxf(bx.z, bx.w)));
-      S.keys[atomicAdd(&S.n, 1u)] = ((uint64_t)__float_as_uint(hi.w) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)i);
+      S.keys[atomicAdd(&S.n, 1u)] = make_key(__float_as_uint(hi.w), (uint32_t)i);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(0xffffffffu, cmax, o));
-  if (lane == 0) S.red[warp] = cmax;
-  __syncthreads();
+  // max_coordinate + 1 (torchvision/ops/boxes.py _batched_nms_coordinate_trick)
+  const float unit = __fadd_rn(block_max<kXThreads>(cmax, S.red), 1.0f);
   const int n = (int)S.n;
-  if (tid == 0) {
-    float m = -CUDART_INF_F;
-    for (int w = 0; w < kXThreads / 32; ++w) m = fmaxf(m, S.red[w]);
-    S.unit = __fadd_rn(m, 1.0f);  // max_coordinate + 1 (torchvision/ops/boxes.py _batched_nms_coordinate_trick)
-  }
   if (n == 0) {
     if (tid == 0) count[b] = 0;
     return;
@@ -870,22 +809,9 @@ __global__ void __launch_bounds__(kXThreads) yolox_nms_kernel(const float* __res
   int npad = 1;
   while (npad < n) npad <<= 1;
   for (int i = n + tid; i < npad; i += kXThreads) S.keys[i] = 0ull;
-  for (int k = 2; k <= npad; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      __syncthreads();
-      for (int t = tid; t < npad / 2; t += kXThreads) {
-        const int i = 2 * j * (t / j) + (t % j);
-        const uint64_t x = S.keys[i], y = S.keys[i + j];
-        const bool desc = (i & k) == 0;
-        if (desc ? (x < y) : (x > y)) {
-          S.keys[i] = y;
-          S.keys[i + j] = x;
-        }
-      }
-    }
+  bitonic_tile(S.keys, npad, 0, 2, npad);
   __syncthreads();
   const bool vanilla = n > vanilla_above;
-  const float unit = S.unit;
   int kept_n = 0;
   for (int base = 0; base < n; base += kXChunk) {
     const int i = base + tid;
@@ -895,7 +821,7 @@ __global__ void __launch_bounds__(kXThreads) yolox_nms_kernel(const float* __res
     int cls = 0;
     uint32_t idx = 0;
     if (alive) {
-      idx = 0xFFFFFFFFu - (uint32_t)(S.keys[i] & 0xFFFFFFFFull);
+      idx = key_id(S.keys[i]);
       const float4 bx = __ldg(reinterpret_cast<const float4*>(cb + (size_t)idx * 8));
       const float4 hi = __ldg(reinterpret_cast<const float4*>(cb + (size_t)idx * 8 + 4));
       cls = (int)hi.z;
@@ -923,68 +849,19 @@ __global__ void __launch_bounds__(kXThreads) yolox_nms_kernel(const float* __res
         }
       }
     }
-    const uint32_t bal = __ballot_sync(0xffffffffu, alive);
-    if (lane == 0) S.warp_cnt[warp] = __popc(bal);
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t v = S.warp_cnt[lane];
-      uint32_t inc = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-      }
-      S.warp_cnt[lane] = inc - v;
-      if (lane == 31) S.m_alive = inc;
-    }
-    __syncthreads();
-    const int m = (int)S.m_alive;
-    if (alive) {
-      const int pos = (int)S.warp_cnt[warp] + __popc(bal & ((1u << lane) - 1));
-      S.cbox[pos] = box;
-      S.carea[pos] = area;
-      S.ccls[pos] = cls;
-      S.cidx[pos] = idx;
-    }
-    __syncthreads();
-    const int words = (m + 31) >> 5;
-    if (tid < m) {
-      const float4 me = S.cbox[tid];
-      const float ma = S.carea[tid];
-      const int mc = S.ccls[tid];
-      for (int wd = 0; wd < words; ++wd) {
-        uint32_t bits = 0;
-        const int c0 = wd << 5;
-        const int c1 = min(m, c0 + 32);
-        for (int c = max(c0, tid + 1); c < c1; ++c)
-          if ((!vanilla || S.ccls[c] == mc) && iou_gt(me, ma, S.cbox[c], S.carea[c], iou_thr)) bits |= 1u << (c & 31);
-        S.mask[tid][wd] = bits;
-      }
-    }
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t removed = 0;
-      int nk = 0;
-      for (int r = 0; r < m; ++r) {
-        const uint32_t rw = __shfl_sync(0xffffffffu, removed, r >> 5);
-        if (!((rw >> (r & 31)) & 1u)) {
-          if (lane == 0) S.keeplist[nk] = (uint32_t)r;
-          ++nk;
-          if (lane < words) removed |= S.mask[r][lane];
-        }
-      }
-      if (lane == 0) S.new_kept = (uint32_t)nk;
-    }
-    __syncthreads();
-    const int nk = (int)S.new_kept;
+    const int nk = greedy_chunk<kXThreads>(S.g, alive, box, area, cls, idx, kXChunk,
+                                           [&](int r, int c) {
+                                             const GreedyChunk<kXChunk>& G = S.g;
+                                             return (!vanilla || G.cls[c] == G.cls[r]) && iou_gt(G.box[r], G.area[r], G.box[c], G.area[c], iou_thr);
+                                           });
     for (int t = tid; t < nk; t += kXThreads) {
-      const int r = (int)S.keeplist[t];
+      const int r = (int)S.g.keep[t];
       const int o = kept_n + t;
-      kbox[o] = S.cbox[r];
-      karea[o] = S.carea[r];
-      kcls[o] = S.ccls[r];
-      knext[o] = atomicExch(&S.cls_head[S.ccls[r] & 1023], o);
-      const float* src = cb + (size_t)S.cidx[r] * 8;
+      kbox[o] = S.g.box[r];
+      karea[o] = S.g.area[r];
+      kcls[o] = S.g.cls[r];
+      knext[o] = atomicExch(&S.cls_head[S.g.cls[r] & 1023], o);
+      const float* src = cb + (size_t)S.g.payload[r] * 8;
       float* d = dout + (size_t)o * 7;
 #pragma unroll
       for (int q = 0; q < 7; ++q) d[q] = __ldg(src + q);
@@ -1066,24 +943,8 @@ __global__ void __launch_bounds__(256) fcos_decode_kernel(const float* __restric
     const int b = (int)(row / npix);
     const int pix = (int)(row - (long long)b * npix);
     const float* c = cls + row * cls_pitch;
-    float best = -1.0f;
-    int bi = 0x7fffffff;
-    for (int k = lane; k < nc; k += 32) {
-      const float p = sigmoid_fast(__ldg(c + k));
-      if (p > best) {
-        best = p;
-        bi = k;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ob > best || (ob == best && oi < bi)) {
-        best = ob;
-        bi = oi;
-      }
-    }
+    float best;
+    const int bi = warp_argmax_first(nc, [&](int k) { return sigmoid_fast(__ldg(c + k)); }, best);
     if (lane == 0) {
       const float* r = rc + row * rc_pitch;
       const float cnt = sigmoid_fast(__ldg(r + 4));
@@ -1106,17 +967,16 @@ constexpr int kFcosSel = 4096;  // candidates sorted in shared memory (top-k <= 
 
 struct FcosSmem {
   uint64_t keys[kFcosSel];                 // 32 KB
-  uint32_t hist[kBins];                    // 64 KB; reused as the suppression mask [512][16] after selection
+  union {
+    uint32_t hist[kBins];                  // 64 KB, top-k selection
+    GreedyChunk<kFcosThreads> g;           // greedy scan, after the selection; payload = sorted key position
+  };
   float4 kbox[2048];                       // kept (class-offset) boxes, 32 KB
   float karea[2048];
-  float4 cbox[kFcosThreads];
-  float carea[kFcosThreads];
-  uint32_t cidx[kFcosThreads];
-  uint32_t keeplist[kFcosThreads];
+  uint32_t seg[kBins / 32];
   uint32_t warp_cnt[kFcosThreads / 32];
   float red[kFcosThreads / 32];
-  uint32_t n_sel, tbin, m_alive, new_kept, overflow;
-  float maxc;
+  uint32_t n_sel, tbin, overflow;
 };
 
 // FCOS IoU: '+1' areas, plain intersection, box j is KEPT iff iou <= thr evaluated in float32 (fcos_detect.py:117,133-135)
@@ -1145,76 +1005,39 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
   for (int i = tid; i < kBins; i += kFcosThreads) S.hist[i] = 0;
   if (tid == 0) {
     S.n_sel = 0;
-    S.tbin = 0;
     S.overflow = 0;
   }
   __syncthreads();
   for (int i = tid; i < N; i += kFcosThreads) {
     const float v = sc[i];
-    if (v >= 0.0f) atomicAdd(&S.hist[min(__float_as_uint(v) >> 17, (uint32_t)(kBins - 1))], 1u);  // NaN / negative never selected
+    if (v >= 0.0f) atomicAdd(&S.hist[nms_score_bin(v)], 1u);  // NaN / negative never selected
   }
   __syncthreads();
-  if (warp == 0) {  // walk the bins top-down, 32 at a time
-    uint32_t run = 0;
-    for (int base = kBins - 32; base >= 0; base -= 32) {
-      const uint32_t v = S.hist[base + (31 - lane)];  // lane 0 = highest bin of the group
-      uint32_t inc = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-      }
-      const uint32_t hit = __ballot_sync(0xffffffffu, run + inc >= (uint32_t)topk);
-      if (hit) {
-        const int l = __ffs(hit) - 1;
-        if (lane == 0) S.tbin = (uint32_t)(base + (31 - l));
-        break;
-      }
-      run += __shfl_sync(0xffffffffu, inc, 31);
-    }
-  }
+  top_bin_search<kFcosThreads>(S.hist, (uint32_t)topk, S.seg, &S.tbin, nullptr);
   __syncthreads();
   const uint32_t tb = S.tbin;
   for (int i0 = 0; i0 < N; i0 += kFcosThreads) {
     const int i = i0 + tid;
-    bool pass = false;
-    uint32_t bits = 0;
-    if (i < N) {
-      const float v = sc[i];
-      bits = __float_as_uint(v);
-      pass = (v >= 0.0f) && (min(bits >> 17, (uint32_t)(kBins - 1)) >= tb);
-    }
-    const uint32_t m = __ballot_sync(0xffffffffu, pass);
-    if (m) {
-      uint32_t base = 0;
-      if (lane == 0) base = atomicAdd(&S.n_sel, (uint32_t)__popc(m));
-      base = __shfl_sync(0xffffffffu, base, 0);
-      if (pass) {
-        const uint32_t pos = base + __popc(m & ((1u << lane) - 1));
-        if (pos < (uint32_t)kFcosSel) S.keys[pos] = ((uint64_t)bits << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)i);
-        else S.overflow = 1;
-      }
+    const float v = (i < N) ? sc[i] : 0.0f;
+    const bool pass = i < N && v >= 0.0f && nms_score_bin(v) >= tb;
+    const uint32_t pos = warp_append(&S.n_sel, pass);
+    if (pass) {
+      if (pos < (uint32_t)kFcosSel) S.keys[pos] = make_key(__float_as_uint(v), (uint32_t)i);
+      else S.overflow = 1;
     }
   }
   __syncthreads();
   uint32_t nsel = min(S.n_sel, (uint32_t)kFcosSel);
   if (S.overflow && status && tid == 0) atomicExch(&status[0], 1);
   for (int i = nsel + tid; i < kFcosSel; i += kFcosThreads) S.keys[i] = 0ull;
-  for (int k = 2; k <= kFcosSel; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      __syncthreads();
-      for (int t = tid; t < kFcosSel / 2; t += kFcosThreads) {
-        const int i = 2 * j * (t / j) + (t % j);
-        cmpswap(S.keys, i, i + j, (i & k) == 0);
-      }
-    }
+  bitonic_tile(S.keys, kFcosSel, 0, 2, kFcosSel);
   __syncthreads();
   // candidates = sorted prefix of length min(topk, nsel) with score >= score_thres (fcos_detect.py:65-67,92-93)
   int ncand = min((int)nsel, topk);
   {
     // scores are sorted descending: count the prefix that passes the threshold
     int cntp = 0;
-    for (int i = tid; i < ncand; i += kFcosThreads) cntp += (__uint_as_float((uint32_t)(S.keys[i] >> 32)) >= score_thres) ? 1 : 0;
+    for (int i = tid; i < ncand; i += kFcosThreads) cntp += (key_score(S.keys[i]) >= score_thres) ? 1 : 0;
     for (int o = 16; o > 0; o >>= 1) cntp += __shfl_xor_sync(0xffffffffu, cntp, o);
     if (lane == 0) S.warp_cnt[warp] = (uint32_t)cntp;
     __syncthreads();
@@ -1226,21 +1049,10 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
   // ---- 2. class offset = cls * (max coordinate of the candidate boxes + 1)   (batched_nms :141-153)
   float mx = -3.402823466e38f;
   for (int i = tid; i < ncand; i += kFcosThreads) {
-    const uint32_t loc = 0xFFFFFFFFu - (uint32_t)(S.keys[i] & 0xFFFFFFFFull);
-    const float4 q = bx[loc];
+    const float4 q = bx[key_id(S.keys[i])];
     mx = fmaxf(mx, fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)));
   }
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if (lane == 0) S.red[warp] = mx;
-  __syncthreads();
-  if (tid == 0) {
-    float m2 = S.red[0];
-    for (int i = 1; i < kFcosThreads / 32; ++i) m2 = fmaxf(m2, S.red[i]);
-    S.maxc = __fadd_rn(m2, 1.0f);
-  }
-  __syncthreads();
-  const float offmul = S.maxc;
-  uint32_t (*mask)[kFcosThreads / 32] = reinterpret_cast<uint32_t (*)[kFcosThreads / 32]>(S.hist);
+  const float offmul = __fadd_rn(block_max<kFcosThreads>(mx, S.red), 1.0f);
 
   // ---- 3. greedy NMS over the candidates in score order (chunks of 512, like the YOLO kernel)
   int kept_n = 0;
@@ -1249,9 +1061,8 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
     bool alive = i < ncand;
     float4 box = make_float4(0, 0, 0, 0);
     float area = 0.0f;
-    uint32_t loc = 0;
     if (alive) {
-      loc = 0xFFFFFFFFu - (uint32_t)(S.keys[i] & 0xFFFFFFFFull);
+      const uint32_t loc = key_id(S.keys[i]);
       const float4 q = bx[loc];
       const float off = __fmul_rn((float)cl[loc], offmul);
       box = make_float4(__fadd_rn(q.x, off), __fadd_rn(q.y, off), __fadd_rn(q.z, off), __fadd_rn(q.w, off));
@@ -1262,65 +1073,18 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
           break;
         }
     }
-    const uint32_t bal = __ballot_sync(0xffffffffu, alive);
-    if (lane == 0) S.warp_cnt[warp] = __popc(bal);
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t v = (lane < kFcosThreads / 32) ? S.warp_cnt[lane] : 0;
-      uint32_t inc = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-      }
-      if (lane < kFcosThreads / 32) S.warp_cnt[lane] = inc - v;
-      if (lane == 31) S.m_alive = inc;
-    }
-    __syncthreads();
-    const int m = (int)S.m_alive;
-    if (alive) {
-      const int pos = (int)S.warp_cnt[warp] + __popc(bal & ((1u << lane) - 1));
-      S.cbox[pos] = box;
-      S.carea[pos] = area;
-      S.cidx[pos] = (uint32_t)i;
-    }
-    __syncthreads();
-    const int words = (m + 31) >> 5;
-    if (tid < m) {
-      const float4 me = S.cbox[tid];
-      const float ma = S.carea[tid];
-      for (int wd = 0; wd < words; ++wd) {
-        uint32_t bits = 0;
-        const int c0 = wd << 5, c1 = min(m, c0 + 32);
-        for (int c = max(c0, tid + 1); c < c1; ++c)
-          if (fcos_suppressed(me, ma, S.cbox[c], S.carea[c], iou_thres)) bits |= 1u << (c & 31);
-        mask[tid][wd] = bits;
-      }
-    }
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t removed = 0;
-      int nk = 0;
-      for (int r = 0; r < m; ++r) {
-        const uint32_t rw = __shfl_sync(0xffffffffu, removed, r >> 5);
-        if (!((rw >> (r & 31)) & 1u)) {
-          if (lane == 0) S.keeplist[nk] = (uint32_t)r;
-          ++nk;
-          if (lane < words) removed |= mask[r][lane];
-        }
-      }
-      if (lane == 0) S.new_kept = (uint32_t)nk;
-    }
-    __syncthreads();
-    const int nk = (int)S.new_kept;
+    const int nk = greedy_chunk<kFcosThreads>(S.g, alive, box, area, 0, (uint32_t)i, kFcosThreads,
+                                              [&](int r, int c) {
+                                                return fcos_suppressed(S.g.box[r], S.g.area[r], S.g.box[c], S.g.area[c], iou_thres);
+                                              });
     for (int t = tid; t < nk; t += kFcosThreads) {
-      const int r = (int)S.keeplist[t];
+      const int r = (int)S.g.keep[t];
       const int o = kept_n + t;
-      S.kbox[o] = S.cbox[r];
-      S.karea[o] = S.carea[r];
-      const uint64_t key = S.keys[S.cidx[r]];
-      const uint32_t l2 = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);
-      out_scores[(size_t)b * topk + o] = __uint_as_float((uint32_t)(key >> 32));
+      S.kbox[o] = S.g.box[r];
+      S.karea[o] = S.g.area[r];
+      const uint64_t key = S.keys[S.g.payload[r]];
+      const uint32_t l2 = key_id(key);
+      out_scores[(size_t)b * topk + o] = key_score(key);
       out_classes[(size_t)b * topk + o] = cl[l2];
       reinterpret_cast<float4*>(out_boxes)[(size_t)b * topk + o] = bx[l2];
       out_loc[(size_t)b * topk + o] = (int)l2;

@@ -63,6 +63,22 @@ def test_nms_other_thresholds(cuda):
     _nms_case(pred, conf=0.05, iou=0.7, multi_label=True, max_det=100)
 
 
+def test_nms_full_path_with_global_sort_steps(cuda):
+    """Image 0: 10 000 copies of one box with distinct scores above a 20 x 20 grid of disjoint boxes.  The top ~3k candidates keep
+    one box, so the image takes the full top-max_nms path, and its 10 400 candidates (> 2 x 4096) need the sort's grid-wide
+    steps.  Image 1 holds the grid only and is finished by the top ~3k candidates."""
+    pred = np.zeros((2, 10400, 85), np.float32)
+    pred[0, :10000, :5] = [320, 320, 100, 100, 1.0]
+    pred[0, :10000, 5] = np.linspace(0.5, 0.9, 10000, dtype=np.float32)
+    gy, gx = np.divmod(np.arange(400), 20)
+    pred[:, 10000:, 0] = 16 + 32 * gx
+    pred[:, 10000:, 1] = 16 + 32 * gy
+    pred[:, 10000:, 2:4] = 20
+    pred[:, 10000:, 4] = 1.0
+    pred[:, 10000:, 6] = np.linspace(0.1, 0.4, 400, dtype=np.float32)
+    _nms_case(pred)
+
+
 def test_decode_matches_reference_formula(cuda):
     from cvpytorch_b200 import ops
     from oracle import yolov5_oracle as YO
