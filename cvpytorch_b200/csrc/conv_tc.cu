@@ -150,7 +150,7 @@ struct alignas(64) ConvKArgs {
   unsigned int* y_hist;        // NMS workspace histogram [B][kNmsBins] (or NULL)
   float* y_rowmax;             // NMS workspace per-row best score [B][y_zrows] (or NULL)
   uint32_t wait_hint;          // suspend-time hint (ns) of the producer's free-slot waits (CVB_WAIT_HINT, 0 = spin)
-  int dbg;                     // diagnostics (CVB_DBG, results are WRONG): bit 0 = no TMA stores, bit 1 = activations loaded only for the first ring pass, bit 2 = epilogue skips the math / staging, bit 5 = fused decode without histogram atomics, bit 6 = without the z copy-out
+  int dbg;                     // diagnostics (CVB_DBG, results are WRONG): bit 0 = no TMA stores, bit 1 = activations loaded only for the first ring pass, bit 2 = epilogue skips the math / staging, bit 5 = fused decode without histogram atomics, bit 6 = without the z copy-out, bits 10 / 11 = classic loader streams weight tiles on every other ring fill / the first ring pass only
   long long* prof;             // diagnostics (cvb_conv_plan_set_profile): per-CTA cycle counters of the three pipeline roles, or NULL
   SmemLayout sm;
 };
@@ -296,8 +296,8 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
       (b_res != smem + a.sm.weights || out_stage0 != smem + a.sm.out || res_stage != smem + a.sm.resid ||
        reinterpret_cast<uint8_t*>(acc_s) != smem + a.sm.acc || reinterpret_cast<uint8_t*>(bias_s) != smem + a.sm.bias ||
        reinterpret_cast<uint8_t*>(bars) != smem + a.sm.bars || stage_bytes != a.sm.slot)) {
-    printf("conv_tc_kernel: shared-memory regions differ from the plan's layout\n");
-    __trap();
+    // (no printf here: its call makes ptxas serialize every wgmma of the diagnostics build, which then times a different main loop)
+    __trap();  // shared-memory regions differ from the plan's layout
   }
   const int SB = halo ? a.sb_stages : 0;
   uint64_t* full = bars;
@@ -409,20 +409,23 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
           }
         }
       } else
-      for (int tile = t_begin; tile < t_end; tile += t_step) {
+      for (int tile = t_begin, fill = 0; tile < t_end; tile += t_step) {
         const TileOrigin to = tile_origin<BLOCK_N>(a, tile);
         const int w0 = to.w0, h0 = to.h0, b0 = to.b0, n0 = to.n0;
         for (int tap = 0; tap < a.taps; ++tap) {
           const CUtensorMap* mapA = &a.tmA[a.tap_map[tap]];
           const int cw = w0 + a.tap_dw[tap];
           const int ch = h0 + a.tap_dh[tap];
-          for (int ck = 0; ck < a.chunks; ++ck) {
+          for (int ck = 0; ck < a.chunks; ++ck, ++fill) {
             CVB_PROF_WAIT(0, mbar_wait(&empty[stage], phase ^ 1, 100 + stage, a.wait_hint));
-            mbar_expect_tx(&full[stage], tx_bytes);
+            // diagnostics: streamed weight tiles on every other ring fill only (bit 10: half the weight traffic from L2), or on the
+            // first ring pass only (bit 11); the other fills reuse whatever the slot holds
+            const bool cut_b = kDiag && !a.b_resident && (((dbg & 1024) && (fill & 1)) || ((dbg & 2048) && fill >= STAGES));
+            mbar_expect_tx(&full[stage], cut_b ? 2 * a.a_box_bytes : tx_bytes);
             uint8_t* sb = stage_base + stage * stage_bytes;
             tma_load_5d(mapA, &full[stage], sb, ck * BLOCK_K, cw, ch, b0, 0);  // fused: both planes in one box
             if (!a.a_fused) tma_load_5d(mapA, &full[stage], sb + A_BYTES, ck * BLOCK_K, cw, ch, b0, 1);
-            if (!a.b_resident) {
+            if (!a.b_resident && !cut_b) {
               const int kc = tap * a.cin + ck * BLOCK_K;
               tma_load_3d(&a.tmB, &full[stage], sb + 2 * A_BYTES, kc, n0, 0);  // box {K, N, 2 planes}: hi then lo
             }
@@ -563,7 +566,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
         const uint32_t wg16 = PP ? 0u : (uint32_t)wg * (4u * SWZ);  // rows 64*wg..: eight 8-row groups of 8 * SWZ bytes
         uint32_t bres_it16 = bres16;
         for (int i = 0; i < k_iters; ++i, bres_it16 += 2u * kB16) {
-          mbar_wait(&full[stage], phase, 300 + stage);
+          CVB_PROF_WAIT(5, mbar_wait(&full[stage], phase, 300 + stage));
           const uint32_t b16 = resident ? bres_it16 : a_ring16 + ((2u * A_BYTES) >> 4);
           wgmma_fence();
           issue_tap<BLOCK_N, KSTEPS, SPLIT>(dm, dc, a_ring16 + wg16, lo16, kHiStd, b16, kB16, kHiStd, ksteps);
@@ -1021,11 +1024,12 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
       if (q == 0 && lane == 0) tma_store_wait_all0();  // thread 0 of each decode group: its bulk stores
     }
     if (tid_e == 0) tma_store_wait_all0();
-    if (prof_on && tid_e == 0) {  // epilogue: total cycles, MMA main loop, staging waits, conversion, barrier, store issue
+    if (prof_on && tid_e == 0) {  // epilogue: total cycles, MMA main loop, staging waits, conversion, barrier, store issue, and (classic
+                                  // loader) the main loop's waits on the ring's full barriers
       long long* pr = a.prof + ((size_t)(PP ? wg : 0) * gridDim.x + blockIdx.x) * 16;  // ping-pong: one counter row per warpgroup
       pr[8] = clock64() - prof_t0;
       pr[9] = prof_acc[0];
-      for (int i = 1; i < 5; ++i) pr[9 + i] = prof_acc[i];
+      for (int i = 1; i < 6; ++i) pr[9 + i] = prof_acc[i];
     }
   }
 }
@@ -1291,14 +1295,14 @@ static int choose_block(const ConvProblem& P, int* bn_out, int* bk_out) {
     bk = 32;   // the 64 KB NMS histogram + 44 KB staging tile leave room for three 32 KB stages
   } else {
     static const int bk_small = [] {
-      const char* e = getenv("CVB_BK_SMALLN");  // tuning knob: K chunk of the block_n <= 64 kernels for 64-channel inputs (default 32)
+      const char* e = getenv("CVB_BK_SMALLN");  // A/B knob: K chunk of the block_n <= 64 kernels for 64-channel inputs (default: full)
       const int v = e ? atoi(e) : 0;
-      return (v == 16 || v == 32 || v == 64) ? v : 32;
+      return (v == 16 || v == 32 || v == 64) ? v : 0;
     }();
-    // 64-channel inputs into narrow cooperative tiles (1x1 convs and the row-window stems): half-size K chunks shrink the ring
-    // stages, so that more of these plans fit two CTAs per SM (see plan_ring below); ping-pong plans go back to full chunks.
-    // Multi-tap 3x3 layers keep 64-wide chunks: measured slower with twice the TMA operations.
-    if (bn <= 64 && (cin == 64 || (cin == 128 && cout > 64)) && (d->kh * d->kw == 1 || P.win > 0)) bk = bk_small;
+    // 64-channel inputs into narrow tiles (1x1 convs and the row-window stems) keep the full 64-wide K chunk.  Half-size chunks shrink
+    // the ring stages so that more of these plans fit two CTAs per SM, but on the H100 the YOLOv5-s step measured 0.3 ms faster with
+    // full chunks (14.06-14.12 vs 14.40-14.41 ms, DESIGN.md 6).  CVB_BK_SMALLN=32 restores the half-size chunks.
+    if (bk_small && bn <= 64 && (cin == 64 || (cin == 128 && cout > 64)) && (d->kh * d->kw == 1 || P.win > 0)) bk = bk_small;
   }
   *bn_out = bn;
   *bk_out = bk;
