@@ -1098,6 +1098,7 @@ struct CvbConvPlan {
   int smem;
   int threads;
   int schedule;  // CVB_SCHED_COOPERATIVE or CVB_SCHED_PINGPONG
+  int epi;       // compile-time epilogue specialisation of fn (0 = generic, see fill_epilogue)
 };
 
 namespace cvb {
@@ -1838,7 +1839,7 @@ static int encode_maps(const ConvProblem& P, int bn, const SchedPlan& S, const H
 }
 
 // ---- epilogue operands, fused-decode arguments, accumulation gain; returns the kernel (compile-time epilogue specialisation)
-static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& S, ConvKArgs& a) {
+static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& S, ConvKArgs& a, int* epi_out) {
   const CvbConvDesc* d = &P.d;
   if (d->residual.base) {
     const CvbView& r = d->residual;
@@ -1897,7 +1898,18 @@ static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& 
     }
   }
   const void* fn = epi ? lookup_kernel(bn, S.bk, P.f32, false, epi, S.pp) : nullptr;
+  *epi_out = fn ? epi : 0;
   return fn ? fn : lookup_kernel(bn, S.bk, P.f32, P.yolo, 0, S.pp);
+}
+
+// programmatic dependent launch (prologue of conv N+1 overlapping the tail of conv N): measured neutral on the YOLOv5-s step (6.57 vs
+// 6.55 ms; the persistent grids leave no idle SMs to overlap into), so it stays opt-in: CVB_PDL=1
+static bool pdl_on() {
+  static const bool on = [] {
+    const char* e = getenv("CVB_PDL");
+    return e && atoi(e) == 1;
+  }();
+  return on;
 }
 
 // ---- diagnostics switches and the persistent launch grid
@@ -1942,9 +1954,10 @@ static int set_launch(const ConvProblem& P, int bn, const SchedPlan& S, CvbConvP
   static const bool dbg = [] { const char* e = getenv("CVB_PLAN_DEBUG"); return e && atoi(e) != 0; }();
   if (dbg)
     fprintf(stderr, "[cvb plan] cin=%d cout=%d k=%dx%d s=%d out=%dx%dx%d bn=%d bk=%d stages=%d resident=%d out_bufs=%d ctas/sm=%d "
-            "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s\n", P.cin, P.cout, P.d.kh, P.d.kw,
-            P.d.stride, P.d.out.B, P.Ho, P.Wo, bn, S.bk, a.stages, a.b_resident, a.out_bufs, S.ctas, p->smem, p->grid, total, a.resid_tma,
-            a.halo, a.n_copies, a.sb_stages, a.halo ? (unsigned)a.sm.slot : 0u, a.kskip, S.pp ? "pingpong" : "cooperative");
+            "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s epi=%d pdl=%d\n", P.cin, P.cout,
+            P.d.kh, P.d.kw, P.d.stride, P.d.out.B, P.Ho, P.Wo, bn, S.bk, a.stages, a.b_resident, a.out_bufs, S.ctas, p->smem, p->grid, total,
+            a.resid_tma, a.halo, a.n_copies, a.sb_stages, a.halo ? (unsigned)a.sm.slot : 0u, a.kskip, S.pp ? "pingpong" : "cooperative",
+            p->epi, (int)pdl_on());
   return CVB_OK;
 }
 
@@ -1971,7 +1984,7 @@ extern "C" int cvb_conv_plan_create(const CvbConvDesc* desc, CvbConvPlan** out_p
   fill_tiles(P, taps, bn, S, halo, p->args);
   rc = encode_maps(P, bn, S, halo, p->args);
   if (rc != CVB_OK) return rc;
-  p->fn = fill_epilogue(P, bn, S, p->args);
+  p->fn = fill_epilogue(P, bn, S, p->args, &p->epi);
   rc = set_launch(P, bn, S, p.get());
   if (rc != CVB_OK) return rc;
   *out_plan = p.release();
@@ -1982,12 +1995,7 @@ extern "C" int cvb_conv_plan_run(const CvbConvPlan* p, void* stream) {
   using namespace cvb;
   CVB_REQUIRE(p != nullptr, "null plan");
   void* kargs[1] = {const_cast<ConvKArgs*>(&p->args)};
-  static const bool pdl = [] {
-    // programmatic dependent launch (prologue of conv N+1 overlapping the tail of conv N): measured neutral on the YOLOv5-s
-    // step (6.57 vs 6.55 ms; the persistent grids leave no idle SMs to overlap into), so it stays opt-in: CVB_PDL=1
-    const char* e = getenv("CVB_PDL");
-    return e && atoi(e) == 1;
-  }();
+  const bool pdl = pdl_on();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(p->grid);

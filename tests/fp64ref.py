@@ -1,4 +1,5 @@
-"""float64 references and an element-wise error bound for the training kernels (tests/test_train_gpu.py).
+"""float64 references and element-wise error bounds for the training kernels (tests/test_train_gpu.py) and for the split-fp16 inference
+conv (split_conv_reference below).
 
 Each reference is computed in float64 on exactly the bf16 values the kernel reads, together with the same operation on the absolute values
 of its inputs (`absref`).  absref bounds every partial sum of a dot product, so the fp32 accumulation error of one output element is at most
@@ -95,6 +96,101 @@ def wgrad_gamma(B, Ho, Wo, cin, cout, k, sms):
     """One CTA chains 8 MMAs (K = 16 pixels each) per tile it owns; `splits` CTAs then add their partial sums with fp32 atomics."""
     _, splits, per = wgrad_split(B, Ho, Wo, cin, cout, k, sms)
     return (8 * per + 16 + splits) * U23
+
+
+# ---------------------------------------------------------------------------------------------------- split-fp16 inference conv
+SPLIT_REL = 2.0 ** -19   # see split_conv_reference
+LAYER_BUDGET = 2e-5      # max|out - ref| / max|ref| of one layer (DESIGN.md 2)
+
+
+def split64(t):
+    """fp16 hi / lo planes [2, B, H, W, C] (a SplitTensor or its data, possibly a channel slice) -> float64 NCHW hi + lo."""
+    d = t if torch.is_tensor(t) else t.data
+    return (d[0].double() + d[1].double()).permute(0, 3, 1, 2)
+
+
+def conv_out64(d):
+    """The conv's output buffer (fp16 hi / lo planes [2, B, H, W, C] or fp32 [B, H, W, C]) -> float64 NCHW."""
+    return split64(d) if d.dtype == torch.float16 else d.double().permute(0, 3, 1, 2)
+
+
+def split_conv_reference(tin, wp, bp, k, s=1, p=0, dil=1, act='silu', residual=None, resid_first=0, resid_scale=1.0, up=None,
+                         w_window=0, block_n=128, cout=None, out_h=None):
+    """float64 reference of the fused conv kernel (csrc/conv_tc.cu) and the element-wise bound of its error -> (ref, bound), NCHW.
+
+    Computed on the GPU from exactly the values the kernel reads: hi + lo of the split input `tin` ([2, B, H, W, C] fp16, a channel slice
+    is fine) and of the packed weights `wp` ([2, cout_pad, K] from ops.pack_conv_weights), the fp32 bias `bp`, the split `residual`
+    ([2, B, Ho, Wo, cout]) times `resid_scale`, and the fp32 `up` partial ([B, ceil(Ho/2), ceil(Wo/2), cout], nearest x2).  absref is the
+    same conv on |x|, |w| plus |bias|, |up| (and |residual| when it enters before the activation): it bounds every partial sum.
+
+        |out - ref| <= 2^-19 (|ref| + |residual|) + slope * gamma * absref
+        gamma = mma_gamma(16 chain) + chain * 2^-25 + 2^-21
+
+    Each constant follows from the kernel's arithmetic:
+      chain   the MMAs (K = 16 each) chained into the hi*hi accumulator of one output element: taps * K_tap / 16.  It is also the
+              chain rz_gain = 1 + 1.9e-8 * chain is computed from; the gain's own correction is at most 2^-25 per MMA of the chain.
+        classic / halo loader, stride 2, dilation: taps = kh * kw, K_tap = cin.  The K order differs between loaders, not the chain.
+        row-window stems (w_window = win): taps = kh filter rows of K_tap = win * C, the all-zero weight columns included; the kernel
+              skips their MMAs (kskip) but rz_gain counts them, and counting them in gamma only loosens it.
+        block_n = 256: hi*hi and both cross terms share one register accumulator (no separate cross accumulator), so the chain is three
+              times as long: chain = 3 * taps * K_tap / 16.
+      mma_gamma  one fp32 ulp (2^-23: the tensor core's adder truncates) per chained MMA plus 16 for the additions inside one MMA.
+      2^-21   the dropped lo * lo products (|lo| <= 2^-11 |hi| on both operands) and the cross terms' own rounding.
+      slope   1.1 for SiLU (|silu'| <= 1.1), 1 for ReLU and for no activation: the accumulation error passes through the activation.
+      2^-19   the epilogue after the accumulator: the fast SiLU (~2^-22 relative), the fp32 additions of bias / up / residual and the
+              hi / lo split of the output (~22 bits), relative to the output and to the residual added after the activation.
+
+    w_window: out_h = the output height (default: the input height); filter row ky reads input row h + ky - p, rows past the input
+    read TMA zero fill, and the input already carries the left zero columns."""
+    x = split64(tin)
+    cout = wp.shape[1] if cout is None else cout
+    w = (wp[0].double() + wp[1].double())[:cout]
+    if w_window:
+        C = x.shape[1]
+        Ho = x.shape[2] if out_h is None else out_h
+        w = w.view(cout, k, w_window, C).permute(0, 3, 1, 2)
+        x = F.pad(x, (0, 0, p, max(0, Ho + k - 1 - p - x.shape[2])))[:, :, :Ho + k - 1]
+        taps, k_tap = k, w_window * C
+        ref, absref = F.conv2d(x, w), F.conv2d(x.abs(), w.abs())
+    else:
+        cin = x.shape[1]
+        w = w.view(cout, k, k, cin).permute(0, 3, 1, 2)
+        taps, k_tap = k * k, cin
+        ref, absref = F.conv2d(x, w, None, s, p, dil), F.conv2d(x.abs(), w.abs(), None, s, p, dil)
+    b = bp[:cout].double().view(1, -1, 1, 1)
+    ref, absref = ref + b, absref + b.abs()
+    Ho, Wo = ref.shape[2:]
+    if up is not None:
+        u = F.interpolate(up.double().permute(0, 3, 1, 2), scale_factor=2, mode='nearest')[:, :, :Ho, :Wo]
+        ref, absref = ref + u, absref + u.abs()
+    rsum = split64(residual) * resid_scale if residual is not None else torch.zeros_like(ref)
+    if resid_first:
+        ref, absref = ref + rsum, absref + rsum.abs()
+    if act == 'silu':
+        ref = F.silu(ref)
+    elif act == 'relu':
+        ref = F.relu(ref)
+    if residual is not None and not resid_first:
+        ref = ref + rsum
+    chain = (3 if block_n > 128 else 1) * taps * k_tap // 16
+    gamma = mma_gamma(16 * chain) + chain * 2.0 ** -25 + 2.0 ** -21
+    bound = SPLIT_REL * (ref.abs() + rsum.abs()) + (1.1 if act == 'silu' else 1.0) * gamma * absref + 1e-30
+    return ref, bound
+
+
+def max_rel(out, ref):
+    """max |out - ref| / max |ref| (NaN if out has a NaN)."""
+    out = out.double().to(ref.device)
+    return float((out - ref).abs().max() / ref.abs().max().clamp_min(1e-300))
+
+
+def check_conv(out, ref, bound, what):
+    """The two checks of a conv output against split_conv_reference: (a) element-wise bound, (b) max |out - ref| / max |ref| within the
+    single-layer budget.  (b) is the tighter one on deep-K layers, (a) on small outputs.  Returns max |out - ref| / bound."""
+    r = check(out, ref, bound, what)
+    e = max_rel(out, ref)
+    assert e < LAYER_BUDGET, f'{what}: max|out - ref| / max|ref| = {e:.3g} exceeds {LAYER_BUDGET}'
+    return r
 
 
 def check(out, ref, bound, what):

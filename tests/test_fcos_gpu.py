@@ -12,6 +12,9 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, 'tests', 'golden')
 sys.path.insert(0, os.path.join(ROOT, 'tools'))
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
+import fp64ref  # noqa: E402
+
 TOL = 1e-3
 
 
@@ -92,9 +95,12 @@ def test_resnet_stem_window_conv(cuda):
     ops.stem_s2d(x.cuda().contiguous(), t.view(), pad_left=2)
     wp, bp = ops.pack_conv_weights(ops.window_weights(resnet_stem_weights_to_s2d(w.double()), 4), b.double())
     out = ops.SplitTensor(B, H // 2, W // 2, 64)
+    out.data.fill_(float('nan'))
     ops.ConvPlan(t.view(), out.view(), wp, bp, 4, 1, 2, 1, 'relu', w_window=4).run()
     torch.cuda.synchronize()
     assert _rel(ops.split_to_nchw(out.view()), ref) < 2e-5
+    ref64, bound = fp64ref.split_conv_reference(t, wp, bp, 4, 1, 2, act='relu', w_window=4)
+    fp64ref.check_conv(fp64ref.conv_out64(out.data), ref64, bound, 'resnet stem 7x7/s2 as 4 window rows')
 
 
 def test_conv_residual_before_activation(cuda):
@@ -104,14 +110,15 @@ def test_conv_residual_before_activation(cuda):
     w = torch.randn(256, 64, 1, 1, generator=g) / 8
     b = torch.randn(256, generator=g)
     r = torch.randn(2, 256, 20, 20, generator=g)
-    ref = F.relu(F.conv2d(x.cuda(), w.cuda(), b.cuda()) + r.cuda())
     tin, tres, tout = ops.SplitTensor(2, 20, 20, 64), ops.SplitTensor(2, 20, 20, 256), ops.SplitTensor(2, 20, 20, 256)
     ops.nchw_to_split(x.cuda(), tin.view())
     ops.nchw_to_split(r.cuda(), tres.view())
+    tout.data.fill_(float('nan'))
     wp, bp = ops.pack_conv_weights(w.double(), b.double())
     ops.ConvPlan(tin.view(), tout.view(), wp, bp, 1, 1, 0, 1, 'relu', residual=tres.view(), residual_before_act=1).run()
     torch.cuda.synchronize()
-    assert _rel(ops.split_to_nchw(tout.view()), ref) < 2e-5
+    ref, bound = fp64ref.split_conv_reference(tin, wp, bp, 1, act='relu', residual=tres, resid_first=1)
+    fp64ref.check_conv(fp64ref.conv_out64(tout.data), ref, bound, 'conv 64->256 1x1 relu(conv + residual)')
 
 
 def test_fcos_forward_vs_reference_golden_128(model):
