@@ -14,7 +14,6 @@ residual_before_act; the 7x7/s2 stem runs as 4 filter rows over the space-to-dep
 (class-offset, '+1'-area) NMS run on device with fixed-capacity outputs.
 """
 import math
-from copy import deepcopy
 
 import numpy as np
 import torch
@@ -22,8 +21,7 @@ import torch.nn as nn
 
 from . import _lib, ops
 from .engine import GraphBuilder
-from .models import _GraphCache, _check_infer_input
-from .modules import folded
+from .modules import _build, _Standalone, folded
 
 
 # =============================================================================================== ResNet-50
@@ -97,7 +95,7 @@ def deep_stem_weights_to_s2d(w64):
     return out
 
 
-class ResNet(_GraphCache):
+class ResNet(_Standalone):
     def __init__(self, subtype='resnet50', out_stages=[2, 3, 4], output_stride=32, frozen_stages=-1, norm_eval=False, conv_cfg=None,
                  norm_cfg=dict(type='BN', requires_grad=True), classifier=False, num_classes=1000, backbone_path=None, pretrained=True):
         super().__init__()
@@ -159,23 +157,11 @@ class ResNet(_GraphCache):
         return outs
 
     def forward(self, x):
-        _check_infer_input(self, x)
-        B, _, H, W = x.shape
-        key = (B, H, W, x.device.index)
-        if key not in self._graphs:
-            g = GraphBuilder(B, x.device)
-            holder = {}
-            outs = self.emit(g, lambda: holder['x'], H, W)
-            self._graphs[key] = (g, holder, outs)
-        g, holder, outs = self._graphs[key]
-        holder['x'] = x.contiguous().float()
-        g.run()
-        res = [ops.split_to_nchw(o.view()) for o in outs]
-        return res if len(self.out_stages) > 1 else res[0]
+        return self._run_image(x)
 
 
 # =============================================================================================== FPN
-class FCOSFPN(_GraphCache):
+class FCOSFPN(_Standalone):
     def __init__(self, in_channels=[512, 1024, 2048], out_channels=256):
         super().__init__()
         self.prj_3 = nn.Conv2d(in_channels[0], out_channels, 1)
@@ -214,18 +200,7 @@ class FCOSFPN(_GraphCache):
         return [P3, P4, P5, P6, P7]
 
     def forward(self, x):
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x)
-        if key not in self._graphs:
-            g = GraphBuilder(x[0].shape[0], x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            outs = self.emit(g, ins)
-            self._graphs[key] = (g, ins, outs)
-        g, ins, outs = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
-        return [ops.split_to_nchw(o.view()) for o in outs]
+        return [ops.split_to_nchw(o.view()) for o in self._run(x)]
 
 
 # =============================================================================================== head
@@ -235,7 +210,7 @@ class ScaleExp(nn.Module):
         self.scale = nn.Parameter(torch.tensor([init_value], dtype=torch.float32))
 
 
-class FCOSHead(_GraphCache):
+class FCOSHead(_Standalone):
     def __init__(self, num_classes, in_channel, GN=True, cnt_on_reg=True, prior=0.01):
         super().__init__()
         if not GN or not cnt_on_reg or in_channel % 8 != 0 or in_channel // 32 != 8:
@@ -289,19 +264,8 @@ class FCOSHead(_GraphCache):
         return outs
 
     def forward(self, inputs):
-        _check_infer_input(self, inputs[0])
-        key = tuple(tuple(t.shape) for t in inputs)
-        if key not in self._graphs:
-            g = GraphBuilder(inputs[0].shape[0], inputs[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in inputs]
-            outs = self.emit(g, ins)
-            self._graphs[key] = (g, ins, outs)
-        g, ins, outs = self._graphs[key]
-        for t, v in zip(inputs, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
         cls_l, cnt_l, reg_l = [], [], []
-        for i, (cls, rc) in enumerate(outs):
+        for i, (cls, rc) in enumerate(self._run(inputs)):
             cls_l.append(ops.f32nhwc_to_nchw(cls.view(0, self.num_classes)))
             r = ops.f32nhwc_to_nchw(rc.view(0, 8))
             cnt_l.append(r[:, 4:5].contiguous())
@@ -341,14 +305,6 @@ _HEADS = {'FCOSHead': FCOSHead}
 _DETECTS = {'FCOSDetect': FCOSDetect}
 
 
-def _build(table, cfg):
-    c = deepcopy(dict(cfg))
-    name = c.pop('name')
-    if name not in table:
-        raise NotImplementedError(name)
-    return table[name](**c)
-
-
 def build_backbone(cfg):
     return _build(_BACKBONES, cfg)
 
@@ -365,7 +321,7 @@ def build_detect(cfg):
     return _build(_DETECTS, cfg)
 
 
-class FCOS(_GraphCache):
+class FCOS(_Standalone):
     """Model-level drop-in for src.models.fcos.FCOS (inference path)."""
 
     def __init__(self, dictionary=None, model_cfg=None):
@@ -398,17 +354,12 @@ class FCOS(_GraphCache):
         return dict(g=g, holder=holder, ws=ws, feats=feats, levels=levels, head=head_outs)
 
     def _graph_for(self, imgs):
-        B, _, H, W = imgs.shape
-        key = (B, H, W, imgs.device.index)
-        if key not in self._graphs:
-            self._graphs[key] = self.build_graph(B, H, W, imgs.device)
-        return self._graphs[key]
+        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device))
 
     def predict(self, imgs):
         """Device-only inference: (scores [B,K], classes [B,K] (1-based), boxes [B,K,4], loc [B,K], count [B]); no host sync.
         Graph-owned buffers (overwritten by the next call).  ``self._graph_for(imgs)['ws'].status[0] != 0`` flags a top-k
         capacity overflow of the last run; ``forward()`` checks it and raises."""
-        _check_infer_input(self, imgs)
         G = self._graph_for(imgs)
         G['holder']['x'] = imgs.contiguous().float()
         G['g'].run()

@@ -19,42 +19,11 @@ import torch.nn as nn
 
 from . import _lib, ops
 from .engine import GraphBuilder
-from .modules import ConvModule, CSPLayer, DownsamplingModule, SPPF, UpsamplingModule, folded
-
-
-def _check_infer_input(module, x):
-    if module.training:
-        raise RuntimeError(f'{type(module).__name__}: the H100 path implements inference only; call .eval() first '
-                           '(training stays on the reference implementation)')
-    if not (isinstance(x, torch.Tensor) and x.is_cuda):
-        raise _lib.CvbError(f'{type(module).__name__}: input must be a CUDA tensor; there is no CPU fallback')
-    if x.device.index != torch.cuda.current_device():
-        # one device per process (INTEGRATION.md): plans, graph buffers and kernel launches all use the CURRENT device
-        raise _lib.CvbError(f'{type(module).__name__}: input lives on cuda:{x.device.index} but the current device is '
-                            f'cuda:{torch.cuda.current_device()}; call torch.cuda.set_device() first (one device per process)')
-
-
-class _GraphCache(nn.Module):
-    """Caches one built graph per input shape; invalidated when weights change."""
-
-    def __init__(self):
-        super().__init__()
-        self._graphs = {}
-        self.register_load_state_dict_post_hook(lambda m, k: m.invalidate())
-
-    def invalidate(self):
-        self._graphs = {}
-        for m in self.children():
-            if isinstance(m, _GraphCache):
-                m.invalidate()
-
-    def train(self, mode=True):
-        self.invalidate()
-        return super().train(mode)
+from .modules import ConvModule, CSPLayer, DownsamplingModule, SPPF, UpsamplingModule, _build, _Standalone, folded
 
 
 # =============================================================================================== backbone
-class YOLOv5CSPDarknet(_GraphCache):
+class YOLOv5CSPDarknet(_Standalone):
     cfg = {"n": [0.33, 0.25], "t": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
 
     def __init__(self, subtype='cspdark_s', in_channels=3, out_channels=[64, 128, 256, 512, 1024], num_blocks=[3, 6, 9, 3],
@@ -112,23 +81,11 @@ class YOLOv5CSPDarknet(_GraphCache):
         return outs
 
     def forward(self, x):
-        _check_infer_input(self, x)
-        B, _, H, W = x.shape
-        key = (B, H, W, x.device.index)
-        if key not in self._graphs:
-            g = GraphBuilder(B, x.device)
-            holder = {}
-            outs = self.emit(g, lambda: holder['x'], H, W)
-            self._graphs[key] = (g, holder, outs)
-        g, holder, outs = self._graphs[key]
-        holder['x'] = x.contiguous().float()
-        g.run()
-        res = [ops.split_to_nchw(o.view()) for o in outs]
-        return res if len(self.out_stages) > 1 else res[0]
+        return self._run_image(x)
 
 
 # =============================================================================================== neck
-class YOLOv5Neck(_GraphCache):
+class YOLOv5Neck(_Standalone):
     def __init__(self, in_channels, out_channels, depth_mul=1.0, width_mul=1.0, **unused):
         super().__init__()
         assert isinstance(in_channels, list)
@@ -159,23 +116,11 @@ class YOLOv5Neck(_GraphCache):
 
     def forward(self, x):
         assert len(x) == len(self.in_channels)
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x) + (x[0].device.index,)
-        if key not in self._graphs:
-            B = x[0].shape[0]
-            g = GraphBuilder(B, x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            outs = self.emit(g, ins)
-            self._graphs[key] = (g, ins, outs)
-        g, ins, outs = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
-        return [ops.split_to_nchw(o.view()) for o in outs]
+        return [ops.split_to_nchw(o.view()) for o in self._run(x)]
 
 
 # =============================================================================================== detect
-class YOLOv5Detect(_GraphCache):
+class YOLOv5Detect(_Standalone):
     def __init__(self, num_classes=80, in_channels=[256, 512, 1024], stride=[8., 16., 32.], anchors=(), depth_mul=1.0, width_mul=1.0):
         super().__init__()
         in_channels = list(map(lambda x: int(x * width_mul), in_channels))
@@ -233,18 +178,7 @@ class YOLOv5Detect(_GraphCache):
         return z, (raws if want_raw else None)
 
     def forward(self, x):
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x) + (x[0].device.index,)
-        if key not in self._graphs:
-            B = x[0].shape[0]
-            g = GraphBuilder(B, x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            z, raws = self.emit(g, ins)
-            self._graphs[key] = (g, ins, z, raws)
-        g, ins, z, raws = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
+        z, raws = self._run(x)
         for i in range(len(x)):  # the reference replaces the list entries in place (yolov5_detect.py:42-44)
             x[i] = raws[i]
         return z, x
@@ -254,14 +188,6 @@ class YOLOv5Detect(_GraphCache):
 _BACKBONES = {'YOLOv5CSPDarknet': YOLOv5CSPDarknet, 'YOLOv5Backbone': YOLOv5CSPDarknet}
 _NECKS = {'YOLOv5Neck': YOLOv5Neck}
 _DETECTS = {'YOLOv5Detect': YOLOv5Detect}
-
-
-def _build(table, cfg):
-    c = deepcopy(dict(cfg))
-    name = c.pop('name')
-    if name not in table:
-        raise NotImplementedError(name)
-    return table[name](**c)
 
 
 def build_backbone(cfg):
@@ -305,7 +231,7 @@ def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=Non
     return out
 
 
-class YOLOv5(_GraphCache):
+class YOLOv5(_Standalone):
     """Model-level drop-in for src.models.yolov5.YOLOv5 (inference path).  forward(imgs, targets, mode) keeps the
     reference contract: mode 'val' -> (losses_dict, outputs list of {'boxes','labels','scores'})."""
     anchors = [[[1.25000, 1.62500], [2.00000, 3.75000], [4.12500, 2.87500]],
@@ -359,10 +285,8 @@ class YOLOv5(_GraphCache):
         B, H, W = (imgs.shape[0], imgs.shape[1], imgs.shape[2]) if u8 else (imgs.shape[0], imgs.shape[2], imgs.shape[3])
         # the thresholds are baked into the decode histogram / NMS steps of a graph: they are part of the key so that changing
         # model.conf_thres / iou_thres / max_det after the first forward takes effect (the reference reads them on every call, yolov5.py:262)
-        key = (B, H, W, imgs.device.index, want_raw, u8, float(self.conf_thres), float(self.iou_thres), int(self.max_det))
-        if key not in self._graphs:
-            self._graphs[key] = self.build_graph(B, H, W, imgs.device, want_raw, u8_input=u8)
-        return self._graphs[key]
+        return self._graph([imgs], lambda: self.build_graph(B, H, W, imgs.device, want_raw, u8_input=u8),
+                           want_raw, u8, float(self.conf_thres), float(self.iou_thres), int(self.max_det))
 
     def predict_frames(self, frames_u8):
         """Device-only inference on camera frames: uint8 CUDA tensor [B,H,W,3] (BGR, already letterboxed to the network size).
@@ -382,7 +306,6 @@ class YOLOv5(_GraphCache):
         The tensors are the GRAPH-OWNED output buffers (overwritten by the next call with the same shape).  ``nms_status(imgs)``
         returns the device status word of the last run ([0] != 0: the NMS candidate capacity overflowed and the result is invalid);
         ``forward()`` checks it and raises."""
-        _check_infer_input(self, imgs)
         G = self._graph_for(imgs)
         G['holder']['x'] = imgs.contiguous().float()
         G['g'].run()

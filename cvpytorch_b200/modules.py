@@ -13,10 +13,13 @@ Mirrors (paths relative to the reference checkout):
   UpsamplingModule, DownsamplingModule  src/models/modules/yolo11_modules.py:388-408
 """
 
+from copy import deepcopy
+
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import _lib, ops
+from .engine import GraphBuilder
 
 BN_EPS = 1e-3
 
@@ -49,39 +52,101 @@ class _EmitModule(nn.Module):
                            'backbone / neck / detect graph (call the parent module), not stand-alone')
 
 
-class _StandaloneBrick(_EmitModule):
-    """Brick-level drop-in (SURVEY.md 8b: ConvModule(conv_cfg=dict(type='B200Conv2d'), ...) inside an otherwise unchanged reference
-    model): called on its own, the brick runs as a one-layer graph with the layout adapters at its boundary -- NCHW fp32 in, NCHW fp32
-    out, like the reference's ConvModule.forward (conv_module.py:201-214).  Inside a H100 parent it is emitted into the parent's graph
-    and this method is never used.  Inference only; one cached plan per input shape (invalidated by load_state_dict / train())."""
+class _Standalone(nn.Module):
+    """Base of every drop-in that runs on its own (model, backbone, neck / head, brick, block): the module is built into a
+    GraphBuilder graph once per input and the graph is replayed on later calls.
 
-    def forward(self, x):
-        from .engine import GraphBuilder
-        if self.training:
-            raise RuntimeError(f'{type(self).__name__} (H100): inference only; call .eval() first')
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 4):
-            raise ops._lib.CvbError(f'{type(self).__name__}: input must be a CUDA tensor [B,C,H,W]; there is no CPU fallback')
-        cache = self.__dict__.setdefault('_brick_graphs', {})
-        key = (tuple(x.shape), x.device.index)
-        if key not in cache:
-            B, C, H, W = x.shape
-            g = GraphBuilder(B, x.device)
-            cpad = (C + 15) // 16 * 16  # the tensor-core path wants cin % 16 == 0: zero channels are free
-            xin = g.new_act(H, W, cpad)
-            out = self._emit_padded(g, xin, C, cpad)
-            cache[key] = (g, xin, out)
-        g, xin, out = cache[key]
-        ops.nchw_to_split(x, xin.tensor.view(0, x.shape[1]))  # the padding channels of the zero-initialised buffer stay zero
-        g.run()
-        return ops.split_to_nchw(out.view())
+    ``_graph`` is the only way to that cache.  It rejects what the graph cannot run -- training mode (RuntimeError), and any input
+    that is not a 4-D CUDA tensor on the current device (CvbError: plans, buffers and TMA descriptors belong to the device a graph
+    was built on, INTEGRATION.md §4) -- before it looks anything up.  A graph is keyed by the input shapes, the device and the
+    caller's extra key.  The weights are folded into the plans when a graph is built, so ``load_state_dict``, ``train()`` /
+    ``eval()`` and ``RepVGGBlock.switch_to_deploy`` drop every graph of the module; weights changed any other way (in place, or
+    by ``switch_to_deploy`` of a block inside a module that has run) take effect after the next ``eval()``.  Inference only: there
+    is no CPU fallback."""
+
+    def __init__(self):
+        super().__init__()
+        self._graphs = {}
+
+    def _drop_graphs(self):
+        self._graphs.clear()
 
     def train(self, mode=True):
-        self.__dict__['_brick_graphs'] = {}
+        self._drop_graphs()
         return super().train(mode)
 
     def _load_from_state_dict(self, *a, **k):
-        self.__dict__['_brick_graphs'] = {}
+        self._drop_graphs()
         return super()._load_from_state_dict(*a, **k)
+
+    def _graph(self, xs, build, *key):
+        """The graph ``build()`` returned for inputs ``xs`` (a list of tensors), built on the first call with these shapes."""
+        name = type(self).__name__
+        if self.training:
+            raise RuntimeError(f'{name}: the H100 path implements inference only; call .eval() first '
+                               '(training stays on the reference implementation)')
+        for x in xs:
+            if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 4):
+                raise _lib.CvbError(f'{name}: every input must be a 4-D CUDA tensor; there is no CPU fallback')
+            if x.device.index != torch.cuda.current_device():
+                raise _lib.CvbError(f'{name}: input lives on cuda:{x.device.index} but the current device is '
+                                    f'cuda:{torch.cuda.current_device()}; call torch.cuda.set_device() first (one device per process)')
+        key = tuple(tuple(x.shape) for x in xs) + (xs[0].device.index,) + key
+        if key not in self._graphs:
+            self._graphs[key] = build()
+        return self._graphs[key]
+
+    def _run(self, xs, emit=None, cin_align=1):
+        """Runs ``emit(g, ins)`` (default ``self.emit``) on the NCHW fp32 maps ``xs`` and returns what it returned.  ``ins`` are
+        split-NHWC input buffers with the channels of ``xs`` rounded up to a multiple of ``cin_align``; the extra channels stay zero."""
+        def build():
+            g = GraphBuilder(xs[0].shape[0], xs[0].device)
+            ins = [g.new_act(x.shape[2], x.shape[3], (x.shape[1] + cin_align - 1) // cin_align * cin_align) for x in xs]
+            return g, ins, (emit or self.emit)(g, ins)
+        g, ins, outs = self._graph(xs, build)
+        for x, v in zip(xs, ins):
+            ops.nchw_to_split(x, v.slice(0, x.shape[1]).view())
+        g.run()
+        return outs
+
+    def _run_image(self, x):
+        """``forward`` of the image backbones: NCHW fp32 images -> the NCHW fp32 maps of ``out_stages`` (the map itself when there
+        is one stage), from ``self.emit(g, image_getter, H, W)``."""
+        def build():
+            g, holder = GraphBuilder(x.shape[0], x.device), {}
+            return g, holder, self.emit(g, lambda: holder['x'], x.shape[2], x.shape[3])
+        g, holder, outs = self._graph([x], build)
+        holder['x'] = x.contiguous().float()
+        g.run()
+        res = [ops.split_to_nchw(o.view()) for o in outs]
+        return res if len(self.out_stages) > 1 else res[0]
+
+
+def _build(table, cfg):
+    """Reference factory contract (src/models/{backbones,necks,heads,detects}/__init__.py): deepcopy the cfg, pop 'name',
+    Class(**cfg); an unknown name raises NotImplementedError."""
+    c = deepcopy(dict(cfg))
+    name = c.pop('name')
+    if name not in table:
+        raise NotImplementedError(name)
+    return table[name](**c)
+
+
+def _pad_cin(w, n):
+    """[O,I,k,k] weights with n zero input channels appended."""
+    return nn.functional.pad(w, (0, 0, 0, 0, 0, n))
+
+
+class _StandaloneBrick(_Standalone):
+    """Brick-level drop-in (SURVEY.md 8b: ConvModule(conv_cfg=dict(type='B200Conv2d'), ...) inside an otherwise unchanged reference
+    model): called on its own, the brick runs as a one-layer graph with the layout adapters at its boundary -- NCHW fp32 in, NCHW fp32
+    out, like the reference's ConvModule.forward (conv_module.py:201-214).  Inside a H100 parent it is emitted into the parent's graph
+    and this method is never used."""
+
+    def forward(self, x):
+        # the tensor-core path wants cin % 16 == 0: the input buffer gets zero channels up to it, read with zero weights.  The pad is
+        # counted from the input's own channels, so an input whose channel count is not the brick's fails the conv's channel check.
+        return ops.split_to_nchw(self._run([x], lambda g, ins: self._emit_padded(g, ins[0], x.shape[1]), cin_align=16).view())
 
 
 class ConvModule(_StandaloneBrick):
@@ -112,18 +177,18 @@ class ConvModule(_StandaloneBrick):
         self.act_name = _act_name(act_cfg)
         nn.init.kaiming_normal_(self.conv.weight, a=0, mode='fan_out', nonlinearity='relu')  # conv_module.py:181-199
 
-    def _emit_padded(self, g, xin, cin, cpad):
-        if self.groups != 1 or cpad == cin:
-            return self.emit(g, xin if cpad == cin else xin.slice(0, cin))
+    def _emit_padded(self, g, x, cin):
+        if self.groups != 1:
+            return self.emit(g, x.slice(0, cin))
         w, b = folded(self.conv, self.bn if self.with_norm else None)
-        w = torch.cat([w, torch.zeros((w.shape[0], cpad - cin) + tuple(w.shape[2:]), dtype=w.dtype)], 1)
-        return g.conv(xin, w, b, self.kernel_size, self.stride, self.padding, self.act_name, dilation=self.dilation)
+        return g.conv(x, _pad_cin(w, x.c - cin), b, self.kernel_size, self.stride, self.padding, self.act_name, dilation=self.dilation)
 
     def emit(self, g, x, name='', **kw):
         w, b = folded(self.conv, self.bn if self.with_norm else None)
         if self.groups != 1:  # depthwise: HBM-bound SIMT kernel (no tensor cores for 9 MACs per output)
             if self.act_name not in (None, 'relu'):
                 raise NotImplementedError('depthwise conv: ReLU / no activation only')
+            assert w.shape[0] == x.c, (name, w.shape[0], x.c)  # the kernel reads one weight column per input channel
             out = kw.get('out') or g.new_act(x.H, x.W, x.c)
             w9c, bias = ops.pack_dw_weights(w, b, device=g.device)
             g.buffers.append((w9c, bias))
@@ -167,11 +232,9 @@ class Conv(_StandaloneBrick):
         if act is not True and act is not False and act is not None:
             raise NotImplementedError('custom activation module')
 
-    def _emit_padded(self, g, xin, cin, cpad):
+    def _emit_padded(self, g, x, cin):
         w, b = folded(self.conv, self.bn)
-        if cpad != cin:
-            w = torch.cat([w, torch.zeros((w.shape[0], cpad - cin) + tuple(w.shape[2:]), dtype=w.dtype)], 1)
-        return g.conv(xin, w, b, self.k, self.s, self.p, self.act_name)
+        return g.conv(x, _pad_cin(w, x.c - cin), b, self.k, self.s, self.p, self.act_name)
 
     def emit(self, g, x, name='', **kw):
         w, b = folded(self.conv, self.bn)

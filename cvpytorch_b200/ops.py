@@ -225,7 +225,7 @@ def nchw_to_split(x, dst_view):
 
 def split_to_nchw(src_view, out=None, device=None):
     """device: where to allocate `out` (default: the current CUDA device -- the library runs one device per process and
-    models._check_infer_input rejects tensors that live elsewhere)."""
+    the stand-alone drop-ins, modules._Standalone, reject tensors that live elsewhere)."""
     if out is None:
         out = torch.empty((src_view.B, src_view.C, src_view.H, src_view.W), dtype=torch.float32,
                           device=device if device is not None else torch.device('cuda', torch.cuda.current_device()))

@@ -11,16 +11,13 @@ so the following GEMM keeps 64-channel K chunks); the image-pool branch is avgpo
 "resize" (a broadcast); depthwise 3x3 (dilated) convs are an HBM-bound SIMT kernel, their 1x1 pointwise convs run on the
 tensor-core kernel; the final bilinear upsample + argmax is one kernel (the [B,19,H,W] fp32 tensor never exists).
 """
-from copy import deepcopy
-
 import torch
 import torch.nn as nn
 
 from . import ops
 from .engine import GraphBuilder
 from .fcos_models import ResNet
-from .models import _GraphCache, _check_infer_input
-from .modules import ConvModule, DepthwiseSeparableConvModule, folded
+from .modules import ConvModule, DepthwiseSeparableConvModule, _build, _Standalone, folded
 
 
 class ASPPModules(nn.ModuleList):
@@ -36,7 +33,7 @@ class ASPPModules(nn.ModuleList):
                 self.append(DepthwiseSeparableConvModule(in_channels, channels, 3, dilation=d, padding=d, norm_cfg=norm_cfg, act_cfg=act_cfg))
 
 
-class Deeplabv3PlusHead(_GraphCache):
+class Deeplabv3PlusHead(_Standalone):
     def __init__(self, low_in_channels, low_channels, dilations=(1, 6, 12, 18), num_classes=19, in_channels=None, channels=None,
                  dropout_ratio=0.1, conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True), act_cfg=dict(type='ReLU')):
         super().__init__()
@@ -97,30 +94,11 @@ class Deeplabv3PlusHead(_GraphCache):
         return logits
 
     def forward(self, x):
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x)
-        if key not in self._graphs:
-            g = GraphBuilder(x[0].shape[0], x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            logits = self.emit(g, ins)
-            self._graphs[key] = (g, ins, logits)
-        g, ins, logits = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
-        return ops.f32nhwc_to_nchw(logits.view(0, self.num_classes))
+        return ops.f32nhwc_to_nchw(self._run(x).view(0, self.num_classes))
 
 
 _BACKBONES = {'ResNet': ResNet}
 _HEADS = {'Deeplabv3PlusHead': Deeplabv3PlusHead}
-
-
-def _build(table, cfg):
-    c = deepcopy(dict(cfg))
-    name = c.pop('name')
-    if name not in table:
-        raise NotImplementedError(name)
-    return table[name](**c)
 
 
 def build_backbone(cfg):
@@ -131,7 +109,7 @@ def build_head(cfg):
     return _build(_HEADS, cfg)
 
 
-class EncoderDecoder(_GraphCache):
+class EncoderDecoder(_Standalone):
     """Model-level drop-in for src.models.segmentors.encoder_decoder.EncoderDecoder (inference: mode='val' -> int64 [B,H,W])."""
 
     def __init__(self, dictionary=None, model_cfg=None, *args, **kwargs):
@@ -162,17 +140,12 @@ class EncoderDecoder(_GraphCache):
         return dict(g=g, holder=holder, logits=logits, labels=labels, feats=feats)
 
     def _graph_for(self, imgs, out_hw=None):
-        B, _, H, W = imgs.shape
-        key = (B, H, W, imgs.device.index, out_hw)
-        if key not in self._graphs:
-            self._graphs[key] = self.build_graph(B, H, W, imgs.device, out_hw)
-        return self._graphs[key]
+        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device, out_hw), out_hw)
 
     def predict(self, imgs, out_hw=None):
         """Device-only inference: int64 label map [B, Ho, Wo] (Ho, Wo default to the input size); no host sync.
         The returned tensor is the GRAPH-OWNED output buffer: the next call with the same shape overwrites it (zero-copy);
         ``forward()`` returns a fresh tensor like the reference does."""
-        _check_infer_input(self, imgs)
         G = self._graph_for(imgs, out_hw)
         G['holder']['x'] = imgs.contiguous().float()
         G['g'].run()

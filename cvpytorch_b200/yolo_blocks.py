@@ -17,25 +17,14 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import GraphBuilder
-from .modules import ConvModule, _EmitModule, folded
+from .modules import ConvModule, _Standalone, folded
 
 
-class _Block(_EmitModule):
+class _Block(_Standalone):
     """stand-alone execution of a block as its own small graph (tests, brick-level use)"""
 
     def forward(self, x):
-        if self.training:
-            raise RuntimeError(f'{type(self).__name__} (H100): inference only; call .eval() first')
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 4):
-            raise ops._lib.CvbError(f'{type(self).__name__}: input must be a CUDA tensor [B,C,H,W]; there is no CPU fallback')
-        B, C, H, W = x.shape
-        g = GraphBuilder(B, x.device)
-        xin = g.new_act(H, W, C)
-        out = self.emit(g, xin)
-        ops.nchw_to_split(x, xin.view())
-        g.run()
-        return ops.split_to_nchw(out.view())
+        return ops.split_to_nchw(self._run([x], lambda g, ins: self.emit(g, ins[0])).view())
 
 
 def _fold_bn_identity(bn, channels):
@@ -90,6 +79,7 @@ class RepVGGBlock(_Block):
             if hasattr(self, name):
                 delattr(self, name)
         self.deploy = True
+        self._drop_graphs()  # the next call runs the deployed conv's weights
 
     def emit(self, g, x, name='', **kw):
         k, b = self.equivalent_kernel_bias()

@@ -16,16 +16,13 @@ re-ordered from the reference's [tl, bl, tr, br] patch order); CSP blocks, zero-
 fold are the YOLOv5 ones; per head level the first cls and reg 3x3 convs share one GEMM (N = 2 x 128), reg (4) and obj (1)
 predictors share one fp32-output 1x1 GEMM, cls (80) is another; `cvb_yolox_decode` turns both into 8-float candidate records
 and `cvb_yolox_nms` applies the score filter + torchvision.ops.batched_nms semantics per image."""
-from copy import deepcopy
-
 import numpy as np
 import torch
 import torch.nn as nn
 
 from . import ops
 from .engine import GraphBuilder
-from .models import _GraphCache, _check_infer_input
-from .modules import ConvModule, CSPLayer, SPPF, _EmitModule, _emit_csp, folded
+from .modules import ConvModule, CSPLayer, SPPF, _build, _EmitModule, _emit_csp, _Standalone, folded
 
 
 class Focus(_EmitModule):
@@ -52,7 +49,7 @@ def focus_weights_to_s2d(w64):
     return out
 
 
-class CSPDarknet(_GraphCache):
+class CSPDarknet(_Standalone):
     cfg = {"n": [0.33, 0.25], "t": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
 
     def __init__(self, subtype='cspdark_s', out_channels=[64, 128, 256, 512, 1024], layers=[3, 9, 9, 3], spp_ksizes=(5, 9, 13),
@@ -92,18 +89,7 @@ class CSPDarknet(_GraphCache):
         return outs
 
     def forward(self, x):
-        _check_infer_input(self, x)
-        B, _, H, W = x.shape
-        key = (B, H, W, x.device.index)
-        if key not in self._graphs:
-            g = GraphBuilder(B, x.device)
-            holder = {}
-            self._graphs[key] = (g, holder, self.emit(g, lambda: holder['x'], H, W))
-        g, holder, outs = self._graphs[key]
-        holder['x'] = x.contiguous().float()
-        g.run()
-        res = [ops.split_to_nchw(o.view()) for o in outs]
-        return res if len(self.out_stages) > 1 else res[0]
+        return self._run_image(x)
 
 
 class BaseConv(ConvModule):
@@ -146,7 +132,7 @@ class XCSPLayer(_EmitModule):
         return _emit_csp(g, x, self.conv1, self.conv2, self.conv3, blocks, sc, name, up_src=up_src, out=out)
 
 
-class YOLOXNeck(_GraphCache):
+class YOLOXNeck(_Standalone):
     def __init__(self, subtype='yolox_s', channels=[256, 512, 1024], depth_mul=1.0, width_mul=1.0):
         super().__init__()
         assert isinstance(channels, list)
@@ -180,17 +166,7 @@ class YOLOXNeck(_GraphCache):
 
     def forward(self, x):
         assert len(x) == len(self.channels)
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x)
-        if key not in self._graphs:
-            g = GraphBuilder(x[0].shape[0], x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            self._graphs[key] = (g, ins, self.emit(g, ins))
-        g, ins, outs = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
-        return [ops.split_to_nchw(o.view()) for o in outs]
+        return [ops.split_to_nchw(o.view()) for o in self._run(x)]
 
 
 class HeadConv(ConvModule):
@@ -201,7 +177,7 @@ class HeadConv(ConvModule):
                          act_cfg=dict(type=activation))
 
 
-class YOLOXHead(_GraphCache):
+class YOLOXHead(_Standalone):
     def __init__(self, num_classes=80, subtype='yolox_s', in_channels=[256, 512, 1024], strides=[8, 16, 32], depth_mul=1.0, width_mul=1.0):
         super().__init__()
         self.num_classes, self.subtype, self.strides, self.n_anchors = num_classes, subtype, strides, 1
@@ -249,33 +225,13 @@ class YOLOXHead(_GraphCache):
 
     def forward(self, x):
         """list of NCHW CUDA feature maps -> list of [B, 5 + num_classes, h+2, w+2] raw outputs (reg, obj, cls), as the reference."""
-        _check_infer_input(self, x[0])
-        key = tuple(tuple(t.shape) for t in x)
-        if key not in self._graphs:
-            g = GraphBuilder(x[0].shape[0], x[0].device)
-            ins = [g.new_act(t.shape[2], t.shape[3], t.shape[1]) for t in x]
-            self._graphs[key] = (g, ins, self.emit(g, ins))
-        g, ins, outs = self._graphs[key]
-        for t, v in zip(x, ins):
-            ops.nchw_to_split(t, v.view())
-        g.run()
-        res = []
-        for ro, cl in outs:
-            res.append(torch.cat([ops.f32nhwc_to_nchw(ro.view(0, 5)), ops.f32nhwc_to_nchw(cl.view(0, self.num_classes))], 1))
-        return res
+        return [torch.cat([ops.f32nhwc_to_nchw(ro.view(0, 5)), ops.f32nhwc_to_nchw(cl.view(0, self.num_classes))], 1)
+                for ro, cl in self._run(x)]
 
 
 _BACKBONES = {'CSPDarknet': CSPDarknet, 'CspDarkNet': CSPDarknet}
 _NECKS = {'YOLOXNeck': YOLOXNeck}
 _HEADS = {'YOLOXHead': YOLOXHead}
-
-
-def _build(table, cfg):
-    c = deepcopy(dict(cfg))
-    name = c.pop('name')
-    if name not in table:
-        raise NotImplementedError(name)
-    return table[name](**c)
 
 
 def build_backbone(cfg):
@@ -290,7 +246,7 @@ def build_head(cfg):
     return _build(_HEADS, cfg)
 
 
-class YOLOX(_GraphCache):
+class YOLOX(_Standalone):
     """Model-level drop-in for src.models.yolox.YOLOX (inference: mode='val')."""
     cfg = {"nano": [0.33, 0.25], "tiny": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
     input_norm = dict(mean=(0.406, 0.456, 0.485), std=(0.225, 0.224, 0.229), reverse_channels=True)
@@ -332,15 +288,10 @@ class YOLOX(_GraphCache):
         return dict(g=g, holder=holder, outs=outs, ws=ws)
 
     def _graph_for(self, imgs):
-        B, _, H, W = imgs.shape
-        key = (B, H, W, imgs.device.index)
-        if key not in self._graphs:
-            self._graphs[key] = self.build_graph(B, H, W, imgs.device)
-        return self._graphs[key]
+        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device))
 
     def predict(self, imgs):
         """Device-only inference: (det [B,A,7] rows (x1,y1,x2,y2,obj,class_conf,class_pred) in kept order, count [B]); no host sync."""
-        _check_infer_input(self, imgs)
         G = self._graph_for(imgs)
         G['holder']['x'] = imgs.contiguous().float()
         G['g'].run()

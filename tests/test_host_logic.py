@@ -66,16 +66,67 @@ def test_stem_space_to_depth_equivalence():
 
 
 def test_factories_follow_reference_contract():
+    """The build_* factories of all four model families: an unknown name raises NotImplementedError, and the cfg is deep-copied,
+    not consumed (not even the 'depth_mul' / 'width_mul' keys YOLOv5's build_backbone drops)."""
+    from copy import deepcopy
+
+    from cvpytorch_b200 import fcos_models as FM
     from cvpytorch_b200 import models as M
-    with pytest.raises(NotImplementedError):
-        M.build_backbone({'name': 'NoSuchBackbone'})
-    with pytest.raises(NotImplementedError):
-        M.build_neck({'name': 'BiFPN'})
+    from cvpytorch_b200 import seg_models as SM
+    from cvpytorch_b200 import synth
+    from cvpytorch_b200 import yolox_models as XM
+    for build in (M.build_backbone, M.build_neck, M.build_detect, XM.build_backbone, XM.build_neck, XM.build_head, FM.build_backbone,
+                  FM.build_neck, FM.build_head, FM.build_detect, SM.build_backbone, SM.build_head):
+        with pytest.raises(NotImplementedError):
+            build({'name': 'NoSuchModule'})
     cfg = {'name': 'YOLOv5Detect', 'in_channels': [256, 512, 1024], 'width_mul': 0.5, 'anchors': M.YOLOv5.anchors, 'num_classes': 80}
     d = M.build_detect(cfg)
-    assert 'name' in cfg and d.m[0].weight.shape == (255, 128, 1, 1)  # cfg is deep-copied, not consumed
+    assert 'name' in cfg and d.m[0].weight.shape == (255, 128, 1, 1)
     bias = d.m[0].bias.view(3, 85)
     assert abs(float(bias[0, 4]) - np.log(8 / (640 / 8) ** 2)) < 1.0  # prior added on top of the default init
+    for build, cfg in ((M.build_backbone, {**synth.YOLOV5S_CFG['BACKBONE'], 'depth_mul': 0.33, 'width_mul': 0.5}),
+                       (M.build_detect, cfg),
+                       (XM.build_neck, {**synth.YOLOX_CFG['NECK'], 'depth_mul': 0.33, 'width_mul': 0.5}),
+                       (FM.build_detect, synth.FCOS_CFG['DETECT']),
+                       (SM.build_head, synth.DEEPLAB_CFG['HEAD'])):
+        before = deepcopy(cfg)
+        build(cfg)
+        assert cfg == before, cfg['name']
+
+
+def test_standalone_dropins_reject_cpu_input_and_training_without_caching():
+    """Every drop-in that runs on its own -- the 3 backbones, the 7 components, the bricks, the yolo_blocks blocks and the 4 models'
+    'val' forward -- raises CvbError on CPU tensors and RuntimeError in training mode (that check first), and caches no graph."""
+    from cvpytorch_b200 import _lib, synth
+    from cvpytorch_b200 import fcos_models as FM
+    from cvpytorch_b200 import models as M
+    from cvpytorch_b200 import seg_models as SM
+    from cvpytorch_b200 import yolo_blocks as YB
+    from cvpytorch_b200 import yolox_models as XM
+    from cvpytorch_b200.modules import Conv, ConvModule
+    cls80 = [{f'c{i}': 1.0} for i in range(80)]
+    v5, yx = M.YOLOv5(cls80, dict(synth.YOLOV5S_CFG)), XM.YOLOX(cls80, dict(synth.YOLOX_CFG))
+    fc, dl = FM.FCOS(cls80, dict(synth.FCOS_CFG)), SM.EncoderDecoder([{f'c{i}': 1.0} for i in range(19)], dict(synth.DEEPLAB_CFG))
+    img = torch.zeros(1, 3, 64, 64)
+    maps = lambda *cs: [torch.zeros(1, c, 8 >> i, 8 >> i) for i, c in enumerate(cs)]  # noqa: E731
+    x = torch.zeros(1, 32, 8, 8)
+    inputs = [(v5.backbone, img), (yx.backbone, img), (fc.backbone, img),
+              (v5.neck, maps(128, 256, 512)), (v5.detect, maps(128, 256, 512)), (yx.neck, maps(128, 256, 512)), (yx.head, maps(128, 256, 512)),
+              (fc.neck, maps(512, 1024, 2048)), (fc.head, maps(256, 256, 256, 256)), (dl.head, maps(256, 2048)),
+              (ConvModule(24, 32, 3, padding=1, norm_cfg=dict(type='BN')), torch.zeros(1, 24, 8, 8)), (Conv(24, 32, 3), torch.zeros(1, 24, 8, 8)),
+              (YB.RepVGGBlock(32, 32), x), (YB.BottleRep(32, 32), x), (YB.RepBlock(32, 32, n=2), x), (YB.Conv_C3(32, 32), x),
+              (YB.BepC3(32, 32, n=2), x), (YB.EELAN(32, 16, 32), x)]
+    calls = [(m, lambda m=m, t=t: m(t)) for m, t in inputs] + [(m, lambda m=m: m(img, None, 'val')) for m in (v5, yx, fc, dl)]
+    for m, call in calls:
+        m.eval()
+        with pytest.raises(_lib.CvbError):
+            call()
+        assert m._graphs == {}, type(m).__name__
+        m.train()
+        with pytest.raises(RuntimeError) as e:
+            call()
+        assert not isinstance(e.value, _lib.CvbError), type(m).__name__
+        assert m._graphs == {}, type(m).__name__
 
 
 def test_model_surface_and_loud_failure_without_cuda():

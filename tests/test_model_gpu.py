@@ -339,6 +339,69 @@ def test_brick_level_convmodule_standalone(cuda):
     assert _rel(c(x), ref) < 2e-5
 
 
+def test_standalone_graph_cache_and_invalidation(cuda):
+    """The stand-alone graph cache of a model, a component, a brick and a yolo_blocks block: after load_state_dict the next call
+    equals, bit for bit, a fresh module holding the new weights; a repeated call with the same shape replays the cached graph;
+    train() + eval() rebuild it.  Every tensor of a list input is checked before a graph is built."""
+    from cvpytorch_b200 import _lib, synth
+    from cvpytorch_b200 import models as M
+    from cvpytorch_b200 import yolo_blocks as YB
+    from cvpytorch_b200.modules import ConvModule
+    torch.manual_seed(11)
+    img = torch.randn(2, 3, 64, 64, device='cuda')
+    feats = [torch.randn(2, c, 8 >> i, 8 >> i, device='cuda') for i, c in enumerate((128, 256, 512))]
+    x24, x64 = torch.randn(2, 24, 12, 20, device='cuda'), torch.randn(2, 64, 12, 20, device='cuda')
+    ncfg = {'name': 'YOLOv5Neck', 'in_channels': [256, 512, 1024], 'out_channels': [256, 512, 1024], 'depth_mul': 0.33, 'width_mul': 0.5}
+    cases = [(lambda: synth.build_yolov5s(True), lambda m: [t.clone() for t in m.predict(img)] + [m._graph_for(img)['z'].clone()]),
+             (lambda: M.build_neck(ncfg).eval(), lambda m: m(feats)),
+             (lambda: ConvModule(24, 32, 3, padding=1, norm_cfg=dict(type='BN'), act_cfg=dict(type='SiLU')).eval(), lambda m: [m(x24)]),
+             (lambda: YB.BepC3(64, 64, n=4).eval(), lambda m: [m(x64)])]
+    for make, run in cases:
+        m = make()
+        before = run(m)
+        sd = {k: v * 0.9 if v.is_floating_point() and 'running' not in k else v for k, v in m.state_dict().items()}
+        m.load_state_dict(sd)
+        assert m._graphs == {}
+        out = run(m)
+        fresh = make()
+        fresh.load_state_dict(sd)
+        ref = run(fresh)
+        torch.cuda.synchronize()
+        name = type(m).__name__
+        assert all(torch.equal(a, b) for a, b in zip(out, ref)) and not all(torch.equal(a, b) for a, b in zip(out, before)), name
+        graph = next(iter(m._graphs.values()))
+        again = run(m)
+        assert len(m._graphs) == 1 and next(iter(m._graphs.values())) is graph, name
+        m.train()
+        m.eval()
+        assert m._graphs == {}, name
+        rebuilt = run(m)
+        assert next(iter(m._graphs.values())) is not graph, name
+        assert all(torch.equal(a, b) and torch.equal(a, c) for a, b, c in zip(out, again, rebuilt)), name
+    neck = M.build_neck(ncfg).eval()
+    with pytest.raises(_lib.CvbError):
+        neck([feats[0], feats[1].cpu(), feats[2]])
+    assert neck._graphs == {}
+    rep = YB.RepVGGBlock(64, 64).eval()
+    y = rep(x64)
+    rep.switch_to_deploy()  # drops the graph of the three-branch fold: the next call runs the deployed conv
+    assert rep._graphs == {}
+    assert _rel(rep(x64), y) < 1e-5 and len(rep._graphs) == 1
+
+
+def test_standalone_brick_rejects_a_wrong_channel_count(cuda):
+    """A brick called on a map whose channel count is not its in_channels raises, as the reference's conv does, instead of reading
+    its weights against the wrong channels: fewer or more channels, with or without channel padding, depthwise included."""
+    from cvpytorch_b200.modules import Conv, ConvModule
+    bn = dict(type='BN')
+    for m, c in ((ConvModule(64, 32, 3, padding=1, norm_cfg=bn), 16), (ConvModule(24, 32, 3, padding=1, norm_cfg=bn), 32),
+                 (ConvModule(24, 32, 3, padding=1, norm_cfg=bn), 20), (Conv(16, 32, 3), 20), (Conv(32, 32, 1), 48),
+                 (ConvModule(32, 32, 3, padding=1, groups=32, norm_cfg=bn), 16), (ConvModule(32, 32, 3, padding=1, groups=32, norm_cfg=bn), 48)):
+        with pytest.raises(AssertionError):
+            m.eval()(torch.randn(1, c, 8, 8, device='cuda'))
+        assert m._graphs == {}
+
+
 def test_drop_in_through_the_reference_trainer_val_step(model):
     """The val branch of the reference's Trainer.run_step (trainer.py:209-231) restated around the drop-in model, including the
     `cfg.distributed` path: reduce_dict(losses) stacks the loss values (src/utils/distributed.py:108-125) and must not see an empty dict."""
