@@ -292,121 +292,21 @@ __global__ void sppf_pool_kernel(const __half* __restrict__ x, int H, int W, int
 }
 
 // ------------------------------------------------------------------ YOLOv5 decode
-// Grid (pixel chunks, B); one warp per output row (a, pix): 85 contiguous floats are read and written coalesced, all
-// index arithmetic is 32-bit and per row.  While the scores are in registers the CTA also builds the NMS score
-// histogram of its image in shared memory (64 KB) and flushes the non-empty bins once -- this replaces the separate
-// counting pass over the 548 MB prediction tensor and keeps the hot bins out of global atomics.
+// Grid (pixel chunks, B); one warp per output row (anchor a, pixel), anchor-major: three 32-lane chunks of the row's no <= 96 floats
+// are read and written coalesced, kDecodeRows rows in flight.  While the scores are in registers the CTA also builds the NMS score
+// histogram of its image in shared memory (64 KB, HIST) and flushes the non-empty bins once -- this replaces the separate counting
+// pass over the 548 MB prediction tensor and keeps the hot bins out of global atomics.  MULTI: one histogram entry per class score
+// above conf, else one per row (its best score).  z may be null without HIST; xperm (the raw rows, permuted) may be null.
 constexpr int kDecodePix = 512;      // pixels per CTA (x na anchor rows)
 constexpr int kDecodeThreads = 512;  // 16 warps
 constexpr int kDecodeRows = 4;       // rows in flight per warp (all loads issued before the first use)
 
+template <bool HIST, bool MULTI>
 __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float* __restrict__ raw, int ny, int nx, int pitch, int na,
                                                                      int no, const float* __restrict__ anchors_px, float stride,
                                                                      float* __restrict__ z, long long z_rows, long long z_off,
                                                                      float* __restrict__ xperm, uint32_t* __restrict__ hist,
-                                                                     float* __restrict__ rowmax, float conf, int multi_label) {
-  extern __shared__ uint32_t s_hist[];  // [kNmsBins] when hist != nullptr
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  constexpr int NW = kDecodeThreads / 32;
-  const int b = blockIdx.y;
-  const int npix = ny * nx;
-  const int pix0 = blockIdx.x * kDecodePix;
-  const int cpix = min(npix, pix0 + kDecodePix) - pix0;
-  if (hist != nullptr) {
-    for (int i = threadIdx.x; i < kNmsBins; i += kDecodeThreads) s_hist[i] = 0;
-    __syncthreads();
-  }
-  const int nrows = cpix * na;
-  const int nchunk = (no + 31) >> 5;  // <= 3 supported in registers (no <= 96); larger class counts loop
-  for (int r0 = warp * kDecodeRows; r0 < nrows; r0 += NW * kDecodeRows) {
-    float v[kDecodeRows][3];
-    int av[kDecodeRows], pv[kDecodeRows];
-#pragma unroll
-    for (int i = 0; i < kDecodeRows; ++i) {
-      const int rr = min(r0 + i, nrows - 1);
-      const int a = rr / cpix;
-      const int pix = pix0 + rr - a * cpix;
-      av[i] = a;
-      pv[i] = pix;
-      const float* src = raw + ((size_t)b * npix + pix) * pitch + a * no;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const int c = k * 32 + lane;
-        v[i][k] = (k < nchunk && c < no) ? __ldg(src + c) : 0.0f;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kDecodeRows; ++i) {
-      if (r0 + i >= nrows) break;
-      const int a = av[i], pix = pv[i];
-      const int py = pix / nx, px = pix - py * nx;
-      const size_t orow = (size_t)a * npix + pix;
-      float* zdst = z ? z + ((size_t)b * z_rows + z_off + orow) * no : nullptr;
-      float* xdst = xperm ? xperm + ((size_t)b * na * npix + orow) * no : nullptr;
-      float obj = 0.0f, best = -1.0f, rbest = 0.0f;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const int c = k * 32 + lane;
-        float o = 0.0f;
-        if (k < nchunk && c < no) {
-          const float x = v[i][k];
-          if (xdst) xdst[c] = x;
-          // reference: y = x.sigmoid(); xy = (y*2 - 0.5 + grid) * stride; wh = (y*2)**2 * anchor_grid   (yolov5_detect.py:50-53)
-          const float y = sigmoid_fast(x);
-          o = y;
-          if (c < 2) {
-            o = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(y, 2.0f), 0.5f), c == 0 ? (float)px : (float)py), stride);
-          } else if (c < 4) {
-            const float t2 = __fmul_rn(y, 2.0f);
-            o = __fmul_rn(__fmul_rn(t2, t2), __ldg(anchors_px + a * 2 + (c - 2)));
-          }
-          if (zdst) zdst[c] = o;
-        }
-        if (hist != nullptr) {
-          if (k == 0) obj = __shfl_sync(0xffffffffu, o, 4);
-          if (obj > conf && c >= 5 && c < no && k < nchunk) {
-            const float sc = __fmul_rn(o, obj);  // same fp32 product the NMS kernels recompute from z (yolov5.py:106)
-            if (multi_label) {
-              if (sc > conf) {
-                atomicAdd(&s_hist[nms_score_bin(sc)], 1u);
-                rbest = fmaxf(rbest, sc);
-              }
-            } else {
-              best = fmaxf(best, sc);
-            }
-          }
-        }
-      }
-      if (hist != nullptr) {
-        if (!multi_label) rbest = best > conf ? best : 0.0f;
-#pragma unroll
-        for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
-        if (lane == 0) {
-          rowmax[(size_t)b * z_rows + z_off + orow] = rbest;
-          if (!multi_label && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
-        }
-      }
-    }
-  }
-  if (hist != nullptr) {
-    __syncthreads();
-    uint32_t* gh = hist + (size_t)b * kNmsBins;
-    for (int i = threadIdx.x; i < kNmsBins; i += kDecodeThreads) {
-      const uint32_t c = s_hist[i];
-      if (c) atomicAdd(&gh[i], c);
-    }
-  }
-}
-
-// Specialised decode for the hot configuration (64 <= no <= 96, decoded output only): one warp per (anchor, pixel) row, three
-// 32-lane chunks, kDecodeRows rows in flight, 32-bit offsets inside the CTA's pixel range, no per-chunk control flow.  Same
-// arithmetic as the generic kernel above (bit-identical z, histogram and rowmax).
-template <bool HIST, bool MULTI>
-__global__ void __launch_bounds__(kDecodeThreads) yolo_decode_fast_kernel(const float* __restrict__ raw, int ny, int nx, int pitch, int na,
-                                                                          int no, const float* __restrict__ anchors_px, float stride,
-                                                                          float* __restrict__ z, long long z_rows, long long z_off,
-                                                                          uint32_t* __restrict__ hist, float* __restrict__ rowmax,
-                                                                          float conf, uint32_t nx_magic) {
+                                                                     float* __restrict__ rowmax, float conf, uint32_t nx_magic) {
   extern __shared__ uint32_t s_hist[];  // [kNmsBins] when HIST
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NW = kDecodeThreads / 32;
@@ -420,63 +320,76 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_fast_kernel(const 
     __syncthreads();
   }
   const float* rbase = raw + ((size_t)b * npix + pix0) * pitch;
-  float* zb = z + ((size_t)b * z_rows + z_off) * no;        // row index inside the level: a * npix + pix
+  const size_t zb = ((size_t)b * z_rows + z_off) * no;  // z element of the level's first row in image b
+  const size_t xb = (size_t)b * na * npix * no;
   float* rmb = HIST ? rowmax + (size_t)b * z_rows + z_off : nullptr;
-  const bool v2 = (64 + lane) < no;
-  const bool is_cls = lane >= 5;
-  // rows = (anchor a, pixel p): explicit loop nest, so the only division left is pixel -> (py, px), done with a multiply-high
-  // (nx_magic = ceil(2^32 / nx), exact while pix * nx < 2^32: checked on the host)
-  for (int a = 0; a < na; ++a)
-  for (int p0 = warp * R; p0 < cpix; p0 += NW * R) {
-    float v[R][3];
+  const bool v0 = lane < no, v1 = 32 + lane < no, v2 = 64 + lane < no;
+  const bool is_cls = v0 && lane >= 5;
+  for (int a = 0; a < na; ++a) {
+    const float anchor = __ldg(anchors_px + a * 2 + (lane & 1));  // w (even lanes) or h (odd lanes) of this anchor, in pixels
+    for (int p0 = warp * R; p0 < cpix; p0 += NW * R) {
+      float v[R][3];
 #pragma unroll
-    for (int i = 0; i < R; ++i) {
-      const int p = min(p0 + i, cpix - 1);
-      const float* src = rbase + (uint32_t)(p * pitch + a * no) + lane;
-      v[i][0] = __ldg(src);
-      v[i][1] = __ldg(src + 32);
-      v[i][2] = v2 ? __ldg(src + 64) : 0.0f;
-    }
-#pragma unroll
-    for (int i = 0; i < R; ++i) {
-      const bool ok = (p0 + i) < cpix;  // tail rows are computed on clamped inputs and not stored (keeps the shuffles convergent)
-      const int pix = pix0 + min(p0 + i, cpix - 1);
-      const int py = (int)__umulhi((uint32_t)pix, nx_magic), px = pix - py * nx;
-      const uint32_t orow = (uint32_t)(a * npix + pix);
-      float* dst = zb + (size_t)orow * no + lane;
-      const float y0 = sigmoid_fast(v[i][0]);
-      const float y1 = sigmoid_fast(v[i][1]);
-      const float y2 = sigmoid_fast(v[i][2]);
-      // reference: y = x.sigmoid(); xy = (y*2 - 0.5 + grid) * stride; wh = (y*2)**2 * anchor_grid   (yolov5_detect.py:50-53)
-      const float t2 = __fmul_rn(y0, 2.0f);
-      const float xy = __fmul_rn(__fadd_rn(__fsub_rn(t2, 0.5f), lane == 0 ? (float)px : (float)py), stride);
-      const float wh = __fmul_rn(__fmul_rn(t2, t2), __ldg(anchors_px + a * 2 + (lane & 1)));
-      const float o0 = lane < 2 ? xy : (lane < 4 ? wh : y0);
-      if (ok) {
-        dst[0] = o0;
-        dst[32] = y1;
-        if (v2) dst[64] = y2;
+      for (int i = 0; i < R; ++i) {
+        const int p = min(p0 + i, cpix - 1);
+        const float* src = rbase + (size_t)(uint32_t)p * (uint32_t)pitch + (uint32_t)(a * no + lane);
+        v[i][0] = v0 ? __ldg(src) : 0.0f;
+        v[i][1] = v1 ? __ldg(src + 32) : 0.0f;
+        v[i][2] = v2 ? __ldg(src + 64) : 0.0f;
       }
-      if (HIST) {
-        const float obj = __shfl_sync(0xffffffffu, o0, 4);
-        float rbest = 0.0f;
-        if (ok && obj > conf) {  // warp-uniform
-          // same fp32 product the NMS kernels recompute from z (yolov5.py:106)
-          const float s0 = is_cls ? __fmul_rn(o0, obj) : 0.0f;
-          const float s1 = __fmul_rn(y1, obj);
-          const float s2 = v2 ? __fmul_rn(y2, obj) : 0.0f;
-          if (MULTI) {
-            if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
-            if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
-            if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
-          }
-          rbest = fmaxf(fmaxf(s0, s1), s2);
-          if (!(rbest > conf)) rbest = 0.0f;
+      int pyv[R];  // pixel row of every row in flight, computed before the row loop (keeps fast_div's branches out of it)
 #pragma unroll
-          for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
-          if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
+      for (int i = 0; i < R; ++i) pyv[i] = fast_div(pix0 + min(p0 + i, cpix - 1), nx, nx_magic);
+      if (xperm != nullptr) {  // kernel-uniform: copy the raw rows
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          if (p0 + i < cpix) {
+            float* dst = xperm + xb + (size_t)(uint32_t)(a * npix + pix0 + p0 + i) * no + lane;
+            if (v0) dst[0] = v[i][0];
+            if (v1) dst[32] = v[i][1];
+            if (v2) dst[64] = v[i][2];
+          }
         }
-        if (ok && lane == 0) rmb[orow] = rbest;
+      }
+#pragma unroll
+      for (int i = 0; i < R; ++i) {
+        const bool ok = (p0 + i) < cpix;  // tail rows are computed on clamped inputs and not stored (keeps the shuffles convergent)
+        const int pix = pix0 + min(p0 + i, cpix - 1);
+        // this lane's element of level row a * npix + pix (na * npix < 2^31: checked on the host)
+        const size_t roff = (size_t)(uint32_t)(a * npix + pix) * no + lane;
+        const int py = pyv[i], px = pix - py * nx;
+        const float y0 = sigmoid_fast(v[i][0]);
+        const float y1 = sigmoid_fast(v[i][1]);
+        const float y2 = sigmoid_fast(v[i][2]);
+        const float xy = yolo_xy(y0, lane == 0 ? (float)px : (float)py, stride);
+        const float wh = yolo_wh(y0, anchor);
+        const float o0 = lane < 2 ? xy : (lane < 4 ? wh : y0);
+        if (ok && z != nullptr) {
+          float* dst = z + zb + roff;
+          if (v0) dst[0] = o0;
+          if (v1) dst[32] = y1;
+          if (v2) dst[64] = y2;
+        }
+        if (HIST) {
+          const float obj = __shfl_sync(0xffffffffu, o0, 4);
+          float rbest = 0.0f;
+          if (ok && obj > conf) {  // warp-uniform
+            const float s0 = is_cls ? yolo_score(o0, obj) : 0.0f;
+            const float s1 = v1 ? yolo_score(y1, obj) : 0.0f;
+            const float s2 = v2 ? yolo_score(y2, obj) : 0.0f;
+            if (MULTI) {
+              if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
+              if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
+              if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
+            }
+            rbest = fmaxf(fmaxf(s0, s1), s2);
+            if (!(rbest > conf)) rbest = 0.0f;
+#pragma unroll
+            for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
+            if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
+          }
+          if (ok && lane == 0) rmb[a * npix + pix] = rbest;
+        }
       }
     }
   }
@@ -1113,44 +1026,21 @@ extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const
   CVB_REQUIRE(z != nullptr || xperm != nullptr, "yolo_decode: nothing to write");
   CVB_REQUIRE(nms_workspace == nullptr || z != nullptr, "yolo_decode: histogram needs the decoded output");
   CVB_REQUIRE((long long)raw->H * raw->W * na < 0x7fffffffLL, "yolo_decode: level too large");
-  const size_t smem = nms_workspace ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
+  CVB_REQUIRE(no <= 96, "yolo_decode: at most 91 classes supported (no=%d)", no);
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
   static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(yolo_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
+    cudaError_t e = cudaFuncSetAttribute(yolo_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(yolo_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
     return e;
   }();
   CVB_CHECK_CUDA(attr_set_err);
-  dim3 grid(ceil_div(raw->H * raw->W, kDecodePix), raw->B);
-  CVB_REQUIRE(no <= 96, "yolo_decode: at most 91 classes supported (no=%d)", no);
   uint32_t* hist = static_cast<uint32_t*>(nms_workspace);
-  float* rowmax = nms_workspace ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(raw->B)) : nullptr;
-  const float* rawp = static_cast<const float*>(raw->base);
-  const uint32_t nx_magic = (uint32_t)((0x100000000ULL + (unsigned long long)raw->W - 1) / (unsigned long long)raw->W);
-  if (xperm == nullptr && no >= 64 && raw->W > 1 && (long long)kDecodePix * raw->c_pitch + (long long)na * no < 0x7fffffffLL &&
-      (unsigned long long)raw->H * raw->W * raw->W < 0x100000000ULL) {
-    // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-    static const cudaError_t fast_attr_set_err = [] {
-      cudaError_t e = cudaSuccess;
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(yolo_decode_fast_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(yolo_decode_fast_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
-      return e;
-    }();
-    CVB_CHECK_CUDA(fast_attr_set_err);
-    cudaStream_t st = as_stream(stream);
-    if (!hist)
-      yolo_decode_fast_kernel<false, false><<<grid, kDecodeThreads, 0, st>>>(rawp, raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows,
-                                                                             z_off, nullptr, nullptr, conf_thres, nx_magic);
-    else if (multi_label)
-      yolo_decode_fast_kernel<true, true><<<grid, kDecodeThreads, smem, st>>>(rawp, raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows,
-                                                                              z_off, hist, rowmax, conf_thres, nx_magic);
-    else
-      yolo_decode_fast_kernel<true, false><<<grid, kDecodeThreads, smem, st>>>(rawp, raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows,
-                                                                               z_off, hist, rowmax, conf_thres, nx_magic);
-  } else {
-    yolo_decode_kernel<<<grid, kDecodeThreads, smem, as_stream(stream)>>>(rawp, raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows,
-                                                                          z_off, xperm, hist, rowmax, conf_thres, multi_label);
-  }
+  float* rowmax = hist ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(raw->B)) : nullptr;
+  const size_t smem = hist ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
+  const auto kernel = !hist ? yolo_decode_kernel<false, false> : multi_label ? yolo_decode_kernel<true, true> : yolo_decode_kernel<true, false>;
+  kernel<<<dim3(ceil_div(raw->H * raw->W, kDecodePix), raw->B), kDecodeThreads, smem, as_stream(stream)>>>(
+      static_cast<const float*>(raw->base), raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows, z_off, xperm, hist, rowmax,
+      conf_thres, fast_div_magic(raw->W, (unsigned long long)raw->H * raw->W));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;

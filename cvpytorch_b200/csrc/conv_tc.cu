@@ -95,7 +95,7 @@ struct alignas(64) ConvKArgs {
   CUtensorMap tmO;     // output (5D; plane dim = 1 for fp32)
   CUtensorMap tmR;     // residual (same box as the output tile), loaded by TMA into a staging tile
   int tiles_w, tiles_h, tiles_b, tiles_n;
-  uint32_t mg_n, mg_w, mg_h;   // ceil(2^32 / tiles_{n,w,h}): tile index -> coordinates by multiply-high (0: use a real division)
+  uint32_t mg_n, mg_w, mg_h;   // fast_div_magic of tiles_{n,w,h}: tile index -> coordinates by multiply-high
   int TW, TH, NB;
   int Ho, Wo, Bn;
   int cout;
@@ -154,10 +154,6 @@ struct alignas(64) ConvKArgs {
   long long* prof;             // diagnostics (cvb_conv_plan_set_profile): per-CTA cycle counters of the three pipeline roles, or NULL
   SmemLayout sm;
 };
-
-// x / d for 0 <= x with x * d < 2^32 (checked on the host, else magic = 0; magic = 1 means d == 1): one multiply-high instead of a
-// ~20-instruction division
-__device__ __forceinline__ int fast_div(int x, int d, uint32_t magic) { return magic == 1u ? x : (magic ? (int)__umulhi((uint32_t)x, magic) : x / d); }
 
 // first output column, row, image and channel of a tile; tile = ((bt * tiles_h + ht) * tiles_w + wt) * tiles_n + nt
 struct TileOrigin {
@@ -750,12 +746,11 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
             yv[4 * j + 3] = sigmoid_fast(v4.w + bias_a[col + 4 * j + 3]);
           }
           int j0 = 0;
-          if (col == 0) {  // (warp-uniform) xy = (y*2 - 0.5 + grid) * stride; wh = (y*2)^2 * anchor  (yolov5_detect.py:50-53)
-            const float t0 = __fmul_rn(yv[0], 2.0f), t1 = __fmul_rn(yv[1], 2.0f), t2 = __fmul_rn(yv[2], 2.0f), t3 = __fmul_rn(yv[3], 2.0f);
-            srow[0] = __fmul_rn(__fadd_rn(__fsub_rn(t0, 0.5f), (float)px), a.y_stride);
-            srow[1] = __fmul_rn(__fadd_rn(__fsub_rn(t1, 0.5f), (float)py), a.y_stride);
-            srow[2] = __fmul_rn(__fmul_rn(t2, t2), a.y_anchor[an * 2]);
-            srow[3] = __fmul_rn(__fmul_rn(t3, t3), a.y_anchor[an * 2 + 1]);
+          if (col == 0) {  // (warp-uniform) box columns
+            srow[0] = yolo_xy(yv[0], (float)px, a.y_stride);
+            srow[1] = yolo_xy(yv[1], (float)py, a.y_stride);
+            srow[2] = yolo_wh(yv[2], a.y_anchor[an * 2]);
+            srow[3] = yolo_wh(yv[3], a.y_anchor[an * 2 + 1]);
             srow[4] = yv[4];
             yv[0] = yv[1] = yv[2] = yv[3] = yv[4] = 0.0f;  // not class scores
             j0 = 5;
@@ -770,12 +765,11 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
               if (j >= j0 && col + j < no) srow[col + j] = yv[j];
           }
           if (any_live) {
-            // scores: the fp32 product the NMS kernels recompute from z (yolov5.py:106).  y = 0 in the padding columns and obj = 0 in
-            // rows outside the level, so `sc > conf` alone decides; the histogram update sits behind a warp vote (a uniform branch):
-            // background pixels cost four instructions per score
+            // y = 0 in the padding columns and obj = 0 in rows outside the level, so `sc > conf` alone decides; the histogram update
+            // sits behind a warp vote (a uniform branch): background pixels cost four instructions per score
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
-              const float sc = __fmul_rn(yv[j], obj);
+              const float sc = yolo_score(yv[j], obj);
               const bool pass = sc > conf;
               rbest = fmaxf(rbest, sc);
               if (multi && __any_sync(0xffffffffu, pass)) hist_inc_if(hist_s32, sc, pass);
@@ -1718,14 +1712,9 @@ static void fill_tiles(const ConvProblem& P, const TapTable& T, int bn, const Sc
   a.tiles_n = ceil_div(P.cout, bn);
   {
     const unsigned long long total_t = (unsigned long long)a.tiles_w * a.tiles_h * a.tiles_b * a.tiles_n;
-    auto magic = [&](int dv) -> uint32_t {  // exact for 0 <= x <= total_t when x * dv < 2^32
-      if (dv <= 1) return 1u;  // sentinel: x / 1
-      if (total_t * (unsigned long long)dv >= 0xFFFFFFFFULL) return 0u;
-      return (uint32_t)((0x100000000ULL + (unsigned long long)dv - 1) / (unsigned long long)dv);
-    };
-    a.mg_n = magic(a.tiles_n);
-    a.mg_w = magic(a.tiles_w);
-    a.mg_h = magic(a.tiles_h);
+    a.mg_n = fast_div_magic(a.tiles_n, total_t);
+    a.mg_w = fast_div_magic(a.tiles_w, total_t);
+    a.mg_h = fast_div_magic(a.tiles_h, total_t);
   }
   a.Ho = P.Ho;
   a.Wo = P.Wo;

@@ -38,6 +38,17 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// Division by a run-time constant d >= 1 with one multiply-high: magic = ceil(2^32 / d) is exact for 0 <= x < x_end while
+// x_end * d < 2^32; otherwise magic = 0 selects real division, and magic = 1 means d == 1.
+inline uint32_t fast_div_magic(int d, unsigned long long x_end) {
+  if (d <= 1) return 1u;
+  if (x_end * (unsigned long long)d >= 0xFFFFFFFFULL) return 0u;
+  return (uint32_t)((0x100000000ULL + (unsigned long long)d - 1) / (unsigned long long)d);
+}
+#ifdef __CUDACC__
+__device__ __forceinline__ int fast_div(int x, int d, uint32_t magic) { return magic == 1u ? x : (magic ? (int)__umulhi((uint32_t)x, magic) : x / d); }
+#endif
+
 // NMS score histogram (shared by nms.cu, the decode kernels and the fused-decode conv epilogue): kNmsBins bins per image
 constexpr int kNmsBins = 16384;
 #ifdef __CUDACC__
@@ -63,6 +74,18 @@ __device__ __forceinline__ float sigmoid_fast(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
   return r;
 }
+
+// The YOLOv5 decode of one z row and its NMS score, written once for the stand-alone decode kernel, the fused-decode conv epilogue
+// and the NMS passes that recompute scores from z, which must all produce the same fp32 bits.  Reference: y = x.sigmoid();
+// xy = (y*2 - 0.5 + grid) * stride; wh = (y*2)**2 * anchor_grid (yolov5_detect.py:50-53); score = cls * obj (yolov5.py:106).
+__device__ __forceinline__ float yolo_xy(float y, float grid, float stride) {
+  return __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(y, 2.0f), 0.5f), grid), stride);
+}
+__device__ __forceinline__ float yolo_wh(float y, float anchor) {
+  const float t2 = __fmul_rn(y, 2.0f);
+  return __fmul_rn(__fmul_rn(t2, t2), anchor);
+}
+__device__ __forceinline__ float yolo_score(float cls, float obj) { return __fmul_rn(cls, obj); }
 #endif
 
 }  // namespace cvb

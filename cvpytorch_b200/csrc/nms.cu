@@ -330,7 +330,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __
       float rbest = 0.0f;
       if (multi_label) {
         for (int c = lane; c < nc; c += 32) {
-          const float sc = __fmul_rn(__ldg(r + 5 + c), ob);
+          const float sc = yolo_score(__ldg(r + 5 + c), ob);
           if (sc > conf) {
             atomicAdd(&hist[nms_score_bin(sc)], 1u);
             rbest = fmaxf(rbest, sc);
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __
         }
       } else {
         // best class only: conf, j = x[:, 5:].max(1)
-        for (int c = lane; c < nc; c += 32) rbest = fmaxf(rbest, __fmul_rn(__ldg(r + 5 + c), ob));
+        for (int c = lane; c < nc; c += 32) rbest = fmaxf(rbest, yolo_score(__ldg(r + 5 + c), ob));
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o));
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
 #pragma unroll
           for (int k = 0; k < 3; ++k) {
             const int c = k * 32 + lane;
-            const float sc = (c < nc) ? __fmul_rn(v[i][k], ob[i]) : 0.0f;
+            const float sc = (c < nc) ? yolo_score(v[i][k], ob[i]) : 0.0f;
             const bool pass = c < nc && sc > conf && nms_score_bin(sc) >= tb;
             const uint32_t slot = warp_append(&s_cnt, pass);
             if (pass) stage[slot] = make_key(__float_as_uint(sc), (uint32_t)an[i] * (uint32_t)nc + (uint32_t)c);
@@ -427,7 +427,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
       if (multi_label) {
         for (int c0 = 0; c0 < nc; c0 += 32) {
           const int c = c0 + lane;
-          const float sc = (c < nc) ? __fmul_rn(__ldg(r + 5 + c), ob) : 0.0f;
+          const float sc = (c < nc) ? yolo_score(__ldg(r + 5 + c), ob) : 0.0f;
           const bool pass = c < nc && sc > conf && nms_score_bin(sc) >= tb;
           const uint32_t slot = warp_append(&s_cnt, pass);
           if (pass) stage[slot] = make_key(__float_as_uint(sc), (uint32_t)anchor * (uint32_t)nc + (uint32_t)c);
@@ -435,7 +435,7 @@ __global__ void __launch_bounds__(kScanThreads) nms_emit_kernel(const float* __r
       } else {
         // best class only: conf, j = x[:, 5:].max(1)
         float best;
-        const int bi = warp_argmax_first(nc, [&](int c) { return __fmul_rn(__ldg(r + 5 + c), ob); }, best);
+        const int bi = warp_argmax_first(nc, [&](int c) { return yolo_score(__ldg(r + 5 + c), ob); }, best);
         if (lane == 0 && best > conf && nms_score_bin(best) >= tb)
           stage[atomicAdd(&s_cnt, 1u)] = make_key(__float_as_uint(best), (uint32_t)anchor * (uint32_t)nc + (uint32_t)bi);
       }

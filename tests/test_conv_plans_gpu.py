@@ -12,9 +12,9 @@ processes of this file (`python tests/test_conv_plans_gpu.py --plans | --run OUT
   - test_plan_coverage parses the default plans and requires every plan dimension of the table (COVERAGE) to occur;
   - test_knob_* compare a knob's outputs with the default ones (bitwise where the K order of every element is unchanged, else the
     float64 bound) and require the plan lines to show that the knob took effect.
-The YOLOv5 decode paths (fused CVB_OUT_YOLO epilogue, yolo_decode_fast_kernel) are checked against the decode formula in float64, and
-their NMS histogram / per-row best score against what the NMS recomputes from their own z.  test_*_teeth show that the checks reject
-subtly wrong outputs.
+The YOLOv5 decode paths (fused CVB_OUT_YOLO epilogue, the stand-alone yolo_decode_kernel) are checked against the decode formula in
+float64, and their NMS histogram / per-row best score against what the NMS recomputes from their own z.  test_*_teeth show that the
+checks reject subtly wrong outputs.
 """
 import math
 import os
@@ -32,6 +32,7 @@ for _p in (ROOT, HERE):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 import fp64ref  # noqa: E402
+from test_post_gpu import _ws_regions  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -641,15 +642,6 @@ def nms_consistency(z, hist, rowmax, conf, multi, what):
     assert torch.equal(hist.long(), ref), f'{what}: histogram differs in {int((hist.long() != ref).sum())} bins'
 
 
-def _ws_regions(ws, B, A):
-    """(histogram i32 [B, 16384], rowmax f32 [B, A]) of an NmsWorkspace (layout: csrc/internal.h)."""
-    al = lambda x, a: (x + a - 1) // a * a  # noqa: E731
-    head = al(B * 16384 * 4, 256) + 6 * al(B * 4, 256)
-    rm_off = head + B * (65536 + 4096) * 8
-    raw = ws.ws[ws.ws_ptr - ws.ws.data_ptr():]
-    return raw[:B * 16384 * 4].view(torch.int32).view(B, 16384), raw[rm_off:rm_off + B * A * 4].view(torch.float32).view(B, A)
-
-
 def _decode_check(z, zref, zbound, what):
     r = fp64ref.check(z, zref, zbound, what)
     print(f'{what}: worst error / bound {r:.3f}')
@@ -690,33 +682,54 @@ def test_fused_decode_vs_formula(cuda, no, multi):
     nms_consistency(zl, hist, rowmax[:, z_off:z_off + na * npix], conf, multi and no - 5 > 1, f'fused decode no={no}')
 
 
-@pytest.mark.parametrize('no,multi,hist', [(64, True, True), (85, True, True), (85, False, True), (96, True, True), (96, False, True),
-                                           (85, True, False)])
-def test_fast_decode_vs_formula(cuda, no, multi, hist):
-    """yolo_decode_fast_kernel (cvb_yolo_decode without xperm, no >= 64) against the float64 decode of its own fp32 input (dx = 0), and
-    its histogram / rowmax (both variants) against its own z."""
+DECODE_CASES = [  # (no, multi, hist, na, nx, xperm)
+    (64, True, True, 3, 13, False), (85, True, True, 3, 13, False), (85, False, True, 3, 13, False), (96, True, True, 3, 13, False),
+    (96, False, True, 3, 13, False), (85, True, False, 3, 13, False),
+    (85, True, False, 3, 13, True),    # xperm: the raw rows of the want_raw graph
+    (85, True, True, 3, 13, True),     # xperm and the histogram
+    (8, True, True, 2, 13, False),     # small no, two anchors
+    (6, False, True, 3, 13, False),    # one class
+    (85, True, True, 3, 1, False),     # nx = 1
+    (6, False, True, 1, 20800, False),  # pix * nx >= 2^32: real division instead of the multiply-high
+]
+
+
+def _decode_id(c):
+    no, multi, hist, na, nx, xperm = c
+    return f'{no}-{multi}-{hist}' + (f'-na{na}' if na != 3 else '') + (f'-nx{nx}' if nx != 13 else '') + ('-xperm' if xperm else '')
+
+
+@pytest.mark.parametrize('no,multi,hist,na,nx,xperm', DECODE_CASES, ids=[_decode_id(c) for c in DECODE_CASES])
+def test_fast_decode_vs_formula(cuda, no, multi, hist, na, nx, xperm):
+    """yolo_decode_kernel (cvb_yolo_decode) against the float64 decode of its own fp32 input (dx = 0), also max-normalised within
+    5e-6; its xperm rows equal the permuted raw tensor bit for bit; its histogram / rowmax (both variants) against its own z."""
     from cvpytorch_b200 import ops
-    B, ny, nx, na, z_off, stride = 2, 10, 13, 3, 2, 8.0
+    B, ny, z_off, stride = 2, 10, 2, 8.0
     g = torch.Generator().manual_seed(60 + no)
     pitch = (na * no + 7) // 8 * 8
     raw = ops.F32Tensor(B, ny, nx, pitch)
     raw.data.copy_(torch.randn(B, ny, nx, pitch, generator=g) * 3)
-    anchors = torch.tensor([[10., 13.], [16., 30.], [33., 23.]])
+    anchors = torch.tensor([[10., 13.], [16., 30.], [33., 23.]])[:na]
     A, conf = na * ny * nx + z_off + 3, 0.05
     ws = ops.NmsWorkspace(B, A, no - 5)
     ops.nms_reset(ws)
     z = torch.full((B, A, no), float('nan'), device='cuda')
-    ops.yolo_decode(raw.view(0, na * no), na, no, anchors.cuda().contiguous(), stride, z, A, z_off, None, ws if hist else None, conf, multi)
+    xp = torch.full((B, na, ny, nx, no), float('nan'), device='cuda') if xperm else None
+    ops.yolo_decode(raw.view(0, na * no), na, no, anchors.cuda().contiguous(), stride, z, A, z_off, xp, ws if hist else None, conf, multi)
     torch.cuda.synchronize()
     npix = ny * nx
-    xr = raw.data[..., :na * no].double().view(B, npix, na, no).permute(0, 2, 1, 3)
+    xr = raw.data[..., :na * no].view(B, npix, na, no).permute(0, 2, 1, 3)
+    if xperm:
+        assert torch.equal(xp.view(B, na, npix, no), xr), 'xperm is not the permuted raw tensor'
+    xr = xr.double()
     zref, zbound = decode_reference(xr, torch.zeros_like(xr), anchors.double().cuda(), stride, nx)
     zl = z[:, z_off:z_off + na * npix]
-    _decode_check(zl.view(B, na, npix, no), zref, zbound, f'fast decode no={no}')
+    _decode_check(zl.view(B, na, npix, no), zref, zbound, f'decode no={no}')
+    assert fp64ref.max_rel(zl.view(B, na, npix, no), zref) < 5e-6
     assert bool(z[:, :z_off].isnan().all()) and bool(z[:, z_off + na * npix:].isnan().all()), 'decode wrote outside its z rows'
     if hist:
         h, rowmax = _ws_regions(ws, B, A)
-        nms_consistency(zl, h, rowmax[:, z_off:z_off + na * npix], conf, multi, f'fast decode no={no}')
+        nms_consistency(zl, h, rowmax[:, z_off:z_off + na * npix], conf, multi and no - 5 > 1, f'decode no={no}')
 
 
 def test_decode_checks_teeth(cuda):

@@ -79,33 +79,6 @@ def test_nms_full_path_with_global_sort_steps(cuda):
     _nms_case(pred)
 
 
-def test_decode_matches_reference_formula(cuda):
-    from cvpytorch_b200 import ops
-    from oracle import yolov5_oracle as YO
-    torch.manual_seed(3)
-    B, ny, nx, na, no = 2, 12, 20, 3, 85
-    raw = ops.F32Tensor(B, ny, nx, 256)
-    raw.data.normal_(0, 2)
-    anchors_px = (torch.tensor(YO.ANCHORS[1]) * 16.0).float().cuda().contiguous()
-    z = torch.zeros(B, na * ny * nx + 5, no, device='cuda')
-    xperm = torch.zeros(B, na, ny, nx, no, device='cuda')
-    ops.yolo_decode(raw.view(0, 255), na, no, anchors_px, 16.0, z, z.shape[1], 5, xperm)
-    torch.cuda.synchronize()
-    r = raw.data[..., :255].view(B, ny, nx, na, no).permute(0, 3, 1, 2, 4).contiguous().cpu()
-    assert torch.equal(xperm.cpu(), r)
-    yv, xv = torch.meshgrid([torch.arange(ny), torch.arange(nx)], indexing='ij')
-    grid = torch.stack((xv, yv), 2).expand((1, na, ny, nx, 2)).float()
-    ag = (torch.tensor(YO.ANCHORS[1]).float() * 16.0).view(1, na, 1, 1, 2).expand(1, na, ny, nx, 2)
-    y = r.sigmoid()
-    y[..., 0:2] = (y[..., 0:2] * 2 - 0.5 + grid) * 16.0
-    y[..., 2:4] = (y[..., 2:4] * 2) ** 2 * ag
-    ref = y.view(B, -1, no)
-    got = z[:, 5:].cpu()
-    err = float((got - ref).abs().max() / ref.abs().max())
-    assert err < 5e-6, err  # sigmoid = ex2.approx + rcp.approx (|rel err| ~ 2^-22)
-    assert float(z[:, :5].abs().max()) == 0.0
-
-
 def test_output_side_rescale_clip_and_confusion_matrix(cuda):
     """SURVEY.md 8(f) rank 2: device-side box rescale/clip == the reference's numpy lines (yolov5.py:274-281) bit for bit;
     device confusion matrix == eval_segmentation.py:52-57 (np.bincount) exactly."""
