@@ -63,6 +63,11 @@ SYMBOLS = {
     'cvb_train_conv_wgrad_pad': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_train_pred_conv': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     'cvb_train_pred_grad': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_yolox_loss_workspace_bytes': (c_size_t, [c_int32, c_int32]),
+    'cvb_train_yolox_loss_fwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), c_int32, c_int32, c_void_p, c_int32, c_int32,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'cvb_train_yolox_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), c_int32, c_int32, c_void_p, c_int32, c_int32,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

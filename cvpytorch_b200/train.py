@@ -10,14 +10,15 @@ Mirrors (paths relative to the reference checkout), with the same constructor ar
   YOLOXNeck    src/models/necks/yolox_neck.py:13-74           top-down (upsample + concat) and bottom-up (stride-2 conv + concat) CSP path
   ConvModule   src/models/modules/convs.py                     conv -> BN -> SiLU as the YOLOX head builds it (1x1 stems with padding 1)
   YOLOXHead    src/models/heads/yolox_head.py:14-88            stems, cls / reg branches, prediction convs with bias -> fp32 NCHW outputs
+  YOLOXLoss    src/losses/det/yolox_loss.py:73-436             SimOTA assignment, IoU / objectness / class losses and their gradient
 
 Channel counts of every convolution: 16, 32 or multiples of 64 (YOLOX-n, -s and -l; the 24 / 48 / 80-wide -t, -m and -x raise).  The
 prediction convs (num_classes, 4 and 1 outputs) run as GEMMs zero-padded to the next such width.
 
 What runs where: every convolution (forward, backward-data, backward-weight) is a bf16 wgmma implicit GEMM and every BatchNorm / SiLU pass
 (statistics, apply, backward reductions, backward apply) is a kernel of libcvb200.so (csrc/train_kernels.cu).  torch.autograd only chains the
-per-layer Functions and adds the gradients of the shortcut / concat fan-outs (tensor plumbing); the loss and the optimiser stay in PyTorch,
-as in the reference trainer (trainer.py:177-207).  Precision: bf16 activations / gradients, fp32 accumulation, fp32 master weights and fp32
+per-layer Functions and adds the gradients of the shortcut / concat fan-outs (tensor plumbing); the YOLOX loss is csrc/yolox_loss.cu
+(YOLOXLoss below); the optimiser stays in PyTorch, as in the reference trainer (trainer.py:177-207).  Precision: bf16 activations / gradients, fp32 accumulation, fp32 master weights and fp32
 weight gradients (BASELINE.json configs[3] asks for a bf16 step).  No CPU fallback: CPU tensors raise.
 
 Inside a block activations are NHWC bf16; `CSPLayer.forward` accepts / returns the reference's NCHW tensors (layout change at the boundary).
@@ -656,3 +657,100 @@ class YOLOXHead(nn.Module):
 
     def forward(self, x):
         return self.forward_nhwc([_to_nhwc(t, 'YOLOX neck / head (H100 training)') for t in x])
+
+
+# ------------------------------------------------------------------------------------------------ YOLOX loss (SimOTA assignment + the three terms)
+def _loss_levels(preds, strides):
+    """-> ctypes (pointer array, shape array, stride array) of the head outputs, validated on the host by the C entry points."""
+    n = len(preds)
+    ptrs = (ctypes.c_void_p * n)(*[p.data_ptr() for p in preds])
+    shapes = (ctypes.c_int32 * (4 * n))(*[int(d) for p in preds for d in (tuple(p.shape) if p.dim() == 4 else (0, 0, 0, 0))])
+    strd = (ctypes.c_float * n)(*[float(s) for s in strides])
+    return ptrs, shapes, strd
+
+
+def yolox_loss_forward(preds, targets, strides, num_classes):
+    """preds: the head's fp32 NCHW outputs [B, 5 + num_classes, h, w] (CUDA, contiguous); targets fp32 [B, max_gt, 5] (class, cx, cy, w, h).
+    -> (out fp32 [6] = loss, iou_loss, conf_loss, cls_loss, num_fg ratio, num_fg; matched_gt int32 [B, A], -1 = background; matched_iou [B, A])."""
+    if len(preds) != len(strides):
+        raise ValueError(f'YOLOXLoss: {len(strides)} strides for {len(preds)} outputs')
+    B = preds[0].shape[0]
+    A = sum(p.shape[2] * p.shape[3] for p in preds)
+    dev = preds[0].device
+    ws = torch.empty((max(int(_lib.lib().cvb_train_yolox_loss_workspace_bytes(B, A)), 1),), dtype=torch.uint8, device=dev)
+    out = torch.empty((6,), dtype=torch.float32, device=dev)
+    matched_gt = torch.empty((B, A), dtype=torch.int32, device=dev)
+    matched_iou = torch.empty((B, A), dtype=torch.float32, device=dev)
+    ptrs, shapes, strd = _loss_levels(preds, strides)
+    _lib.check(_lib.lib().cvb_train_yolox_loss_fwd(ptrs, shapes, strd, len(preds), num_classes, _p(targets), B, targets.shape[1], _p(matched_gt),
+                                                   _p(matched_iou), _p(out), _p(ws), ws.numel(), _stream()), 'cvb_train_yolox_loss_fwd')
+    return out, matched_gt, matched_iou
+
+
+def yolox_loss_backward(preds, targets, strides, num_classes, matched_gt, matched_iou, out, grad_out):
+    """d(sum_i grad_out[i] * out[i], i < 4) / d(preds) under the forward's assignment -> fp32 NCHW gradients shaped like preds."""
+    grads = [torch.empty_like(p) for p in preds]
+    ptrs, shapes, strd = _loss_levels(preds, strides)
+    gptrs = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+    _lib.check(_lib.lib().cvb_train_yolox_loss_bwd(ptrs, shapes, strd, len(preds), num_classes, _p(targets), preds[0].shape[0], targets.shape[1],
+                                                   _p(matched_gt), _p(matched_iou), _p(out), _p(grad_out), gptrs, _stream()), 'cvb_train_yolox_loss_bwd')
+    return grads
+
+
+class _YOLOXLossFn(torch.autograd.Function):
+    """out [6] = (loss, iou_loss, conf_loss, cls_loss, num_fg ratio, num_fg) of the head outputs; the assignment is kept for the backward
+    (two [B, A] tensors), the gradient is recomputed from it and scaled by the incoming gradients of the four loss entries."""
+
+    @staticmethod
+    def forward(ctx, targets, strides, num_classes, *preds):
+        out, matched_gt, matched_iou = yolox_loss_forward(preds, targets, strides, num_classes)
+        ctx.save_for_backward(targets, matched_gt, matched_iou, out, *preds)
+        ctx.strides, ctx.num_classes = strides, num_classes
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        targets, matched_gt, matched_iou, out, *preds = ctx.saved_tensors
+        grads = yolox_loss_backward(preds, targets, ctx.strides, ctx.num_classes, matched_gt, matched_iou, out, g.float().contiguous())
+        return (None, None, None, *grads)
+
+
+def _loss_targets(targets, B, device):
+    """The reference's targets [B, max_gt, 5] as the contiguous fp32 CUDA tensor of the kernels (an empty GT list becomes one zero row)."""
+    if not isinstance(targets, torch.Tensor) or targets.dim() != 3 or targets.shape[0] != B or targets.shape[2] != 5:
+        raise ValueError(f'YOLOXLoss: targets must be a [B={B}, max_gt, 5] tensor of (class, cx, cy, w, h) rows')
+    _check_cuda(targets, 'YOLOXLoss targets')
+    t = targets.detach().to(device=device, dtype=torch.float32)
+    if t.shape[1] == 0:
+        t = torch.zeros((B, 1, 5), dtype=torch.float32, device=device)
+    return t.contiguous()
+
+
+class YOLOXLoss(nn.Module):
+    """src/losses/det/yolox_loss.py:73-282 on the H100 kernels (csrc/yolox_loss.cu): same constructor, no parameters or buffers.
+    forward(preds, targets) takes the head's list of fp32 NCHW outputs [B, 5 + num_classes, h, w] (CUDA) and targets [B, max_gt, 5] (class, cx,
+    cy, w, h in pixels; at most 1024 rows) and returns the reference's dict {loss, conf_loss, cls_loss, iou_loss, num_fg} of device scalars,
+    with no host sync: the whole loss can be captured in a CUDA graph.  The L1 (use_l1) and re-ID (reid_dim > 0) branches raise
+    NotImplementedError."""
+
+    def __init__(self, num_classes, reid_dim=0, id_nums=None, strides=[8, 16, 32], in_channels=[256, 512, 1024]):
+        super().__init__()
+        if reid_dim > 0:
+            raise NotImplementedError('H100 YOLOXLoss: the re-ID branch (reid_dim > 0) is not implemented')
+        self.n_anchors = 1
+        self.num_classes = num_classes
+        self.strides = strides
+        self.reid_dim = reid_dim
+        self.use_l1 = False
+        self.in_channels = in_channels
+
+    def forward(self, preds, targets, imgs=None):
+        if self.use_l1:
+            raise NotImplementedError('H100 YOLOXLoss: the L1 branch (use_l1 = True) is not implemented')
+        if len(preds) != len(self.strides):
+            raise ValueError(f'YOLOXLoss: {len(self.strides)} strides for {len(preds)} outputs')
+        for p in preds:
+            _check_cuda(p, 'YOLOXLoss')
+        preds = [p.float().contiguous() for p in preds]
+        out = _YOLOXLossFn.apply(_loss_targets(targets, preds[0].shape[0], preds[0].device), tuple(self.strides), self.num_classes, *preds)
+        return {'loss': out[0], 'conf_loss': out[2], 'cls_loss': out[3], 'iou_loss': out[1], 'num_fg': out[4].detach()}

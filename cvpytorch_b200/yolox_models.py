@@ -20,7 +20,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import _lib, ops, train
 from .engine import GraphBuilder
 from .modules import ConvModule, CSPLayer, SPPF, _build, _EmitModule, _emit_csp, _Standalone, folded
 
@@ -247,7 +247,8 @@ def build_head(cfg):
 
 
 class YOLOX(_Standalone):
-    """Model-level drop-in for src.models.yolox.YOLOX (inference: mode='val')."""
+    """Model-level drop-in for src.models.yolox.YOLOX: mode='val' runs the cached inference graph (eval()), mode='train' the training
+    kernels and the YOLOXLoss (train()) over the same parameters."""
     cfg = {"nano": [0.33, 0.25], "tiny": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
     input_norm = dict(mean=(0.406, 0.456, 0.485), std=(0.225, 0.224, 0.229), reverse_channels=True)
 
@@ -271,6 +272,16 @@ class YOLOX(_Standalone):
         self.head = build_head(hcfg)
         self.stride = [8, 16, 32]
         self.conf_thr, self.nms_thr = 0.01, 0.65   # src/models/yolox.py:94-95
+        lcfg = model_cfg.get('LOSS') if isinstance(model_cfg, dict) else getattr(model_cfg, 'LOSS', None)
+        lcfg = dict(lcfg) if lcfg else {'name': 'YOLOXLoss'}
+        if lcfg.pop('name', 'YOLOXLoss') != 'YOLOXLoss':
+            raise NotImplementedError('YOLOX (H100): only the YOLOXLoss is on the training path')
+        lcfg['num_classes'] = self.num_classes
+        self.loss = train.YOLOXLoss(**lcfg)  # (no parameters or buffers: the state_dict keys stay the inference model's)
+        # the training modules (train.CSPDarknet / YOLOXNeck / YOLOXHead), built on the first training forward over this model's own
+        # parameters and buffers; kept out of the module tree so that state_dict(), parameters() and .to() see each tensor once
+        self.__dict__['_train_modules'] = None
+        self._cfgs = (bcfg, ncfg, hcfg)
 
     def build_graph(self, B, H, W, device, u8_input=False):
         g = GraphBuilder(B, device)
@@ -297,11 +308,61 @@ class YOLOX(_Standalone):
         G['g'].run()
         return G['ws'].det, G['ws'].count
 
+    def _training_modules(self):
+        """(train.CSPDarknet, train.YOLOXNeck, train.YOLOXHead) whose parameters and buffers ARE this model's (re-bound on every call: .to()
+        replaces buffer tensors).  Widths the training kernels refuse (YOLOX-t, -m, -x) raise NotImplementedError."""
+        if self._train_modules is None:
+            strip = lambda c: {k: v for k, v in c.items() if k != 'name'}  # noqa: E731
+            bcfg, ncfg, hcfg = self._cfgs
+            mods = (train.CSPDarknet(**strip(bcfg)), train.YOLOXNeck(**strip(ncfg)), train.YOLOXHead(**strip(hcfg)))
+            binds = []
+            for tm, im in zip(mods, (self.backbone, self.neck, self.head)):
+                if list(tm.state_dict()) != list(im.state_dict()):
+                    raise NotImplementedError(f'YOLOX (H100) training: {type(im).__name__} keys differ from the training module\'s')
+                for name, sub in tm.named_modules():  # (bound by name: the key lists are equal)
+                    if sub._parameters or sub._buffers:
+                        src = im.get_submodule(name)
+                        binds += [(sub._parameters, k, src._parameters) for k in sub._parameters]
+                        binds += [(sub._buffers, k, src._buffers) for k in sub._buffers]
+            self.__dict__['_train_modules'] = (mods, binds)
+        mods, binds = self._train_modules
+        for dst, k, src in binds:
+            dst[k] = src[k]
+        return mods
+
+    def pack_targets(self, imgs, targets):
+        """trans_specific_format (yolox.py:112-139): the per-image target dicts -> gt [B, max_labels, 5] rows (label, box) on the images'
+        device, zero rows after each image's boxes.  A [B, max_labels, 5] tensor is taken as already packed."""
+        if isinstance(targets, torch.Tensor):
+            return targets
+        max_labels = max(t['labels'].shape[0] for t in targets)
+        gt = torch.zeros((len(targets), max_labels, 5), device=imgs.device)
+        for i, t in enumerate(targets):
+            n = t['labels'].shape[0]
+            gt[i, :n, 0] = t['labels'].to(imgs.device, torch.float32)
+            gt[i, :n, 1:] = t['boxes'].to(imgs.device, torch.float32)
+        return gt
+
+    def forward_train(self, imgs, targets):
+        """The reference's training forward (yolox.py:150-157, 186-187) on the H100 training kernels: backbone -> neck -> head -> loss,
+        over this model's parameters; returns the loss dict {loss, conf_loss, cls_loss, iou_loss, num_fg} (device scalars, no host sync)."""
+        if not self.training:
+            raise RuntimeError("YOLOX (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
+        if isinstance(imgs, (list, tuple)):
+            imgs = torch.stack(list(imgs))
+        if not imgs.is_cuda:
+            raise _lib.CvbError('YOLOX (H100) training: CUDA images required (the training path has no CPU fallback)')
+        gt = self.pack_targets(imgs, targets)
+        bb, nk, hd = self._training_modules()
+        return self.loss(hd.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gt)
+
     def forward(self, imgs, targets=None, mode='infer', **kwargs):
         if mode == 'infer':
             return  # the reference returns None here (yolox.py:144-149)
+        if mode == 'train':
+            return self.forward_train(imgs, targets)
         if mode != 'val':
-            raise RuntimeError("YOLOX (H100): only mode='val' (inference) is implemented; training stays on the reference")
+            raise RuntimeError(f"YOLOX (H100): unknown mode {mode!r}")
         if isinstance(imgs, (list, tuple)):
             imgs = torch.stack(list(imgs))
         det, cnt = self.predict(imgs)

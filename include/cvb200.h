@@ -416,6 +416,26 @@ int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t 
 int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int32_t h, int32_t w, int32_t c_off, int32_t cout, int32_t cout_pad, void* dy, float* dbias,
                         void* stream);
 
+/* YOLOX training loss (src/losses/det/yolox_loss.py:73-436; csrc/yolox_loss.cu): SimOTA assignment, the IoU / objectness / class losses
+ * and their gradient with respect to the head outputs.  preds[l]: fp32 NCHW [B, 5 + nc, h_l, w_l] (read in place), shapes[4 l ..] =
+ * (B, 5 + nc, h_l, w_l), strides[l] > 0, 1 <= nlev <= 4; anchors in level order, row-major within a level (A = sum h_l w_l).
+ * targets: fp32 [B, max_gt, 5] rows (class, cx, cy, w, h) in pixels, 1 <= max_gt <= 1024; an image uses its first nlabel rows, nlabel =
+ * the number of rows with a positive sum.
+ * cvb_train_yolox_loss_fwd: out fp32 [6] = (loss, iou_loss, conf_loss, cls_loss, num_fg / max(num_gt, 1), num_fg) with num_fg = max(foreground
+ *   anchors, 1); matched_gt int32 [B, A] (the matched GT row, -1 = background) and matched_iou fp32 [B, A] (0 for background).  Ties: the lower
+ *   anchor index in a GT's top-k, the lower GT index in the conflict argmin; a GT in an image without candidate anchors matches nothing.
+ *   workspace: cvb_train_yolox_loss_workspace_bytes(B, A) bytes, 256-byte aligned, owned by the caller.  No host sync; bitwise reproducible.
+ * cvb_train_yolox_loss_bwd: grads[l] fp32 NCHW, shapes of preds[l] (every element written) = d(sum_i grad_out[i] out[i]) / d(preds[l]) for
+ *   i < 4, under the forward's assignment (matched_gt, matched_iou, fwd_out = its out).  grad_out: fp32 [4] on the device.
+ */
+size_t cvb_train_yolox_loss_workspace_bytes(int32_t B, int32_t A);
+int cvb_train_yolox_loss_fwd(const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, const float* targets,
+                             int32_t B, int32_t max_gt, int32_t* matched_gt, float* matched_iou, float* out, void* workspace, size_t ws_bytes,
+                             void* stream);
+int cvb_train_yolox_loss_bwd(const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, const float* targets,
+                             int32_t B, int32_t max_gt, const int32_t* matched_gt, const float* matched_iou, const float* fwd_out,
+                             const float* grad_out, float* const* grads, void* stream);
+
 /* Library info / errors */
 const char* cvb_last_error_string(void);
 int cvb_version(void);
