@@ -7,19 +7,15 @@
 
 namespace cvb {
 
-__device__ __forceinline__ void split_f32(float x, __half* hi, __half* lo) {
-  x = fminf(fmaxf(x, -65504.0f), 65504.0f);
-  const __half h = __float2half_rn(x);
-  *hi = h;
-  *lo = __float2half_rn(x - __half2float(h));
-}
-
 // ------------------------------------------------------------------ NCHW fp32 -> split16 NHWC
-// grid (ceil(W/32), ceil(C/32), B*H), block (32, 8): smem transpose so both sides are coalesced.
+// grid (ceil(W/32), ceil(C/32), image rows), block (32, 8): smem transpose so both sides are coalesced.  Image row b*H + h =
+// bh0 + blockIdx.z: the host launches chunks of at most kMaxGridZ rows (the grid's z limit), so any B*H converts.
+constexpr int kMaxGridZ = 65535;
+
 __global__ void nchw_to_split_kernel(const float* __restrict__ src, int B, int C, int H, int W, __half* __restrict__ dst, int pitch,
-                                     long long plane) {
+                                     long long plane, int bh0) {
   __shared__ float tile[32][33];
-  const int bh = blockIdx.z;
+  const int bh = bh0 + (int)blockIdx.z;
   const int b = bh / H, h = bh % H;
   const int w0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += 8) {
@@ -30,20 +26,21 @@ __global__ void nchw_to_split_kernel(const float* __restrict__ src, int B, int C
   for (int i = threadIdx.y; i < 32; i += 8) {
     const int w = w0 + i, c = c0 + threadIdx.x;
     if (w < W && c < C) {
-      __half hi, lo;
-      split_f32(tile[threadIdx.x][i], &hi, &lo);
+      const float v = tile[threadIdx.x][i];
+      uint32_t hi, lo;
+      split_pair(v, v, hi, lo);
       const size_t o = (((size_t)b * H + h) * W + w) * pitch + c;
-      dst[o] = hi;
-      dst[o + plane] = lo;
+      dst[o] = __ushort_as_half((unsigned short)hi);
+      dst[o + plane] = __ushort_as_half((unsigned short)lo);
     }
   }
 }
 
 // split16 NHWC -> NCHW fp32 (x = hi + lo)
 __global__ void split_to_nchw_kernel(const __half* __restrict__ src, int B, int C, int H, int W, int pitch, long long plane,
-                                     float* __restrict__ dst) {
+                                     float* __restrict__ dst, int bh0) {
   __shared__ float tile[32][33];
-  const int bh = blockIdx.z;
+  const int bh = bh0 + (int)blockIdx.z;
   const int b = bh / H, h = bh % H;
   const int w0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += 8) {
@@ -62,9 +59,10 @@ __global__ void split_to_nchw_kernel(const __half* __restrict__ src, int B, int 
   }
 }
 
-__global__ void f32nhwc_to_nchw_kernel(const float* __restrict__ src, int B, int C, int H, int W, int pitch, float* __restrict__ dst) {
+__global__ void f32nhwc_to_nchw_kernel(const float* __restrict__ src, int B, int C, int H, int W, int pitch, float* __restrict__ dst,
+                                       int bh0) {
   __shared__ float tile[32][33];
-  const int bh = blockIdx.z;
+  const int bh = bh0 + (int)blockIdx.z;
   const int b = bh / H, h = bh % H;
   const int w0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += 8) {
@@ -104,11 +102,7 @@ __global__ void stem_s2d_kernel(const float* __restrict__ src, int B, int H, int
     uint32_t hq[8], lq[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      __half h0, l0, h1, l1;
-      split_f32(v[2 * k], &h0, &l0);
-      split_f32(v[2 * k + 1], &h1, &l1);
-      hq[k] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-      lq[k] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+      split_pair(v[2 * k], v[2 * k + 1], hq[k], lq[k]);
     }
     __half* o = dst + (((size_t)b * H2 + h2) * Wd + (w2 + col_off)) * pitch;  // Wd > W2: zero-padded row-window layout
     reinterpret_cast<uint4*>(o)[0] = make_uint4(hq[0], hq[1], hq[2], hq[3]);
@@ -191,11 +185,7 @@ __global__ void __launch_bounds__(256) stem_s2d_u8_kernel(const uint8_t* __restr
       uint32_t hq[8], lq[8];
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        __half h0, l0, h1, l1;
-        split_f32(v[2 * k], &h0, &l0);
-        split_f32(v[2 * k + 1], &h1, &l1);
-        hq[k] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-        lq[k] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+        split_pair(v[2 * k], v[2 * k + 1], hq[k], lq[k]);
       }
       __half* o = dst + (((size_t)b * H2 + h2) * Wd + (w2 + q + col_off)) * pitch;
       reinterpret_cast<uint4*>(o)[0] = make_uint4(hq[0], hq[1], hq[2], hq[3]);
@@ -208,7 +198,7 @@ __global__ void __launch_bounds__(256) stem_s2d_u8_kernel(const uint8_t* __restr
 
 // ------------------------------------------------------------------ SPPF: three chained 5x5/s1/p2 max pools
 // One CTA per (image, 8-channel slice): the whole HxW map of the slice lives in shared memory as fp32;
-// each pool is a separable row-max / column-max pass.  y2 == 9x9 pool, y3 == 13x13 pool of x.
+// each pool is a separable row-max / column-max pass.  y2 == 9x9 pool, y3 == 13x13 pool of x.  NaN propagates (nan_max).
 __global__ void sppf_pool_kernel(const __half* __restrict__ x, int H, int W, int xp, long long xplane, __half* __restrict__ y1, int p1,
                                  long long plane1, __half* __restrict__ y2, int p2, long long plane2, __half* __restrict__ y3, int p3,
                                  long long plane3, int cgroups) {
@@ -246,10 +236,10 @@ __global__ void sppf_pool_kernel(const __half* __restrict__ x, int H, int W, int
         const int ww = w + d;
         if (d != 0 && ww >= 0 && ww < W) {
           const float4 v = cur4[(p + d) * 2 + hf];
-          m.x = fmaxf(m.x, v.x);
-          m.y = fmaxf(m.y, v.y);
-          m.z = fmaxf(m.z, v.z);
-          m.w = fmaxf(m.w, v.w);
+          m.x = nan_max(m.x, v.x);
+          m.y = nan_max(m.y, v.y);
+          m.z = nan_max(m.z, v.z);
+          m.w = nan_max(m.w, v.w);
         }
       }
       tmp4[i] = m;
@@ -264,10 +254,10 @@ __global__ void sppf_pool_kernel(const __half* __restrict__ x, int H, int W, int
         const int hh = h + d;
         if (d != 0 && hh >= 0 && hh < H) {
           const float4 v = tmp4[(p + d * W) * 2 + hf];
-          m.x = fmaxf(m.x, v.x);
-          m.y = fmaxf(m.y, v.y);
-          m.z = fmaxf(m.z, v.z);
-          m.w = fmaxf(m.w, v.w);
+          m.x = nan_max(m.x, v.x);
+          m.y = nan_max(m.y, v.y);
+          m.z = nan_max(m.z, v.z);
+          m.w = nan_max(m.w, v.w);
         }
       }
       curw4[i] = m;
@@ -277,11 +267,7 @@ __global__ void sppf_pool_kernel(const __half* __restrict__ x, int H, int W, int
       uint32_t hq[4], lq[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        __half h0, l0, h1, l1;
-        split_f32(cur[p * 8 + 2 * k], &h0, &l0);
-        split_f32(cur[p * 8 + 2 * k + 1], &h1, &l1);
-        hq[k] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-        lq[k] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+        split_pair(cur[p * 8 + 2 * k], cur[p * 8 + 2 * k + 1], hq[k], lq[k]);
       }
       const size_t o = ((size_t)b * npix + p) * pitches[r] + c0;
       *reinterpret_cast<uint4*>(outs[r] + o) = make_uint4(hq[0], hq[1], hq[2], hq[3]);
@@ -404,7 +390,8 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
 }
 
 // ------------------------------------------------------------------ 3x3 / stride 2 / pad 1 max pool (ResNet stem)
-// one thread per (output pixel, 8-channel vector); max over hi+lo values, result re-split exactly (max is one of the inputs)
+// one thread per (output pixel, 8-channel vector); max over hi+lo values, result re-split exactly (max is one of the inputs).  A NaN
+// is taken and then kept, like F.max_pool2d; the running maximum starts as -inf (hi = 0xFC00) so an all -inf window gives -inf.
 __global__ void maxpool3x3s2_kernel(const __half* __restrict__ x, int B, int H, int W, int C, int xp, long long xplane,
                                     __half* __restrict__ y, int Ho, int Wo, int yp, long long yplane) {
   const int cv = C / 8;
@@ -417,7 +404,7 @@ __global__ void maxpool3x3s2_kernel(const __half* __restrict__ x, int B, int H, 
     const int ho = (int)(t % Ho);
     const int b = (int)(t / Ho);
     float best[8];
-    uint4 bh = make_uint4(0, 0, 0, 0), bl = make_uint4(0, 0, 0, 0);
+    uint4 bh = make_uint4(0xFC00FC00u, 0xFC00FC00u, 0xFC00FC00u, 0xFC00FC00u), bl = make_uint4(0, 0, 0, 0);
     uint32_t* bhw = reinterpret_cast<uint32_t*>(&bh);
     uint32_t* blw = reinterpret_cast<uint32_t*>(&bl);
 #pragma unroll
@@ -438,12 +425,12 @@ __global__ void maxpool3x3s2_kernel(const __half* __restrict__ x, int B, int H, 
           const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[e]));
           const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(&lw[e]));
           const float v0 = hf.x + lf.x, v1 = hf.y + lf.y;
-          if (v0 > best[2 * e]) {
+          if (v0 > best[2 * e] || (v0 != v0 && best[2 * e] == best[2 * e])) {
             best[2 * e] = v0;
             bhw[e] = (bhw[e] & 0xFFFF0000u) | (hw[e] & 0xFFFFu);
             blw[e] = (blw[e] & 0xFFFF0000u) | (lw[e] & 0xFFFFu);
           }
-          if (v1 > best[2 * e + 1]) {
+          if (v1 > best[2 * e + 1] || (v1 != v1 && best[2 * e + 1] == best[2 * e + 1])) {
             best[2 * e + 1] = v1;
             bhw[e] = (bhw[e] & 0xFFFFu) | (hw[e] & 0xFFFF0000u);
             blw[e] = (blw[e] & 0xFFFFu) | (lw[e] & 0xFFFF0000u);
@@ -561,11 +548,7 @@ __global__ void gn_apply_kernel(const __half* __restrict__ x, int npix, int C, i
         v0 = fmaxf(v0, 0.0f);
         v1 = fmaxf(v1, 0.0f);
       }
-      __half h0, l0, h1, l1;
-      split_f32(v0, &h0, &l0);
-      split_f32(v1, &h1, &l1);
-      oh[e] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-      ol[e] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+      split_pair(v0, v1, oh[e], ol[e]);
     }
     const size_t oo = ((size_t)b * npix + p) * yp + g * 8;
     *reinterpret_cast<uint4*>(y + oo) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
@@ -625,11 +608,7 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const __half* __restrict
         v0 = fmaxf(v0, 0.0f);
         v1 = fmaxf(v1, 0.0f);
       }
-      __half h0, l0, h1, l1;
-      split_f32(v0, &h0, &l0);
-      split_f32(v1, &h1, &l1);
-      oh[e] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-      ol[e] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+      split_pair(v0, v1, oh[e], ol[e]);
     }
     const size_t oo = (((size_t)b * H + h) * W + w) * yp + c8 * 8;
     *reinterpret_cast<uint4*>(y + oo) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
@@ -709,11 +688,7 @@ __global__ void __launch_bounds__(256) dwconv3x3_d1_kernel(const __half* __restr
         v0 = fmaxf(v0, 0.0f);
         v1 = fmaxf(v1, 0.0f);
       }
-      __half h0, l0, h1, l1;
-      split_f32(v0, &h0, &l0);
-      split_f32(v1, &h1, &l1);
-      oh[e] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-      ol[e] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+      split_pair(v0, v1, oh[e], ol[e]);
     }
     const size_t oo = (((size_t)b * H + h) * W + (w0 + j)) * yp + c8 * 8;
     *reinterpret_cast<uint4*>(y + oo) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
@@ -752,10 +727,11 @@ __global__ void global_avgpool_kernel(const __half* __restrict__ x, int npix, in
     __syncthreads();
   }
   if (threadIdx.x < 8) {
-    __half h, l;
-    split_f32(red[threadIdx.x][0] / (float)npix, &h, &l);
-    y[(size_t)b * yp + c8 * 8 + threadIdx.x] = h;
-    y[(size_t)b * yp + c8 * 8 + threadIdx.x + yplane] = l;
+    const float m = red[threadIdx.x][0] / (float)npix;
+    uint32_t h, l;
+    split_pair(m, m, h, l);
+    y[(size_t)b * yp + c8 * 8 + threadIdx.x] = __ushort_as_half((unsigned short)h);
+    y[(size_t)b * yp + c8 * 8 + threadIdx.x + yplane] = __ushort_as_half((unsigned short)l);
   }
 }
 
@@ -806,11 +782,7 @@ __global__ void __launch_bounds__(256) bilinear_resize_kernel(const __half* __re
     uint32_t oh[4], ol[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      __half a0, b0, a1, b1;
-      split_f32(acc[2 * e], &a0, &b0);
-      split_f32(acc[2 * e + 1], &a1, &b1);
-      oh[e] = (uint32_t)__half_as_ushort(a0) | ((uint32_t)__half_as_ushort(a1) << 16);
-      ol[e] = (uint32_t)__half_as_ushort(b0) | ((uint32_t)__half_as_ushort(b1) << 16);
+      split_pair(acc[2 * e], acc[2 * e + 1], oh[e], ol[e]);
     }
     const size_t oo = (((size_t)b * Ho + ho) * Wo + wo) * yp + c8 * 8;
     *reinterpret_cast<uint4*>(y + oo) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
@@ -911,11 +883,14 @@ extern "C" int cvb_nchw_to_split(const float* src, int32_t B, int32_t C, int32_t
   int rc = check_split_view(dst, "nchw_to_split");
   if (rc) return rc;
   CVB_REQUIRE(src && dst->B == B && dst->C == C && dst->H == H && dst->W == W, "nchw_to_split: shape mismatch");
-  dim3 grid(ceil_div(W, 32), ceil_div(C, 32), B * H), block(32, 8);
-  nchw_to_split_kernel<<<grid, block, 0, as_stream(stream)>>>(src, B, C, H, W, static_cast<__half*>(dst->base), dst->c_pitch,
-                                                              dst->plane_stride / 2);
-  CVB_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  CVB_REQUIRE((long long)B * H < 0x7fffffffLL, "nchw_to_split: too many image rows");
+  for (int bh0 = 0; bh0 < B * H; bh0 += kMaxGridZ) {
+    dim3 grid(ceil_div(W, 32), ceil_div(C, 32), min(B * H - bh0, kMaxGridZ)), block(32, 8);
+    nchw_to_split_kernel<<<grid, block, 0, as_stream(stream)>>>(src, B, C, H, W, static_cast<__half*>(dst->base), dst->c_pitch,
+                                                                dst->plane_stride / 2, bh0);
+    CVB_CHECK_CUDA(cudaGetLastError());
+    count_launch();
+  }
   return CVB_OK;
 }
 
@@ -923,21 +898,29 @@ extern "C" int cvb_split_to_nchw(const CvbView* src, float* dst, void* stream) {
   int rc = check_split_view(src, "split_to_nchw");
   if (rc) return rc;
   CVB_REQUIRE(dst != nullptr, "split_to_nchw: null dst");
-  dim3 grid(ceil_div(src->W, 32), ceil_div(src->C, 32), src->B * src->H), block(32, 8);
-  split_to_nchw_kernel<<<grid, block, 0, as_stream(stream)>>>(static_cast<const __half*>(src->base), src->B, src->C, src->H, src->W,
-                                                              src->c_pitch, src->plane_stride / 2, dst);
-  CVB_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  CVB_REQUIRE((long long)src->B * src->H < 0x7fffffffLL, "split_to_nchw: too many image rows");
+  const int rows = src->B * src->H;
+  for (int bh0 = 0; bh0 < rows; bh0 += kMaxGridZ) {
+    dim3 grid(ceil_div(src->W, 32), ceil_div(src->C, 32), min(rows - bh0, kMaxGridZ)), block(32, 8);
+    split_to_nchw_kernel<<<grid, block, 0, as_stream(stream)>>>(static_cast<const __half*>(src->base), src->B, src->C, src->H, src->W,
+                                                                src->c_pitch, src->plane_stride / 2, dst, bh0);
+    CVB_CHECK_CUDA(cudaGetLastError());
+    count_launch();
+  }
   return CVB_OK;
 }
 
 extern "C" int cvb_f32nhwc_to_nchw(const CvbView* src, float* dst, void* stream) {
   CVB_REQUIRE(src && src->base && dst, "f32nhwc_to_nchw: null argument");
-  dim3 grid(ceil_div(src->W, 32), ceil_div(src->C, 32), src->B * src->H), block(32, 8);
-  f32nhwc_to_nchw_kernel<<<grid, block, 0, as_stream(stream)>>>(static_cast<const float*>(src->base), src->B, src->C, src->H, src->W,
-                                                                src->c_pitch, dst);
-  CVB_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  CVB_REQUIRE((long long)src->B * src->H < 0x7fffffffLL, "f32nhwc_to_nchw: too many image rows");
+  const int rows = src->B * src->H;
+  for (int bh0 = 0; bh0 < rows; bh0 += kMaxGridZ) {
+    dim3 grid(ceil_div(src->W, 32), ceil_div(src->C, 32), min(rows - bh0, kMaxGridZ)), block(32, 8);
+    f32nhwc_to_nchw_kernel<<<grid, block, 0, as_stream(stream)>>>(static_cast<const float*>(src->base), src->B, src->C, src->H, src->W,
+                                                                  src->c_pitch, dst, bh0);
+    CVB_CHECK_CUDA(cudaGetLastError());
+    count_launch();
+  }
   return CVB_OK;
 }
 
@@ -1102,6 +1085,7 @@ extern "C" int cvb_groupnorm_relu(const CvbView* x, int32_t groups, const float*
   cudaStream_t st = as_stream(stream);
   CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, cvb_groupnorm_workspace_bytes(x->B, groups), st));
   const int npix = x->H * x->W;
+  CVB_REQUIRE(groups <= 1024, "groupnorm: at most 1024 groups (one CTA thread per group), got %d", groups);
   const int threads = 256 / groups * groups > 0 ? (256 / groups) * groups : groups;
   int chunks = (npix + 255) / 256;
   if (chunks > kSmCount * 4) chunks = kSmCount * 4;

@@ -181,13 +181,6 @@ __device__ __forceinline__ float silu_fast(float x) {
   return x * r;
 }
 
-// (x0, x1) -> packed fp16 hi pair and lo = x - hi pair; saturating converts (one F2FP per pair) keep |x| > 65504 finite
-__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
-  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x1 - hf.y), "f"(x0 - hf.x));
-}
-
 // diagnostics: cycles spent in a waiting primitive, accumulated per role (only when a profile buffer is attached)
 #define CVB_PROF_WAIT(slot, stmt)              \
   do {                                         \

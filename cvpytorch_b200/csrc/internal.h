@@ -4,6 +4,9 @@
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdint.h>
+#ifdef __CUDACC__
+#include <cuda_fp16.h>
+#endif
 
 #include "../../include/cvb200.h"
 
@@ -66,6 +69,18 @@ inline size_t nms_ws_head_bytes(int B) { return nms_align_up((size_t)B * kNmsBin
 inline size_t nms_ws_rowmax_offset(int B) { return nms_ws_head_bytes(B) + (size_t)B * (kNmsCap + kNmsCapA) * 8; }
 
 #ifdef __CUDACC__
+// The one fp32 -> split16 (hi, lo) conversion, for a pair of values (one F2FP per plane).  hi = fp16_rn(x) and lo = fp16_rn(x - hi), both
+// saturating to +-65504 (cvt .satfinite): |x| <= 65504 is kept to ~22 bits, up to 131008 survives with lo carrying the excess, larger values
+// and +-inf saturate to +-131008, and NaN stays NaN (DESIGN.md 2).  Every kernel that stores split16 calls it.
+__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x1 - hf.y), "f"(x0 - hf.x));
+}
+
+// Max that propagates NaN like F.max_pool2d: once the running maximum m is NaN it stays NaN.
+__device__ __forceinline__ float nan_max(float m, float v) { return (v > m || v != v) ? v : m; }
+
 // sigmoid with two MUFU ops (ex2, rcp), |rel err| ~ 2^-22 (the reference's own CPU sigmoid is ~1 ulp; parity budget 1e-3).  Shared by
 // the YOLOv5 / YOLOX / FCOS decode kernels so that every pass that recomputes a score gets the identical value.
 __device__ __forceinline__ float sigmoid_fast(float x) {

@@ -1,5 +1,5 @@
-"""float64 references and element-wise error bounds for the training kernels (tests/test_train_gpu.py) and for the split-fp16 inference
-conv (split_conv_reference below).
+"""float64 references and element-wise error bounds for the training kernels (tests/test_train_gpu.py), for the split-fp16 inference
+conv (split_conv_reference below) and for the split16 format and the aux kernels (tests/test_aux_kernels_gpu.py, test_fcos_gpu.py).
 
 Each reference is computed in float64 on exactly the bf16 values the kernel reads, together with the same operation on the absolute values
 of its inputs (`absref`).  absref bounds every partial sum of a dot product, so the fp32 accumulation error of one output element is at most
@@ -175,6 +175,61 @@ def split_conv_reference(tin, wp, bp, k, s=1, p=0, dil=1, act='silu', residual=N
     chain = (3 if block_n > 128 else 1) * taps * k_tap // 16
     gamma = mma_gamma(16 * chain) + chain * 2.0 ** -25 + 2.0 ** -21
     bound = SPLIT_REL * (ref.abs() + rsum.abs()) + (1.1 if act == 'silu' else 1.0) * gamma * absref + 1e-30
+    return ref, bound
+
+
+# ---------------------------------------------------------------------------------------------------- split16 format, aux kernels
+SPLIT_OUT_REL = 2.0 ** -22  # hi + lo of an fp32 value keeps ~22 bits: |lo| <= 2^-11 |x|, rounded to 11 bits
+SPLIT_OUT_ABS = 2.0 ** -25  # ... and where lo is an fp16 subnormal (spacing 2^-24) it is off by up to half a spacing
+
+
+def split16(x):
+    """The split16 format of fp32 values x (any shape, on any device) -> (hi, lo) fp16: hi = fp16_rn(sat(x)), lo = fp16_rn(sat(x - hi)),
+    sat = saturate to +-65504 (NaN stays NaN): csrc/internal.h split_pair, DESIGN.md 2."""
+    x = x.float()
+    hi = x.clamp(-65504.0, 65504.0).half()
+    lo = (x - hi.float()).clamp(-65504.0, 65504.0).half()
+    return hi, lo
+
+
+def split_out_bound(ref):
+    """Rounding of an fp32 result to the split16 output format, element-wise."""
+    return SPLIT_OUT_REL * ref.abs() + SPLIT_OUT_ABS
+
+
+def gamma_n(n):
+    """gamma_n = n u / (1 - n u), u = 2^-24: bound on the relative error of n chained fp32 roundings (Higham, Accuracy and Stability of
+    Numerical Algorithms, lemma 3.1)."""
+    return n * U24 / (1 - n * U24)
+
+
+def groupnorm_reference(x64, groups, gamma, beta, eps, relu):
+    """float64 GroupNorm (8 channels per group) of x64 [B, C, H, W] and the element-wise bound of csrc/aux_kernels.cu gn_stats / gn_apply
+    -> (ref, bound).  From the kernels' arithmetic (u = 2^-24):
+      the statistics sum x - pivot (pivot: the group's first channel at pixel 0) in fp32 over <= 64 values (+ the pivot subtraction and
+      the square), then in double:  e_sum = 68 u mean|x - pivot|,  e_mean = e_sum + u |mean|  (fp32 mean),
+      e_var = 68 u mean (x - pivot)^2 + 2 |mean - pivot| e_sum
+      apply: |gamma| (|x - mean| rstd (e_var / (2 (var + eps)) + 2 u) + rstd e_mean) + 4 u (|gamma| rstd |x - mean| + |beta|)
+      hi / lo fp16 output: split_out_bound."""
+    B = x64.shape[0]
+    u = U24
+    g64, b64 = gamma.double()[None, :, None, None], beta.double()[None, :, None, None]
+    ref = F.group_norm(x64, groups, g64.flatten(), b64.flatten(), eps)
+    if relu:
+        ref = F.relu(ref)
+    xg = x64.reshape(B, groups, -1)
+    d = xg - x64[:, ::8, 0, 0][..., None]
+    mean, var = xg.mean(-1), xg.var(-1, unbiased=False)
+    e_sum = 68 * u * d.abs().mean(-1)
+    e_mean = e_sum + u * mean.abs()
+    e_var = 68 * u * (d * d).mean(-1) + 2 * d.mean(-1).abs() * e_sum
+    rstd = 1 / torch.sqrt(var + eps)
+
+    def per_channel(s):
+        return s.repeat_interleave(8, dim=1)[:, :, None, None]
+    xm = (x64 - per_channel(mean)).abs()
+    bound = (g64.abs() * (xm * per_channel(rstd * (e_var / (2 * (var + eps)) + 2 * u)) + per_channel(rstd * e_mean))
+             + 4 * u * (g64.abs() * per_channel(rstd) * xm + b64.abs()) + split_out_bound(ref))
     return ref, bound
 
 

@@ -39,13 +39,7 @@ def test_maxpool_and_groupnorm_kernels(cuda):
     ops.maxpool3x3s2(t.view(), y.view())
     assert torch.equal(ops.split_to_nchw(y.view()), F.max_pool2d(xr, 3, 2, 1))
     # GroupNorm(32, 256) + ReLU vs float64 GroupNorm of the split tensor's own values: mean / std = 1/3 (as in the towers), 10 and 100, on
-    # a small map and a P3-sized one.  Bound per element, from the kernels' arithmetic (u = 2^-24):
-    #   the statistics sum x - pivot (pivot: the group's first channel at pixel 0) in fp32 over <= 64 values (+ the pivot subtraction and
-    #   the square), then in double:  e_sum = 68 u mean|x - pivot|,  e_mean = e_sum + u |mean|  (fp32 mean),
-    #   e_var = 68 u mean (x - pivot)^2 + 2 |mean - pivot| e_sum
-    #   apply: |gamma| (|x - mean| rstd (e_var / (2 (var + eps)) + 2 u) + rstd e_mean) + 4 u (|gamma| rstd |x - mean| + |beta|)
-    #   hi / lo fp16 output: 2^-22 relative, and 2^-25 absolute where lo is subnormal
-    u = 2.0 ** -24
+    # a small map and a P3-sized one.  Bound per element: fp64ref.groupnorm_reference (derived from the kernels' arithmetic there).
     for (B, H, W), shift in [((3, 13, 17), 1 / 3), ((3, 13, 17), 10), ((3, 13, 17), 100), ((2, 100, 136), 1 / 3), ((2, 100, 136), 10), ((2, 100, 136), 100)]:
         x = (torch.randn(B, 256, H, W, device='cuda') + shift) * 3
         t = ops.SplitTensor(B, H, W, 256)
@@ -57,21 +51,7 @@ def test_maxpool_and_groupnorm_kernels(cuda):
         xs = ops.split_to_nchw(t.view())
         out = ops.split_to_nchw(z.view())
         assert _rel(out, F.relu(F.group_norm(xs, 32, gamma, beta, 1e-5))) < 2e-5
-        x64, g64, b64 = xs.double(), gamma.double()[None, :, None, None], beta.double()[None, :, None, None]
-        ref = F.relu(F.group_norm(x64, 32, g64.flatten(), b64.flatten(), 1e-5))
-        xg = x64.reshape(B, 32, -1)
-        d = xg - x64[:, ::8, 0, 0][..., None]
-        mean, var = xg.mean(-1), xg.var(-1, unbiased=False)
-        e_sum = 68 * u * d.abs().mean(-1)
-        e_mean = e_sum + u * mean.abs()
-        e_var = 68 * u * (d * d).mean(-1) + 2 * d.mean(-1).abs() * e_sum
-        rstd = 1 / torch.sqrt(var + 1e-5)
-
-        def per_channel(s):
-            return s.repeat_interleave(8, dim=1)[:, :, None, None]
-        xm = (x64 - per_channel(mean)).abs()
-        bound = (g64.abs() * (xm * per_channel(rstd * (e_var / (2 * (var + 1e-5)) + 2 * u)) + per_channel(rstd * e_mean))
-                 + 4 * u * (g64.abs() * per_channel(rstd) * xm + b64.abs()) + 2.0 ** -22 * ref.abs() + 2.0 ** -25)
+        ref, bound = fp64ref.groupnorm_reference(xs.double(), 32, gamma, beta, 1e-5, relu=True)
         ratio = float(((out.double() - ref).abs() / bound).max())
         print(f'groupnorm {B}x256x{H}x{W} mean/std {shift:.3g}: worst error / bound {ratio:.3f}')
         assert ratio <= 1.0, (B, H, W, shift, ratio)

@@ -54,6 +54,33 @@ p = ops.SplitTensor(1, 20, 20, 256)
 ops.nchw_to_split(torch.randn(1, 64, 20, 20, device='cuda'), p.view(0, 64))
 ops.sppf_pool(p.view(0, 64), p.view(64, 64), p.view(128, 64), p.view(192, 64))
 ops.split_to_nchw(p.view())
+# one channel-slice case per aux kernel: inputs and outputs are slices of wider buffers, 24 channels = a partial 32-channel slab
+q = ops.SplitTensor(1, 9, 13, 64)
+ops.nchw_to_split(torch.randn(1, 24, 9, 13, device='cuda'), q.view(8, 24))
+ops.split_to_nchw(q.view(8, 24))
+f = ops.F32Tensor(1, 9, 13, 40)
+ops.split_to_f32(q.view(8, 24), f.view(8, 24))
+ops.f32nhwc_to_nchw(f.view(4, 24))
+ops.stem_s2d(x, ops.SplitTensor(1, 32, 35, 16).view(), pad_left=2)
+ops.maxpool3x3s2(q.view(8, 24), ops.SplitTensor(1, 5, 7, 40).view(16, 24))
+d = ops.SplitTensor(1, 9, 13, 48)
+w9c, bias = ops.pack_dw_weights(torch.randn(24, 1, 3, 3, dtype=torch.float64), torch.randn(24, dtype=torch.float64))
+for dil in (1, 6):
+    ops.dwconv3x3(q.view(8, 24), w9c, bias, dil, d.view(16, 24), True)
+gp = ops.SplitTensor(1, 1, 1, 40)
+ops.global_avgpool(q.view(8, 24), gp.view(16, 24))
+r = ops.SplitTensor(1, 17, 23, 64)
+ops.bilinear_resize(q.view(8, 24), r.view(24, 24))
+ops.bilinear_resize(gp.view(16, 24), r.view(40, 24))
+ops.groupnorm_relu(q.view(8, 24), 3, torch.ones(24, device='cuda'), torch.zeros(24, device='cuda'), 1e-5, d.view(16, 24),
+                   ops.GroupNormWorkspace(1, 3), relu=False)
+lg = ops.F32Tensor(1, 9, 13, 24)
+ops.upsample_argmax(lg.view(0, 19), 19, torch.zeros((1, 17, 23), dtype=torch.int64, device='cuda'))
+ro = ops.F32Tensor(1, 9, 13, 8)
+ops.yolox_decode(ro.view(0, 5), lg.view(0, 19), 19, 8.0, ops.YoloxWorkspace(1, 9 * 13 + 8), 4)
+ops.fcos_decode(lg.view(0, 19), ro.view(0, 5), 19, 8.0, 1.0, ops.FcosWorkspace(1, 9 * 13 + 8), 4)
+torch.cuda.synchronize()
+print('aux kernels ok')
 
 # YOLOv5 decode + NMS (both phases) on a small stress tensor
 pred = torch.from_numpy(NO.make_stress_prediction(1, A=25200, regime='typical', seed=2)).cuda()
