@@ -11,6 +11,8 @@
 //             dy = gamma * rstd * (dz - mean(dz) - xhat * mean(dz * xhat))   bn_silu_bwd_apply_kernel
 //             dx = conv(dy, W rotated by 180 degrees, in/out swapped)   tconv_kernel again (optionally with the PRODUCER's SiLU' in the epilogue)
 //             dW[co][tap][ci] = sum_pixels dy[p][co] * x[p + tap][ci]    twgrad_kernel   (K = pixels: both operands MN-major in shared memory)
+// nn.SyncBatchNorm (statistics over every rank's pixels): bn_stats_kernel + bn_partial_kernel -> all-gather of the fp64 records ->
+// bn_merge_kernel; backward bn_silu_bwd_reduce_kernel -> all-reduce of the two sums -> bn_silu_bwd_apply_kernel with the global count.
 //
 // Layout: activations and gradients are NHWC bf16, dense (pitch == C; C = 16, 32 or a multiple of 64, and TMA zero-fills a box's channels
 // past a 16- or 32-channel C); weights bf16 [cout][kh*kw][kpad(cin)] (K-major rows, zero-padded to 64 channels), fp32 master weights / fp32
@@ -427,16 +429,11 @@ __global__ void __launch_bounds__(kEwThreads) bn_stats_kernel(const __nv_bfloat1
   red_finish(a1, a2, v, pl, np, active, C, s_part, sums);
 }
 
-// batch statistics -> mean, rstd, folded scale / shift; running statistics updated like nn.BatchNorm2d (unbiased variance, momentum)
-__global__ void bn_finalize_kernel(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ y, long long npix, int C, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean, float* __restrict__ running_var,
-                                   float* __restrict__ stat /* [4][C]: mean, rstd, scale, shift */) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const double n = (double)npix;
-  const double d1 = (double)sums[c] / n;  // mean - pivot
-  const double mean = (double)__bfloat162float(y[c]) + d1;
-  double var = (double)sums[C + c] / n - d1 * d1;
+// channel c's batch mean and biased variance over n pixels -> mean, rstd, folded scale / shift; running statistics updated like
+// nn.BatchNorm2d (unbiased variance, momentum).  Shared by the local (bn_finalize_kernel) and the cross-rank (bn_merge_kernel) statistics.
+__device__ __forceinline__ void bn_finalize_channel(int c, int C, double mean, double var, double n, const float* __restrict__ gamma,
+                                                    const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean,
+                                                    float* __restrict__ running_var, float* __restrict__ stat) {
   if (var < 0.0) var = 0.0;
   const float rstd = (float)(1.0 / sqrt(var + (double)eps));
   const float s = gamma[c] * rstd;
@@ -448,6 +445,55 @@ __global__ void bn_finalize_kernel(const float* __restrict__ sums, const __nv_bf
     running_mean[c] = (1.0f - momentum) * running_mean[c] + momentum * (float)mean;
     running_var[c] = (1.0f - momentum) * running_var[c] + momentum * (float)(var * n / (n > 1.0 ? n - 1.0 : 1.0));
   }
+}
+
+// batch statistics of this device's pixels (bn_stats_kernel's pivoted sums) -> stat [4][C], running statistics
+__global__ void bn_finalize_kernel(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ y, long long npix, int C, const float* __restrict__ gamma,
+                                   const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean, float* __restrict__ running_var,
+                                   float* __restrict__ stat /* [4][C]: mean, rstd, scale, shift */) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double n = (double)npix;
+  const double d1 = (double)sums[c] / n;  // mean - pivot
+  const double mean = (double)__bfloat162float(y[c]) + d1;
+  const double var = (double)sums[C + c] / n - d1 * d1;
+  bn_finalize_channel(c, C, mean, var, n, gamma, beta, eps, momentum, running_mean, running_var, stat);
+}
+
+// Cross-rank (SyncBatchNorm) statistics.  Every rank's pivot y[0][c] is a different sample, so the pivoted sums of two ranks do not add;
+// each rank turns its sums into a record of (count, mean, M2 = sum of squared deviations from its own mean), which merge exactly.
+// Record layout, fp64 [2C + 1]: mean[C], M2[C], count.
+__global__ void bn_partial_kernel(const float* __restrict__ sums, const __nv_bfloat16* __restrict__ y, long long npix, int C, double* __restrict__ rec) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double n = (double)npix;
+  const double s1 = (double)sums[c];
+  const double d1 = s1 / n;  // mean - pivot
+  rec[c] = (double)__bfloat162float(y[c]) + d1;
+  const double m2 = (double)sums[C + c] - s1 * d1;  // = n * (S2 / n - d1^2), the variance bn_finalize_kernel takes, times n
+  rec[C + c] = m2 > 0.0 ? m2 : 0.0;
+  if (c == 0) rec[2 * C] = n;
+}
+
+// records [world][2C + 1] (as all_gather lays them out) -> Chan's pairwise merge in rank order, in fp64, so every rank computes the same bits
+// -> stat [4][C] and running statistics as bn_finalize_kernel; *count = the global pixel count, for the backward's 1 / N.
+__global__ void bn_merge_kernel(const double* __restrict__ recs, int world, int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                float momentum, float* __restrict__ running_mean, float* __restrict__ running_var, float* __restrict__ stat,
+                                double* __restrict__ count) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const long long len = 2 * (long long)C + 1;
+  double n = recs[2 * C], mean = recs[c], m2 = recs[C + c];
+  for (int r = 1; r < world; ++r) {
+    const double* rb = recs + r * len;
+    const double nb = rb[2 * C], nab = n + nb;
+    const double delta = rb[c] - mean;
+    mean += delta * (nb / nab);
+    m2 += rb[C + c] + delta * delta * (n * nb / nab);
+    n = nab;
+  }
+  bn_finalize_channel(c, C, mean, m2 / n, n, gamma, beta, eps, momentum, running_mean, running_var, stat);
+  if (c == 0) *count = n;
 }
 
 // a = silu(y * scale + shift)
@@ -529,10 +575,12 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_reduce_kernel(const __
   red_finish(a1, a2, v, pl, np, active, C, s_part, sums);
 }
 
-// dy = gamma * rstd * (dz - sum_dz / N - xhat * sum_dzx / N)
+// dy = gamma * rstd * (dz - sum_dz / N - xhat * sum_dzx / N);  1 / N = inv_n, or (DEV_COUNT: N over every rank) 1 / *count, read on the device
+template <bool DEV_COUNT>
 __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, long long nvec, int C,
                                                                        const float* __restrict__ stat, const float* __restrict__ gamma, const float* __restrict__ sums,
-                                                                       float inv_n, int g_is_dz, __nv_bfloat16* __restrict__ dy) {
+                                                                       float inv_n, const double* __restrict__ count, int g_is_dz, __nv_bfloat16* __restrict__ dy) {
+  if (DEV_COUNT) inv_n = (float)(1.0 / __ldg(count));
   const int cv = C / 8;
   const long long stride = (long long)gridDim.x * kEwThreads;
   for (long long i = (long long)blockIdx.x * kEwThreads + threadIdx.x; i < nvec; i += 2 * stride) {
@@ -1180,20 +1228,81 @@ extern "C" int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, con
   return CVB_OK;
 }
 
-extern "C" int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, float* sums /* [2][C]: out = dbeta, dgamma */,
-                                     void* dy, void* stream) {
-  CVB_REQUIRE(g && y && stat && gamma && sums && dy && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd: bad argument");
-  cudaStream_t st = as_stream(stream);
+static int bn_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, cudaStream_t st) {
   CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 2 * (size_t)C * sizeof(float), st));
   const int np = kEwThreads / (C / 8);
   bn_silu_bwd_reduce_kernel<<<red_grid(npix, np), kEwThreads, 0, st>>>(
       static_cast<const __nv_bfloat16*>(g), static_cast<const __nv_bfloat16*>(y), npix, C, stat, g_is_dz, sums);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+// count == nullptr: 1 / npix (this device's pixels); otherwise 1 / *count, the global count bn_merge_kernel left on the device
+static int bn_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, const float* sums,
+                        const double* count, void* dy, cudaStream_t st) {
   const long long nvec = npix * (C / 8);
-  bn_silu_bwd_apply_kernel<<<ew_grid(nvec), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(g), static_cast<const __nv_bfloat16*>(y), nvec, C, stat, gamma, sums,
-                                                                 (float)(1.0 / (double)npix), g_is_dz, static_cast<__nv_bfloat16*>(dy));
+  const auto* gb = static_cast<const __nv_bfloat16*>(g);
+  const auto* yb = static_cast<const __nv_bfloat16*>(y);
+  auto* dyb = static_cast<__nv_bfloat16*>(dy);
+  if (count == nullptr)
+    bn_silu_bwd_apply_kernel<false><<<ew_grid(nvec), kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, (float)(1.0 / (double)npix), nullptr, g_is_dz, dyb);
+  else
+    bn_silu_bwd_apply_kernel<true><<<ew_grid(nvec), kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, 0.0f, count, g_is_dz, dyb);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, float* sums /* [2][C]: out = dbeta, dgamma */,
+                                     void* dy, void* stream) {
+  CVB_REQUIRE(g && y && stat && gamma && sums && dy && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd: bad argument");
+  cudaStream_t st = as_stream(stream);
+  const int rc = bn_bwd_reduce(g, g_is_dz, y, npix, C, stat, sums, st);
+  return rc != CVB_OK ? rc : bn_bwd_apply(g, g_is_dz, y, npix, C, stat, gamma, sums, nullptr, dy, st);
+}
+
+// ---- SyncBatchNorm: the statistics and the backward split where a collective sits between the two halves
+extern "C" int cvb_train_bn_partial(const void* y, int64_t npix, int32_t C, float* sums_scratch, double* record, void* stream) {
+  CVB_REQUIRE(y && sums_scratch && record, "train_bn_partial: null pointer");
+  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_partial: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
+              (long long)npix, C);
+  CVB_REQUIRE((reinterpret_cast<uintptr_t>(y) & 15) == 0 && (reinterpret_cast<uintptr_t>(record) & 7) == 0, "train_bn_partial: y must be 16-byte, record 8-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  CVB_CHECK_CUDA(cudaMemsetAsync(sums_scratch, 0, 2 * (size_t)C * sizeof(float), st));
+  bn_stats_kernel<<<red_grid(npix, kEwThreads / (C / 8)), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
+  bn_partial_kernel<<<ceil_div(C, 128), 128, 0, st>>>(sums_scratch, static_cast<const __nv_bfloat16*>(y), npix, C, record);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
   return CVB_OK;
+}
+
+extern "C" int cvb_train_bn_merge(const double* records, int32_t world, int32_t C, const float* gamma, const float* beta, float eps, float momentum,
+                                  float* running_mean, float* running_var, float* stat, double* count, void* stream) {
+  CVB_REQUIRE(records && gamma && beta && stat && count, "train_bn_merge: null pointer");
+  CVB_REQUIRE((running_mean == nullptr) == (running_var == nullptr), "train_bn_merge: running_mean and running_var go together");
+  CVB_REQUIRE(world >= 1 && C > 0 && C % 8 == 0 && C <= 2048, "train_bn_merge: world must be >= 1 and C a multiple of 8 up to 2048 (world=%d C=%d)", world, C);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(records) | reinterpret_cast<uintptr_t>(count)) & 7) == 0, "train_bn_merge: records / count must be 8-byte aligned");
+  bn_merge_kernel<<<ceil_div(C, 128), 128, 0, as_stream(stream)>>>(records, world, C, gamma, beta, eps, momentum, running_mean, running_var, stat, count);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_bn_silu_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream) {
+  CVB_REQUIRE(g && y && stat && sums, "train_bn_silu_bwd_reduce: null pointer");
+  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd_reduce: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
+              (long long)npix, C);
+  return bn_bwd_reduce(g, g_is_dz, y, npix, C, stat, sums, as_stream(stream));
+}
+
+extern "C" int cvb_train_bn_silu_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma,
+                                           const float* sums, const double* count, void* dy, void* stream) {
+  CVB_REQUIRE(g && y && stat && gamma && sums && count && dy, "train_bn_silu_bwd_apply: null pointer");
+  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd_apply: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
+              (long long)npix, C);
+  CVB_REQUIRE((reinterpret_cast<uintptr_t>(count) & 7) == 0, "train_bn_silu_bwd_apply: count must be 8-byte aligned");
+  return bn_bwd_apply(g, g_is_dz, y, npix, C, stat, gamma, sums, count, dy, as_stream(stream));
 }
 
 extern "C" int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream) {

@@ -27,6 +27,7 @@ import ctypes
 import math
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib
@@ -140,9 +141,20 @@ def _set_bn(m):
             mod.eps, mod.momentum = 1e-3, 0.03
 
 
-def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1, pad=None):
-    """a = silu(bn_train(conv(x, weight))) -> (a, (y, stat, g32, wb)): what _bn_silu_backward and the backward convolutions need (the conv
-    output, the BN statistics, fp32 gamma and the backward-data weights).  Updates the running statistics."""
+def _sync_group(bn):
+    """The process group whose ranks' pixels `bn` normalises over, or None (this device's batch only).  Decided at every forward as
+    nn.SyncBatchNorm.forward decides it: an nn.SyncBatchNorm in training mode, torch.distributed initialised, and more than one rank in the
+    module's process_group (None: the default group)."""
+    if not (isinstance(bn, nn.SyncBatchNorm) and bn.training and dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group else dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None):
+    """a = silu(bn_train(conv(x, weight))) -> (a, (y, stat, g32, wb), count): what _bn_silu_backward and the backward convolutions need (the
+    conv output, the BN statistics, fp32 gamma and the backward-data weights) and, with a process group (SyncBatchNorm), the global pixel count
+    on the device (None otherwise).  Updates the running statistics."""
     cout = weight.shape[0]
     L = _lib.lib()
     wf, wb = pack_weights(weight)
@@ -151,34 +163,55 @@ def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, moment
     stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
     scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
     g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-    _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
-                                    _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
+    count = None
+    if group is None:
+        _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                        _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
+    else:  # every rank's (mean, M2, count) record, gathered in rank order and merged on the device
+        world = dist.get_world_size(group)
+        rec = torch.empty((2 * cout + 1,), dtype=torch.float64, device=x.device)
+        _lib.check(L.cvb_train_bn_partial(_p(y), npix, cout, _p(scratch), _p(rec), _stream()), 'cvb_train_bn_partial')
+        recs = torch.empty((world * (2 * cout + 1),), dtype=torch.float64, device=x.device)  # (flat: gloo's all-gather wants world x the input)
+        dist.all_gather_into_tensor(recs, rec, group=group)
+        count = torch.empty((1,), dtype=torch.float64, device=x.device)
+        _lib.check(L.cvb_train_bn_merge(_p(recs), world, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                        _p(stat), _p(count), _stream()), 'cvb_train_bn_merge')
     a = torch.empty_like(y)
     _lib.check(L.cvb_train_bn_silu_fwd(_p(y), npix, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_silu_fwd')
-    return a, (y, stat, g32, wb)
+    return a, (y, stat, g32, wb), count
 
 
-def _bn_silu_backward(g, g_is_dz, y, stat, g32):
+def _bn_silu_backward(g, g_is_dz, y, stat, g32, group=None, count=None):
     """g = d(loss)/d(a), or d(loss)/d(z) with z the BN output when g_is_dz (a SiLU' epilogue already applied) -> (dy = d(loss)/d(y),
-    dgamma, dbeta)."""
+    dgamma, dbeta).  With a process group (SyncBatchNorm): dgamma and dbeta stay this rank's sums (DDP averages them like every other
+    gradient); dy takes the sums over every rank and the global pixel count `count` of the forward."""
     g = g.contiguous()
     cout = y.shape[3]
+    npix = y.shape[0] * y.shape[1] * y.shape[2]
+    L = _lib.lib()
     sums = torch.empty((2, cout), dtype=torch.float32, device=y.device)
     dy = torch.empty_like(y)
-    _lib.check(_lib.lib().cvb_train_bn_silu_bwd(_p(g), int(g_is_dz), _p(y), y.shape[0] * y.shape[1] * y.shape[2], cout, _p(stat), _p(g32), _p(sums), _p(dy),
-                                                _stream()), 'cvb_train_bn_silu_bwd')
-    return dy, sums[1].clone(), sums[0].clone()
+    if group is None:
+        _lib.check(L.cvb_train_bn_silu_bwd(_p(g), int(g_is_dz), _p(y), npix, cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()), 'cvb_train_bn_silu_bwd')
+        return dy, sums[1].clone(), sums[0].clone()
+    _lib.check(L.cvb_train_bn_silu_bwd_reduce(_p(g), int(g_is_dz), _p(y), npix, cout, _p(stat), _p(sums), _stream()), 'cvb_train_bn_silu_bwd_reduce')
+    dgamma, dbeta = sums[1].clone(), sums[0].clone()
+    dist.all_reduce(sums, group=group)
+    _lib.check(L.cvb_train_bn_silu_bwd_apply(_p(g), int(g_is_dz), _p(y), npix, cout, _p(stat), _p(g32), _p(sums), _p(count), _p(dy), _stream()),
+               'cvb_train_bn_silu_bwd_apply')
+    return dy, dgamma, dbeta
 
 
 class _ConvBnSiLU(torch.autograd.Function):
     """a = silu(bn_train(conv(x, W))) with the backward the reference obtains from torch.autograd, on the H100 kernels."""
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride=1, pad=None):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None):
         _check_cuda(x, 'BaseConv (H100 training)')
-        a, saved = _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, k, stride, pad)
+        a, saved, count = _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride, pad)
         ctx.save_for_backward(x, *saved)
         ctx.k, ctx.stride, ctx.pad = k, stride, pad
+        ctx.group, ctx.count = group, count
         ctx.need_dx = x.requires_grad
         return a
 
@@ -187,7 +220,7 @@ class _ConvBnSiLU(torch.autograd.Function):
         x, y, stat, g32, wb = ctx.saved_tensors
         k = ctx.k
         B, H, W, cin = x.shape
-        dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32)
+        dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32, ctx.group, ctx.count)
         dw = conv_wgrad(x, dy, k, ctx.stride, ctx.pad)
         dx = None
         if ctx.need_dx:
@@ -195,7 +228,7 @@ class _ConvBnSiLU(torch.autograd.Function):
                 dx = conv_dgrad_s2(dy, wb, cin, H, W)
             else:  # backward-data of a padding-p conv: the same conv over dy with the rotated weights and padding k - 1 - p
                 dx = conv(dy, wb, cin, k, pad=None if ctx.pad is None else k - 1 - ctx.pad)
-        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None
+        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None
 
 
 class _BottleneckChain(torch.autograd.Function):
@@ -203,24 +236,26 @@ class _BottleneckChain(torch.autograd.Function):
     the 1x1 layer's SiLU' in its epilogue (dz_t leaves the tensor core already multiplied; d(loss)/dt is never written)."""
 
     @staticmethod
-    def forward(ctx, x, w1, g1, b1, rm1, rv1, eps1, mom1, w2, g2, b2, rm2, rv2, eps2, mom2):
+    def forward(ctx, x, w1, g1, b1, rm1, rv1, eps1, mom1, grp1, w2, g2, b2, rm2, rv2, eps2, mom2, grp2):
         _check_cuda(x, 'Bottleneck (H100 training)')
-        t, saved1 = _conv_bn_silu(x, w1, g1, b1, rm1, rv1, eps1, mom1, 1)
-        u, saved2 = _conv_bn_silu(t, w2, g2, b2, rm2, rv2, eps2, mom2, 3)
+        t, saved1, n1 = _conv_bn_silu(x, w1, g1, b1, rm1, rv1, eps1, mom1, grp1, 1)
+        u, saved2, n2 = _conv_bn_silu(t, w2, g2, b2, rm2, rv2, eps2, mom2, grp2, 3)
         ctx.save_for_backward(x, t, *saved1, *saved2)
+        ctx.sync = ((grp1, n1), (grp2, n2))
         ctx.need_dx = x.requires_grad
         return u
 
     @staticmethod
     def backward(ctx, du):
         x, t, y1, st1, g1f, wb1, y2, st2, g2f, wb2 = ctx.saved_tensors
-        dy2, dg2, db2 = _bn_silu_backward(du, False, y2, st2, g2f)
+        sync1, sync2 = ctx.sync
+        dy2, dg2, db2 = _bn_silu_backward(du, False, y2, st2, g2f, *sync2)
         dw2 = conv_wgrad(t, dy2, 3)
         dz1 = conv(dy2, wb2, y1.shape[3], 3, y_prev=y1, stat_prev=st1)  # backward-data of the 3x3 with the 1x1 layer's SiLU' in the epilogue
-        dy1, dg1, db1 = _bn_silu_backward(dz1, True, y1, st1, g1f)
+        dy1, dg1, db1 = _bn_silu_backward(dz1, True, y1, st1, g1f, *sync1)
         dw1 = conv_wgrad(x, dy1, 1)
         dx = conv(dy1, wb1, x.shape[3], 1) if ctx.need_dx else None
-        return dx, dw1, dg1, db1, None, None, None, None, dw2, dg2, db2, None, None, None, None
+        return dx, dw1, dg1, db1, None, None, None, None, None, dw2, dg2, db2, None, None, None, None, None
 
 
 class _ConvBnSiLULayer(nn.Module):
@@ -236,9 +271,10 @@ class _ConvBnSiLULayer(nn.Module):
         self.ksize, self.stride, self.padding = ksize, stride, padding
 
     def _bn_inputs(self):
-        """Counts the step -> the _ConvBnSiLU / _BottleneckChain arguments of this layer's BatchNorm."""
+        """Counts the step -> the _ConvBnSiLU / _BottleneckChain arguments of this layer's BatchNorm (an nn.BatchNorm2d, or the
+        nn.SyncBatchNorm convert_sync_batchnorm put in its place: then the statistics span the ranks of its process group)."""
         bn = self.bn
-        return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, _bn_momentum(bn)
+        return bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, _bn_momentum(bn), _sync_group(bn)
 
     def forward(self, x):
         return self._layer(x, self.conv.weight)

@@ -416,6 +416,27 @@ int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t 
 int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int32_t h, int32_t w, int32_t c_off, int32_t cout, int32_t cout_pad, void* dy, float* dbias,
                         void* stream);
 
+/* SyncBatchNorm (nn.SyncBatchNorm in training mode: batch statistics over every rank's pixels).  The caller runs the collectives between
+ * the calls; nothing here synchronises the host, so the whole sequence can be captured in a CUDA graph.
+ * cvb_train_bn_partial: y [npix][C] bf16 (16-byte aligned, C % 8 == 0, C <= 2048) -> record fp64 [2C + 1] = (mean [C], M2 [C] = sum of
+ *   squared deviations from that mean, npix).  sums_scratch: [2][C] fp32, as cvb_train_bn_stats.  Records merge; the pivoted sums of
+ *   cvb_train_bn_stats do not (every rank's pivot is a different pixel).  npix = 0 is refused: unlike nn.SyncBatchNorm, a rank with an
+ *   empty shard cannot take part (the training convolutions refuse B = 0 before the BatchNorm is reached).
+ * cvb_train_bn_merge: records fp64 [world][2C + 1] (every rank's record, in rank order, as all_gather lays them out) -> Chan's pairwise merge
+ *   in rank order in fp64 (every rank computes the same bits) -> stat [4][C] and the running statistics exactly as cvb_train_bn_stats computes
+ *   them from a mean, a biased variance and a count; count fp64 [1] = the global pixel count, left on the device for the backward.
+ *   Every record's count must be positive (as cvb_train_bn_partial writes them); a zero count would divide 0 by 0 in the merge.
+ * cvb_train_bn_silu_bwd_reduce: the first half of cvb_train_bn_silu_bwd: sums [2][C] = this rank's (dbeta, dgamma).
+ * cvb_train_bn_silu_bwd_apply: the second half, from the sums summed over every rank and N = *count (device fp64, e.g. cvb_train_bn_merge's):
+ *   dy = gamma * rstd * (dz - sums[0] / N - xhat * sums[1] / N).
+ */
+int cvb_train_bn_partial(const void* y, int64_t npix, int32_t C, float* sums_scratch, double* record, void* stream);
+int cvb_train_bn_merge(const double* records, int32_t world, int32_t C, const float* gamma, const float* beta, float eps, float momentum,
+                       float* running_mean, float* running_var, float* stat, double* count, void* stream);
+int cvb_train_bn_silu_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream);
+int cvb_train_bn_silu_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma,
+                                const float* sums, const double* count, void* dy, void* stream);
+
 /* YOLOX training loss (src/losses/det/yolox_loss.py:73-436; csrc/yolox_loss.cu): SimOTA assignment, the IoU / objectness / class losses
  * and their gradient with respect to the head outputs.  preds[l]: fp32 NCHW [B, 5 + nc, h_l, w_l] (read in place), shapes[4 l ..] =
  * (B, 5 + nc, h_l, w_l), strides[l] > 0, 1 <= nlev <= 4; anchors in level order, row-major within a level (A = sum h_l w_l).
