@@ -988,6 +988,10 @@ __device__ __forceinline__ bool fcos_suppressed(const float4& a, float aa, const
   return !(iou <= thr32);
 }
 
+// Score as the top-k selection sees it.  -0.0f equals 0 (torch.topk and the score threshold treat it so), but its bit pattern would
+// land in the top histogram bin and sort above every positive score: it is selected as +0.0f.
+__device__ __forceinline__ float fcos_score(float v) { return v == 0.0f ? 0.0f : v; }
+
 __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __restrict__ scores, const int* __restrict__ classes,
                                                                 const float* __restrict__ boxes, int N, float score_thres,
                                                                 float iou_thres, int topk, float* __restrict__ out_scores,
@@ -1009,7 +1013,7 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
   }
   __syncthreads();
   for (int i = tid; i < N; i += kFcosThreads) {
-    const float v = sc[i];
+    const float v = fcos_score(sc[i]);
     if (v >= 0.0f) atomicAdd(&S.hist[nms_score_bin(v)], 1u);  // NaN / negative never selected
   }
   __syncthreads();
@@ -1018,7 +1022,7 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_nms_kernel(const float* __r
   const uint32_t tb = S.tbin;
   for (int i0 = 0; i0 < N; i0 += kFcosThreads) {
     const int i = i0 + tid;
-    const float v = (i < N) ? sc[i] : 0.0f;
+    const float v = (i < N) ? fcos_score(sc[i]) : 0.0f;
     const bool pass = i < N && v >= 0.0f && nms_score_bin(v) >= tb;
     const uint32_t pos = warp_append(&S.n_sel, pass);
     if (pass) {

@@ -126,21 +126,23 @@ def fcos_detect(cls, cnt, reg, score_threshold=0.05, nms_iou_threshold=0.6, max_
     sc = torch.sqrt(sc * cnt_p.squeeze(-1))
     cl = cl + 1
     boxes = torch.cat([coords[None] - reg_p[..., :2], coords[None] + reg_p[..., 2:]], -1)
-    out = []
-    k = min(max_num, sc.shape[-1])
-    for b in range(B):
-        s = sc[b].numpy()
-        top = np.argsort(-s, kind='stable')[:k]  # torch.topk(sorted=True); ties: lower index first (defined here)
-        s_t, c_t, b_t = s[top], cl[b].numpy()[top], boxes[b].numpy()[top]
-        m = s_t >= np.float32(score_threshold)
-        s_m, c_m, b_m, loc = s_t[m], c_t[m], b_t[m], top[m]
-        if s_m.size == 0:
-            out.append((s_m, c_m, b_m, loc))
-            continue
-        off = c_m.astype(np.float32) * (b_m.max() + np.float32(1))  # batched_nms (:141-153)
-        keep = box_nms(b_m + off[:, None], s_m, nms_iou_threshold)
-        out.append((s_m[keep], c_m[keep], b_m[keep], loc[keep]))
+    out = [post_process(sc[b].numpy(), cl[b].numpy(), boxes[b].numpy(), score_threshold, nms_iou_threshold, max_num) for b in range(B)]
     return out, (sc, cl, boxes)
+
+
+def post_process(s, c, b, score_threshold=0.05, nms_iou_threshold=0.6, max_num=1000):
+    """FCOSDetect._post_process (:60-105) on the decoded arrays of ONE image: scores [N], classes [N] (1-based), boxes [N,4]
+    -> (scores [n], classes [n], boxes [n,4], loc [n])."""
+    k = min(max_num, s.shape[-1])
+    top = np.argsort(-s, kind='stable')[:k]  # torch.topk(sorted=True); ties: lower index first (defined here)
+    s_t, c_t, b_t = s[top], c[top], b[top]
+    m = s_t >= np.float32(score_threshold)
+    s_m, c_m, b_m, loc = s_t[m], c_t[m], b_t[m], top[m]
+    if s_m.size == 0:
+        return s_m, c_m, b_m, loc
+    off = c_m.astype(np.float32) * (b_m.max() + np.float32(1))  # batched_nms (:141-153)
+    keep = box_nms(b_m + off[:, None], s_m, nms_iou_threshold)
+    return s_m[keep], c_m[keep], b_m[keep], loc[keep]
 
 
 def forward(x, sd):

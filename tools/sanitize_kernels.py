@@ -17,6 +17,7 @@ from cvpytorch_b200 import ops  # noqa: E402
 from oracle import nms_oracle as NO  # noqa: E402
 from oracle import yolox_oracle as XO  # noqa: E402
 import test_conv_gpu as T  # noqa: E402
+import test_nms_kernels_gpu as TN  # noqa: E402
 
 torch.backends.cudnn.allow_tf32 = False  # the torch fp32 reference must not run on TF32 tensor cores
 torch.backends.cuda.matmul.allow_tf32 = False
@@ -87,14 +88,23 @@ pred = torch.from_numpy(NO.make_stress_prediction(1, A=25200, regime='typical', 
 M.non_max_suppression(pred, 0.001, 0.6, multi_label=True)
 pred = torch.from_numpy(NO.make_stress_prediction(1, A=25200, regime='capped', seed=3)).cuda()
 M.non_max_suppression(pred, 0.001, 0.6, multi_label=True)
+# full path with the sort's grid-wide steps: 9000 candidates whose top ~3k keep fewer than max_det boxes
+wsb = ops.NmsWorkspace(1, 9000, 4)
+ops.yolo_nms(torch.from_numpy(TN.big_scene(9000)[None]).cuda(), wsb)
 torch.cuda.synchronize()
+assert int(TN.ws_regions(wsb)['cntB'][0]) == 9000 and int(wsb.status[0]) == 0
 print('yolo nms ok')
 
 # YOLOX post-process
 rec = XO.make_stress_records(regime='typical', seed=2)
 ws = ops.YoloxWorkspace(1, rec.shape[0])
 ops.yolox_nms(ws, 0.01, 0.65, cand=torch.from_numpy(rec[None]).cuda().contiguous())
+# 1001 candidates > vanilla_above: per-class chains of kept boxes
+rec = TN._switch_scene(1001)
+ws = ops.YoloxWorkspace(1, rec.shape[0])
+ops.yolox_nms(ws, 0.01, 0.65, vanilla_above=1000, cand=torch.from_numpy(rec[None]).cuda().contiguous())
 torch.cuda.synchronize()
+assert int(ws.count[0]) == 1001
 print('yolox nms ok')
 
 # FCOS NMS
@@ -107,7 +117,13 @@ wh = torch.rand(B, N, 2, generator=g) * 90 + 4
 bx = torch.cat([xy, xy + wh], 2).cuda().contiguous()
 fw = ops.FcosWorkspace(B, N)
 ops.fcos_nms(fw, 0.05, 0.6, scores=sc, classes=cl, boxes=bx)
+# more locations than the 4096 keys of the selection
+fs, fc, fb = TN.fcos_scene(6000)
+fw = ops.FcosWorkspace(1, 6000)
+ops.fcos_nms(fw, 0.05, 0.6, scores=torch.from_numpy(fs[None]).cuda(), classes=torch.from_numpy(fc[None].astype('int32')).cuda(),
+             boxes=torch.from_numpy(fb[None]).cuda())
 torch.cuda.synchronize()
+assert int(fw.out_count[0]) == 1000 and int(fw.status[0]) == 0
 print('fcos nms ok')
 
 # whole model at a tiny size (every graph step incl. the fused decode histogram path)
