@@ -61,6 +61,8 @@ SYMBOLS = {
     'cvb_train_focus_s2d': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_train_spp_pool_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_spp_pool_bwd': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    'cvb_train_sppf_chain_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_sppf_chain_bwd': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_upsample_cat_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p]),
     'cvb_train_upsample_cat_bwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_conv_pad': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -72,6 +74,12 @@ SYMBOLS = {
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'cvb_train_yolox_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), c_int32, c_int32, c_void_p, c_int32, c_int32,
                                            c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
+    'cvb_train_yolov5_loss_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32]),
+    'cvb_train_yolov5_loss_fwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_int32, c_int32, c_int32, c_void_p,
+                                            c_int32, POINTER(c_float), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'cvb_train_yolov5_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_int32, c_int32, c_int32, c_void_p,
+                                            c_int32, POINTER(c_float), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, POINTER(c_void_p),
+                                            c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

@@ -101,6 +101,14 @@ __device__ __forceinline__ float yolo_wh(float y, float anchor) {
   return __fmul_rn(__fmul_rn(t2, t2), anchor);
 }
 __device__ __forceinline__ float yolo_score(float cls, float obj) { return __fmul_rn(cls, obj); }
+
+// The training losses' fp32 sigmoid and BCEWithLogits (pos_weight 1), shared by yolox_loss.cu and yolov5_loss.cu:
+// BCEWithLogits(x, t) = (1 - t) x + m + log(exp(-m) + exp(-x - m)), m = max(-x, 0)
+__device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
+__device__ __forceinline__ float bce_logits(float x, float t) {
+  const float m = fmaxf(-x, 0.0f);
+  return (1.0f - t) * x + m + logf(expf(-m) + expf(-x - m));
+}
 #endif
 
 }  // namespace cvb

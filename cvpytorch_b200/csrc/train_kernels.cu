@@ -690,6 +690,7 @@ __global__ void __launch_bounds__(kEwThreads) spp_pool_fwd_kernel(const __nv_bfl
 #pragma unroll
     for (int s = 0; s < 3; ++s) {
       crow[(s + 1) * cv] = float_to_bf16x8(m[s]);  // (bf16 values: the conversion is exact)
+      if (idx == nullptr) continue;  // (the chained SPPF takes the values only: sppf_chain_idx_kernel records its winners)
       uint2 u;
       u.x = (uint32_t)k[s][0] | ((uint32_t)k[s][1] << 8) | ((uint32_t)k[s][2] << 16) | ((uint32_t)k[s][3] << 24);
       u.y = (uint32_t)k[s][4] | ((uint32_t)k[s][5] << 8) | ((uint32_t)k[s][6] << 16) | ((uint32_t)k[s][7] << 24);
@@ -744,6 +745,70 @@ __global__ void __launch_bounds__(kEwThreads) spp_pool_bwd_kernel(const __nv_bfl
       }
     }
     reinterpret_cast<uint4*>(da + p * C)[v] = float_to_bf16x8(acc);
+  }
+}
+
+// Chained SPPF (yolo_modules.py:165-194 with kernel_sizes = 5): y1 = mp5(x), y2 = mp5(y1), y3 = mp5(y2).  The values are those of the
+// parallel 5 / 9 / 13 pools (spp_pool_fwd_kernel writes cat = [x | y1 | y2 | y3]), but autograd through the chain routes each stage's
+// gradient to the winner of the 5 x 5 window of that stage's own input, which on ties is not the parallel pools' winner.  idx [3][B*H*W][C]
+// uint8: per stage s, the row-major offset (0..24) in the window over cat slice s of its first maximum (NaN wins; the window starts at its
+// first in-map element, as in max_pool2d).  Thread = one (pixel, channel).
+__global__ void __launch_bounds__(kEwThreads) sppf_chain_idx_kernel(const __nv_bfloat16* __restrict__ cat, int B, int H, int W, int C, uint8_t* __restrict__ idx) {
+  const long long npix = (long long)B * H * W, n = npix * C;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int c = (int)(i % C);
+    const long long p = i / C;
+    const int w = (int)(p % W);
+    const long long t = p / W;
+    const int h = (int)(t % H);
+    const long long img = (t / H) * H * W;
+    for (int s = 0; s < 3; ++s) {
+      float m = -INFINITY;
+      int k = (max(-h, -2) + 2) * 5 + max(-w, -2) + 2;
+      for (int dy = -2; dy <= 2; ++dy) {
+        const int y = h + dy;
+        if (y < 0 || y >= H) continue;
+        for (int dx = -2; dx <= 2; ++dx) {
+          const int x = w + dx;
+          if (x < 0 || x >= W) continue;
+          const float f = __bfloat162float(cat[(img + (long long)y * W + x) * 4 * C + s * C + c]);
+          if (f > m || f != f) { m = f; k = (dy + 2) * 5 + dx + 2; }
+        }
+      }
+      idx[(s * npix + p) * C + c] = (uint8_t)k;
+    }
+  }
+}
+
+// One backward stage of the chain: D_s = g[..., s C + c] + the D_{s+1} of every q in the 5 x 5 around p whose stage-s window chose p, in
+// row-major q order (D_3 = g[..., 3C + c]).  d_next: fp32 D_{s+1}, or nullptr for s = 2; the result goes to d_out (fp32) or, for s = 0, to
+// da (bf16, rounded once).  A deterministic gather: no atomics.
+__global__ void __launch_bounds__(kEwThreads) sppf_chain_bwd_kernel(const __nv_bfloat16* __restrict__ g, const uint8_t* __restrict__ idx, int s,
+                                                                    const float* __restrict__ d_next, float* __restrict__ d_out, __nv_bfloat16* __restrict__ da,
+                                                                    int B, int H, int W, int C) {
+  const long long npix = (long long)B * H * W, n = npix * C;
+  const uint8_t* is = idx + s * n;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int c = (int)(i % C);
+    const long long p = i / C;
+    const int w = (int)(p % W);
+    const long long t = p / W;
+    const int h = (int)(t % H);
+    const long long img = (t / H) * H * W;
+    float acc = __bfloat162float(g[p * 4 * C + s * C + c]);
+    for (int ey = -2; ey <= 2; ++ey) {  // q = (h + ey, w + ex): p sits at (-ey, -ex) from q's centre
+      const int y = h + ey;
+      if (y < 0 || y >= H) continue;
+      for (int ex = -2; ex <= 2; ++ex) {
+        const int x = w + ex;
+        if (x < 0 || x >= W) continue;
+        const long long q = img + (long long)y * W + x;
+        if (is[q * C + c] != (uint8_t)((2 - ey) * 5 + (2 - ex))) continue;
+        acc += d_next ? d_next[q * C + c] : __bfloat162float(g[q * 4 * C + (s + 1) * C + c]);
+      }
+    }
+    if (d_out) d_out[i] = acc;
+    else da[i] = __float2bfloat16_rn(acc);
   }
 }
 
@@ -1339,6 +1404,35 @@ extern "C" int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B,
                                                                          static_cast<__nv_bfloat16*>(da));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_sppf_chain_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream) {
+  CVB_REQUIRE(a && cat && idx && B > 0 && H > 0 && W > 0 && C > 0, "train_sppf_chain_fwd: bad argument");
+  CVB_REQUIRE(C % 8 == 0, "train_sppf_chain_fwd: C must be a multiple of 8 (C=%d)", C);
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0, "train_sppf_chain_fwd: a / cat must be 16-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  const long long n = (long long)B * H * W * C;
+  spp_pool_fwd_kernel<<<ew_grid(n / 8), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat), nullptr);
+  sppf_chain_idx_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(cat), B, H, W, C, static_cast<uint8_t*>(idx));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(2);
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_sppf_chain_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, float* scratch, void* da, void* stream) {
+  CVB_REQUIRE(g && idx && scratch && da && B > 0 && H > 0 && W > 0 && C > 0, "train_sppf_chain_bwd: bad argument");
+  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da) | reinterpret_cast<uintptr_t>(scratch)) & 3) == 0,
+              "train_sppf_chain_bwd: g / scratch / da must be 4-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  const long long n = (long long)B * H * W * C;
+  const __nv_bfloat16* gb = static_cast<const __nv_bfloat16*>(g);
+  const uint8_t* ib = static_cast<const uint8_t*>(idx);
+  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 2, nullptr, scratch, nullptr, B, H, W, C);
+  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 1, scratch, scratch + n, nullptr, B, H, W, C);
+  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 0, scratch + n, nullptr, static_cast<__nv_bfloat16*>(da), B, H, W, C);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(3);
   return CVB_OK;
 }
 

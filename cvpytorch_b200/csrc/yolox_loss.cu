@@ -63,17 +63,9 @@ __device__ __forceinline__ Anchor anchor_at(const LossLevels& L, int b, int a) {
   return r;
 }
 
-__device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 // F.binary_cross_entropy with target 0 / 1: -max(log1p(-q), -100) / -max(log(q), -100)
 __device__ __forceinline__ float bce0(float q) { return -fmaxf(log1pf(-q), -100.0f); }
 __device__ __forceinline__ float bce1(float q) { return -fmaxf(logf(q), -100.0f); }
-
-// BCEWithLogits(x, t) = (1 - t) x + m + log(exp(-m) + exp(-x - m)), m = max(-x, 0)
-__device__ __forceinline__ float bce_logits(float x, float t) {
-  const float m = fmaxf(-x, 0.0f);
-  return (1.0f - t) * x + m + logf(expf(-m) + expf(-x - m));
-}
 
 // decoded prediction (yolox_loss.py:150-152): xy = (p + grid) * s, wh = exp(p) * s
 __device__ __forceinline__ float4 decode(const Anchor& an) {

@@ -17,7 +17,7 @@ from copy import deepcopy
 import torch
 import torch.nn as nn
 
-from . import _lib, ops
+from . import _lib, ops, train, yolov5_train
 from .engine import GraphBuilder
 from .modules import ConvModule, CSPLayer, DownsamplingModule, SPPF, UpsamplingModule, _build, _Standalone, folded
 
@@ -232,8 +232,9 @@ def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=Non
 
 
 class YOLOv5(_Standalone):
-    """Model-level drop-in for src.models.yolov5.YOLOv5 (inference path).  forward(imgs, targets, mode) keeps the
-    reference contract: mode 'val' -> (losses_dict, outputs list of {'boxes','labels','scores'})."""
+    """Model-level drop-in for src.models.yolov5.YOLOv5.  forward(imgs, targets, mode) keeps the reference contract: mode 'val' (eval()) ->
+    (losses_dict, outputs list of {'boxes','labels','scores'}) from the cached inference graph; mode 'train' (train()) -> the loss dict
+    {'loss', 'box_loss', 'obj_loss', 'cls_loss'} from the training kernels and the YOLOv5Loss over the same parameters."""
     anchors = [[[1.25000, 1.62500], [2.00000, 3.75000], [4.12500, 2.87500]],
                [[1.87500, 3.81250], [3.87500, 2.81250], [3.68750, 7.43750]],
                [[3.62500, 2.81250], [4.87500, 6.18750], [11.65625, 10.18750]]]
@@ -259,11 +260,20 @@ class YOLOv5(_Standalone):
         self.conf_thres = 0.001   # yolov5.py:189
         self.iou_thres = 0.6      # yolov5.py:190
         self.max_det = 300
-        self.loss = None          # training loss stays with the reference (SURVEY.md §2 row 17, out of scope)
+        lcfg = model_cfg.get('LOSS') if isinstance(model_cfg, dict) else getattr(model_cfg, 'LOSS', None)
+        lcfg = dict(lcfg) if lcfg else {'name': 'YOLOv5Loss'}
+        if lcfg.pop('name', 'YOLOv5Loss') != 'YOLOv5Loss':
+            raise NotImplementedError('YOLOv5 (H100): only the YOLOv5Loss is on the training path')
+        lcfg.update(anchors=self.anchors, num_classes=self.num_classes)  # yolov5.py:210-219 (setup_extra_params)
+        self.loss = yolov5_train.YOLOv5Loss(**lcfg)  # (no parameters or buffers: the state_dict keys stay the inference model's)
         for m in self.modules():
             if isinstance(m, nn.BatchNorm2d):
                 m.eps = 1e-3
                 m.momentum = 0.03
+        # the training modules (yolov5_train.YOLOv5CSPDarknet / YOLOv5Neck / YOLOv5Detect), built on the first training forward over this
+        # model's own parameters and buffers (train.bound_training_modules)
+        self.__dict__['_train_modules'] = None
+        self._cfgs = (bcfg, ncfg, dcfg)
 
     # ------------------------------------------------------------------ fused graph
     # ToTensor + Normalize of conf/coco_yolov5_s.yml:58-59 (det_transforms.py:85-109), used only by the uint8-frame entry points
@@ -315,11 +325,47 @@ class YOLOv5(_Standalone):
         """Device int32[4] status of the NMS stage of the graph that serves `imgs` ([0] = candidate-capacity overflow flag)."""
         return self._graph_for(imgs)['ws'].status
 
+    def _training_modules(self):
+        """(yolov5_train.YOLOv5CSPDarknet, YOLOv5Neck, YOLOv5Detect) over this model's own parameters, buffers and BatchNorm modules.  Widths
+        the training kernels refuse (YOLOv5-m, -x) raise NotImplementedError."""
+        def build():
+            strip = lambda c: {k: v for k, v in c.items() if k not in ('name', 'depth_mul', 'width_mul')}  # noqa: E731
+            bcfg, ncfg, dcfg = self._cfgs
+            return (yolov5_train.YOLOv5CSPDarknet(**strip(bcfg)), yolov5_train.YOLOv5Neck(**{k: v for k, v in ncfg.items() if k != 'name'}),
+                    yolov5_train.YOLOv5Detect(**{k: v for k, v in dcfg.items() if k != 'name'}))
+        return train.bound_training_modules(self, (self.backbone, self.neck, self.detect), build)
+
+    @staticmethod
+    def pack_targets(imgs, targets):
+        """trans_specific_format (yolov5.py:221-245): the per-image target dicts -> gts [nt, 6] rows (image, label, cx, cy, w, h) on the
+        images' device.  A tensor is taken as already packed."""
+        if isinstance(targets, torch.Tensor):
+            return targets
+        rows = [torch.cat([torch.full((t['labels'].shape[0], 1), float(i), device=imgs.device), t['labels'].to(imgs.device, torch.float32).view(-1, 1),
+                           t['boxes'].to(imgs.device, torch.float32).view(-1, 4)], 1) for i, t in enumerate(targets)]
+        return torch.cat(rows, 0) if rows else torch.zeros((0, 6), device=imgs.device)
+
+    def forward_train(self, imgs, targets):
+        """The reference's training forward (yolov5.py:247-262) on the H100 training kernels: backbone -> neck -> detect -> YOLOv5Loss over this
+        model's parameters; returns {loss [1], box_loss, obj_loss, cls_loss} (device tensors, no host sync)."""
+        if not self.training:
+            raise RuntimeError("YOLOv5 (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
+        if isinstance(imgs, (list, tuple)):
+            imgs = torch.stack(list(imgs))
+        if not imgs.is_cuda:
+            raise _lib.CvbError('YOLOv5 (H100) training: CUDA images required (the training path has no CPU fallback)')
+        gts = self.pack_targets(imgs, targets)
+        bb, nk, dt = self._training_modules()
+        loss, items = self.loss(dt.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gts)
+        return {'loss': loss, 'box_loss': items[0], 'obj_loss': items[1], 'cls_loss': items[2]}
+
     def forward(self, imgs, targets=None, mode='infer', **kwargs):
         if mode == 'infer':
             return  # the reference returns None here (yolov5.py:247-249)
+        if mode == 'train':
+            return self.forward_train(imgs, targets)
         if mode != 'val':
-            raise RuntimeError("YOLOv5 (H100): only mode='val' (inference) is implemented; training stays on the reference")
+            raise RuntimeError(f"YOLOv5 (H100): unknown mode {mode!r}")
         det, _, cnt = self.predict(imgs)
         losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
         # yolov5.py:258: the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps

@@ -280,7 +280,7 @@ class _ConvBnSiLULayer(nn.Module):
         return self._layer(x, self.conv.weight)
 
     def _layer(self, x, weight):
-        _require_training(self, f'cvpytorch_b200.train.{self.drop_in} is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
+        _require_training(self, f'{type(self).__module__}.{self.drop_in} is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
         return _ConvBnSiLU.apply(x, weight, *self._bn_inputs(), self.ksize, self.stride, self.padding)
 
 
@@ -314,12 +314,16 @@ class Bottleneck(nn.Module):
         self.use_add = shortcut and in_channels == out_channels
 
     def forward(self, x):
-        _require_training(self, 'training drop-in: call .train()')
-        c1, c2 = self.conv1, self.conv2
-        y = _BottleneckChain.apply(x, c1.conv.weight, *c1._bn_inputs(), c2.conv.weight, *c2._bn_inputs())
-        if self.use_add:
-            y = y + x
-        return y
+        return _bottleneck(self, x, self.conv1, self.conv2, self.use_add)
+
+
+def _bottleneck(m, x, c1, c2, use_add):
+    """The body of a YOLOX Bottleneck / YOLOv5 C3 bottleneck: c2(c1(x)) as one _BottleneckChain (+ x when use_add)."""
+    _require_training(m, 'training drop-in: call .train()')
+    y = _BottleneckChain.apply(x, c1.conv.weight, *c1._bn_inputs(), c2.conv.weight, *c2._bn_inputs())
+    if use_add:
+        y = y + x
+    return y
 
 
 class CSPLayer(nn.Module):
@@ -420,23 +424,62 @@ class Focus(nn.Module):
         return _to_nchw(self.forward_nhwc(x), x.dtype)
 
 
+def sppf_chain(a):
+    """a NHWC bf16 [B,H,W,C] -> (cat [B,H,W,4C] = [a | y1 | y2 | y3], y_i = maxpool5(y_(i-1)), idx uint8 [3,B,H,W,C]: each stage's winner in
+    the 5x5 window of its own input)."""
+    B, H, W, C = a.shape
+    cat = torch.empty((B, H, W, 4 * C), dtype=torch.bfloat16, device=a.device)
+    idx = torch.empty((3, B, H, W, C), dtype=torch.uint8, device=a.device)
+    _lib.check(_lib.lib().cvb_train_sppf_chain_fwd(_p(a), B, H, W, C, _p(cat), _p(idx), _stream()), 'cvb_train_sppf_chain_fwd')
+    return cat, idx
+
+
+def sppf_chain_backward(g, idx):
+    """g = d(loss)/d(cat) [B,H,W,4C], idx of sppf_chain -> d(loss)/d(a) [B,H,W,C]: autograd through the chain (deterministic fp32 gathers)."""
+    B, H, W, C4 = g.shape
+    da = torch.empty((B, H, W, C4 // 4), dtype=torch.bfloat16, device=g.device)
+    scratch = torch.empty((2, B, H, W, C4 // 4), dtype=torch.float32, device=g.device)
+    _lib.check(_lib.lib().cvb_train_sppf_chain_bwd(_p(g), _p(idx), B, H, W, C4 // 4, _p(scratch), _p(da), _stream()), 'cvb_train_sppf_chain_bwd')
+    return da
+
+
+class _SppfChain(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, a):
+        _check_cuda(a, 'SPPF (H100 training)')
+        cat, idx = sppf_chain(a.contiguous())
+        ctx.save_for_backward(idx)
+        return cat
+
+    @staticmethod
+    def backward(ctx, g):
+        idx, = ctx.saved_tensors
+        return sppf_chain_backward(g.contiguous(), idx)
+
+
 class SPPF(nn.Module):
-    """src/models/modules/yolo_modules.py:165-194 with kernel_sizes (5, 9, 13): conv1 (C -> C/2) -> [x | mp5 | mp9 | mp13] (parallel pools,
-    one kernel that writes the concatenation conv2 reads) -> conv2 (2C -> C).  forward: NCHW; forward_nhwc: NHWC bf16."""
+    """src/models/modules/yolo_modules.py:165-194: conv1 (C -> C/2) -> pools -> conv2 (2C -> C), with kernel_sizes (5, 9, 13) (YOLOX: the
+    parallel pools [x | mp5 | mp9 | mp13]) or 5 (YOLOv5: the chained pools [x | y1 | y2 | y3], y_i = mp5(y_(i-1)): the same values, but the
+    gradient of a tie goes where autograd through the chain sends it).  One kernel writes the concatenation conv2 reads.  forward: NCHW;
+    forward_nhwc: NHWC bf16."""
 
     def __init__(self, in_channels, out_channels, kernel_sizes=(5, 9, 13), conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True),
                  act_cfg=dict(type='Swish'), init_cfg=None):
         super().__init__()
-        if isinstance(kernel_sizes, int) or tuple(kernel_sizes) != (5, 9, 13):
-            raise NotImplementedError(f'H100 training SPPF: kernel_sizes (5, 9, 13) only (got {kernel_sizes})')
+        chained = isinstance(kernel_sizes, int) and kernel_sizes == 5
+        if not chained and (isinstance(kernel_sizes, int) or tuple(kernel_sizes) != (5, 9, 13)):
+            raise NotImplementedError(f'H100 training SPPF: kernel_sizes (5, 9, 13) or 5 only (got {kernel_sizes})')
         self.kernel_sizes = kernel_sizes
         hidden_channels = in_channels // 2
         self.conv1 = BaseConv(in_channels, hidden_channels, 1, stride=1)
-        self.m = nn.ModuleList([nn.MaxPool2d(kernel_size=ks, stride=1, padding=ks // 2) for ks in kernel_sizes])  # (parameter-free; module-tree parity)
+        # (parameter-free; module-tree parity)
+        self.m = (nn.MaxPool2d(kernel_size=5, stride=1, padding=2) if chained else
+                  nn.ModuleList([nn.MaxPool2d(kernel_size=ks, stride=1, padding=ks // 2) for ks in kernel_sizes]))
         self.conv2 = BaseConv(hidden_channels * 4, out_channels, 1, stride=1)
+        self._pool = _SppfChain if chained else _SppPool
 
     def forward_nhwc(self, x):
-        return self.conv2(_SppPool.apply(self.conv1(x)))
+        return self.conv2(self._pool.apply(self.conv1(x)))
 
     def forward(self, x):
         return _to_nchw(self.forward_nhwc(_to_nhwc(x, 'SPPF (H100 training)')), x.dtype)
@@ -444,6 +487,33 @@ class SPPF(nn.Module):
 
 def _nhwc(m, x):
     return m.forward_nhwc(x) if isinstance(m, (CSPLayer, SPPF)) else m(x)
+
+
+def bound_training_modules(model, inference_modules, build):
+    """The training modules of a model-level drop-in (build() -> a tuple, one per inference module), kept out of the model's module tree and
+    whose parameters, buffers and BatchNorm modules ARE the inference modules' (re-bound by name on every call: .to() replaces buffer tensors,
+    convert_sync_batchnorm replaces the BatchNorm modules, and the layers sync their statistics when they see an nn.SyncBatchNorm).  So
+    state_dict(), the optimiser's parameters and the statistics eval() folds are the same tensors.  Built on the first call and cached in
+    model.__dict__['_train_modules']; a training module whose keys differ from its inference module's raises NotImplementedError."""
+    if model.__dict__.get('_train_modules') is None:
+        mods = build()
+        binds = []
+        for tm, im in zip(mods, inference_modules):
+            if list(tm.state_dict()) != list(im.state_dict()):
+                raise NotImplementedError(f'{type(model).__name__} (H100) training: {type(im).__name__} keys differ from the training module\'s')
+            for name, sub in tm.named_modules():  # (bound by name: the key lists are equal)
+                if isinstance(sub, nn.modules.batchnorm._BatchNorm):  # the module itself, with its parameters and buffers
+                    parent, _, leaf = name.rpartition('.')
+                    binds.append((tm.get_submodule(parent)._modules, leaf, im.get_submodule(parent)._modules))
+                elif sub._parameters or sub._buffers:
+                    src = im.get_submodule(name)
+                    binds += [(sub._parameters, k, src._parameters) for k in sub._parameters]
+                    binds += [(sub._buffers, k, src._buffers) for k in sub._buffers]
+        model.__dict__['_train_modules'] = (mods, binds)
+    mods, binds = model._train_modules
+    for dst, k, src in binds:
+        dst[k] = src[k]
+    return mods
 
 
 class CSPDarknet(nn.Module):

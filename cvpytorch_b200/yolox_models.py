@@ -309,30 +309,13 @@ class YOLOX(_Standalone):
         return G['ws'].det, G['ws'].count
 
     def _training_modules(self):
-        """(train.CSPDarknet, train.YOLOXNeck, train.YOLOXHead) whose parameters, buffers and BatchNorm modules ARE this model's (re-bound on
-        every call: .to() replaces buffer tensors, convert_sync_batchnorm replaces the BatchNorm modules, and the layers sync their statistics
-        when they see an nn.SyncBatchNorm).  Widths the training kernels refuse (YOLOX-t, -m, -x) raise NotImplementedError."""
-        if self._train_modules is None:
+        """(train.CSPDarknet, train.YOLOXNeck, train.YOLOXHead) over this model's own parameters, buffers and BatchNorm modules
+        (train.bound_training_modules).  Widths the training kernels refuse (YOLOX-t, -m, -x) raise NotImplementedError."""
+        def build():
             strip = lambda c: {k: v for k, v in c.items() if k != 'name'}  # noqa: E731
             bcfg, ncfg, hcfg = self._cfgs
-            mods = (train.CSPDarknet(**strip(bcfg)), train.YOLOXNeck(**strip(ncfg)), train.YOLOXHead(**strip(hcfg)))
-            binds = []
-            for tm, im in zip(mods, (self.backbone, self.neck, self.head)):
-                if list(tm.state_dict()) != list(im.state_dict()):
-                    raise NotImplementedError(f'YOLOX (H100) training: {type(im).__name__} keys differ from the training module\'s')
-                for name, sub in tm.named_modules():  # (bound by name: the key lists are equal)
-                    if isinstance(sub, nn.modules.batchnorm._BatchNorm):  # the module itself, with its parameters and buffers
-                        parent, _, leaf = name.rpartition('.')
-                        binds.append((tm.get_submodule(parent)._modules, leaf, im.get_submodule(parent)._modules))
-                    elif sub._parameters or sub._buffers:
-                        src = im.get_submodule(name)
-                        binds += [(sub._parameters, k, src._parameters) for k in sub._parameters]
-                        binds += [(sub._buffers, k, src._buffers) for k in sub._buffers]
-            self.__dict__['_train_modules'] = (mods, binds)
-        mods, binds = self._train_modules
-        for dst, k, src in binds:
-            dst[k] = src[k]
-        return mods
+            return train.CSPDarknet(**strip(bcfg)), train.YOLOXNeck(**strip(ncfg)), train.YOLOXHead(**strip(hcfg))
+        return train.bound_training_modules(self, (self.backbone, self.neck, self.head), build)
 
     def pack_targets(self, imgs, targets):
         """trans_specific_format (yolox.py:112-139): the per-image target dicts -> gt [B, max_labels, 5] rows (label, box) on the images'

@@ -372,6 +372,11 @@ int cvb_coco_pack(const float* rows, int32_t B, int32_t M, int32_t row_stride, c
  *   (ties: the first maximal element, as torch's max_pool2d).
  * cvb_train_spp_pool_bwd: g = d(loss)/d(cat) [B,H,W,4C], idx of the forward -> da [B,H,W,C] = g[..., :C] + the pooled gradients routed to
  *   their winners; a gather summed in fp32 in a fixed order (bitwise reproducible).
+ * cvb_train_sppf_chain_fwd: the chained SPPF of YOLOv5 (kernel_sizes = 5: y1 = maxpool5(a), y2 = maxpool5(y1), y3 = maxpool5(y2)) ->
+ *   cat [B,H,W,4C] = [a | y1 | y2 | y3] (the values of the parallel pools) and idx uint8 [3][B*H*W][C]: per stage, the row-major offset
+ *   (0..24) of the first maximum of the 5 x 5 window of that stage's input (NaN propagates, as torch's max_pool2d).
+ * cvb_train_sppf_chain_bwd: g = d(loss)/d(cat), idx of the forward -> da [B,H,W,C], autograd through the chain (y3 -> y2 -> y1 -> a, each
+ *   stage adding its slice of g); deterministic fp32 gathers, scratch: 2 * B*H*W*C floats owned by the caller.
  *
  * YOLOX neck and head training (src/models/necks/yolox_neck.py:13-74, src/models/heads/yolox_head.py:14-88) adds:
  * cvb_train_upsample_cat_fwd: cat [B,2h,2w,Ca+Cb] = [nearest_up2(a [B,h,w,Ca]) | b [B,2h,2w,Cb]] (the neck's top-down upsample + concat,
@@ -405,6 +410,8 @@ int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void* y, int64_t
 int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream);
 int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream);
 int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, void* da, void* stream);
+int cvb_train_sppf_chain_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream);
+int cvb_train_sppf_chain_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, float* scratch, void* da, void* stream);
 int cvb_train_upsample_cat_fwd(const void* a, int32_t B, int32_t h, int32_t w, int32_t Ca, const void* b, int32_t Cb, void* cat, void* stream);
 int cvb_train_upsample_cat_bwd(const void* g, int32_t B, int32_t h, int32_t w, int32_t Ca, int32_t Cb, void* da, void* db, void* stream);
 int cvb_train_conv_pad(const void* x, int32_t B, int32_t H, int32_t W, int32_t cin, const void* w_packed, int32_t cout, int32_t k, int32_t pad, void* out,
@@ -449,6 +456,27 @@ int cvb_train_bn_silu_bwd_apply(const void* g, int32_t g_is_dz, const void* y, i
  * cvb_train_yolox_loss_bwd: grads[l] fp32 NCHW, shapes of preds[l] (every element written) = d(sum_i grad_out[i] out[i]) / d(preds[l]) for
  *   i < 4, under the forward's assignment (matched_gt, matched_iou, fwd_out = its out).  grad_out: fp32 [4] on the device.
  */
+/* YOLOv5 training loss (src/losses/yolov5_loss.py:135-278; csrc/yolov5_loss.cu): build_targets' candidate list, the CIoU box,
+ * objectness and class BCE losses and their gradient with respect to the detect convs' outputs.  preds[l]: fp32 NCHW [B, na (5 + nc), ny_l,
+ * nx_l] (read in place as [B, na, 5 + nc, ny, nx]), shapes[4 l ..] = (B, na (5 + nc), ny_l, nx_l), 1 <= nlev <= 4, 1 <= na <= 8.
+ * anchors: host fp32 [nlev][na][2] in grid units; balance: host fp32 [nlev]; hyp: host fp32 [5] = (anchor_t, box, obj, cls, gr).
+ * targets: fp32 [nt, 6] rows (image, class, cx, cy, w, h) normalised to [0, 1] on the device, nt >= 0.  A class outside [0, nc) gets no
+ * one-hot entry; an image index outside [0, B) matches nothing.  cap = 5 na nt candidates per level.
+ * cvb_train_yolov5_loss_fwd: out fp32 [4] = (loss, lbox, lobj, lcls) of the reference ((lbox + lobj + lcls) B with the hyper-parameter
+ *   weights applied); per level l the candidate list in the reference's order: ncand[l], cand_idx int32 [nlev][cap][5] = (image, anchor,
+ *   gj, gi, class) and cand_box fp32 [nlev][cap][6] = (tbox x, y, w, h, anchor w, h).  workspace: cvb_train_yolov5_loss_workspace_bytes(nlev,
+ *   na, nt) bytes, 256-byte aligned, kept for the backward.  No host sync; bitwise reproducible.
+ * cvb_train_yolov5_loss_bwd: grads[l] fp32, shapes of preds[l] (every element written) = grad_out[0] d(loss)/d(preds[l]) under the
+ *   forward's candidates and workspace.  grad_out: fp32 [1] on the device.
+ */
+size_t cvb_train_yolov5_loss_workspace_bytes(int32_t nlev, int32_t na, int32_t nt);
+int cvb_train_yolov5_loss_fwd(const float* const* preds, const int32_t* shapes, const float* anchors, const float* balance, int32_t nlev, int32_t na,
+                              int32_t nc, const float* targets, int32_t nt, const float* hyp, int32_t* cand_idx, float* cand_box, int32_t* ncand,
+                              float* out, void* workspace, size_t ws_bytes, void* stream);
+int cvb_train_yolov5_loss_bwd(const float* const* preds, const int32_t* shapes, const float* anchors, const float* balance, int32_t nlev, int32_t na,
+                              int32_t nc, const float* targets, int32_t nt, const float* hyp, const int32_t* cand_idx, const float* cand_box,
+                              const int32_t* ncand, const void* workspace, size_t ws_bytes, const float* grad_out, float* const* grads, void* stream);
+
 size_t cvb_train_yolox_loss_workspace_bytes(int32_t B, int32_t A);
 int cvb_train_yolox_loss_fwd(const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, const float* targets,
                              int32_t B, int32_t max_gt, int32_t* matched_gt, float* matched_iou, float* out, void* workspace, size_t ws_bytes,
