@@ -39,6 +39,12 @@ class CvbNmsParams(ctypes.Structure):
                 ('max_wh', c_float), ('hist_ready', c_int32)]
 
 
+class CvbEmaEntry(ctypes.Structure):
+    _fields_ = [('ema', c_void_p), ('src', c_void_p), ('numel', c_int64)]
+
+
+CVB_EMA_TABLE_ENTRY_BYTES = 32
+
 # name -> (restype, argtypes); must list every symbol include/cvb200.h declares
 SYMBOLS = {
     'cvb_conv_plan_create': (c_int32, [POINTER(CvbConvDesc), POINTER(c_void_p)]),
@@ -80,6 +86,8 @@ SYMBOLS = {
     'cvb_train_yolov5_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_int32, c_int32, c_int32, c_void_p,
                                             c_int32, POINTER(c_float), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, POINTER(c_void_p),
                                             c_void_p]),
+    'cvb_ema_table_upload': (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
+    'cvb_ema_update': (c_int32, [c_void_p, c_int32, c_float, c_float, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

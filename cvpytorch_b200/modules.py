@@ -71,6 +71,16 @@ class _Standalone(nn.Module):
     def _drop_graphs(self):
         self._graphs.clear()
 
+    def __getstate__(self):
+        """What copy.deepcopy and pickle take: the module without its device caches.  The graphs (plans that own C handles, buffers, TMA
+        descriptors) are rebuilt on the copy's first eval-mode call, and the training modules (train.bound_training_modules, bound to THIS
+        model's tensors) on its first training call, so the copy never runs on the original's parameters.  The original keeps both."""
+        state = super().__getstate__()
+        state['_graphs'] = {}
+        if '_train_modules' in state:
+            state['_train_modules'] = None
+        return state
+
     def train(self, mode=True):
         self._drop_graphs()
         return super().train(mode)

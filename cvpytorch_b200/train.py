@@ -494,7 +494,8 @@ def bound_training_modules(model, inference_modules, build):
     whose parameters, buffers and BatchNorm modules ARE the inference modules' (re-bound by name on every call: .to() replaces buffer tensors,
     convert_sync_batchnorm replaces the BatchNorm modules, and the layers sync their statistics when they see an nn.SyncBatchNorm).  So
     state_dict(), the optimiser's parameters and the statistics eval() folds are the same tensors.  Built on the first call and cached in
-    model.__dict__['_train_modules']; a training module whose keys differ from its inference module's raises NotImplementedError."""
+    model.__dict__['_train_modules'], which a deepcopy or pickle of the model leaves None (modules._Standalone.__getstate__) so that the copy
+    binds its own tensors; a training module whose keys differ from its inference module's raises NotImplementedError."""
     if model.__dict__.get('_train_modules') is None:
         mods = build()
         binds = []

@@ -485,6 +485,24 @@ int cvb_train_yolox_loss_bwd(const float* const* preds, const int32_t* shapes, c
                              int32_t B, int32_t max_gt, const int32_t* matched_gt, const float* matched_iou, const float* fwd_out,
                              const float* grad_out, float* const* grads, void* stream);
 
+/* Model EMA (src/utils/ema.py ModelEMA.update; csrc/ema.cu): one EMA step over every entry of a table in ONE launch,
+ * ema[j] = fl(fl(ema[j] * decay) + fl(src[j] * one_minus_decay)) for j < numel, fp32, no FMA contraction: bitwise the reference's
+ * `item *= decay; item += (1 - decay) * src` with decay = (float)d and one_minus_decay = (float)(1.0 - d) rounded from the host's double d.
+ * cvb_ema_table_upload: checks the host table entries [n] (n >= 1; numel >= 0; ema and src non-null when numel > 0) and enqueues its copy
+ *   on `stream` into `table`, caller-owned device memory of n * CVB_EMA_TABLE_ENTRY_BYTES bytes, 16-byte aligned.  The entries' ema ranges
+ *   must not overlap each other or any src range.  Not capturable (host-to-device copy from pageable memory).
+ * cvb_ema_update: the step over an uploaded table of n entries; any pointer alignment (float4 where ema and src are both 16-byte aligned).
+ *   No host sync, CUDA-graph capturable.
+ */
+#define CVB_EMA_TABLE_ENTRY_BYTES 32
+typedef struct {
+  float* ema;       /* fp32, contiguous, updated in place */
+  const float* src; /* fp32, contiguous, the model's tensor */
+  int64_t numel;
+} CvbEmaEntry;
+int cvb_ema_table_upload(const CvbEmaEntry* entries, int32_t n, void* table, void* stream);
+int cvb_ema_update(const void* table, int32_t n, float decay, float one_minus_decay, void* stream);
+
 /* Library info / errors */
 const char* cvb_last_error_string(void);
 int cvb_version(void);
