@@ -45,6 +45,21 @@ class CvbEmaEntry(ctypes.Structure):
 
 CVB_EMA_TABLE_ENTRY_BYTES = 32
 
+
+class CvbSgdGroup(ctypes.Structure):
+    _fields_ = [('lr', c_float), ('weight_decay', c_float), ('momentum', c_float), ('flags', c_int32)]
+
+
+class CvbSgdEntry(ctypes.Structure):
+    _fields_ = [('param', c_void_p), ('grad', c_void_p), ('momentum_buffer', c_void_p), ('valid', c_void_p), ('numel', c_int64),
+                ('group', c_int32)]
+
+
+CVB_SGD_TABLE_ENTRY_BYTES = 64
+CVB_SGD_CHUNK = 4096
+CVB_SGD_MAX_GROUPS = 1024
+CVB_SGD_NESTEROV, CVB_SGD_WEIGHT_DECAY, CVB_SGD_MOMENTUM = 1, 2, 4
+
 # name -> (restype, argtypes); must list every symbol include/cvb200.h declares
 SYMBOLS = {
     'cvb_conv_plan_create': (c_int32, [POINTER(CvbConvDesc), POINTER(c_void_p)]),
@@ -88,6 +103,8 @@ SYMBOLS = {
                                             c_void_p]),
     'cvb_ema_table_upload': (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
     'cvb_ema_update': (c_int32, [c_void_p, c_int32, c_float, c_float, c_void_p]),
+    'cvb_sgd_table_upload': (c_int32, [POINTER(CvbSgdEntry), c_int32, c_int32, c_void_p, c_void_p]),
+    'cvb_sgd_step': (c_int32, [c_void_p, c_int32, POINTER(CvbSgdGroup), c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

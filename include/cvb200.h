@@ -503,6 +503,44 @@ typedef struct {
 int cvb_ema_table_upload(const CvbEmaEntry* entries, int32_t n, void* table, void* stream);
 int cvb_ema_update(const void* table, int32_t n, float decay, float one_minus_decay, void* stream);
 
+/* SGD step (torch.optim.SGD under torch.amp.GradScaler; csrc/sgd.cu): every parameter of every group in ONE launch, fp32, bitwise the
+ * reference's GradScaler.unscale_ + _multi_tensor_sgd on the same GPU (the per-element formula is in sgd.cu).  Momentum buffer validity
+ * lives on the device: `valid` holds one int32 per CVB_SGD_CHUNK elements of the parameter (one for an empty parameter), 0 while the
+ * buffer has never been written (the next applied step copies d into it, as the reference's first step clones it), 1 after.
+ * cvb_sgd_table_upload: checks the host table entries [n] (n >= 1; 1 <= n_groups <= CVB_SGD_MAX_GROUPS; numel >= 0; 0 <= group < n_groups;
+ *   param and grad non-null when numel > 0; valid non-null with a momentum_buffer, and a momentum_buffer with valid when numel > 0) and
+ *   enqueues its copy on `stream` into `table`, caller-owned device memory of n * CVB_SGD_TABLE_ENTRY_BYTES bytes, 16-byte aligned.  Every
+ *   entry of a group with CVB_SGD_MOMENTUM needs valid (and a momentum_buffer when numel > 0); the params must not overlap each other.
+ *   Not capturable (host-to-device copy from pageable memory).
+ * cvb_sgd_step: the step over an uploaded table of n entries with the groups [n_groups] passed by value (no copy of their own).
+ *   grad_scale (optional, device fp32 scalar): the gradients are multiplied by (float)(1.0 / (double)*grad_scale) first.  found_inf
+ *   (optional, device fp32 scalar): when non-zero, nothing is written.  Any pointer alignment (float4 where param, grad and buffer are
+ *   16-byte aligned).  No host sync, CUDA-graph capturable.
+ */
+#define CVB_SGD_TABLE_ENTRY_BYTES 64
+#define CVB_SGD_CHUNK 4096
+#define CVB_SGD_MAX_GROUPS 1024 /* 16 KB of kernel arguments */
+#define CVB_SGD_NESTEROV 1      /* CvbSgdGroup.flags: nesterov=True */
+#define CVB_SGD_WEIGHT_DECAY 2  /* weight_decay != 0 (in the Python double) */
+#define CVB_SGD_MOMENTUM 4      /* momentum != 0 (in the Python double) */
+typedef struct {
+  float lr;
+  float weight_decay;
+  float momentum;
+  int32_t flags;
+} CvbSgdGroup;
+typedef struct {
+  float* param;           /* fp32, contiguous, updated in place */
+  const float* grad;      /* fp32, contiguous, shaped as param; read only */
+  float* momentum_buffer; /* fp32, contiguous, shaped as param; NULL in a group without momentum */
+  int32_t* valid;         /* max(1, ceil(numel / CVB_SGD_CHUNK)) flags; NULL in a group without momentum */
+  int64_t numel;
+  int32_t group;
+} CvbSgdEntry;
+int cvb_sgd_table_upload(const CvbSgdEntry* entries, int32_t n, int32_t n_groups, void* table, void* stream);
+int cvb_sgd_step(const void* table, int32_t n, const CvbSgdGroup* groups, int32_t n_groups, const float* grad_scale, const float* found_inf,
+                 void* stream);
+
 /* Library info / errors */
 const char* cvb_last_error_string(void);
 int cvb_version(void);
