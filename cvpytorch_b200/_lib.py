@@ -60,6 +60,14 @@ CVB_SGD_CHUNK = 4096
 CVB_SGD_MAX_GROUPS = 1024
 CVB_SGD_NESTEROV, CVB_SGD_WEIGHT_DECAY, CVB_SGD_MOMENTUM = 1, 2, 4
 
+CVB_COCO_IOU_THRS, CVB_COCO_REC_THRS = 10, 101
+CVB_COCO_MAX_IMAGES, CVB_COCO_MAX_CATS, CVB_COCO_MAX_GT, CVB_COCO_MAX_DETS = 1 << 20, 4000, 1 << 26, 1 << 28
+
+
+class CvbCocoEvalParams(ctypes.Structure):
+    _fields_ = [('n_images', c_int32), ('n_cats', c_int32), ('n_gt', c_int32), ('n_det', c_int32), ('iou_thrs', c_double * CVB_COCO_IOU_THRS),
+                ('rec_thrs', c_double * CVB_COCO_REC_THRS)]
+
 # name -> (restype, argtypes); must list every symbol include/cvb200.h declares
 SYMBOLS = {
     'cvb_conv_plan_create': (c_int32, [POINTER(CvbConvDesc), POINTER(c_void_p)]),
@@ -105,6 +113,9 @@ SYMBOLS = {
     'cvb_ema_update': (c_int32, [c_void_p, c_int32, c_float, c_float, c_void_p]),
     'cvb_sgd_table_upload': (c_int32, [POINTER(CvbSgdEntry), c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_sgd_step': (c_int32, [c_void_p, c_int32, POINTER(CvbSgdGroup), c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_coco_eval_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32]),
+    'cvb_coco_eval_bbox': (c_int32, [POINTER(CvbCocoEvalParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

@@ -520,3 +520,43 @@ def coco_pack(rows, count, image_ids, id2category=None):
                                         int(cat.numel()) if cat is not None else 0, rec_ids.data_ptr(), rec_box.data_ptr(), total.data_ptr(), _stream()),
                'cvb_coco_pack')
     return rec_ids, rec_box, total
+
+
+# --------------------------------------------------------------------------------------- output side: COCO box mAP (csrc/coco_eval.cu)
+def coco_eval_bbox(gt_key, gt_box, gt_area, gt_crowd, img_evaluated, det_img, det_cat, det_score, det_box, n_cats, iou_thrs, rec_thrs):
+    """pycocotools COCOeval (bbox, default parameters) evaluate + accumulate + summarize on the device.  Ground truths: gt_key [G] int32
+    (category index * n_images + image index, ascending, annotation order within a key), gt_box [G,4] xywh float64, gt_area [G] float64,
+    gt_crowd [G] uint8.  img_evaluated [n_images] uint8 (images by ascending id).  Detections: det_img / det_cat [N] int32 (category -1:
+    not evaluated), det_score [N] fp32, det_box [N,4] xywh float64.  All CUDA, contiguous.  Returns device tensors precision
+    [10,101,K,4,3], recall [10,K,4,3], stats [12] (float64) and det_masks [N,4] int32 (bits 0..9 matched, 16..25 ignored per threshold)."""
+    n_images, n_gt, n_det = img_evaluated.numel(), gt_key.numel(), det_img.numel()
+    for name, lim, v in (('images', _lib.CVB_COCO_MAX_IMAGES, n_images), ('categories', _lib.CVB_COCO_MAX_CATS, n_cats),
+                         ('ground truths', _lib.CVB_COCO_MAX_GT, n_gt), ('detections', _lib.CVB_COCO_MAX_DETS, n_det)):
+        if v > lim:
+            raise _lib.CvbError(f'coco_eval_bbox: {v} {name} exceed the limit of {lim}')
+    specs = ((gt_key, torch.int32, (n_gt,)), (gt_box, torch.float64, (n_gt, 4)), (gt_area, torch.float64, (n_gt,)), (gt_crowd, torch.uint8, (n_gt,)),
+             (img_evaluated, torch.uint8, (n_images,)), (det_img, torch.int32, (n_det,)), (det_cat, torch.int32, (n_det,)),
+             (det_score, torch.float32, (n_det,)), (det_box, torch.float64, (n_det, 4)))
+    for t, dtype, shape in specs:
+        _require_cuda(t, 'coco_eval_bbox')
+        if t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous() or t.device != img_evaluated.device:
+            raise _lib.CvbError(f'coco_eval_bbox: expected a contiguous {dtype} {shape} tensor on {img_evaluated.device}, got {t.dtype} '
+                                f'{tuple(t.shape)} on {t.device}')
+    dev = img_evaluated.device
+    p = _lib.CvbCocoEvalParams(n_images, n_cats, n_gt, n_det)
+    p.iou_thrs[:] = [float(x) for x in iou_thrs]
+    p.rec_thrs[:] = [float(x) for x in rec_thrs]
+    ws_bytes = _lib.lib().cvb_coco_eval_workspace_bytes(n_det, n_gt, n_cats)
+    if ws_bytes == 0:
+        raise _lib.CvbError(f'coco_eval_bbox: sizes outside the limits (n_det={n_det}, n_gt={n_gt}, n_cats={n_cats})')
+    ws = torch.empty(ws_bytes + 256, dtype=torch.uint8, device=dev)
+    ws_ptr = (ws.data_ptr() + 255) & ~255
+    precision = torch.empty((10, 101, n_cats, 4, 3), dtype=torch.float64, device=dev)
+    recall = torch.empty((10, n_cats, 4, 3), dtype=torch.float64, device=dev)
+    stats = torch.empty((12,), dtype=torch.float64, device=dev)
+    masks = torch.empty((n_det, 4), dtype=torch.int32, device=dev)
+    ptr = lambda t: t.data_ptr() if t.numel() else None  # noqa: E731
+    _lib.check(_lib.lib().cvb_coco_eval_bbox(ctypes.byref(p), ptr(gt_key), ptr(gt_box), ptr(gt_area), ptr(gt_crowd), img_evaluated.data_ptr(),
+                                             ptr(det_img), ptr(det_cat), ptr(det_score), ptr(det_box), ptr(masks), precision.data_ptr(),
+                                             recall.data_ptr(), stats.data_ptr(), ws_ptr, ws_bytes, _stream()), 'cvb_coco_eval_bbox')
+    return precision, recall, stats, masks

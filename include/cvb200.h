@@ -541,6 +541,40 @@ int cvb_sgd_table_upload(const CvbSgdEntry* entries, int32_t n, int32_t n_groups
 int cvb_sgd_step(const void* table, int32_t n, const CvbSgdGroup* groups, int32_t n_groups, const float* grad_scale, const float* found_inf,
                  void* stream);
 
+/* COCO box mAP (pycocotools COCOeval, iouType 'bbox', default parameters; csrc/coco_eval.cu): matching, precision / recall accumulation and
+ * the 12 summary statistics on the device, stream-ordered, no host sync.  Area ranges all / small / medium / large are [0, 1e10] /
+ * [0, 1024] / [1024, 9216] / [9216, 1e10] (inclusive bounds), maxDets 1 / 10 / 100, every detection segment cut to its best 100.
+ * Ground truths: gt_key [n_gt] = category index * n_images + image index, ascending, annotation order within a key; gt_box [n_gt][4] xywh
+ *   float64; gt_area [n_gt] (the annotation's area field); gt_crowd [n_gt] (1 = iscrowd: ignored, matched by any number of detections).
+ * Images are indexed in ascending image id order; img_evaluated [n_images] is 1 for the images the evaluation covers.
+ * Detections [n_det]: det_img (image index, evaluated), det_cat (category index, or -1 for a category the ground truth does not list: not
+ *   evaluated), det_score (fp32, no NaN), det_box [n_det][4] xywh float64.
+ * Outputs (device): det_masks [n_det][4] per area range (bits 0..9 matched at IoU threshold t, bits 16..25 ignored; 0 for detections past
+ *   rank 100 or of no category); precision [T=10][R=101][n_cats][4][3] and recall [10][n_cats][4][3] float64 laid out as COCOeval's
+ *   eval['precision'] / eval['recall'] (-1 where a category has no non-ignored ground truth); stats [12] float64 in summarize() order.
+ * workspace: cvb_coco_eval_workspace_bytes(n_det, n_gt, n_cats) bytes of device memory, 256-byte aligned (0 = sizes outside the limits).
+ * Limits: n_images <= CVB_COCO_MAX_IMAGES, 1 <= n_cats <= CVB_COCO_MAX_CATS, n_gt <= CVB_COCO_MAX_GT, n_det <= CVB_COCO_MAX_DETS (LVIS
+ *   val has 1 203 categories and 20 k images).  Index ranges and the key order are the caller's contract; the sizes and pointers are checked.
+ */
+#define CVB_COCO_IOU_THRS 10
+#define CVB_COCO_REC_THRS 101
+#define CVB_COCO_MAX_IMAGES (1 << 20)
+#define CVB_COCO_MAX_CATS 4000
+#define CVB_COCO_MAX_GT (1 << 26)
+#define CVB_COCO_MAX_DETS (1 << 28)
+typedef struct {
+  int32_t n_images;
+  int32_t n_cats;
+  int32_t n_gt;
+  int32_t n_det;
+  double iou_thrs[CVB_COCO_IOU_THRS]; /* np.linspace(.5, .95, 10) */
+  double rec_thrs[CVB_COCO_REC_THRS]; /* np.linspace(0, 1, 101) */
+} CvbCocoEvalParams;
+size_t cvb_coco_eval_workspace_bytes(int32_t n_det, int32_t n_gt, int32_t n_cats);
+int cvb_coco_eval_bbox(const CvbCocoEvalParams* params, const uint32_t* gt_key, const double* gt_box, const double* gt_area, const uint8_t* gt_crowd,
+                       const uint8_t* img_evaluated, const int32_t* det_img, const int32_t* det_cat, const float* det_score, const double* det_box,
+                       uint32_t* det_masks, double* precision, double* recall, double* stats, void* workspace, size_t ws_bytes, void* stream);
+
 /* Library info / errors */
 const char* cvb_last_error_string(void);
 int cvb_version(void);
