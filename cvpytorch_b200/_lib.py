@@ -109,7 +109,14 @@ SYMBOLS = {
     'cvb_train_yolov5_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_int32, c_int32, c_int32, c_void_p,
                                             c_int32, POINTER(c_float), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, POINTER(c_void_p),
                                             c_void_p]),
-    'cvb_ema_table_upload': (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
+    'cvb_train_fcos_loss_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32]),
+    'cvb_train_fcos_loss_fwd': (c_int32, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float),
+                                          c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                          c_void_p]),
+    'cvb_train_fcos_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float),
+                                          c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, POINTER(c_void_p),
+                                          POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    'cvb_ema_table_upload':(c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
     'cvb_ema_update': (c_int32, [c_void_p, c_int32, c_float, c_float, c_void_p]),
     'cvb_sgd_table_upload': (c_int32, [POINTER(CvbSgdEntry), c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_sgd_step': (c_int32, [c_void_p, c_int32, POINTER(CvbSgdGroup), c_int32, c_void_p, c_void_p, c_void_p]),

@@ -477,6 +477,32 @@ int cvb_train_yolov5_loss_bwd(const float* const* preds, const int32_t* shapes, 
                               int32_t nc, const float* targets, int32_t nt, const float* hyp, const int32_t* cand_idx, const float* cand_box,
                               const int32_t* ncand, const void* workspace, size_t ws_bytes, const float* grad_out, float* const* grads, void* stream);
 
+/* FCOS training loss (src/losses/fcos_loss.py; csrc/fcos_loss.cu): GenTargets' point assignment, the sigmoid focal, centerness BCE and
+ * 1 - GIoU losses and their gradient with respect to the head outputs.  Per level l (1 <= nlev <= 8): cls[l] fp32 NCHW [B, nc, h_l, w_l],
+ * cnt[l] [B, 1, h_l, w_l], reg[l] [B, 4, h_l, w_l] (ltrb), all read in place; shapes[12 l ..] = the three shapes in that order.
+ * strides[l]: positive integers (as fp32); limit_range fp32 [nlev][2] = (lo, hi), lo < hi.  Points in level order, row-major within a level
+ * (A = sum h_l w_l), at (column stride + stride / 2, row stride + stride / 2).  boxes: fp32 [B, m, 4] (x1, y1, x2, y2 in pixels, 16-byte
+ * aligned), labels: int32 [B, m], 0 <= m <= 1024 (both may be NULL when m = 0); padded rows are -1.  A (point, GT) pair is positive when the
+ * point is strictly inside the box, max(l, t, r, b) is in (lo, hi] and the centre offset is below 1.5 stride; a point's GT is the first
+ * minimum of the area over the m rows (99999999 for a pair that is not positive), and a point without a positive pair is background.  A
+ * label outside 1..nc gives an all-zero one-hot row.  m = 0 gives an all-background batch (the reference raises).
+ * cvb_train_fcos_loss_fwd: out fp32 [4] = (cls_loss, cnt_loss, reg_loss, total), each term the batch mean of the image's sum over
+ *   max(num_pos_b, 1); matched_gt int32 [B, A] (-1 = background) and num_pos int32 [B], both kept for the backward; targets (optional,
+ *   NULL to skip) fp32 [B, A, 5] = the point's centerness and (l, t, r, b) regression targets, -1 for background.  workspace:
+ *   cvb_train_fcos_loss_workspace_bytes(B, A, nc) bytes, 256-byte aligned, owned by the caller.  No host sync; bitwise reproducible.
+ * cvb_train_fcos_loss_bwd: gcls / gcnt / greg[l] fp32 NCHW, shapes of cls / cnt / reg[l] (every element written) = d(sum_i grad_out[i]
+ *   out[i]) / d(outputs) under the forward's matched_gt and num_pos.  grad_out: fp32 [4] on the device.  A logit whose sigmoid saturates
+ *   against its target gives an inf loss and a NaN gradient, as the reference does.
+ */
+size_t cvb_train_fcos_loss_workspace_bytes(int32_t B, int32_t A, int32_t nc);
+int cvb_train_fcos_loss_fwd(const float* const* cls, const float* const* cnt, const float* const* reg, const int32_t* shapes, const float* strides,
+                            const float* limit_range, int32_t nlev, const float* boxes, const int32_t* labels, int32_t B, int32_t m,
+                            int32_t* matched_gt, int32_t* num_pos, float* targets, float* out, void* workspace, size_t ws_bytes, void* stream);
+int cvb_train_fcos_loss_bwd(const float* const* cls, const float* const* cnt, const float* const* reg, const int32_t* shapes, const float* strides,
+                            const float* limit_range, int32_t nlev, const float* boxes, const int32_t* labels, int32_t B, int32_t m,
+                            const int32_t* matched_gt, const int32_t* num_pos, const float* grad_out, float* const* gcls, float* const* gcnt,
+                            float* const* greg, void* stream);
+
 size_t cvb_train_yolox_loss_workspace_bytes(int32_t B, int32_t A);
 int cvb_train_yolox_loss_fwd(const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, const float* targets,
                              int32_t B, int32_t max_gt, int32_t* matched_gt, float* matched_iou, float* out, void* workspace, size_t ws_bytes,
