@@ -68,6 +68,11 @@ class CvbCocoEvalParams(ctypes.Structure):
     _fields_ = [('n_images', c_int32), ('n_cats', c_int32), ('n_gt', c_int32), ('n_det', c_int32), ('iou_thrs', c_double * CVB_COCO_IOU_THRS),
                 ('rec_thrs', c_double * CVB_COCO_REC_THRS)]
 
+
+CVB_SEG_U8, CVB_SEG_I32, CVB_SEG_I64 = 0, 1, 2
+CVB_SEG_ERR_NEGATIVE, CVB_SEG_ERR_OVERFLOW = 1, 2
+CVB_SEG_MAX_N = (1 << 31) - 1  # pixels per cvb_seg_confusion_update call
+
 # name -> (restype, argtypes); must list every symbol include/cvb200.h declares
 SYMBOLS = {
     'cvb_conv_plan_create': (c_int32, [POINTER(CvbConvDesc), POINTER(c_void_p)]),
@@ -123,6 +128,8 @@ SYMBOLS = {
     'cvb_coco_eval_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32]),
     'cvb_coco_eval_bbox': (c_int32, [POINTER(CvbCocoEvalParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'cvb_seg_confusion_nc_max': (c_int32, []),
+    'cvb_seg_confusion_update': (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

@@ -17,7 +17,7 @@ FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler
 TMP="$(mktemp -d)"
 trap 'rm -rf "$TMP"' EXIT
 pids=()
-for src in api conv_tc aux_kernels nms train_kernels yolox_loss yolov5_loss fcos_loss ema sgd coco_eval; do
+for src in api conv_tc aux_kernels nms train_kernels yolox_loss yolov5_loss fcos_loss ema sgd coco_eval seg_eval; do
   FILE_FLAGS=()
   # the losses, the EMA and SGD follow the reference's fp32 operation order, and the COCO evaluation pycocotools' float64 one: no contracted
   # multiply-adds

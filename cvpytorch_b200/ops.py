@@ -560,3 +560,38 @@ def coco_eval_bbox(gt_key, gt_box, gt_area, gt_crowd, img_evaluated, det_img, de
                                              ptr(det_img), ptr(det_cat), ptr(det_score), ptr(det_box), ptr(masks), precision.data_ptr(),
                                              recall.data_ptr(), stats.data_ptr(), ws_ptr, ws_bytes, _stream()), 'cvb_coco_eval_bbox')
     return precision, recall, stats, masks
+
+
+# --------------------------------------------------------------------------------------- output side: segmentation confusion matrix (csrc/seg_eval.cu)
+SEG_DTYPES = {torch.uint8: _lib.CVB_SEG_U8, torch.int32: _lib.CVB_SEG_I32, torch.int64: _lib.CVB_SEG_I64}
+
+
+def seg_nc_max():
+    """The largest class count cvb_seg_confusion_update accepts (nc² uint32 bins in one CTA's shared memory)."""
+    return int(_lib.lib().cvb_seg_confusion_nc_max())
+
+
+def seg_confusion_update(gt, pred, nc, matrix, err):
+    """matrix [nc,nc] uint64 CUDA += the confusion matrix of the label maps gt / pred (uint8, int32 or int64, any shape, equal numel) by
+    eval_segmentation.py's rule: pixels with 0 <= gt < nc count at flat index nc * gt + pred; flat indices outside [0, nc²) OR bit 0
+    (negative) or bit 1 (too large) into err (int32 CUDA, first element).  Non-contiguous maps are made contiguous on the device; no host
+    sync.  Batches above 2^31 - 1 pixels are counted in several launches."""
+    for t in (gt, pred, matrix, err):
+        _require_cuda(t, 'seg_confusion_update')
+    dev = matrix.device
+    if gt.device != dev or pred.device != dev or err.device != dev:
+        raise _lib.CvbError(f'seg_confusion_update: gt on {gt.device}, pred on {pred.device}, err on {err.device}, the matrix on {dev}')
+    if gt.dtype not in SEG_DTYPES or pred.dtype not in SEG_DTYPES:
+        raise TypeError(f'seg_confusion_update: label maps must be uint8, int32 or int64 (got gt {gt.dtype}, pred {pred.dtype})')
+    if gt.numel() != pred.numel():
+        raise ValueError(f'seg_confusion_update: gt has {gt.numel()} elements and pred {pred.numel()}')
+    if matrix.dtype != torch.uint64 or tuple(matrix.shape) != (nc, nc) or not matrix.is_contiguous():
+        raise _lib.CvbError(f'seg_confusion_update: matrix must be a contiguous uint64 [{nc}, {nc}] tensor (got {matrix.dtype} {tuple(matrix.shape)})')
+    if err.dtype != torch.int32 or err.numel() < 1:
+        raise _lib.CvbError(f'seg_confusion_update: err must be an int32 tensor (got {err.dtype} with {err.numel()} elements)')
+    gt, pred = gt.contiguous().view(-1), pred.contiguous().view(-1)
+    n = gt.numel()
+    for off in range(0, n, _lib.CVB_SEG_MAX_N):
+        k = min(_lib.CVB_SEG_MAX_N, n - off)
+        _lib.check(_lib.lib().cvb_seg_confusion_update(gt[off:].data_ptr(), SEG_DTYPES[gt.dtype], pred[off:].data_ptr(), SEG_DTYPES[pred.dtype], k, nc,
+                                                       matrix.data_ptr(), err.data_ptr(), _stream()), 'cvb_seg_confusion_update')
