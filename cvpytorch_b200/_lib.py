@@ -130,6 +130,12 @@ SYMBOLS = {
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'cvb_seg_confusion_nc_max': (c_int32, []),
     'cvb_seg_confusion_update': (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_seg_ce_nc_max': (c_int32, []),
+    'cvb_train_seg_ce_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32]),
+    'cvb_train_seg_ce_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_int32, c_int64, c_int64, c_int64,
+                                       c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'cvb_train_seg_ce_bwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_int32, c_int64, c_int64, c_int64,
+                                       c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_conv_plan_set_profile': (c_int32, [c_void_p, c_void_p, POINTER(c_int32)]),
     'cvb_nchw_to_split': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, POINTER(CvbView), c_void_p]),
     'cvb_split_to_nchw': (c_int32, [POINTER(CvbView), c_void_p, c_void_p]),

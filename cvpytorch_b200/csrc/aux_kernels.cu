@@ -736,16 +736,6 @@ __global__ void global_avgpool_kernel(const __half* __restrict__ x, int npix, in
 }
 
 // ------------------------------------------------------------------ bilinear resize (align_corners = False), split16 -> split16
-// PyTorch semantics (F.interpolate / upsample_bilinear2d): src = max((dst + 0.5) * in/out - 0.5, 0), i1 = min(i0 + 1, in - 1).
-__device__ __forceinline__ void bilinear_src(int dst, float scale, int in_size, int* i0, int* i1, float* l1) {
-  float s = fmaxf(((float)dst + 0.5f) * scale - 0.5f, 0.0f);
-  int a = (int)s;
-  if (a > in_size - 1) a = in_size - 1;
-  *i0 = a;
-  *i1 = a + ((a < in_size - 1) ? 1 : 0);
-  *l1 = s - (float)a;
-}
-
 // CTA = 8 x 8 output pixels x four 8-channel vectors, grid (pixel tiles, channel slabs, B): 32-bit index math, 64-byte runs per pixel.
 __global__ void __launch_bounds__(256) bilinear_resize_kernel(const __half* __restrict__ x, int Hi, int Wi, int C, int xp, long long xplane,
                                                               __half* __restrict__ y, int Ho, int Wo, int yp, long long yplane, int tiles_x) {

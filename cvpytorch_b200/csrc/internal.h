@@ -102,6 +102,18 @@ __device__ __forceinline__ float yolo_wh(float y, float anchor) {
 }
 __device__ __forceinline__ float yolo_score(float cls, float obj) { return __fmul_rn(cls, obj); }
 
+// Source taps of output index dst of a bilinear resize with align_corners = False, PyTorch's upsample_bilinear2d with size= given:
+// scale = (float)in / out, src = max((dst + 0.5) * scale - 0.5, 0), i0 = (int)src, i1 = i0 + (i0 < in - 1), l1 = src - i0 (the weight of
+// i1; i0's is 1 - l1).  Shared by the split16 resize, the fused upsample + argmax and the segmentation loss, so that they interpolate alike.
+__device__ __forceinline__ void bilinear_src(int dst, float scale, int in_size, int* i0, int* i1, float* l1) {
+  float s = fmaxf(((float)dst + 0.5f) * scale - 0.5f, 0.0f);
+  int a = (int)s;
+  if (a > in_size - 1) a = in_size - 1;
+  *i0 = a;
+  *i1 = a + ((a < in_size - 1) ? 1 : 0);
+  *l1 = s - (float)a;
+}
+
 // The training losses' fp32 sigmoid and BCEWithLogits (pos_weight 1), shared by yolox_loss.cu and yolov5_loss.cu:
 // BCEWithLogits(x, t) = (1 - t) x + m + log(exp(-m) + exp(-x - m)), m = max(-x, 0)
 __device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }

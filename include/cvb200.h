@@ -623,6 +623,31 @@ int32_t cvb_seg_confusion_nc_max(void);
 int cvb_seg_confusion_update(const void* gt, int32_t gt_dtype, const void* pred, int32_t pred_dtype, int64_t n, int32_t nc, uint64_t* matrix,
                              int32_t* err, void* stream);
 
+/* Segmentation cross-entropy with the bilinear upsample to label size fused in (src/losses/seg/cross_entropy_loss.py CrossEntropyLoss2d
+ * after F.interpolate(preds, size=targets.shape[-2:], mode='bilinear', align_corners=False) in EncoderDecoder.loss_forward;
+ * csrc/seg_loss.cu).  The upsampled logits z [B, C, H, W] are never written: both passes recompute them from the taps.
+ * preds: fp32 NCHW [B, C, h, w], contiguous, read in place.  labels [B, H, W] of dtype CVB_SEG_U8, _I32 or _I64, element strides (sb, sh, sw)
+ *   >= 0, aligned to the element size, read as they are.  z = torch's upsample_bilinear2d of preds (scale = (float)in / out,
+ *   src = max((dst + 0.5) scale - 0.5, 0)); equal sizes are the identity.  Any h, w -> H, W, up or down.
+ * A pixel whose label equals ignore_index is ignored; a valid one (0 <= label < C) adds lse(z) - z_label.  A label outside [0, C) that is
+ *   not ignore_index (torch raises / asserts) is counted in n_bad and makes the loss and every gradient element NaN.
+ * cvb_train_seg_ce_fwd: loss fp32 [1] = loss_weight * (sum / n_valid) (NaN when n_valid = 0, as torch's 'mean'); record int64 [2] =
+ *   (n_valid, n_bad) and lse fp32 [B, H, W] (the log-sum-exp of valid pixels), both kept for the backward.  workspace:
+ *   cvb_train_seg_ce_workspace_bytes(B, H, W) bytes, 256-byte aligned, owned by the caller.  No host sync; bitwise reproducible.
+ * cvb_train_seg_ce_bwd: grad_preds fp32 [B, C, h, w] (every element written) = grad_out[0] d(loss)/d(preds), a gather with no atomics:
+ *   bitwise reproducible.  Ignored pixels contribute 0, so every pixel ignored gives an all-zero gradient.  grad_out: fp32 [1] on the device.
+ * Limits, checked before any launch: 1 <= C <= cvb_train_seg_ce_nc_max() (1024), 1 <= B, h, w, H, W <= 65535, B H W < 2^31, known dtype
+ *   code, non-null aligned pointers, a large enough workspace.
+ */
+int32_t cvb_train_seg_ce_nc_max(void);
+size_t cvb_train_seg_ce_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int cvb_train_seg_ce_fwd(const float* preds, int32_t B, int32_t C, int32_t h, int32_t w, const void* labels, int32_t label_dtype, int32_t H, int32_t W,
+                         int64_t sb, int64_t sh, int64_t sw, int64_t ignore_index, float loss_weight, float* lse, int64_t* record, float* loss,
+                         void* workspace, size_t ws_bytes, void* stream);
+int cvb_train_seg_ce_bwd(const float* preds, int32_t B, int32_t C, int32_t h, int32_t w, const void* labels, int32_t label_dtype, int32_t H, int32_t W,
+                         int64_t sb, int64_t sh, int64_t sw, int64_t ignore_index, float loss_weight, const float* lse, const int64_t* record,
+                         const float* grad_out, float* grad_preds, void* stream);
+
 /* Library info / errors */
 const char* cvb_last_error_string(void);
 int cvb_version(void);

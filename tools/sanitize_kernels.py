@@ -171,3 +171,17 @@ xt = torch.randn(1, 128, 8, 8, device='cuda', requires_grad=True)
 mt(xt).sum().backward()
 torch.cuda.synchronize()
 print('training kernels ok')
+
+# segmentation loss: forward + backward at x4, a non-integer ratio with a strided int32 label view, a downsample, a footprint larger than
+# one shared-memory block (1 x 1 -> 200 x 300), an all-ignored batch and an out-of-range label
+from cvpytorch_b200 import seg_train as ST  # noqa: E402
+for (Bs, Cs, hs, ws_, Hs, Ws, dt) in ((2, 19, 8, 12, 32, 48, torch.uint8), (1, 5, 13, 29, 40, 61, torch.int32), (1, 3, 20, 28, 9, 11, torch.int64),
+                                      (1, 2, 1, 1, 200, 300, torch.uint8)):
+    ps = torch.randn(Bs, Cs, hs, ws_, device='cuda', requires_grad=True)
+    ts = torch.randint(0, Cs, (Bs, Hs, Ws + 3), device='cuda').to(dt)[:, :, 1:Ws + 1]
+    ST.CrossEntropyLoss2d()(ps, ts).backward()
+    ST.CrossEntropyLoss2d()(ps, torch.full_like(ts, 255)).backward()
+    ts[0, 0, 0] = Cs
+    ST.CrossEntropyLoss2d()(ps, ts).backward()
+torch.cuda.synchronize()
+print('segmentation loss ok')
