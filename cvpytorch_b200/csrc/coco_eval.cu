@@ -337,31 +337,26 @@ static size_t cub_tmp_bytes(int n) {
   return std::max<size_t>(std::max(a, b), 1);
 }
 
-static CocoWs coco_ws(char* base, int n_det, int n_gt, int n_cats) {
+static CocoWs coco_ws(void* base, int n_det, int n_gt, int n_cats) {
+  WsCarver c(base);
   CocoWs w{};
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    char* ptr = base ? base + off : nullptr;
-    off += (bytes + 255) & ~(size_t)255;
-    return ptr;
-  };
   const size_t n = (size_t)n_det;
-  w.keys_in = (uint64_t*)take(n * 8);
-  w.keys = (uint64_t*)take(n * 8);
-  w.key2_in = (uint64_t*)take(n * 8);
-  w.key2 = (uint64_t*)take(n * 8);
-  w.vals_in = (int32_t*)take(n * 4);
-  w.order = (int32_t*)take(n * 4);
-  w.order2 = (int32_t*)take(n * 4);
-  w.seg_start = (int32_t*)take(n * 4);
-  w.num_segs = (int32_t*)take(4);
-  w.det_rank = (int32_t*)take(n * 4);
-  w.npig = (int32_t*)take((size_t)n_cats * kCocoA * 4);
-  w.flags = (uint8_t*)take(n);
-  w.gt_matched = (uint8_t*)take((size_t)n_gt * kScans);
+  w.keys_in = (uint64_t*)c.take(n * 8);
+  w.keys = (uint64_t*)c.take(n * 8);
+  w.key2_in = (uint64_t*)c.take(n * 8);
+  w.key2 = (uint64_t*)c.take(n * 8);
+  w.vals_in = (int32_t*)c.take(n * 4);
+  w.order = (int32_t*)c.take(n * 4);
+  w.order2 = (int32_t*)c.take(n * 4);
+  w.seg_start = (int32_t*)c.take(n * 4);
+  w.num_segs = (int32_t*)c.take(4);
+  w.det_rank = (int32_t*)c.take(n * 4);
+  w.npig = (int32_t*)c.take((size_t)n_cats * kCocoA * 4);
+  w.flags = (uint8_t*)c.take(n);
+  w.gt_matched = (uint8_t*)c.take((size_t)n_gt * kScans);
   w.cub_bytes = cub_tmp_bytes(n_det);
-  w.cub_tmp = take(w.cub_bytes);
-  w.total = w.cub_bytes ? off : 0;
+  w.cub_tmp = c.take(w.cub_bytes);
+  w.total = w.cub_bytes ? c.bytes() : 0;
   return w;
 }
 
@@ -392,8 +387,8 @@ extern "C" int cvb_coco_eval_bbox(const CvbCocoEvalParams* params, const uint32_
   CVB_REQUIRE(img_evaluated && precision && recall && stats && workspace, "coco_eval_bbox: null pointer");
   CVB_REQUIRE(p.n_gt == 0 || (gt_key && gt_box && gt_area && gt_crowd), "coco_eval_bbox: null ground-truth pointer");
   CVB_REQUIRE(p.n_det == 0 || (det_img && det_cat && det_score && det_box && det_masks), "coco_eval_bbox: null detection pointer");
-  CVB_REQUIRE(((uintptr_t)workspace & 255) == 0, "coco_eval_bbox: workspace must be 256-byte aligned");
-  const CocoWs w = coco_ws(static_cast<char*>(workspace), p.n_det, p.n_gt, p.n_cats);
+  CVB_REQUIRE(is_aligned(workspace, 256), "coco_eval_bbox: workspace must be 256-byte aligned");
+  const CocoWs w = coco_ws(workspace, p.n_det, p.n_gt, p.n_cats);
   CVB_REQUIRE(w.total > 0, "coco_eval_bbox: CUB could not size its temporary storage for %d detections", p.n_det);
   CVB_REQUIRE(ws_bytes >= w.total, "coco_eval_bbox: workspace of %zu bytes < %zu", ws_bytes, w.total);
   cudaStream_t st = as_stream(stream);

@@ -33,20 +33,13 @@ __device__ __forceinline__ float ema_step(float e, float m, float d, float c) { 
 __global__ void __launch_bounds__(kEmaThreads) ema_update_kernel(const EmaRecord* __restrict__ table, int n, float d, float c) {
   const int64_t total = table[n - 1].first_chunk + (table[n - 1].numel + kEmaChunk - 1) / kEmaChunk;
   for (int64_t w = blockIdx.x; w < total; w += gridDim.x) {
-    // the last record with first_chunk <= w owns item w (an empty entry shares its first_chunk with the next entry, which wins)
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (table[mid].first_chunk <= w) lo = mid;
-      else hi = mid - 1;
-    }
-    const EmaRecord r = table[lo];
+    const EmaRecord r = owning_record(table, n, w);
     const int64_t begin = (w - r.first_chunk) * kEmaChunk;
     const int len = (int)min(kEmaChunk, r.numel - begin);
     float* e = r.ema + begin;
     const float* s = r.src + begin;
     int scalar_from = 0;
-    if (((reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(s)) & 15) == 0) {
+    if (is_aligned(e, 16) & is_aligned(s, 16)) {  // (& rather than &&: one branch-free test)
       float4* e4 = reinterpret_cast<float4*>(e);
       const float4* s4 = reinterpret_cast<const float4*>(s);
       const int nvec = len >> 2;
@@ -79,7 +72,7 @@ using namespace cvb;
 extern "C" int cvb_ema_table_upload(const CvbEmaEntry* entries, int32_t n, void* table, void* stream) {
   CVB_REQUIRE(entries && table, "ema_table_upload: null pointer");
   CVB_REQUIRE(n > 0, "ema_table_upload: n_entries must be > 0 (n=%d)", n);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(table) & 15) == 0, "ema_table_upload: table must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(table, 16), "ema_table_upload: table must be 16-byte aligned");
   std::vector<EmaRecord> recs(n);
   int64_t chunks = 0;
   for (int i = 0; i < n; ++i) {
@@ -97,7 +90,7 @@ extern "C" int cvb_ema_table_upload(const CvbEmaEntry* entries, int32_t n, void*
 extern "C" int cvb_ema_update(const void* table, int32_t n, float decay, float one_minus_decay, void* stream) {
   CVB_REQUIRE(table, "ema_update: null pointer");
   CVB_REQUIRE(n > 0, "ema_update: n_entries must be > 0 (n=%d)", n);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(table) & 15) == 0, "ema_update: table must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(table, 16), "ema_update: table must be 16-byte aligned");
   ema_update_kernel<<<kEmaGrid, kEmaThreads, 0, as_stream(stream)>>>(static_cast<const EmaRecord*>(table), n, decay, one_minus_decay);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();

@@ -164,29 +164,6 @@ __device__ __forceinline__ int target_class(const FcosLevels& L, const int32_t* 
   return (lab >= 1 && lab <= L.nc) ? lab - 1 : -1;
 }
 
-// Block-wide fp64 sum of N values per thread in a fixed tree; thread 0 gets the totals.
-template <int N>
-__device__ __forceinline__ void block_sum(double (&v)[N], double (*red)[N]) {
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < N; ++k) red[threadIdx.x >> 5][k] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      double t = 0.0;
-      for (int w = 0; w < kFcosThreads / 32; ++w) t += red[w][k];
-      v[k] = t;
-    }
-  }
-}
-
 // --------------------------------------------------------------------------------------------------------------------------- forward
 __global__ void __launch_bounds__(kFcosThreads) fcos_assign_kernel(FcosLevels L, const float* __restrict__ boxes, int32_t* __restrict__ matched_gt,
                                                                    float* __restrict__ tgt, double* __restrict__ partial) {
@@ -220,7 +197,7 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_assign_kernel(FcosLevels L,
       for (int k = 0; k < 5; ++k) tgt[((size_t)b * L.A + a) * 5 + k] = t[k];
     }
   }
-  block_sum<3>(v, red);
+  block_sum<kFcosThreads>(v, red);
   if (threadIdx.x == 0) {
     double* d = partial + ((size_t)b * L.nblk + blockIdx.x) * 3;
     d[0] = v[0];
@@ -247,7 +224,7 @@ __global__ void __launch_bounds__(kFcosThreads) fcos_focal_kernel(FcosLevels L, 
     for (int j = 0; j < kFcosClsChunk; ++j)
       if (c0 + j < c1) v[0] += focal(e[j], c0 + j == k);
   }
-  block_sum<1>(v, red);
+  block_sum<kFcosThreads>(v, red);
   if (threadIdx.x == 0) partial[((size_t)b * L.nchunk + blockIdx.y) * L.nblk + blockIdx.x] = v[0];
 }
 
@@ -272,10 +249,7 @@ __global__ void __launch_bounds__(kFcosFinalThreads) fcos_final_kernel(FcosLevel
         v[3] += d[2];
       }
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-      }
+      for (int k = 0; k < 4; ++k) v[k] = warp_sum(v[k]);
       if (lane == 0) {
         const double np = fmax(v[3], 1.0);
         img[wid][0] = v[0] / np;
@@ -357,18 +331,14 @@ inline int point_blocks(int A) { return ceil_div(A, kFcosThreads); }
 inline int class_chunks(int nc) { return ceil_div(nc, kFcosClsChunk); }
 
 FcosWs fcos_ws(void* base, int B, int A, int nc) {
+  WsCarver c(base);
   FcosWs w{};
-  size_t o = 0;
-  char* p = static_cast<char*>(base);
-  auto take = [&](size_t bytes) { char* r = p ? p + o : nullptr; o = nms_align_up(o + bytes, 256); return r; };
   const size_t nb = (size_t)B * point_blocks(A);
-  w.pt_partial = reinterpret_cast<double*>(take(nb * 3 * sizeof(double)));
-  w.cls_partial = reinterpret_cast<double*>(take(nb * class_chunks(nc) * sizeof(double)));
-  w.bytes = o;
+  w.pt_partial = static_cast<double*>(c.take(nb * 3 * sizeof(double)));
+  w.cls_partial = static_cast<double*>(c.take(nb * class_chunks(nc) * sizeof(double)));
+  w.bytes = c.bytes();
   return w;
 }
-
-inline bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 // Validates the description shared by the forward and the backward and fills L (gradients: may be NULL in the forward).
 int make_levels(const char* what, const float* const* cls, const float* const* cnt, const float* const* reg, const int32_t* shapes, const float* strides,
@@ -379,7 +349,7 @@ int make_levels(const char* what, const float* const* cls, const float* const* c
   CVB_REQUIRE(B >= 1, "%s: batch must be >= 1 (got %d)", what, B);
   CVB_REQUIRE(m >= 0 && m <= kFcosMaxGt, "%s: m must be in [0, %d] GT rows per image (got %d)", what, kFcosMaxGt, m);
   if (m > 0)
-    CVB_REQUIRE(boxes && labels && aligned(boxes, 16) && aligned(labels, 4), "%s: boxes (16-byte aligned) and labels (4-byte aligned) are required", what);
+    CVB_REQUIRE(boxes && labels && is_aligned(boxes, 16) && is_aligned(labels, 4), "%s: boxes (16-byte aligned) and labels (4-byte aligned) are required", what);
   const int nc = shapes[1];
   CVB_REQUIRE(nc >= 1 && nc <= 65536, "%s: num_classes must be in [1, 65536] (got %d)", what, nc);
   *L = FcosLevels{};
@@ -397,10 +367,10 @@ int make_levels(const char* what, const float* const* cls, const float* const* c
     CVB_REQUIRE(s >= 1.0f && s <= 65536.0f && s == floorf(s), "%s: level %d stride must be a positive integer (got %g)", what, l, (double)s);
     const float lo = limit_range[2 * l], hi = limit_range[2 * l + 1];
     CVB_REQUIRE(lo < hi, "%s: level %d limit range must have lo < hi (got [%g, %g])", what, l, (double)lo, (double)hi);
-    CVB_REQUIRE(cls[l] && cnt[l] && reg[l] && aligned(cls[l], 4) && aligned(cnt[l], 4) && aligned(reg[l], 4),
+    CVB_REQUIRE(cls[l] && cnt[l] && reg[l] && is_aligned(cls[l], 4) && is_aligned(cnt[l], 4) && is_aligned(reg[l], 4),
                 "%s: level %d output missing or not 4-byte aligned", what, l);
     if (gcls)
-      CVB_REQUIRE(gcls[l] && gcnt[l] && greg[l] && aligned(gcls[l], 4) && aligned(gcnt[l], 4) && aligned(greg[l], 4),
+      CVB_REQUIRE(gcls[l] && gcnt[l] && greg[l] && is_aligned(gcls[l], 4) && is_aligned(gcnt[l], 4) && is_aligned(greg[l], 4),
                   "%s: level %d gradient missing or not 4-byte aligned", what, l);
     CVB_REQUIRE((long long)c[2] * c[3] * s < (1LL << 24) && (long long)c[2] * s < (1LL << 24) && (long long)c[3] * s < (1LL << 24),
                 "%s: level %d map too large for exact fp32 point coordinates", what, l);
@@ -453,11 +423,11 @@ extern "C" int cvb_train_fcos_loss_fwd(const float* const* cls, const float* con
   FcosLevels L;
   const int rc = make_levels("train_fcos_loss_fwd", cls, cnt, reg, shapes, strides, limit_range, nlev, boxes, labels, B, m, nullptr, nullptr, nullptr, &L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(matched_gt && num_pos && out && aligned(matched_gt, 4) && aligned(num_pos, 4) && aligned(out, 4),
+  CVB_REQUIRE(matched_gt && num_pos && out && is_aligned(matched_gt, 4) && is_aligned(num_pos, 4) && is_aligned(out, 4),
               "train_fcos_loss_fwd: matched_gt, num_pos and out are required, 4-byte aligned");
-  CVB_REQUIRE(aligned(targets, 4), "train_fcos_loss_fwd: targets must be 4-byte aligned");
+  CVB_REQUIRE(is_aligned(targets, 4), "train_fcos_loss_fwd: targets must be 4-byte aligned");
   const FcosWs w = fcos_ws(workspace, B, L.A, L.nc);
-  CVB_REQUIRE(workspace && aligned(workspace, 256), "train_fcos_loss_fwd: workspace required, 256-byte aligned");
+  CVB_REQUIRE(workspace && is_aligned(workspace, 256), "train_fcos_loss_fwd: workspace required, 256-byte aligned");
   CVB_REQUIRE(ws_bytes >= w.bytes, "train_fcos_loss_fwd: workspace of %zu bytes too small (%zu needed)", ws_bytes, w.bytes);
   cudaStream_t st = as_stream(stream);
   fcos_assign_kernel<<<dim3(L.nblk, B), kFcosThreads, (size_t)m * sizeof(float4), st>>>(L, boxes, matched_gt, targets, w.pt_partial);
@@ -476,7 +446,7 @@ extern "C" int cvb_train_fcos_loss_bwd(const float* const* cls, const float* con
   FcosLevels L;
   const int rc = make_levels("train_fcos_loss_bwd", cls, cnt, reg, shapes, strides, limit_range, nlev, boxes, labels, B, m, gcls, gcnt, greg, &L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(matched_gt && num_pos && grad_out && aligned(matched_gt, 4) && aligned(num_pos, 4) && aligned(grad_out, 4),
+  CVB_REQUIRE(matched_gt && num_pos && grad_out && is_aligned(matched_gt, 4) && is_aligned(num_pos, 4) && is_aligned(grad_out, 4),
               "train_fcos_loss_bwd: matched_gt, num_pos and grad_out are required, 4-byte aligned");
   fcos_bwd_kernel<<<dim3(L.nblk, L.nchunk, B), kFcosThreads, 0, as_stream(stream)>>>(L, boxes, labels, matched_gt, num_pos, grad_out);
   CVB_CHECK_CUDA(cudaGetLastError());

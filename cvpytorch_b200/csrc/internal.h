@@ -41,6 +41,31 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// p is a multiple of a (a power of two)
+__host__ __device__ inline bool is_aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// Lays the pieces of a workspace out one after another, each on a 256-byte boundary.  Constructed on nullptr it only sizes: take()
+// returns nullptr and bytes() is what the workspace needs.
+class WsCarver {
+ public:
+  explicit WsCarver(void* base) : base_(static_cast<char*>(base)) {}
+  void* take(size_t bytes) {
+    char* r = base_ ? base_ + off_ : nullptr;
+    off_ = align_up(off_ + bytes, 256);
+    return r;
+  }
+  size_t bytes() const { return off_; }
+
+ private:
+  char* base_;
+  size_t off_ = 0;
+};
+
+// bytes per element of a CVB_SEG_* label dtype code
+inline int seg_label_bytes(int32_t code) { return code == CVB_SEG_U8 ? 1 : code == CVB_SEG_I32 ? 4 : 8; }
+
 // Division by a run-time constant d >= 1 with one multiply-high: magic = ceil(2^32 / d) is exact for 0 <= x < x_end while
 // x_end * d < 2^32; otherwise magic = 0 selects real division, and magic = 1 means d == 1.
 inline uint32_t fast_div_magic(int d, unsigned long long x_end) {
@@ -64,8 +89,7 @@ constexpr int kNmsCapA = 4096;   // phase-A candidate capacity = one shared-memo
 // NMS workspace layout (bytes): [hist B*kNmsBins u32][6 slots of B u32][keysB B*kNmsCap u64][keysA B*kNmsCapA u64][rowmax B*A f32]
 // rowmax[b][anchor] = best score (obj*cls, > conf) of the anchor row, 0 when it has no candidate: written by the pass that
 // builds the histogram (decode kernel or the NMS count pass) and lets the emit passes skip rows below the threshold bin.
-inline size_t nms_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-inline size_t nms_ws_head_bytes(int B) { return nms_align_up((size_t)B * kNmsBins * 4, 256) + 6 * nms_align_up((size_t)B * 4, 256); }
+inline size_t nms_ws_head_bytes(int B) { return align_up((size_t)B * kNmsBins * 4, 256) + 6 * align_up((size_t)B * 4, 256); }
 inline size_t nms_ws_rowmax_offset(int B) { return nms_ws_head_bytes(B) + (size_t)B * (kNmsCap + kNmsCapA) * 8; }
 
 #ifdef __CUDACC__
@@ -120,6 +144,50 @@ __device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(
 __device__ __forceinline__ float bce_logits(float x, float t) {
   const float m = fmaxf(-x, 0.0f);
   return (1.0f - t) * x + m + logf(expf(-m) + expf(-x - m));
+}
+
+// The one fp64 summation order of the losses' per-CTA and final reductions (DESIGN.md 2), so that every loss adds alike: a warp adds its
+// lanes by an xor butterfly (offsets 16, 8, 4, 2, 1; every lane ends with the warp total), then the warp totals are added in ascending warp
+// order starting from 0.0.
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Block-wide sum of N values per thread of a kThreads-thread CTA, in the order above; thread 0 gets the totals in v.  red is shared
+// [kThreads / 32][N]; the leading barrier lets calls follow one another on the same red.  (Only thread 0 adds the warp totals: every
+// thread doing so costs kThreads * N fp64 adds per CTA, which slowed the 4096-CTA segmentation forward by about 1 us.)
+template <int kThreads, int N>
+__device__ __forceinline__ void block_sum(double (&v)[N], double (*red)[N]) {
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < N; ++k) v[k] = warp_sum(v[k]);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) red[threadIdx.x >> 5][k] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    double t = 0.0;
+    for (int w = 0; w < kThreads / 32; ++w) t += red[w][k];
+    v[k] = t;
+  }
+}
+
+// The record of a work table (ema.cu, sgd.cu) that owns work item w: the last of table[0, n) with first_chunk <= w, first_chunk being
+// non-decreasing from 0 (an entry with no items shares its first_chunk with the next one, which wins).
+template <typename R>
+__device__ __forceinline__ R owning_record(const R* __restrict__ table, int n, int64_t w) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (table[mid].first_chunk <= w) lo = mid;
+    else hi = mid - 1;
+  }
+  return table[lo];
 }
 #endif
 

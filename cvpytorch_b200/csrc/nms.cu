@@ -49,9 +49,9 @@ struct NmsWs {
 static NmsWs carve_ws(void* ws, int B, int phase) {
   NmsWs w;
   uint8_t* p = static_cast<uint8_t*>(ws);
-  const size_t slot = nms_align_up((size_t)B * 4, 256);
+  const size_t slot = align_up((size_t)B * 4, 256);
   w.hist = reinterpret_cast<uint32_t*>(p);
-  p += nms_align_up((size_t)B * kBins * 4, 256);
+  p += align_up((size_t)B * kBins * 4, 256);
   uint32_t* cntB = reinterpret_cast<uint32_t*>(p);
   uint32_t* tbinB = reinterpret_cast<uint32_t*>(p + slot);
   uint32_t* cntA = reinterpret_cast<uint32_t*>(p + 2 * slot);
@@ -643,7 +643,7 @@ using namespace cvb;
 extern "C" size_t cvb_nms_workspace_bytes(int32_t B, int32_t A, int32_t nc) {
   (void)nc;
   if (B <= 0 || A <= 0) return 0;
-  return nms_ws_rowmax_offset(B) + nms_align_up((size_t)B * A * sizeof(float), 256);
+  return nms_ws_rowmax_offset(B) + align_up((size_t)B * A * sizeof(float), 256);
 }
 
 extern "C" int cvb_nms_workspace_reset(void* workspace, size_t workspace_bytes, int32_t B, void* stream) {

@@ -101,19 +101,14 @@ __global__ void __launch_bounds__(kSegThreads, 4) seg_confusion_kernel(const G* 
   }
 }
 
-static int seg_size(int32_t code) {
-  return code == CVB_SEG_U8 ? 1 : code == CVB_SEG_I32 ? 4 : 8;
-}
-
 template <typename G, typename P>
 static int seg_launch(const void* gt, const void* pred, long long n, int nc, unsigned long long* matrix, int* err, cudaStream_t stream) {
   constexpr int kW = sizeof(G) > sizeof(P) ? (int)sizeof(G) : (int)sizeof(P);
   constexpr int E = 16 / kW;
   // first pixel where gt and pred both sit on their vector width (the step advances both by a whole vector); none: all scalar
-  const uintptr_t ag = reinterpret_cast<uintptr_t>(gt), ap = reinterpret_cast<uintptr_t>(pred);
   long long head = n;
   for (int h = 0; h < E; ++h) {
-    if ((ag + h * sizeof(G)) % (E * sizeof(G)) == 0 && (ap + h * sizeof(P)) % (E * sizeof(P)) == 0) {
+    if (is_aligned(static_cast<const G*>(gt) + h, E * sizeof(G)) && is_aligned(static_cast<const P*>(pred) + h, E * sizeof(P))) {
       head = h < n ? h : n;
       break;
     }
@@ -167,10 +162,9 @@ extern "C" int cvb_seg_confusion_update(const void* gt, int32_t gt_dtype, const 
   CVB_REQUIRE(known(gt_dtype) && known(pred_dtype), "seg_confusion_update: unknown dtype code (gt %d, pred %d)", gt_dtype, pred_dtype);
   if (n == 0) return CVB_OK;
   CVB_REQUIRE(gt && pred && matrix && err, "seg_confusion_update: null pointer");
-  const int gs = seg_size(gt_dtype), ps = seg_size(pred_dtype);
-  CVB_REQUIRE(reinterpret_cast<uintptr_t>(gt) % gs == 0 && reinterpret_cast<uintptr_t>(pred) % ps == 0,
+  CVB_REQUIRE(is_aligned(gt, seg_label_bytes(gt_dtype)) && is_aligned(pred, seg_label_bytes(pred_dtype)),
               "seg_confusion_update: gt / pred not aligned to their element size");
-  CVB_REQUIRE(reinterpret_cast<uintptr_t>(matrix) % 8 == 0 && reinterpret_cast<uintptr_t>(err) % 4 == 0,
+  CVB_REQUIRE(is_aligned(matrix, 8) && is_aligned(err, 4),
               "seg_confusion_update: matrix must be 8-byte and err 4-byte aligned");
   unsigned long long* m = reinterpret_cast<unsigned long long*>(matrix);
   int* e = reinterpret_cast<int*>(err);

@@ -111,20 +111,10 @@ __global__ void __launch_bounds__(kCeThreads) seg_ce_fwd_kernel(const float* __r
     }
     lse_out[p] = lse;
   }
+  block_sum<kCeThreads>(v, red);
+  if (threadIdx.x == 0) {
 #pragma unroll
-  for (int k = 0; k < 3; ++k) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) red[threadIdx.x >> 5][k] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    double a = 0.0;
-    for (int w = 0; w < kCeThreads / 32; ++w) a += red[w][threadIdx.x];
-    partial[(size_t)blockIdx.x * 3 + threadIdx.x] = a;
+    for (int k = 0; k < 3; ++k) partial[(size_t)blockIdx.x * 3 + k] = v[k];
   }
 }
 
@@ -137,29 +127,14 @@ __global__ void __launch_bounds__(kCeFinalThreads) seg_ce_final_kernel(const dou
     v[1] += partial[(size_t)i * 3 + 1];
     v[2] += partial[(size_t)i * 3 + 2];
   }
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) red[threadIdx.x >> 5][k] = v[k];
-  }
-  __syncthreads();
+  block_sum<kCeFinalThreads>(v, red);
   if (threadIdx.x == 0) {
-    double a[3] = {0.0, 0.0, 0.0};
-    for (int w = 0; w < kCeFinalThreads / 32; ++w) {
-      a[0] += red[w][0];
-      a[1] += red[w][1];
-      a[2] += red[w][2];
-    }
-    const long long n_valid = (long long)a[1], n_bad = (long long)a[2];
+    const long long n_valid = (long long)v[1], n_bad = (long long)v[2];
     record[0] = n_valid;
     record[1] = n_bad;
     // the mean over valid pixels (0 / 0 = NaN when every pixel is ignored, as torch's 'mean'), then the weight, as the reference does;
     // a label outside [0, C) makes the loss NaN (torch raises there)
-    loss[0] = n_bad ? __int_as_float(0x7fffffff) : loss_weight * (float)(a[0] / a[1]);
+    loss[0] = n_bad ? __int_as_float(0x7fffffff) : loss_weight * (float)(v[0] / v[1]);
   }
 }
 
@@ -305,7 +280,7 @@ __global__ void __launch_bounds__(kCeThreads) seg_ce_bwd_kernel(const float* __r
 // --------------------------------------------------------------------------------------------------------------------------- host
 inline int fwd_blocks(long long n) { return (int)((n + (long long)kCeThreads * kCePix - 1) / ((long long)kCeThreads * kCePix)); }
 
-inline size_t ws_bytes_for(long long n) { return nms_align_up((size_t)fwd_blocks(n) * 3 * sizeof(double), 256); }
+inline size_t ws_bytes_for(long long n) { return align_up((size_t)fwd_blocks(n) * 3 * sizeof(double), 256); }
 
 inline int pow2_at_most(double v, int hi) {
   int p = 1;
@@ -333,10 +308,6 @@ size_t ce_smem_bytes(const CeTile& K) {
   return (2 * bpx + (size_t)K.FYB * K.TJ + K.FYB + K.FXB) * 4 + (2 * (size_t)K.FYB + 2 * K.FXB + 2 * K.TI + 2 * K.TJ) * 4 + bpx * 2;
 }
 
-inline bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
-int label_size(int32_t code) { return code == CVB_SEG_U8 ? 1 : code == CVB_SEG_I32 ? 4 : 8; }
-
 // Validates what the forward and the backward share and fills S.
 int make_shape(const char* what, const float* preds, int32_t B, int32_t C, int32_t h, int32_t w, const void* labels, int32_t dtype, int32_t H,
                int32_t W, int64_t sb, int64_t sh, int64_t sw, int64_t ignore_index, CeShape* S) {
@@ -350,8 +321,8 @@ int make_shape(const char* what, const float* preds, int32_t B, int32_t C, int32
   CVB_REQUIRE(sb >= 0 && sh >= 0 && sw >= 0, "%s: label strides must be >= 0 (got %lld, %lld, %lld)", what, (long long)sb, (long long)sh,
               (long long)sw);
   CVB_REQUIRE((B - 1) * sb + (H - 1) * sh + (W - 1) * sw < (1LL << 40), "%s: label strides too large", what);
-  CVB_REQUIRE(preds && aligned(preds, 4), "%s: preds missing or not 4-byte aligned", what);
-  CVB_REQUIRE(labels && aligned(labels, label_size(dtype)), "%s: labels missing or not aligned to their element size", what);
+  CVB_REQUIRE(preds && is_aligned(preds, 4), "%s: preds missing or not 4-byte aligned", what);
+  CVB_REQUIRE(labels && is_aligned(labels, seg_label_bytes(dtype)), "%s: labels missing or not aligned to their element size", what);
   *S = CeShape{B, C, h, w, H, W, sb, sh, sw, ignore_index, (float)h / (float)H, (float)w / (float)W};
   return CVB_OK;
 }
@@ -374,10 +345,10 @@ extern "C" int cvb_train_seg_ce_fwd(const float* preds, int32_t B, int32_t C, in
   CeShape S;
   const int rc = make_shape("train_seg_ce_fwd", preds, B, C, h, w, labels, label_dtype, H, W, sb, sh, sw, ignore_index, &S);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(lse && record && loss && aligned(lse, 4) && aligned(record, 8) && aligned(loss, 4),
+  CVB_REQUIRE(lse && record && loss && is_aligned(lse, 4) && is_aligned(record, 8) && is_aligned(loss, 4),
               "train_seg_ce_fwd: lse, loss (4-byte aligned) and record (8-byte aligned) are required");
   const long long n = (long long)B * H * W;
-  CVB_REQUIRE(workspace && aligned(workspace, 256), "train_seg_ce_fwd: workspace required, 256-byte aligned");
+  CVB_REQUIRE(workspace && is_aligned(workspace, 256), "train_seg_ce_fwd: workspace required, 256-byte aligned");
   CVB_REQUIRE(ws_bytes >= ws_bytes_for(n), "train_seg_ce_fwd: workspace of %zu bytes too small (%zu needed)", ws_bytes, ws_bytes_for(n));
   double* partial = static_cast<double*>(workspace);
   const int nblk = fwd_blocks(n);
@@ -413,7 +384,7 @@ extern "C" int cvb_train_seg_ce_bwd(const float* preds, int32_t B, int32_t C, in
   CeShape S;
   const int rc = make_shape("train_seg_ce_bwd", preds, B, C, h, w, labels, label_dtype, H, W, sb, sh, sw, ignore_index, &S);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(lse && record && grad_out && grad_preds && aligned(lse, 4) && aligned(record, 8) && aligned(grad_out, 4) && aligned(grad_preds, 4),
+  CVB_REQUIRE(lse && record && grad_out && grad_preds && is_aligned(lse, 4) && is_aligned(record, 8) && is_aligned(grad_out, 4) && is_aligned(grad_preds, 4),
               "train_seg_ce_bwd: lse, grad_out, grad_preds (4-byte aligned) and record (8-byte aligned) are required");
   const cudaStream_t st = as_stream(stream);
   switch (label_dtype) {

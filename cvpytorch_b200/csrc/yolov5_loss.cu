@@ -10,8 +10,8 @@
 //   4. v5_seg_kernel    one thread per sorted position; the first of each cell's run takes the last candidate in candidate order (the
 //                       reference's index_put_ on the CPU: last write wins) for tobj = (1 - gr) + gr * clamp(CIoU, 0), and the objectness
 //                       correction BCE(x, tobj) - BCE(x, 0) of that cell.
-//   5. v5_obj_kernel    every objectness logit: BCE(x, 0), summed per CTA in a fixed tree.
-//   6. v5_final_kernel  one CTA: the per-level means from fp64 sums in fixed trees -> loss, lbox, lobj, lcls.
+//   5. v5_obj_kernel    every objectness logit: BCE(x, 0), summed per CTA (block_sum).
+//   6. v5_final_kernel  one CTA: the per-level means from fp64 sums (block_sum) -> loss, lbox, lobj, lcls.
 // Backward (cvb_train_yolov5_loss_bwd): v5_fill_kernel writes every gradient element (objectness d/dx of BCE(x, 0), zeros elsewhere);
 // v5_cell_grad_kernel then rewrites the channels of each candidate cell, summing its candidates' box and class gradients in candidate
 // order.  No float atomics: the loss and the gradient are bitwise reproducible.
@@ -268,50 +268,39 @@ __global__ void __launch_bounds__(kV5Threads) v5_seg_kernel(V5Levels L, const in
   corr[off + p] = c;
 }
 
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  for (int w = 0; w < kV5Threads / 32; ++w) t += red[w];
-  return t;
-}
-
 __global__ void __launch_bounds__(kV5Threads) v5_obj_kernel(V5Levels L, double* __restrict__ partial) {
-  __shared__ double red[kV5Threads / 32];
+  __shared__ double red[kV5Threads / 32][1];
   const int l = blockIdx.y;
   const long long hw = (long long)L.ny[l] * L.nx[l], n = (long long)L.B * L.na * hw;
-  double v = 0.0;
+  double v[1] = {0.0};
   for (long long i = blockIdx.x * (long long)kV5Threads + threadIdx.x; i < n; i += (long long)kV5ObjBlocks * kV5Threads) {
     const long long ba = i / hw;
-    v += (double)bce_logits(L.p[l][(ba * (5 + L.nc) + 4) * hw + i % hw], 0.0f);
+    v[0] += (double)bce_logits(L.p[l][(ba * (5 + L.nc) + 4) * hw + i % hw], 0.0f);
   }
-  const double t = block_sum(v, red);
-  if (threadIdx.x == 0) partial[l * kV5ObjBlocks + blockIdx.x] = t;
+  block_sum<kV5Threads>(v, red);
+  if (threadIdx.x == 0) partial[l * kV5ObjBlocks + blockIdx.x] = v[0];
 }
 
 __global__ void __launch_bounds__(kV5Threads) v5_final_kernel(V5Levels L, const int* __restrict__ ncand, const double* __restrict__ term,
                                                               const double* __restrict__ corr, const double* __restrict__ partial, float* __restrict__ out) {
-  __shared__ double red[kV5Threads / 32];
+  __shared__ double red[kV5Threads / 32][3];
   float lbox = 0.0f, lobj = 0.0f, lcls = 0.0f;
   for (int l = 0; l < L.nlev; ++l) {
     const int n = ncand[l];
     const size_t off = (size_t)l * L.cap;
-    double vb = 0.0, vc = 0.0, vo = 0.0;
+    double v[3] = {0.0, 0.0, 0.0};  // box, class, objectness
     for (int k = threadIdx.x; k < n; k += kV5Threads) {
-      vb += term[2 * (off + k)];
-      vc += term[2 * (off + k) + 1];
-      vo += corr[off + k];
+      v[0] += term[2 * (off + k)];
+      v[1] += term[2 * (off + k) + 1];
+      v[2] += corr[off + k];
     }
-    for (int j = threadIdx.x; j < kV5ObjBlocks; j += kV5Threads) vo += partial[l * kV5ObjBlocks + j];
-    const double sb = block_sum(vb, red), sc = block_sum(vc, red), so = block_sum(vo, red);
+    for (int j = threadIdx.x; j < kV5ObjBlocks; j += kV5Threads) v[2] += partial[l * kV5ObjBlocks + j];
+    block_sum<kV5Threads>(v, red);
     if (n > 0) {
-      lbox += (float)(sb / n);
-      if (L.nc > 1) lcls += (float)(sc / ((double)n * L.nc));
+      lbox += (float)(v[0] / n);
+      if (L.nc > 1) lcls += (float)(v[1] / ((double)n * L.nc));
     }
-    lobj += (float)(so / ((double)L.B * L.na * L.ny[l] * L.nx[l])) * L.balance[l];
+    lobj += (float)(v[2] / ((double)L.B * L.na * L.ny[l] * L.nx[l])) * L.balance[l];
   }
   if (threadIdx.x == 0) {
     lbox *= L.hyp_box;
@@ -388,22 +377,18 @@ struct V5Ws {
 };
 
 V5Ws v5_ws(void* base, int nlev, int cap) {
+  WsCarver c(base);
   V5Ws w{};
-  size_t o = 0;
-  char* p = static_cast<char*>(base);
-  auto take = [&](size_t bytes) { char* r = p ? p + o : nullptr; o = nms_align_up(o + bytes, 256); return r; };
   const size_t n = (size_t)nlev * (cap > 0 ? cap : 1);
-  w.key = reinterpret_cast<int*>(take(n * 4));
-  w.sorted = reinterpret_cast<int*>(take(n * 4));
-  w.score = reinterpret_cast<float*>(take(n * 4));
-  w.term = reinterpret_cast<double*>(take(n * 2 * sizeof(double)));
-  w.corr = reinterpret_cast<double*>(take(n * sizeof(double)));
-  w.partial = reinterpret_cast<double*>(take((size_t)nlev * kV5ObjBlocks * sizeof(double)));
-  w.bytes = o;
+  w.key = static_cast<int*>(c.take(n * 4));
+  w.sorted = static_cast<int*>(c.take(n * 4));
+  w.score = static_cast<float*>(c.take(n * 4));
+  w.term = static_cast<double*>(c.take(n * 2 * sizeof(double)));
+  w.corr = static_cast<double*>(c.take(n * sizeof(double)));
+  w.partial = static_cast<double*>(c.take((size_t)nlev * kV5ObjBlocks * sizeof(double)));
+  w.bytes = c.bytes();
   return w;
 }
-
-inline bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 int make_levels(const char* what, const float* const* preds, const int32_t* shapes, const float* anchors, const float* balance, int32_t nlev, int32_t na,
                 int32_t nc, const float* targets, int32_t nt, const float* hyp, float* const* grads, V5Levels* L) {
@@ -412,7 +397,7 @@ int make_levels(const char* what, const float* const* preds, const int32_t* shap
   CVB_REQUIRE(na >= 1 && na <= kV5MaxAnchors, "%s: 1 to %d anchors per level supported (got %d)", what, kV5MaxAnchors, na);
   CVB_REQUIRE(nc >= 1, "%s: num_classes must be >= 1 (got %d)", what, nc);
   CVB_REQUIRE(nt >= 0, "%s: nt must be >= 0 (got %d)", what, nt);
-  CVB_REQUIRE(nt == 0 || (targets && aligned(targets, 4)), "%s: targets [nt, 6] required, 4-byte aligned", what);
+  CVB_REQUIRE(nt == 0 || (targets && is_aligned(targets, 4)), "%s: targets [nt, 6] required, 4-byte aligned", what);
   CVB_REQUIRE((long long)5 * na * nt < (1LL << 28), "%s: too many targets (%d)", what, nt);
   CVB_REQUIRE(hyp[0] > 1.0f, "%s: anchor_t must be > 1 (got %g)", what, (double)hyp[0]);
   *L = V5Levels{};
@@ -420,11 +405,11 @@ int make_levels(const char* what, const float* const* preds, const int32_t* shap
   CVB_REQUIRE(B >= 1, "%s: batch must be >= 1 (got %d)", what, B);
   for (int l = 0; l < nlev; ++l) {
     const int32_t* s = shapes + 4 * l;
-    CVB_REQUIRE(preds[l] && aligned(preds[l], 4), "%s: level %d output missing or not 4-byte aligned", what, l);
+    CVB_REQUIRE(preds[l] && is_aligned(preds[l], 4), "%s: level %d output missing or not 4-byte aligned", what, l);
     CVB_REQUIRE(s[0] == B && s[1] == na * (5 + nc) && s[2] > 0 && s[3] > 0,
                 "%s: level %d output must be [B=%d, na * (5 + nc)=%d, ny > 0, nx > 0] (got [%d, %d, %d, %d])", what, l, B, na * (5 + nc), s[0], s[1], s[2], s[3]);
     CVB_REQUIRE((long long)B * na * (5 + nc) * s[2] * s[3] < INT_MAX, "%s: level %d too large", what, l);
-    if (grads) CVB_REQUIRE(grads[l] && aligned(grads[l], 4), "%s: level %d gradient missing or not 4-byte aligned", what, l);
+    if (grads) CVB_REQUIRE(grads[l] && is_aligned(grads[l], 4), "%s: level %d gradient missing or not 4-byte aligned", what, l);
     for (int a = 0; a < na; ++a) {
       const float aw = anchors[(l * na + a) * 2], ah = anchors[(l * na + a) * 2 + 1];
       CVB_REQUIRE(aw > 0.0f && ah > 0.0f, "%s: level %d anchor %d must be positive (got %g x %g)", what, l, a, (double)aw, (double)ah);
@@ -452,10 +437,10 @@ int make_levels(const char* what, const float* const* preds, const int32_t* shap
 }
 
 int check_outputs(const char* what, const int32_t* cand_idx, const float* cand_box, const int32_t* ncand, const void* workspace, size_t ws_bytes, const V5Levels& L) {
-  CVB_REQUIRE(cand_idx && cand_box && ncand && aligned(cand_idx, 4) && aligned(cand_box, 4) && aligned(ncand, 4),
+  CVB_REQUIRE(cand_idx && cand_box && ncand && is_aligned(cand_idx, 4) && is_aligned(cand_box, 4) && is_aligned(ncand, 4),
               "%s: cand_idx, cand_box and ncand are required, 4-byte aligned", what);
   const size_t need = v5_ws(nullptr, L.nlev, L.cap).bytes;
-  CVB_REQUIRE(workspace && aligned(workspace, 256), "%s: workspace required, 256-byte aligned", what);
+  CVB_REQUIRE(workspace && is_aligned(workspace, 256), "%s: workspace required, 256-byte aligned", what);
   CVB_REQUIRE(ws_bytes >= need, "%s: workspace of %zu bytes too small (%zu needed)", what, ws_bytes, need);
   return CVB_OK;
 }
@@ -478,7 +463,7 @@ extern "C" int cvb_train_yolov5_loss_fwd(const float* const* preds, const int32_
   if (rc != CVB_OK) return rc;
   rc = check_outputs("train_yolov5_loss_fwd", cand_idx, cand_box, ncand, workspace, ws_bytes, L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(out && aligned(out, 4), "train_yolov5_loss_fwd: out [4] required, 4-byte aligned");
+  CVB_REQUIRE(out && is_aligned(out, 4), "train_yolov5_loss_fwd: out [4] required, 4-byte aligned");
   const V5Ws w = v5_ws(workspace, nlev, L.cap);
   cudaStream_t st = as_stream(stream);
   const int cblk = ceil_div(L.cap > 0 ? L.cap : 1, kV5Threads);
@@ -502,7 +487,7 @@ extern "C" int cvb_train_yolov5_loss_bwd(const float* const* preds, const int32_
   if (rc != CVB_OK) return rc;
   rc = check_outputs("train_yolov5_loss_bwd", cand_idx, cand_box, ncand, workspace, ws_bytes, L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(grad_out && aligned(grad_out, 4), "train_yolov5_loss_bwd: grad_out [1] required, 4-byte aligned");
+  CVB_REQUIRE(grad_out && is_aligned(grad_out, 4), "train_yolov5_loss_bwd: grad_out [1] required, 4-byte aligned");
   const V5Ws w = v5_ws(const_cast<void*>(workspace), nlev, L.cap);
   cudaStream_t st = as_stream(stream);
   for (int l = 0; l < nlev; ++l) {

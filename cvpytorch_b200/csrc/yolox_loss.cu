@@ -9,8 +9,8 @@
 //   4. loss_gt_kernel       one CTA per (GT, image): IoU and cost over the image's candidates, the top-10 IoUs (dynamic k) and the k
 //                           lowest costs (ties: the lower anchor index), kept per thread in registers and merged across the CTA.
 //   5. loss_resolve_kernel  one thread per anchor: an anchor taken by several GTs goes to the argmin of its cost over all GTs (ties: the
-//                           lower GT index); the matched GT / IoU and the anchor's three loss terms, summed per CTA in a fixed tree.
-//   6. loss_final_kernel    one CTA: the CTA partials in a fixed order -> loss, iou_loss, conf_loss, cls_loss, num_fg ratio, num_fg.
+//                           lower GT index); the matched GT / IoU and the anchor's three loss terms, summed per CTA (block_sum).
+//   6. loss_final_kernel    one CTA: the CTA partials by a halving tree (DESIGN.md 2) -> loss, iou_loss, conf_loss, cls_loss, num_fg ratio, num_fg.
 // Backward (cvb_train_yolox_loss_bwd): loss_bwd_kernel, one thread per anchor, writes every channel of the fp32 NCHW gradients from the
 // saved assignment, scaled by the incoming gradients of the four loss outputs.  No float atomics anywhere: results are bitwise reproducible.
 //
@@ -365,20 +365,10 @@ __global__ void __launch_bounds__(kLossThreads) loss_resolve_kernel(LossLevels L
     matched_gt[idx] = m;
     matched_iou[idx] = miou;
   }
+  block_sum<kLossThreads>(v, red);
+  if (threadIdx.x == 0) {
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) red[threadIdx.x >> 5][k] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x < 4) {
-    double t = 0.0;
-    for (int w = 0; w < kLossThreads / 32; ++w) t += red[w][threadIdx.x];
-    partial[(size_t)blockIdx.x * 4 + threadIdx.x] = t;
+    for (int k = 0; k < 4; ++k) partial[(size_t)blockIdx.x * 4 + k] = v[k];
   }
 }
 
@@ -459,25 +449,21 @@ struct LossWs {
 inline int resolve_blocks(int B, int A) { return (int)(((long long)B * A + kLossThreads - 1) / kLossThreads); }
 
 LossWs loss_ws(void* base, int B, int A) {
+  WsCarver c(base);
   LossWs w{};
-  size_t o = 0;
-  char* p = static_cast<char*>(base);
-  auto take = [&](size_t bytes) { char* r = p ? p + o : nullptr; o = nms_align_up(o + bytes, 256); return r; };
   const size_t n = (size_t)B * A;
-  w.box = reinterpret_cast<float4*>(take(n * sizeof(float4)));
-  w.sc = reinterpret_cast<float2*>(take(n * sizeof(float2)));
-  w.flag = reinterpret_cast<uint8_t*>(take(n));
-  w.cand = reinterpret_cast<int*>(take(n * 4));
-  w.cnt = reinterpret_cast<int*>(take(n * 4));
-  w.taker = reinterpret_cast<int*>(take(n * 4));
-  w.nlabel = reinterpret_cast<int*>(take((size_t)B * 4));
-  w.ncand = reinterpret_cast<int*>(take((size_t)B * 4));
-  w.partial = reinterpret_cast<double*>(take((size_t)resolve_blocks(B, A) * 4 * sizeof(double)));
-  w.bytes = o;
+  w.box = static_cast<float4*>(c.take(n * sizeof(float4)));
+  w.sc = static_cast<float2*>(c.take(n * sizeof(float2)));
+  w.flag = static_cast<uint8_t*>(c.take(n));
+  w.cand = static_cast<int*>(c.take(n * 4));
+  w.cnt = static_cast<int*>(c.take(n * 4));
+  w.taker = static_cast<int*>(c.take(n * 4));
+  w.nlabel = static_cast<int*>(c.take((size_t)B * 4));
+  w.ncand = static_cast<int*>(c.take((size_t)B * 4));
+  w.partial = static_cast<double*>(c.take((size_t)resolve_blocks(B, A) * 4 * sizeof(double)));
+  w.bytes = c.bytes();
   return w;
 }
-
-inline bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 // Validates the level description shared by the forward and the backward and fills L (gradients: grads, may be NULL in the forward).
 int make_levels(const char* what, const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, int32_t B,
@@ -487,16 +473,16 @@ int make_levels(const char* what, const float* const* preds, const int32_t* shap
   CVB_REQUIRE(nc >= 1, "%s: num_classes must be >= 1 (got %d)", what, nc);
   CVB_REQUIRE(B >= 1, "%s: batch must be >= 1 (got %d)", what, B);
   CVB_REQUIRE(max_gt >= 1 && max_gt <= kLossMaxGt, "%s: max_gt must be in [1, %d] GT rows per image (got %d)", what, kLossMaxGt, max_gt);
-  CVB_REQUIRE(aligned(targets, 4), "%s: targets must be 4-byte aligned", what);
+  CVB_REQUIRE(is_aligned(targets, 4), "%s: targets must be 4-byte aligned", what);
   *L = LossLevels{};
   long long A = 0;
   for (int l = 0; l < nlev; ++l) {
     const int32_t* s = shapes + 4 * l;
-    CVB_REQUIRE(preds[l] && aligned(preds[l], 4), "%s: level %d output missing or not 4-byte aligned", what, l);
+    CVB_REQUIRE(preds[l] && is_aligned(preds[l], 4), "%s: level %d output missing or not 4-byte aligned", what, l);
     CVB_REQUIRE(s[0] == B && s[1] == 5 + nc && s[2] > 0 && s[3] > 0,
                 "%s: level %d output must be [B=%d, 5 + num_classes=%d, h > 0, w > 0] (got [%d, %d, %d, %d])", what, l, B, 5 + nc, s[0], s[1], s[2], s[3]);
     CVB_REQUIRE(strides[l] > 0.0f, "%s: level %d stride must be > 0 (got %g)", what, l, (double)strides[l]);
-    if (grads) CVB_REQUIRE(grads[l] && aligned(grads[l], 4), "%s: level %d gradient missing or not 4-byte aligned", what, l);
+    if (grads) CVB_REQUIRE(grads[l] && is_aligned(grads[l], 4), "%s: level %d gradient missing or not 4-byte aligned", what, l);
     L->p[l] = preds[l];
     L->g[l] = grads ? grads[l] : nullptr;
     L->h[l] = s[2];
@@ -531,10 +517,10 @@ extern "C" int cvb_train_yolox_loss_fwd(const float* const* preds, const int32_t
   LossLevels L;
   const int rc = make_levels("train_yolox_loss_fwd", preds, shapes, strides, nlev, nc, B, max_gt, targets, nullptr, &L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(matched_gt && matched_iou && out && aligned(matched_gt, 4) && aligned(matched_iou, 4) && aligned(out, 4),
+  CVB_REQUIRE(matched_gt && matched_iou && out && is_aligned(matched_gt, 4) && is_aligned(matched_iou, 4) && is_aligned(out, 4),
               "train_yolox_loss_fwd: matched_gt, matched_iou and out are required, 4-byte aligned");
   const LossWs w = loss_ws(workspace, B, L.A);
-  CVB_REQUIRE(workspace && aligned(workspace, 256), "train_yolox_loss_fwd: workspace required, 256-byte aligned");
+  CVB_REQUIRE(workspace && is_aligned(workspace, 256), "train_yolox_loss_fwd: workspace required, 256-byte aligned");
   CVB_REQUIRE(ws_bytes >= w.bytes, "train_yolox_loss_fwd: workspace of %zu bytes too small (%zu needed)", ws_bytes, w.bytes);
   cudaStream_t st = as_stream(stream);
   CVB_CHECK_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)B * L.A * sizeof(int), st));
@@ -557,8 +543,8 @@ extern "C" int cvb_train_yolox_loss_bwd(const float* const* preds, const int32_t
   LossLevels L;
   const int rc = make_levels("train_yolox_loss_bwd", preds, shapes, strides, nlev, nc, B, max_gt, targets, grads, &L);
   if (rc != CVB_OK) return rc;
-  CVB_REQUIRE(matched_gt && matched_iou && fwd_out && grad_out && aligned(matched_gt, 4) && aligned(matched_iou, 4) && aligned(fwd_out, 4) &&
-                  aligned(grad_out, 4),
+  CVB_REQUIRE(matched_gt && matched_iou && fwd_out && grad_out && is_aligned(matched_gt, 4) && is_aligned(matched_iou, 4) &&
+                  is_aligned(fwd_out, 4) && is_aligned(grad_out, 4),
               "train_yolox_loss_bwd: matched_gt, matched_iou, fwd_out and grad_out are required, 4-byte aligned");
   loss_bwd_kernel<<<dim3(ceil_div(L.A, kLossThreads), B), kLossThreads, 0, as_stream(stream)>>>(L, targets, matched_gt, matched_iou, fwd_out, grad_out);
   CVB_CHECK_CUDA(cudaGetLastError());

@@ -7,30 +7,19 @@ The network (ResNet-50, FPN, the GN heads, ScaleExp) stays in torch.  The head o
 outputs under autocast work and their gradients flow back through the cast; the fp32 computation is the contract.  No CPU fallback: CPU
 tensors raise CvbError.  Divergence: an empty GT list (m = 0) is an all-background batch here; the reference raises in torch.min.
 """
-import ctypes
-
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .train import _check_cuda, _p, _stream
+from .train import _check_cuda, _floats, _p, _ptrs, _shapes4, _stream, _workspace
 
 MAX_GT = 1024
 
 
 def _levels(preds, strides, limit_range):
-    """-> ctypes (cls, cnt, reg pointer arrays, shape array, strides, limit ranges), validated on the host by the C entry points."""
+    """-> ctypes (cls, cnt, reg pointer arrays, shapes of each level's cls, cnt, reg, strides, limit ranges), validated by the C entry points."""
     cls, cnt, reg = preds
-    n = len(cls)
-
-    def ptrs(ts):
-        return (ctypes.c_void_p * n)(*[t.data_ptr() for t in ts])
-
-    dims = [int(d) for lv in zip(cls, cnt, reg) for t in lv for d in (tuple(t.shape) if t.dim() == 4 else (0, 0, 0, 0))]
-    shapes = (ctypes.c_int32 * (12 * n))(*dims)
-    strd = (ctypes.c_float * n)(*[float(s) for s in strides])
-    lim = (ctypes.c_float * (2 * n))(*[float(v) for r in limit_range for v in r])
-    return ptrs(cls), ptrs(cnt), ptrs(reg), shapes, strd, lim
+    return _ptrs(cls), _ptrs(cnt), _ptrs(reg), _shapes4([t for lv in zip(cls, cnt, reg) for t in lv]), _floats(strides), _floats(v for r in limit_range for v in r)
 
 
 def fcos_loss_forward(preds, boxes, labels, strides, limit_range, return_targets=False):
@@ -44,7 +33,7 @@ def fcos_loss_forward(preds, boxes, labels, strides, limit_range, return_targets
     B, nc = cls[0].shape[0], cls[0].shape[1]
     A = sum(c.shape[2] * c.shape[3] for c in cls)
     dev = cls[0].device
-    ws = torch.empty((max(int(_lib.lib().cvb_train_fcos_loss_workspace_bytes(B, A, nc)), 1),), dtype=torch.uint8, device=dev)
+    ws = _workspace(_lib.lib().cvb_train_fcos_loss_workspace_bytes(B, A, nc), dev)
     out = torch.empty((4,), dtype=torch.float32, device=dev)
     matched_gt = torch.empty((B, A), dtype=torch.int32, device=dev)
     num_pos = torch.empty((B,), dtype=torch.int32, device=dev)
@@ -61,7 +50,7 @@ def fcos_loss_backward(preds, boxes, labels, strides, limit_range, matched_gt, n
     grads = [[torch.empty_like(t) for t in ts] for ts in preds]
     pc, pn, pr, shapes, strd, lim = _levels(preds, strides, limit_range)
     n = len(preds[0])
-    gc, gn, gr = ((ctypes.c_void_p * n)(*[t.data_ptr() for t in ts]) for ts in grads)
+    gc, gn, gr = (_ptrs(ts) for ts in grads)
     _lib.check(_lib.lib().cvb_train_fcos_loss_bwd(pc, pn, pr, shapes, strd, lim, n, _p(boxes), _p(labels), preds[0][0].shape[0], boxes.shape[1],
                                                   _p(matched_gt), _p(num_pos), _p(grad_out), gc, gn, gr, _stream()), 'cvb_train_fcos_loss_bwd')
     return grads

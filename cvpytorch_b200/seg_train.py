@@ -19,7 +19,7 @@ from torch import Tensor
 
 from . import _lib
 from .ops import SEG_DTYPES
-from .train import _check_cuda, _p, _stream
+from .train import _check_cuda, _p, _stream, _workspace
 
 
 def nc_max():
@@ -38,7 +38,7 @@ def seg_ce_forward(pred, target, ignore_index=255, loss_weight=1.0):
     [B, H, W], record int64 [2] = (n_valid, n_bad)); lse and record are what the backward needs."""
     B, H, W = target.shape
     dev = pred.device
-    ws = torch.empty((max(int(_lib.lib().cvb_train_seg_ce_workspace_bytes(B, H, W)), 1),), dtype=torch.uint8, device=dev)
+    ws = _workspace(_lib.lib().cvb_train_seg_ce_workspace_bytes(B, H, W), dev)
     loss = torch.empty((), dtype=torch.float32, device=dev)
     lse = torch.empty((B, H, W), dtype=torch.float32, device=dev)
     record = torch.empty((2,), dtype=torch.int64, device=dev)

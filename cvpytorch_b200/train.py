@@ -41,6 +41,27 @@ def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _ptrs(ts):
+    """ctypes void* array of the tensors' data pointers."""
+    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+def _shapes4(ts):
+    """ctypes int32 array of four dims per tensor: its 4-D shape, or zeros for a tensor that is not 4-D (which the C entry points refuse)."""
+    return (ctypes.c_int32 * (4 * len(ts)))(*[int(d) for t in ts for d in (tuple(t.shape) if t.dim() == 4 else (0, 0, 0, 0))])
+
+
+def _floats(vs):
+    """ctypes float array of the values."""
+    vs = [float(v) for v in vs]
+    return (ctypes.c_float * len(vs))(*vs)
+
+
+def _workspace(nbytes, dev):
+    """A device workspace of the size a *_workspace_bytes entry point returned (at least one byte, so it has an address)."""
+    return torch.empty((max(int(nbytes), 1),), dtype=torch.uint8, device=dev)
+
+
 def _check_cuda(t, what):
     if not t.is_cuda:
         raise _lib.CvbError(f'{what}: CUDA tensor required (the H100 training path has no CPU fallback)')
@@ -767,15 +788,6 @@ class YOLOXHead(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ YOLOX loss (SimOTA assignment + the three terms)
-def _loss_levels(preds, strides):
-    """-> ctypes (pointer array, shape array, stride array) of the head outputs, validated on the host by the C entry points."""
-    n = len(preds)
-    ptrs = (ctypes.c_void_p * n)(*[p.data_ptr() for p in preds])
-    shapes = (ctypes.c_int32 * (4 * n))(*[int(d) for p in preds for d in (tuple(p.shape) if p.dim() == 4 else (0, 0, 0, 0))])
-    strd = (ctypes.c_float * n)(*[float(s) for s in strides])
-    return ptrs, shapes, strd
-
-
 def yolox_loss_forward(preds, targets, strides, num_classes):
     """preds: the head's fp32 NCHW outputs [B, 5 + num_classes, h, w] (CUDA, contiguous); targets fp32 [B, max_gt, 5] (class, cx, cy, w, h).
     -> (out fp32 [6] = loss, iou_loss, conf_loss, cls_loss, num_fg ratio, num_fg; matched_gt int32 [B, A], -1 = background; matched_iou [B, A])."""
@@ -784,12 +796,11 @@ def yolox_loss_forward(preds, targets, strides, num_classes):
     B = preds[0].shape[0]
     A = sum(p.shape[2] * p.shape[3] for p in preds)
     dev = preds[0].device
-    ws = torch.empty((max(int(_lib.lib().cvb_train_yolox_loss_workspace_bytes(B, A)), 1),), dtype=torch.uint8, device=dev)
+    ws = _workspace(_lib.lib().cvb_train_yolox_loss_workspace_bytes(B, A), dev)
     out = torch.empty((6,), dtype=torch.float32, device=dev)
     matched_gt = torch.empty((B, A), dtype=torch.int32, device=dev)
     matched_iou = torch.empty((B, A), dtype=torch.float32, device=dev)
-    ptrs, shapes, strd = _loss_levels(preds, strides)
-    _lib.check(_lib.lib().cvb_train_yolox_loss_fwd(ptrs, shapes, strd, len(preds), num_classes, _p(targets), B, targets.shape[1], _p(matched_gt),
+    _lib.check(_lib.lib().cvb_train_yolox_loss_fwd(_ptrs(preds), _shapes4(preds), _floats(strides), len(preds), num_classes, _p(targets), B, targets.shape[1], _p(matched_gt),
                                                    _p(matched_iou), _p(out), _p(ws), ws.numel(), _stream()), 'cvb_train_yolox_loss_fwd')
     return out, matched_gt, matched_iou
 
@@ -797,10 +808,9 @@ def yolox_loss_forward(preds, targets, strides, num_classes):
 def yolox_loss_backward(preds, targets, strides, num_classes, matched_gt, matched_iou, out, grad_out):
     """d(sum_i grad_out[i] * out[i], i < 4) / d(preds) under the forward's assignment -> fp32 NCHW gradients shaped like preds."""
     grads = [torch.empty_like(p) for p in preds]
-    ptrs, shapes, strd = _loss_levels(preds, strides)
-    gptrs = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
-    _lib.check(_lib.lib().cvb_train_yolox_loss_bwd(ptrs, shapes, strd, len(preds), num_classes, _p(targets), preds[0].shape[0], targets.shape[1],
-                                                   _p(matched_gt), _p(matched_iou), _p(out), _p(grad_out), gptrs, _stream()), 'cvb_train_yolox_loss_bwd')
+    _lib.check(_lib.lib().cvb_train_yolox_loss_bwd(_ptrs(preds), _shapes4(preds), _floats(strides), len(preds), num_classes, _p(targets), preds[0].shape[0],
+                                                   targets.shape[1], _p(matched_gt), _p(matched_iou), _p(out), _p(grad_out), _ptrs(grads), _stream()),
+               'cvb_train_yolox_loss_bwd')
     return grads
 
 

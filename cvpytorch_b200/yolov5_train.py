@@ -13,15 +13,15 @@ channel counts must be 16, 32 or multiples of 64, which YOLOv5-s meets (YOLOv5-m
 momentum 0.03.  CPU tensors raise; evaluation goes through the inference modules of models.py, which load these modules' state_dict
 with strict=True.
 """
-import ctypes
 import math
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .train import (BaseConv, CSPLayer, SPPF, _bottleneck, _check_cuda, _ConvBnSiLULayer, _nhwc, _p, _require_training, _require_widths, _set_bn, _stream,
-                    _to_nchw, _to_nhwc, _UpsampleCat, conv, conv_wgrad, focus_s2d, pack_weights, pred_conv, pred_cout_pad, pred_grad)
+from .train import (BaseConv, CSPLayer, SPPF, _bottleneck, _check_cuda, _ConvBnSiLULayer, _floats, _nhwc, _p, _ptrs, _require_training, _require_widths,
+                    _set_bn, _shapes4, _stream, _to_nchw, _to_nhwc, _UpsampleCat, _workspace, conv, conv_wgrad, focus_s2d, pack_weights, pred_conv,
+                    pred_cout_pad, pred_grad)
 
 
 # ------------------------------------------------------------------------------------------------ backbone
@@ -258,13 +258,7 @@ class YOLOv5Detect(nn.Module):
 
 # ------------------------------------------------------------------------------------------------ loss
 def _loss_args(preds, anchors, balance, hyp):
-    n = len(preds)
-    ptrs = (ctypes.c_void_p * n)(*[p.data_ptr() for p in preds])
-    shapes = (ctypes.c_int32 * (4 * n))(*[int(d) for p in preds for d in (tuple(p.shape) if p.dim() == 4 else (0, 0, 0, 0))])
-    anc = (ctypes.c_float * anchors.numel())(*anchors.flatten().tolist())
-    bal = (ctypes.c_float * n)(*balance[:n])
-    hy = (ctypes.c_float * 5)(*hyp)
-    return ptrs, shapes, anc, bal, hy
+    return _ptrs(preds), _shapes4(preds), _floats(anchors.flatten().tolist()), _floats(balance[:len(preds)]), _floats(hyp)
 
 
 def yolov5_loss_forward(preds, targets, anchors, balance, hyp, num_classes):
@@ -276,7 +270,7 @@ def yolov5_loss_forward(preds, targets, anchors, balance, hyp, num_classes):
     dev = preds[0].device
     cap = max(5 * na * nt, 1)
     L = _lib.lib()
-    ws = torch.empty((max(int(L.cvb_train_yolov5_loss_workspace_bytes(nlev, na, nt)), 1),), dtype=torch.uint8, device=dev)
+    ws = _workspace(L.cvb_train_yolov5_loss_workspace_bytes(nlev, na, nt), dev)
     out = torch.empty((4,), dtype=torch.float32, device=dev)
     cand_idx = torch.empty((nlev, cap, 5), dtype=torch.int32, device=dev)
     cand_box = torch.empty((nlev, cap, 6), dtype=torch.float32, device=dev)
@@ -291,11 +285,10 @@ def yolov5_loss_backward(preds, targets, anchors, balance, hyp, num_classes, can
     """grad_out [1] (device) x d(loss)/d(preds) under the forward's candidates -> fp32 NCHW gradients shaped like preds."""
     grads = [torch.empty_like(p) for p in preds]
     ptrs, shapes, anc, bal, hy = _loss_args(preds, anchors, balance, hyp)
-    gptrs = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
     cand_idx, cand_box, ncand = cands
     nt = targets.shape[0]
     _lib.check(_lib.lib().cvb_train_yolov5_loss_bwd(ptrs, shapes, anc, bal, len(preds), anchors.shape[1], num_classes, _p(targets) if nt else None, nt, hy,
-                                                    _p(cand_idx), _p(cand_box), _p(ncand), _p(ws), ws.numel(), _p(grad_out), gptrs, _stream()),
+                                                    _p(cand_idx), _p(cand_box), _p(ncand), _p(ws), ws.numel(), _p(grad_out), _ptrs(grads), _stream()),
                'cvb_train_yolov5_loss_bwd')
     return grads
 
