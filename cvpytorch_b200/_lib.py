@@ -8,6 +8,8 @@ import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_size_t, c_void_p
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # CVB_DIAG_LIB=1 (developer tools only) loads the diagnostics build of the same sources (csrc/build.sh diag: cycle counters + CVB_DBG switches)
 LIB_PATH = os.path.join(_HERE, 'libcvb200_diag.so' if os.environ.get('CVB_DIAG_LIB') == '1' else 'libcvb200.so')
@@ -200,6 +202,16 @@ def check(rc, what=''):
     if rc != 0:
         msg = lib().cvb_last_error_string()
         raise CvbError(f'{what}: cvb error {rc}: {msg.decode() if msg else "?"}')
+
+
+def _stream():
+    """The `void* stream` argument of a launching call: the current CUDA stream."""
+    return c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _p(t):
+    """The `void*` argument of an optional tensor: its data pointer, or NULL for None."""
+    return c_void_p(t.data_ptr()) if t is not None else None
 
 
 def launch_count():

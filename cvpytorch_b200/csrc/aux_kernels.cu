@@ -920,7 +920,7 @@ extern "C" int cvb_stem_s2d(const float* src, int32_t B, int32_t H, int32_t W, c
   CVB_REQUIRE(src && H % 2 == 0 && W % 2 == 0, "stem_s2d: H and W must be even");
   CVB_REQUIRE(dst->B == B && dst->H == H / 2 && dst->W >= W / 2 + pad_left && pad_left >= 0 && dst->C == 16 && dst->c_pitch == 16,
               "stem_s2d: dst must be [B,H/2,>=W/2+pad_left,16]");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(src) & 7) == 0 && (reinterpret_cast<uintptr_t>(dst->base) & 15) == 0 && dst->plane_stride % 16 == 0,
+  CVB_REQUIRE(is_aligned(src, 8) && is_aligned(dst->base, 16) && dst->plane_stride % 16 == 0,
               "stem_s2d: alignment");
   const long long n = (long long)B * (H / 2) * (W / 2);
   const int block = 256;
@@ -941,9 +941,9 @@ extern "C" int cvb_stem_s2d_u8(const uint8_t* src, int32_t B, int32_t H, int32_t
   CVB_REQUIRE(std[0] != 0.0f && std[1] != 0.0f && std[2] != 0.0f, "stem_s2d_u8: zero std");
   CVB_REQUIRE(dst->B == B && dst->H == H / 2 && dst->W >= W / 2 + pad_left && pad_left >= 0 && dst->C == 16 && dst->c_pitch == 16,
               "stem_s2d_u8: dst must be [B,H/2,>=W/2+pad_left,16]");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(src) & 1) == 0 && (reinterpret_cast<uintptr_t>(dst->base) & 15) == 0 && dst->plane_stride % 16 == 0,
+  CVB_REQUIRE(is_aligned(src, 2) && is_aligned(dst->base, 16) && dst->plane_stride % 16 == 0,
               "stem_s2d_u8: alignment");
-  const bool pair = (W % 4 == 0) && (reinterpret_cast<uintptr_t>(src) & 3) == 0;
+  const bool pair = (W % 4 == 0) && is_aligned(src, 4);
   const long long n = (long long)B * (H / 2) * (W / 2) / (pair ? 2 : 1);
   const int block = 256;
   long long grid = (n + block - 1) / block;
@@ -969,18 +969,14 @@ extern "C" int cvb_sppf_pool(const CvbView* x, const CvbView* y1, const CvbView*
   const CvbView* vs[4] = {x, y1, y2, y3};
   for (int i = 0; i < 4; ++i) {
     CVB_REQUIRE(vs[i]->B == x->B && vs[i]->H == x->H && vs[i]->W == x->W && vs[i]->C == x->C, "sppf: view %d shape mismatch", i);
-    CVB_REQUIRE(vs[i]->c_pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(vs[i]->base) & 15) == 0 && vs[i]->plane_stride % 16 == 0,
+    CVB_REQUIRE(vs[i]->c_pitch % 8 == 0 && is_aligned(vs[i]->base, 16) && vs[i]->plane_stride % 16 == 0,
                 "sppf: view %d alignment", i);
   }
   CVB_REQUIRE(x->C % 8 == 0, "sppf: C must be a multiple of 8");
   const size_t smem = (size_t)x->H * x->W * 8 * sizeof(float) * 2;
   CVB_REQUIRE(smem <= 200 * 1024, "sppf: map %dx%d too large for the shared-memory pool kernel", x->H, x->W);
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sppf_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    return e;
-  }();
+  static const cudaError_t attr_set_err = opt_in_smem(sppf_pool_kernel, 200 * 1024);
   CVB_CHECK_CUDA(attr_set_err);
   const int cgroups = x->C / 8;
   sppf_pool_kernel<<<x->B * cgroups, 256, smem, as_stream(stream)>>>(
@@ -1001,12 +997,10 @@ extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const
   CVB_REQUIRE((long long)raw->H * raw->W * na < 0x7fffffffLL, "yolo_decode: level too large");
   CVB_REQUIRE(no <= 96, "yolo_decode: at most 91 classes supported (no=%d)", no);
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaFuncSetAttribute(yolo_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(yolo_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kNmsBins * (int)sizeof(uint32_t));
-    return e;
-  }();
-  CVB_CHECK_CUDA(attr_set_err);
+  static const cudaError_t multi_smem_err = opt_in_smem(yolo_decode_kernel<true, true>, kNmsBins * (int)sizeof(uint32_t));
+  static const cudaError_t single_smem_err = opt_in_smem(yolo_decode_kernel<true, false>, kNmsBins * (int)sizeof(uint32_t));
+  CVB_CHECK_CUDA(multi_smem_err);
+  CVB_CHECK_CUDA(single_smem_err);
   uint32_t* hist = static_cast<uint32_t*>(nms_workspace);
   float* rowmax = hist ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(raw->B)) : nullptr;
   const size_t smem = hist ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
@@ -1022,7 +1016,7 @@ extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const
 static int check_vec_view(const CvbView* v, const char* what) {
   int rc = check_split_view(v, what);
   if (rc) return rc;
-  CVB_REQUIRE(v->C % 8 == 0 && v->c_pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(v->base) & 15) == 0 && v->plane_stride % 16 == 0,
+  CVB_REQUIRE(v->C % 8 == 0 && v->c_pitch % 8 == 0 && is_aligned(v->base, 16) && v->plane_stride % 16 == 0,
               "%s: channels/pitch must be multiples of 8 and 16-byte aligned", what);
   return CVB_OK;
 }
@@ -1048,7 +1042,7 @@ extern "C" int cvb_split_to_f32nhwc(const CvbView* x, const CvbView* y, void* st
   int rc = check_vec_view(x, "split_to_f32 x");
   if (rc) return rc;
   CVB_REQUIRE(y && y->base && y->B == x->B && y->H == x->H && y->W == x->W && y->C == x->C && y->c_pitch % 4 == 0 &&
-                  (reinterpret_cast<uintptr_t>(y->base) & 15) == 0,
+                  is_aligned(y->base, 16),
               "split_to_f32: output view mismatch");
   const long long npix = (long long)x->B * x->H * x->W;
   long long grid = (npix * (x->C / 8) + 255) / 256;
@@ -1070,7 +1064,7 @@ extern "C" int cvb_groupnorm_relu(const CvbView* x, int32_t groups, const float*
   CVB_REQUIRE(gamma && beta && workspace, "groupnorm: null argument");
   CVB_REQUIRE(groups > 0 && x->C == groups * 8, "groupnorm: only 8 channels per group are supported (C=%d, groups=%d)", x->C, groups);
   CVB_REQUIRE(y->B == x->B && y->H == x->H && y->W == x->W && y->C == x->C, "groupnorm: output view mismatch");
-  CVB_REQUIRE(workspace_bytes >= cvb_groupnorm_workspace_bytes(x->B, groups) && (reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
+  CVB_REQUIRE(workspace_bytes >= cvb_groupnorm_workspace_bytes(x->B, groups) && is_aligned(workspace, 8),
               "groupnorm: workspace too small / misaligned");
   cudaStream_t st = as_stream(stream);
   CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, cvb_groupnorm_workspace_bytes(x->B, groups), st));
@@ -1099,7 +1093,7 @@ extern "C" int cvb_dwconv3x3(const CvbView* x, const float* weights, const float
   if (rc) return rc;
   CVB_REQUIRE(weights && bias && dilation >= 1, "dwconv3x3: bad argument");
   CVB_REQUIRE(y->B == x->B && y->H == x->H && y->W == x->W && y->C == x->C, "dwconv3x3: output view mismatch (stride 1, 'same' padding)");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(weights) & 15) == 0, "dwconv3x3: weights must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(weights, 16), "dwconv3x3: weights must be 16-byte aligned");
   const int tiles_x = ceil_div(x->W, 8), tiles_y = ceil_div(x->H, 8);
   CVB_REQUIRE(x->B <= 65535 && ceil_div(x->C / 8, 4) <= 65535, "dwconv3x3: batch / channel count too large for the launch grid");
   if (dilation == 1) {
@@ -1150,7 +1144,7 @@ extern "C" int cvb_bilinear_resize(const CvbView* x, const CvbView* y, void* str
 
 extern "C" int cvb_upsample_argmax(const CvbView* logits, int32_t nc, int64_t* labels, int32_t Ho, int32_t Wo, void* stream) {
   CVB_REQUIRE(logits && logits->base && labels && nc > 0 && logits->c_pitch >= nc && Ho > 0 && Wo > 0, "upsample_argmax: bad argument");
-  CVB_REQUIRE(logits->c_pitch % 4 == 0 && (reinterpret_cast<uintptr_t>(logits->base) & 15) == 0 && logits->c_pitch >= (nc + 3) / 4 * 4,
+  CVB_REQUIRE(logits->c_pitch % 4 == 0 && is_aligned(logits->base, 16) && logits->c_pitch >= (nc + 3) / 4 * 4,
               "upsample_argmax: logits rows must be 16-byte aligned and padded to a multiple of 4 classes");
   CVB_REQUIRE(Ho <= 65535 && logits->B <= 65535, "upsample_argmax: output too tall / batch too large for the launch grid");
   dim3 grid(ceil_div(Wo, 256), Ho, logits->B);

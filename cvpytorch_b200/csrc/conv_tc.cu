@@ -24,7 +24,6 @@
 
 #include <cstdlib>
 #include <memory>
-#include <mutex>
 #include <new>
 #include <type_traits>
 
@@ -1090,24 +1089,6 @@ struct CvbConvPlan {
 
 namespace cvb {
 
-static int encode_map(CUtensorMap* m, CUtensorMapDataType dt, int rank, void* base, const cuuint64_t* dims,
-                      const cuuint64_t* strides_bytes /*rank-1*/, const cuuint32_t* box, CUtensorMapSwizzle swz) {
-  EncodeTiledFn enc = get_encode_tiled();
-  if (!enc) return set_error(CVB_ERR_NO_DEVICE, "cuTensorMapEncodeTiled entry point not found (no CUDA driver?)");
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = enc(m, dt, (cuuint32_t)rank, base, dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    return set_error(CVB_ERR_CUDA,
-                     "cuTensorMapEncodeTiled failed (%d): rank %d dims [%llu %llu %llu %llu %llu] box [%u %u %u %u %u] base %p", (int)r,
-                     rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
-                     (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0),
-                     (unsigned long long)(rank > 4 ? dims[4] : 0), box[0], rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0,
-                     rank > 3 ? box[3] : 0, rank > 4 ? box[4] : 0, base);
-  }
-  return CVB_OK;
-}
-
 static CUtensorMapSwizzle swizzle_for_bytes(int bytes) {
   return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
@@ -1118,7 +1099,7 @@ static int encode_5d(CUtensorMap* m, CUtensorMapDataType dt, const void* base, i
   const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B, (cuuint64_t)planes};
   const cuuint64_t str[4] = {(cuuint64_t)s_w, (cuuint64_t)s_h, (cuuint64_t)s_b, (cuuint64_t)s_plane};
   const cuuint32_t bx[5] = {(cuuint32_t)box[0], (cuuint32_t)box[1], (cuuint32_t)box[2], (cuuint32_t)box[3], (cuuint32_t)box[4]};
-  return encode_map(m, dt, 5, const_cast<void*>(base), dims, str, bx, swz);
+  return encode_map(m, dt, 5, base, dims, str, bx, swz);
 }
 
 // Pick the output pixel box (TW x TH x NB <= rows: the tile's accumulator rows) that wastes the fewest accumulator rows.
@@ -1149,8 +1130,6 @@ static void choose_box(int B, int H, int W, int rows, int* TW, int* TH, int* NB)
   *TH = bh;
   *NB = bb;
 }
-
-static int g_num_sms = 0;
 
 // A/B knobs read once per process
 static bool two_ctas_on() {
@@ -1220,13 +1199,12 @@ static int validate_desc(const CvbConvDesc& desc, ConvProblem* P) {
     CVB_REQUIRE(d->kh == 1 && d->kw == 1 && d->stride == 1 && d->pad == 0 && win == 0, "conv(yolo): the detect conv is 1x1 / stride 1");
     CVB_REQUIRE(out.C == d->yolo->na * 128 && d->cout_pad == out.C, "conv(yolo): weights must be packed one anchor per 128-wide n-tile (C = na*128)");
     CVB_REQUIRE(!d->residual.base && !d->up_partial.base && d->act == CVB_ACT_NONE, "conv(yolo): no residual / partial / activation");
-    CVB_REQUIRE((reinterpret_cast<uintptr_t>(d->yolo->z) & 3) == 0, "conv(yolo): z must be 4-byte aligned");
+    CVB_REQUIRE(is_aligned(d->yolo->z, 4), "conv(yolo): z must be 4-byte aligned");
   }
   const int cout = out.C;
   CVB_REQUIRE(cin % 16 == 0, "conv: cin=%d must be a multiple of 16", cin);
   CVB_REQUIRE(in.c_pitch % 8 == 0 && (P->yolo || out.c_pitch % 8 == 0), "conv: channel pitch must be a multiple of 8");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(in.base) & 15) == 0 && (P->yolo || (reinterpret_cast<uintptr_t>(out.base) & 15) == 0) &&
-                  (reinterpret_cast<uintptr_t>(d->weights) & 15) == 0,
+  CVB_REQUIRE(is_aligned(in.base, 16) && (P->yolo || is_aligned(out.base, 16)) && is_aligned(d->weights, 16),
               "conv: pointers must be 16-byte aligned");
   // window mode: the caller fixes the output height (asymmetric vertical padding is expressed by `pad` = rows above; rows
   // below come from TMA zero fill), e.g. the 7x7/s2/p3 ResNet stem == 4 filter rows over the space-to-depth input, pad 2.
@@ -1240,13 +1218,13 @@ static int validate_desc(const CvbConvDesc& desc, ConvProblem* P) {
   if (d->residual.base) {
     const CvbView& r = d->residual;
     CVB_REQUIRE(r.B == out.B && r.H == Ho && r.W == Wo && r.C == cout && r.c_pitch % 8 == 0 && cout % 32 == 0 &&
-                    (reinterpret_cast<uintptr_t>(r.base) & 15) == 0 && r.plane_stride % 16 == 0,
+                    is_aligned(r.base, 16) && r.plane_stride % 16 == 0,
                 "conv: residual view mismatch");
   }
   if (d->up_partial.base) {
     const CvbView& u = d->up_partial;
     CVB_REQUIRE(u.B == out.B && u.H == (Ho + 1) / 2 && u.W == (Wo + 1) / 2 && u.C == cout && u.c_pitch % 4 == 0 && cout % 32 == 0 &&
-                    (reinterpret_cast<uintptr_t>(u.base) & 15) == 0,
+                    is_aligned(u.base, 16),
                 "conv: up_partial view mismatch");
   }
   P->win = win;
@@ -1801,7 +1779,7 @@ static int encode_maps(const ConvProblem& P, int bn, const SchedPlan& S, const H
     const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)d->cout_pad, 2};
     const cuuint64_t str[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(K * 2 * d->cout_pad)};
     const cuuint32_t wbox[3] = {(cuuint32_t)bk, (cuuint32_t)bn, 2};
-    rc = encode_map(&a.tmB, f16, 3, const_cast<void*>(d->weights), dims, str, wbox, swizzle_for_bytes(bk * 2));
+    rc = encode_map(&a.tmB, f16, 3, d->weights, dims, str, wbox, swizzle_for_bytes(bk * 2));
   }
   // output and residual tiles: one output group of the tile box (fp32: one plane)
   const ConvGeom g = conv_geom(bn, bk, P.f32, P.yolo, S.pp);
@@ -1909,23 +1887,10 @@ static int set_launch(const ConvProblem& P, int bn, const SchedPlan& S, CvbConvP
   p->smem = S.sm.total;
   p->threads = kThreads;
   p->schedule = S.pp ? CVB_SCHED_PINGPONG : CVB_SCHED_COOPERATIVE;
-  static std::mutex mu;
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    if (g_num_sms == 0) {
-      int dev = 0;
-      cudaError_t e = cudaGetDevice(&dev);
-      if (e == cudaSuccess) e = cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-      if (e != cudaSuccess || g_num_sms <= 0) {
-        g_num_sms = 0;
-        return set_error(CVB_ERR_NO_DEVICE, "no CUDA device: %s", cudaGetErrorString(e));
-      }
-    }
-    cudaError_t e = cudaFuncSetAttribute(p->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-    if (e != cudaSuccess) return set_error(CVB_ERR_CUDA, "cudaFuncSetAttribute(smem) failed: %s", cudaGetErrorString(e));
-  }
+  int sms = sm_count();
+  if (sms == 0) return CVB_ERR_NO_DEVICE;
+  CVB_CHECK_CUDA(opt_in_smem(p->fn, kSmemBudget));
   const long long total = (long long)a.tiles_w * a.tiles_h * a.tiles_b * a.tiles_n;
-  int sms = g_num_sms;
   if (P.d.sm_limit > 0 && P.d.sm_limit < sms) sms = P.d.sm_limit;
   sms *= S.ctas;
   p->grid = (int)(total < sms ? total : sms);

@@ -31,11 +31,19 @@ void count_launch(int n = 1);
     if (!(cond)) return ::cvb::set_error(CVB_ERR_INVALID, __VA_ARGS__); \
   } while (0)
 
-// cuTensorMapEncodeTiled resolved through the runtime (no link-time dependency on libcuda).
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode_tiled();
+// Tiled tensor map with unit element strides, no interleave, 256-byte L2 promotion and zero OOB fill: strides_bytes has rank - 1 entries.
+// A missing driver entry point is CVB_ERR_NO_DEVICE, a refused encoding CVB_ERR_CUDA with the extents and box in the message.
+int encode_map(CUtensorMap* m, CUtensorMapDataType dt, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+               const cuuint32_t* box, CUtensorMapSwizzle swz);
+
+// SM count of the current device, queried once per process; 0 (with CVB_ERR_NO_DEVICE set) when there is no device.
+int sm_count();
+
+// Opt-in of kernel fn to `bytes` of dynamic shared memory per CTA (above the default 48 KB).
+template <typename F>
+inline cudaError_t opt_in_smem(F* fn, int bytes) {
+  return cudaFuncSetAttribute(reinterpret_cast<const void*>(fn), cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+}
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 

@@ -659,7 +659,7 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   CVB_REQUIRE(p->max_det > 0 && p->max_det <= 4096 && p->max_nms > 0, "nms: bad limits");
   CVB_REQUIRE((long long)p->A * p->nc < 0x7fffffffLL, "nms: candidate id overflow");
   CVB_REQUIRE(workspace_bytes >= cvb_nms_workspace_bytes(p->B, p->A, p->nc), "nms: workspace too small");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "nms: workspace must be 256-byte aligned");
+  CVB_REQUIRE(is_aligned(workspace, 256), "nms: workspace must be 256-byte aligned");
   cudaStream_t st = as_stream(stream);
   NmsWs wsA = carve_ws(workspace, p->B, 0), wsB = carve_ws(workspace, p->B, 1);
   if (!p->hist_ready) CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, nms_ws_head_bytes(p->B), st));
@@ -674,13 +674,10 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   const size_t gsmem = sizeof(GreedySmem) + (size_t)p->max_det * (sizeof(float4) + sizeof(float));
   CVB_REQUIRE(gsmem <= 200 * 1024, "nms: max_det too large");
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nms_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nms_greedy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    return e;
-  }();
-  CVB_CHECK_CUDA(attr_set_err);
+  static const cudaError_t emit_smem_err = opt_in_smem(nms_emit_kernel, 160 * 1024);
+  static const cudaError_t greedy_smem_err = opt_in_smem(nms_greedy_kernel, 200 * 1024);
+  CVB_CHECK_CUDA(emit_smem_err);
+  CVB_CHECK_CUDA(greedy_smem_err);
   if (!p->hist_ready) {
     nms_count_kernel<<<sgrid, kScanThreads, 0, st>>>(prediction, p->A, p->nc, p->conf_thres, p->multi_label, wsB);
     count_launch();
@@ -701,11 +698,10 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   {
     // one CTA per SM: co-residency is guaranteed (required by the grid barriers); resolved once, thread-safe static initialisation
     static const int coop_grid = [] {
-      int dev = 0, sms = 0, per_sm = 0;
-      if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-      if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bitonic_full_sort_kernel, 1024, 0) != cudaSuccess) return 0;
-      return (sms > 0 && per_sm > 0) ? sms : 0;
+      const int sms = sm_count();
+      int per_sm = 0;
+      if (sms == 0 || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bitonic_full_sort_kernel, 1024, 0) != cudaSuccess) return 0;
+      return per_sm > 0 ? sms : 0;
     }();
     CVB_REQUIRE(coop_grid > 0, "nms: cooperative sort kernel cannot be resident");
     int Bn = p->B;
@@ -887,7 +883,7 @@ extern "C" int cvb_yolox_decode(const CvbView* reg_obj, const CvbView* cls, int3
   CVB_REQUIRE(reg_obj->plane_stride == 0 && cls->plane_stride == 0, "yolox_decode: inputs must be fp32 NHWC views");
   CVB_REQUIRE(reg_obj->B == cls->B && reg_obj->H == cls->H && reg_obj->W == cls->W && reg_obj->C >= 5 && cls->C >= nc && nc > 0,
               "yolox_decode: shape mismatch");
-  CVB_REQUIRE(off >= 0 && off + (int64_t)cls->H * cls->W <= A && (reinterpret_cast<uintptr_t>(cand) & 15) == 0, "yolox_decode: bad output range");
+  CVB_REQUIRE(off >= 0 && off + (int64_t)cls->H * cls->W <= A && is_aligned(cand, 16), "yolox_decode: bad output range");
   const long long npix = (long long)cls->B * cls->H * cls->W;
   const long long blocks = (npix * 32 + 255) / 256;
   yolox_decode_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(static_cast<const float*>(reg_obj->base), reg_obj->c_pitch,
@@ -903,14 +899,10 @@ extern "C" int cvb_yolox_nms(const float* cand, int32_t B, int32_t A, float conf
   using namespace cvb;
   CVB_REQUIRE(cand && det && det_count && workspace && B > 0 && A > 0, "yolox_nms: null argument / bad shape");
   CVB_REQUIRE(A <= kXKeys, "yolox_nms: at most %d locations per image (got %d)", kXKeys, A);
-  CVB_REQUIRE(workspace_bytes >= cvb_yolox_workspace_bytes(B, A) && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "yolox_nms: workspace");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(cand) & 15) == 0, "yolox_nms: candidate records must be 16-byte aligned");
+  CVB_REQUIRE(workspace_bytes >= cvb_yolox_workspace_bytes(B, A) && is_aligned(workspace, 16), "yolox_nms: workspace");
+  CVB_REQUIRE(is_aligned(cand, 16), "yolox_nms: candidate records must be 16-byte aligned");
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(yolox_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(YoloxSmem));
-    return e;
-  }();
+  static const cudaError_t attr_set_err = opt_in_smem(yolox_nms_kernel, (int)sizeof(YoloxSmem));
   CVB_CHECK_CUDA(attr_set_err);
   float4* kbox = static_cast<float4*>(workspace);
   float* karea = reinterpret_cast<float*>(kbox + (size_t)B * A);
@@ -1107,7 +1099,7 @@ extern "C" int cvb_fcos_decode(const CvbView* cls, const CvbView* regcnt, int32_
   CVB_REQUIRE(cls && regcnt && cls->base && regcnt->base && scores && classes && boxes, "fcos_decode: null argument");
   CVB_REQUIRE(cls->B == regcnt->B && cls->H == regcnt->H && cls->W == regcnt->W && cls->c_pitch >= nc && regcnt->c_pitch >= 5,
               "fcos_decode: view mismatch");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(boxes) & 15) == 0, "fcos_decode: boxes must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(boxes, 16), "fcos_decode: boxes must be 16-byte aligned");
   const long long rows = (long long)cls->B * cls->H * cls->W;
   long long grid = (rows + 7) / 8;
   if (grid > kSmCount * 16) grid = kSmCount * 16;
@@ -1125,7 +1117,7 @@ extern "C" int cvb_fcos_nms(const float* scores, const int32_t* classes, const f
   using namespace cvb;
   CVB_REQUIRE(scores && classes && boxes && out_scores && out_classes && out_boxes && out_loc && out_count, "fcos_nms: null argument");
   CVB_REQUIRE(B > 0 && N > 0 && topk > 0 && topk <= 2048, "fcos_nms: bad sizes (topk <= 2048)");
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(boxes) & 15) == 0 && (reinterpret_cast<uintptr_t>(out_boxes) & 15) == 0, "fcos_nms: box arrays must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(boxes, 16) && is_aligned(out_boxes, 16), "fcos_nms: box arrays must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
   if (status) CVB_CHECK_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), st));
   CVB_CHECK_CUDA(cudaMemsetAsync(out_scores, 0, (size_t)B * topk * sizeof(float), st));
@@ -1133,11 +1125,7 @@ extern "C" int cvb_fcos_nms(const float* scores, const int32_t* classes, const f
   CVB_CHECK_CUDA(cudaMemsetAsync(out_boxes, 0, (size_t)B * topk * 4 * sizeof(float), st));
   CVB_CHECK_CUDA(cudaMemsetAsync(out_loc, 0xFF, (size_t)B * topk * sizeof(int32_t), st));
   // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t attr_set_err = [] {
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(fcos_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FcosSmem));
-    return e;
-  }();
+  static const cudaError_t attr_set_err = opt_in_smem(fcos_nms_kernel, (int)sizeof(FcosSmem));
   CVB_CHECK_CUDA(attr_set_err);
   fcos_nms_kernel<<<B, kFcosThreads, sizeof(FcosSmem), st>>>(scores, classes, boxes, N, score_thres, iou_thres, topk, out_scores, out_classes,
                                                             out_boxes, out_loc, out_count, status);

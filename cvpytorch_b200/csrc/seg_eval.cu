@@ -120,10 +120,10 @@ static int seg_launch(const void* gt, const void* pred, long long n, int nc, uns
   replicas = replicas < 1 ? 1 : replicas > kSegMaxReplicas ? kSegMaxReplicas : replicas;
   const int smem = replicas * stride * 4;
   auto fn = seg_confusion_kernel<G, P>;
-  CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  int dev = 0, sms = 0, per_sm = 0;
-  CVB_CHECK_CUDA(cudaGetDevice(&dev));
-  CVB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CVB_CHECK_CUDA(opt_in_smem(fn, smem));
+  const int sms = sm_count();
+  if (sms == 0) return CVB_ERR_NO_DEVICE;
+  int per_sm = 0;
   CVB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kSegThreads, smem));
   CVB_REQUIRE(per_sm > 0, "seg_confusion_update: %d bytes of shared memory do not fit a CTA", smem);
   constexpr int U = kSegUnroll<E>;

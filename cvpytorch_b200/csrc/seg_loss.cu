@@ -370,7 +370,7 @@ static int ce_bwd_launch(const float* preds, const T* labels, const CeShape& S, 
   const CeTile K = ce_tile(S);
   const size_t smem = ce_smem_bytes(K);
   auto fn = seg_ce_bwd_kernel<T>;
-  CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CVB_CHECK_CUDA(opt_in_smem(fn, (int)smem));
   const dim3 grid(ceil_div(S.w, K.TJ), ceil_div(S.h, K.TI), S.B);
   fn<<<grid, kCeThreads, smem, st>>>(preds, labels, S, K, lse, reinterpret_cast<const long long*>(record), grad_out, loss_weight, grad_preds);
   CVB_CHECK_CUDA(cudaGetLastError());

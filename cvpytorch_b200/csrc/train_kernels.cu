@@ -925,14 +925,9 @@ __global__ void pack_train_weights_kernel(const float* __restrict__ w, int cout,
 }
 
 // ------------------------------------------------------------------------------------------------ host
+// every training operand is bf16 with 64-element (128-byte) K rows
 static int encode_tiled(CUtensorMap* m, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box) {
-  EncodeTiledFn enc = get_encode_tiled();
-  if (!enc) return set_error(CVB_ERR_NO_DEVICE, "cuTensorMapEncodeTiled entry point not found (no CUDA driver?)");
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(CVB_ERR_CUDA, "cuTensorMapEncodeTiled (training) failed: %d", (int)r);
-  return CVB_OK;
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, base, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // pixel box TW x TH x NB with exactly 128 pixels (powers of two) that wastes the fewest rows on out-of-bounds pixels
@@ -957,15 +952,6 @@ static int act_map(CUtensorMap* m, const void* base, int B, int H, int W, int C,
   const cuuint64_t str[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2 * W, (cuuint64_t)C * 2 * W * H};
   const cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)NB};
   return encode_tiled(m, 4, base, dims, str, box);
-}
-
-static int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSmCount;
-  }
-  return n;
 }
 
 }  // namespace cvb
@@ -1078,7 +1064,7 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
   const int k_iters = a.taps * (kpad64(a.cin) / 64);
   a.stages = k_iters < kTStagesFwd ? k_iters : kTStagesFwd;
   const int smem = a.stages * (128 * 128 + bn * 128) + 256 + 2 * bn * 4;
-  CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  CVB_CHECK_CUDA(opt_in_smem(fn, smem));
   void* kargs[1] = {&a};
   const dim3 grid((unsigned)(a.tiles_w * a.tiles_h * a.tiles_b), (unsigned)ceil_div(a.cout, bn));
   CVB_CHECK_CUDA(cudaLaunchKernel(fn, grid, dim3(kTThreads), kargs, (size_t)smem, as_stream(stream)));
@@ -1090,25 +1076,25 @@ static int launch_tconv(TConvArgs& a, const void* w_packed, int wblocks, const v
 // k - 1 - 1 = -1, the backward-data of that stem
 static bool train_pad_ok(int k, int pad) { return k == 1 ? (pad >= -1 && pad <= 1) : (k == 3 && pad == 1); }
 
-// Shape rules of a training convolution (forward / backward-data and backward-weight alike).  aligned: the OR of the addresses that must
-// be 16-byte aligned.  A stride-1 output is (H + 2 pad - k + 1) x (W + 2 pad - k + 1): TMA zero-fills the pixels outside the input
+// Shape rules of a training convolution (forward / backward-data and backward-weight alike).  a, b, c: the operands, which must be 16-byte
+// aligned (c may be null).  A stride-1 output is (H + 2 pad - k + 1) x (W + 2 pad - k + 1): TMA zero-fills the pixels outside the input
 // (pad > 0), a negative pad crops its border instead.
-static int check_conv_shape(const char* fn, int B, int H, int W, int cin, int cout, int k, int stride, int pad, uintptr_t aligned) {
+static int check_conv_shape(const char* fn, int B, int H, int W, int cin, int cout, int k, int stride, int pad, const void* a, const void* b,
+                            const void* c = nullptr) {
   CVB_REQUIRE((k == 1 || k == 3) && train_channels_ok(cin) && train_channels_ok(cout),
               "%s: k in {1,3}, channels must be 16, 32 or multiples of 64 (cin=%d cout=%d k=%d)", fn, cin, cout, k);
   CVB_REQUIRE(stride == 1 || (stride == 2 && k == 3), "%s: stride 1, or stride 2 with k = 3", fn);
   CVB_REQUIRE(train_pad_ok(k, pad), "%s: padding must be -1, 0 or 1 with k = 1, and 1 with k = 3 (k=%d pad=%d)", fn, k, pad);
   CVB_REQUIRE(B > 0 && H > 0 && W > 0 && H + 2 * pad - k + 1 > 0 && W + 2 * pad - k + 1 > 0, "%s: empty output (B=%d H=%d W=%d k=%d pad=%d)", fn, B, H, W,
               k, pad);
-  CVB_REQUIRE((aligned & 15) == 0, "%s: pointers must be 16-byte aligned", fn);
+  CVB_REQUIRE(is_aligned(a, 16) && is_aligned(b, 16) && is_aligned(c, 16), "%s: pointers must be 16-byte aligned", fn);
   return CVB_OK;
 }
 
 static int train_conv(const void* x, int B, int H, int W, int cin, const void* w_packed, int cout, int k, int stride, int pad, void* out, const void* y_prev,
                       const float* bn_stat_prev, void* stream) {
   CVB_REQUIRE(x && w_packed && out, "train_conv: null tensor");
-  int rc = check_conv_shape("train_conv", B, H, W, cin, cout, k, stride, pad,
-                            reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed) | reinterpret_cast<uintptr_t>(out));
+  int rc = check_conv_shape("train_conv", B, H, W, cin, cout, k, stride, pad, x, w_packed, out);
   if (rc != CVB_OK) return rc;
   CVB_REQUIRE((y_prev == nullptr) == (bn_stat_prev == nullptr), "train_conv: the SiLU' epilogue needs both y_prev and its BN statistics");
   TConvArgs a;
@@ -1144,8 +1130,7 @@ extern "C" int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t 
   CVB_REQUIRE(train_channels_ok(cin) && B > 0 && H > 0 && W > 0, "train_pred_conv: cin must be 16, 32 or a multiple of 64 (cin=%d)", cin);
   CVB_REQUIRE(cout > 0 && cout_pad == pred_cout_pad(cout), "train_pred_conv: cout_pad must be the next training width of cout (cout=%d cout_pad=%d)", cout, cout_pad);
   CVB_REQUIRE(c_off >= 0 && c_off + cout <= c_tot, "train_pred_conv: channels [%d, %d) outside the %d-channel output", c_off, c_off + cout, c_tot);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_packed)) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0 &&
-                  (reinterpret_cast<uintptr_t>(bias) & 3) == 0,
+  CVB_REQUIRE(is_aligned(x, 16) && is_aligned(w_packed, 16) && is_aligned(out, 4) && is_aligned(bias, 4),
               "train_pred_conv: x / w_packed must be 16-byte, out / bias 4-byte aligned");
   TConvArgs a;
   tconv_geometry(a, B, H, W, cin, cout_pad, nullptr, H, W, 1, 0, 0);
@@ -1198,7 +1183,7 @@ extern "C" int cvb_train_conv_dgrad_s2(const void* dy, int32_t B, int32_t Ho, in
 
 static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int cin, int cout, int k, int stride, int pad, float* dw, void* stream) {
   CVB_REQUIRE(x && dy && dw, "train_conv_wgrad: null tensor");
-  int rc = check_conv_shape("train_conv_wgrad", B, H, W, cin, cout, k, stride, pad, reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy));
+  int rc = check_conv_shape("train_conv_wgrad", B, H, W, cin, cout, k, stride, pad, x, dy);
   if (rc != CVB_OK) return rc;
   TWgradArgs a;
   memset(&a, 0, sizeof(a));
@@ -1218,7 +1203,9 @@ static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, 
   const bool narrow = cout < 64;
   const int npan = narrow ? 1 : ((cout / 64) % 4 == 0 ? 4 : ((cout / 64) % 2 == 0 ? 2 : 1));
   a.nblocks = narrow ? 1 : cout / (64 * npan);
-  int splits = (2 * num_sms()) / (a.taps * cblocks * a.nblocks);  // ~two waves of CTAs: (split, tap, cin block x cout block)
+  const int sms = sm_count();
+  if (sms == 0) return CVB_ERR_NO_DEVICE;
+  int splits = (2 * sms) / (a.taps * cblocks * a.nblocks);  // ~two waves of CTAs: (split, tap, cin block x cout block)
   if (splits < 1) splits = 1;
   if (splits > m_tiles) splits = m_tiles;
   a.splits = splits;
@@ -1239,7 +1226,7 @@ static int train_conv_wgrad(const void* x, const void* dy, int B, int H, int W, 
   const int stages = npan == 4 ? 2 : kTStagesWg;
   const int smem = stages * ((2 + npan) * 128 * 128) + 256;
   CVB_REQUIRE(smem <= 232448, "train_conv_wgrad: cout=%d needs %d bytes of shared memory", cout, smem);
-  CVB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  CVB_CHECK_CUDA(opt_in_smem(fn, smem));
   void* kargs[1] = {&a};
   const dim3 grid((unsigned)splits, (unsigned)ntaps, (unsigned)(cblocks * a.nblocks));
   CVB_CHECK_CUDA(cudaLaunchKernel(fn, grid, dim3(kTThreads), kargs, (size_t)smem, as_stream(stream)));
@@ -1257,17 +1244,25 @@ extern "C" int cvb_train_conv_wgrad_pad(const void* x, const void* dy, int32_t B
   return train_conv_wgrad(x, dy, B, H, W, cin, cout, k, 1, pad, dw, stream);
 }
 
-// reduction kernels: `np` pixel lanes per CTA, at least ~4 pixels per thread, at most four CTAs per SM (2C global atomics per CTA)
+// Grids of the reduction and element-wise kernels; 0 when there is no device (sm_count() has set CVB_ERR_NO_DEVICE, which the caller
+// returns).  Reduction kernels: `np` pixel lanes per CTA, at least ~4 pixels per thread, at most four CTAs per SM (2C global atomics per CTA).
 static int red_grid(long long npix, int np) {
   long long g = (npix + (long long)np * 4 - 1) / ((long long)np * 4);
-  const long long cap = (long long)num_sms() * 4;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+  const long long cap = (long long)sm_count() * 4;
+  return (int)(cap == 0 ? 0 : g < 1 ? 1 : (g > cap ? cap : g));
 }
 
 static int ew_grid(long long work_items) {
   long long g = (work_items + kEwThreads - 1) / kEwThreads;
-  const long long cap = (long long)num_sms() * 8;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+  const long long cap = (long long)sm_count() * 8;
+  return (int)(cap == 0 ? 0 : g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// the npix / C rule of the SyncBatchNorm entry points (one lane per 8 channels of a kEwThreads-thread CTA)
+static int check_bn_shape(const char* fn, int64_t npix, int32_t C) {
+  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "%s: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)", fn,
+              (long long)npix, C);
+  return CVB_OK;
 }
 
 extern "C" int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const float* gamma, const float* beta, float eps, float momentum, float* running_mean,
@@ -1277,7 +1272,9 @@ extern "C" int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const 
   CVB_CHECK_CUDA(cudaMemsetAsync(sums_scratch, 0, 2 * (size_t)C * sizeof(float), st));
   const int np = kEwThreads / (C / 8) > 0 ? kEwThreads / (C / 8) : 1;
   CVB_REQUIRE(C / 8 <= kEwThreads, "train_bn_stats: C too large");
-  bn_stats_kernel<<<red_grid(npix, np), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
+  const int grid = red_grid(npix, np);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  bn_stats_kernel<<<grid, kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
   bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, st>>>(sums_scratch, static_cast<const __nv_bfloat16*>(y), npix, C, gamma, beta, eps, momentum, running_mean, running_var, stat);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
@@ -1287,7 +1284,9 @@ extern "C" int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const 
 extern "C" int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream) {
   CVB_REQUIRE(y && stat && out && C % 8 == 0, "train_bn_silu_fwd: bad argument");
   const long long nvec = npix * (C / 8);
-  bn_silu_fwd_kernel<<<ew_grid(nvec), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(y), nvec, C, stat, static_cast<__nv_bfloat16*>(out));
+  const int grid = ew_grid(nvec);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  bn_silu_fwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(y), nvec, C, stat, static_cast<__nv_bfloat16*>(out));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
@@ -1295,8 +1294,9 @@ extern "C" int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, con
 
 static int bn_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, cudaStream_t st) {
   CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 2 * (size_t)C * sizeof(float), st));
-  const int np = kEwThreads / (C / 8);
-  bn_silu_bwd_reduce_kernel<<<red_grid(npix, np), kEwThreads, 0, st>>>(
+  const int grid = red_grid(npix, kEwThreads / (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  bn_silu_bwd_reduce_kernel<<<grid, kEwThreads, 0, st>>>(
       static_cast<const __nv_bfloat16*>(g), static_cast<const __nv_bfloat16*>(y), npix, C, stat, g_is_dz, sums);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1307,13 +1307,15 @@ static int bn_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t 
 static int bn_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, const float* sums,
                         const double* count, void* dy, cudaStream_t st) {
   const long long nvec = npix * (C / 8);
+  const int grid = ew_grid(nvec);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
   const auto* gb = static_cast<const __nv_bfloat16*>(g);
   const auto* yb = static_cast<const __nv_bfloat16*>(y);
   auto* dyb = static_cast<__nv_bfloat16*>(dy);
   if (count == nullptr)
-    bn_silu_bwd_apply_kernel<false><<<ew_grid(nvec), kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, (float)(1.0 / (double)npix), nullptr, g_is_dz, dyb);
+    bn_silu_bwd_apply_kernel<false><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, (float)(1.0 / (double)npix), nullptr, g_is_dz, dyb);
   else
-    bn_silu_bwd_apply_kernel<true><<<ew_grid(nvec), kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, 0.0f, count, g_is_dz, dyb);
+    bn_silu_bwd_apply_kernel<true><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, 0.0f, count, g_is_dz, dyb);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
@@ -1330,12 +1332,14 @@ extern "C" int cvb_train_bn_silu_bwd(const void* g, int32_t g_is_dz, const void*
 // ---- SyncBatchNorm: the statistics and the backward split where a collective sits between the two halves
 extern "C" int cvb_train_bn_partial(const void* y, int64_t npix, int32_t C, float* sums_scratch, double* record, void* stream) {
   CVB_REQUIRE(y && sums_scratch && record, "train_bn_partial: null pointer");
-  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_partial: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
-              (long long)npix, C);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(y) & 15) == 0 && (reinterpret_cast<uintptr_t>(record) & 7) == 0, "train_bn_partial: y must be 16-byte, record 8-byte aligned");
+  const int rc = check_bn_shape("train_bn_partial", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(y, 16) && is_aligned(record, 8), "train_bn_partial: y must be 16-byte, record 8-byte aligned");
   cudaStream_t st = as_stream(stream);
   CVB_CHECK_CUDA(cudaMemsetAsync(sums_scratch, 0, 2 * (size_t)C * sizeof(float), st));
-  bn_stats_kernel<<<red_grid(npix, kEwThreads / (C / 8)), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
+  const int grid = red_grid(npix, kEwThreads / (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  bn_stats_kernel<<<grid, kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(y), npix, C, sums_scratch);
   bn_partial_kernel<<<ceil_div(C, 128), 128, 0, st>>>(sums_scratch, static_cast<const __nv_bfloat16*>(y), npix, C, record);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
@@ -1347,7 +1351,7 @@ extern "C" int cvb_train_bn_merge(const double* records, int32_t world, int32_t 
   CVB_REQUIRE(records && gamma && beta && stat && count, "train_bn_merge: null pointer");
   CVB_REQUIRE((running_mean == nullptr) == (running_var == nullptr), "train_bn_merge: running_mean and running_var go together");
   CVB_REQUIRE(world >= 1 && C > 0 && C % 8 == 0 && C <= 2048, "train_bn_merge: world must be >= 1 and C a multiple of 8 up to 2048 (world=%d C=%d)", world, C);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(records) | reinterpret_cast<uintptr_t>(count)) & 7) == 0, "train_bn_merge: records / count must be 8-byte aligned");
+  CVB_REQUIRE(is_aligned(records, 8) && is_aligned(count, 8), "train_bn_merge: records / count must be 8-byte aligned");
   bn_merge_kernel<<<ceil_div(C, 128), 128, 0, as_stream(stream)>>>(records, world, C, gamma, beta, eps, momentum, running_mean, running_var, stat, count);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1356,26 +1360,26 @@ extern "C" int cvb_train_bn_merge(const double* records, int32_t world, int32_t 
 
 extern "C" int cvb_train_bn_silu_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream) {
   CVB_REQUIRE(g && y && stat && sums, "train_bn_silu_bwd_reduce: null pointer");
-  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd_reduce: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
-              (long long)npix, C);
-  return bn_bwd_reduce(g, g_is_dz, y, npix, C, stat, sums, as_stream(stream));
+  const int rc = check_bn_shape("train_bn_silu_bwd_reduce", npix, C);
+  return rc != CVB_OK ? rc : bn_bwd_reduce(g, g_is_dz, y, npix, C, stat, sums, as_stream(stream));
 }
 
 extern "C" int cvb_train_bn_silu_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma,
                                            const float* sums, const double* count, void* dy, void* stream) {
   CVB_REQUIRE(g && y && stat && gamma && sums && count && dy, "train_bn_silu_bwd_apply: null pointer");
-  CVB_REQUIRE(npix > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads, "train_bn_silu_bwd_apply: npix must be > 0 and C a multiple of 8 up to 2048 (npix=%lld C=%d)",
-              (long long)npix, C);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(count) & 7) == 0, "train_bn_silu_bwd_apply: count must be 8-byte aligned");
+  const int rc = check_bn_shape("train_bn_silu_bwd_apply", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(count, 8), "train_bn_silu_bwd_apply: count must be 8-byte aligned");
   return bn_bwd_apply(g, g_is_dz, y, npix, C, stat, gamma, sums, count, dy, as_stream(stream));
 }
 
 extern "C" int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32_t W, void* out, void* stream) {
   CVB_REQUIRE(img && out && B > 0 && H > 0 && W > 0, "train_focus_s2d: bad argument");
   CVB_REQUIRE(H % 2 == 0 && W % 2 == 0, "train_focus_s2d: H and W must be even (H=%d W=%d)", H, W);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(img) & 7) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "train_focus_s2d: img must be 8-byte, out 16-byte aligned");
-  const long long n = (long long)B * (H / 2) * (W / 2);
-  focus_s2d_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(img, B, H, W, static_cast<__nv_bfloat16*>(out));
+  CVB_REQUIRE(is_aligned(img, 8) && is_aligned(out, 16), "train_focus_s2d: img must be 8-byte, out 16-byte aligned");
+  const int grid = ew_grid((long long)B * (H / 2) * (W / 2));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  focus_s2d_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(img, B, H, W, static_cast<__nv_bfloat16*>(out));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
@@ -1384,10 +1388,10 @@ extern "C" int cvb_train_focus_s2d(const float* img, int32_t B, int32_t H, int32
 extern "C" int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream) {
   CVB_REQUIRE(a && cat && idx && B > 0 && H > 0 && W > 0 && C > 0, "train_spp_pool_fwd: bad argument");
   CVB_REQUIRE(C % 8 == 0, "train_spp_pool_fwd: C must be a multiple of 8 (C=%d)", C);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0 && (reinterpret_cast<uintptr_t>(idx) & 7) == 0,
-              "train_spp_pool_fwd: a / cat must be 16-byte, idx 8-byte aligned");
-  const long long n = (long long)B * H * W * (C / 8);
-  spp_pool_fwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat),
+  CVB_REQUIRE(is_aligned(a, 16) && is_aligned(cat, 16) && is_aligned(idx, 8), "train_spp_pool_fwd: a / cat must be 16-byte, idx 8-byte aligned");
+  const int grid = ew_grid((long long)B * H * W * (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  spp_pool_fwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat),
                                                                          static_cast<uint8_t*>(idx));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1397,10 +1401,10 @@ extern "C" int cvb_train_spp_pool_fwd(const void* a, int32_t B, int32_t H, int32
 extern "C" int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, void* da, void* stream) {
   CVB_REQUIRE(g && idx && da && B > 0 && H > 0 && W > 0 && C > 0, "train_spp_pool_bwd: bad argument");
   CVB_REQUIRE(C % 8 == 0, "train_spp_pool_bwd: C must be a multiple of 8 (C=%d)", C);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da)) & 15) == 0 && (reinterpret_cast<uintptr_t>(idx) & 7) == 0,
-              "train_spp_pool_bwd: g / da must be 16-byte, idx 8-byte aligned");
-  const long long n = (long long)B * H * W * (C / 8);
-  spp_pool_bwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), static_cast<const uint8_t*>(idx), B, H, W, C,
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(da, 16) && is_aligned(idx, 8), "train_spp_pool_bwd: g / da must be 16-byte, idx 8-byte aligned");
+  const int grid = ew_grid((long long)B * H * W * (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  spp_pool_bwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), static_cast<const uint8_t*>(idx), B, H, W, C,
                                                                          static_cast<__nv_bfloat16*>(da));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1410,11 +1414,13 @@ extern "C" int cvb_train_spp_pool_bwd(const void* g, const void* idx, int32_t B,
 extern "C" int cvb_train_sppf_chain_fwd(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, void* cat, void* idx, void* stream) {
   CVB_REQUIRE(a && cat && idx && B > 0 && H > 0 && W > 0 && C > 0, "train_sppf_chain_fwd: bad argument");
   CVB_REQUIRE(C % 8 == 0, "train_sppf_chain_fwd: C must be a multiple of 8 (C=%d)", C);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0, "train_sppf_chain_fwd: a / cat must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(a, 16) && is_aligned(cat, 16), "train_sppf_chain_fwd: a / cat must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
   const long long n = (long long)B * H * W * C;
-  spp_pool_fwd_kernel<<<ew_grid(n / 8), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat), nullptr);
-  sppf_chain_idx_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(cat), B, H, W, C, static_cast<uint8_t*>(idx));
+  const int pool_grid = ew_grid(n / 8), idx_grid = ew_grid(n);
+  if (pool_grid == 0 || idx_grid == 0) return CVB_ERR_NO_DEVICE;
+  spp_pool_fwd_kernel<<<pool_grid, kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(a), B, H, W, C, static_cast<__nv_bfloat16*>(cat), nullptr);
+  sppf_chain_idx_kernel<<<idx_grid, kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(cat), B, H, W, C, static_cast<uint8_t*>(idx));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
   return CVB_OK;
@@ -1422,15 +1428,16 @@ extern "C" int cvb_train_sppf_chain_fwd(const void* a, int32_t B, int32_t H, int
 
 extern "C" int cvb_train_sppf_chain_bwd(const void* g, const void* idx, int32_t B, int32_t H, int32_t W, int32_t C, float* scratch, void* da, void* stream) {
   CVB_REQUIRE(g && idx && scratch && da && B > 0 && H > 0 && W > 0 && C > 0, "train_sppf_chain_bwd: bad argument");
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da) | reinterpret_cast<uintptr_t>(scratch)) & 3) == 0,
-              "train_sppf_chain_bwd: g / scratch / da must be 4-byte aligned");
+  CVB_REQUIRE(is_aligned(g, 4) && is_aligned(da, 4) && is_aligned(scratch, 4), "train_sppf_chain_bwd: g / scratch / da must be 4-byte aligned");
   cudaStream_t st = as_stream(stream);
   const long long n = (long long)B * H * W * C;
+  const int grid = ew_grid(n);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
   const __nv_bfloat16* gb = static_cast<const __nv_bfloat16*>(g);
   const uint8_t* ib = static_cast<const uint8_t*>(idx);
-  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 2, nullptr, scratch, nullptr, B, H, W, C);
-  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 1, scratch, scratch + n, nullptr, B, H, W, C);
-  sppf_chain_bwd_kernel<<<ew_grid(n), kEwThreads, 0, st>>>(gb, ib, 0, scratch + n, nullptr, static_cast<__nv_bfloat16*>(da), B, H, W, C);
+  sppf_chain_bwd_kernel<<<grid, kEwThreads, 0, st>>>(gb, ib, 2, nullptr, scratch, nullptr, B, H, W, C);
+  sppf_chain_bwd_kernel<<<grid, kEwThreads, 0, st>>>(gb, ib, 1, scratch, scratch + n, nullptr, B, H, W, C);
+  sppf_chain_bwd_kernel<<<grid, kEwThreads, 0, st>>>(gb, ib, 0, scratch + n, nullptr, static_cast<__nv_bfloat16*>(da), B, H, W, C);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(3);
   return CVB_OK;
@@ -1439,10 +1446,10 @@ extern "C" int cvb_train_sppf_chain_bwd(const void* g, const void* idx, int32_t 
 extern "C" int cvb_train_upsample_cat_fwd(const void* a, int32_t B, int32_t h, int32_t w, int32_t Ca, const void* b, int32_t Cb, void* cat, void* stream) {
   CVB_REQUIRE(a && b && cat && B > 0 && h > 0 && w > 0 && Ca > 0 && Cb > 0, "train_upsample_cat_fwd: bad argument");
   CVB_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "train_upsample_cat_fwd: channels must be multiples of 8 (Ca=%d Cb=%d)", Ca, Cb);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(cat)) & 15) == 0,
-              "train_upsample_cat_fwd: pointers must be 16-byte aligned");
-  const long long n = (long long)B * 4 * h * w * ((Ca + Cb) / 8);
-  upsample_cat_fwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, h, w, Ca, static_cast<const __nv_bfloat16*>(b),
+  CVB_REQUIRE(is_aligned(a, 16) && is_aligned(b, 16) && is_aligned(cat, 16), "train_upsample_cat_fwd: pointers must be 16-byte aligned");
+  const int grid = ew_grid((long long)B * 4 * h * w * ((Ca + Cb) / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  upsample_cat_fwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(a), B, h, w, Ca, static_cast<const __nv_bfloat16*>(b),
                                                                              Cb, static_cast<__nv_bfloat16*>(cat));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1452,10 +1459,10 @@ extern "C" int cvb_train_upsample_cat_fwd(const void* a, int32_t B, int32_t h, i
 extern "C" int cvb_train_upsample_cat_bwd(const void* g, int32_t B, int32_t h, int32_t w, int32_t Ca, int32_t Cb, void* da, void* db, void* stream) {
   CVB_REQUIRE(g && da && db && B > 0 && h > 0 && w > 0 && Ca > 0 && Cb > 0, "train_upsample_cat_bwd: bad argument");
   CVB_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "train_upsample_cat_bwd: channels must be multiples of 8 (Ca=%d Cb=%d)", Ca, Cb);
-  CVB_REQUIRE(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(da) | reinterpret_cast<uintptr_t>(db)) & 15) == 0,
-              "train_upsample_cat_bwd: pointers must be 16-byte aligned");
-  const long long n = (long long)B * h * w * (Ca / 8) + (long long)B * 4 * h * w * (Cb / 8);
-  upsample_cat_bwd_kernel<<<ew_grid(n), kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), B, h, w, Ca, Cb, static_cast<__nv_bfloat16*>(da),
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(da, 16) && is_aligned(db, 16), "train_upsample_cat_bwd: pointers must be 16-byte aligned");
+  const int grid = ew_grid((long long)B * h * w * (Ca / 8) + (long long)B * 4 * h * w * (Cb / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  upsample_cat_bwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(g), B, h, w, Ca, Cb, static_cast<__nv_bfloat16*>(da),
                                                                              static_cast<__nv_bfloat16*>(db));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1467,11 +1474,12 @@ extern "C" int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int
   CVB_REQUIRE(g && dy && dbias && B > 0 && h > 0 && w > 0, "train_pred_grad: bad argument");
   CVB_REQUIRE(cout > 0 && cout_pad == pred_cout_pad(cout), "train_pred_grad: cout_pad must be the next training width of cout (cout=%d cout_pad=%d)", cout, cout_pad);
   CVB_REQUIRE(c_off >= 0 && c_off + cout <= c_tot, "train_pred_grad: channels [%d, %d) outside the %d-channel gradient", c_off, c_off + cout, c_tot);
-  CVB_REQUIRE((reinterpret_cast<uintptr_t>(dy) & 15) == 0 && ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dbias)) & 3) == 0,
-              "train_pred_grad: dy must be 16-byte, g / dbias 4-byte aligned");
+  CVB_REQUIRE(is_aligned(dy, 16) && is_aligned(g, 4) && is_aligned(dbias, 4), "train_pred_grad: dy must be 16-byte, g / dbias 4-byte aligned");
   cudaStream_t st = as_stream(stream);
   const long long hw = (long long)h * w;
-  pred_grad_nhwc_kernel<<<ew_grid((long long)B * hw * (cout_pad / 8)), kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, cout, cout_pad, static_cast<__nv_bfloat16*>(dy));
+  const int grid = ew_grid((long long)B * hw * (cout_pad / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  pred_grad_nhwc_kernel<<<grid, kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, cout, cout_pad, static_cast<__nv_bfloat16*>(dy));
   pred_bias_grad_kernel<<<cout, kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, dbias);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);

@@ -18,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._lib import _stream
 
 
 def is_parallel(model):
@@ -98,8 +99,7 @@ class ModelEMA:
         dev = devices.pop()
         with torch.cuda.device(dev):
             table = torch.empty((len(pairs) * _lib.CVB_EMA_TABLE_ENTRY_BYTES,), dtype=torch.uint8, device=dev)
-            _lib.check(_lib.lib().cvb_ema_table_upload(entries, len(pairs), table.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                       'cvb_ema_table_upload')
+            _lib.check(_lib.lib().cvb_ema_table_upload(entries, len(pairs), table.data_ptr(), _stream()), 'cvb_ema_table_upload')
         return table, len(pairs)
 
     def update(self, model):
@@ -118,7 +118,7 @@ class ModelEMA:
                 self._sig = sig
             table, n = self._table
             with torch.cuda.device(table.device):
-                _lib.check(_lib.lib().cvb_ema_update(table.data_ptr(), n, d, 1 - d, torch.cuda.current_stream().cuda_stream), 'cvb_ema_update')
+                _lib.check(_lib.lib().cvb_ema_update(table.data_ptr(), n, d, 1 - d, _stream()), 'cvb_ema_update')
 
     def update_attr(self, model, include=(), exclude=('process_group', 'reducer')):
         copy_attr(self.ema, model, include, exclude)

@@ -10,13 +10,9 @@ import torch
 
 from . import _lib
 from ._lib import (CVB_ACT_NONE, CVB_ACT_RELU, CVB_ACT_SILU, CVB_OUT_F32, CVB_OUT_SPLIT16, CVB_OUT_YOLO, CvbConvDesc, CvbNmsParams, CvbView,
-                   CvbYoloDecode)
+                   CvbYoloDecode, _stream)
 
 ACTS = {None: CVB_ACT_NONE, 'none': CVB_ACT_NONE, 'silu': CVB_ACT_SILU, 'swish': CVB_ACT_SILU, 'relu': CVB_ACT_RELU}
-
-
-def _stream():
-    return c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _require_cuda(t, what):

@@ -26,6 +26,7 @@ device, when a group's momentum turns on or off, or when the set of params with 
 import torch
 
 from . import _lib
+from ._lib import _p, _stream
 
 
 def _refuse(group, gi):
@@ -115,7 +116,7 @@ class SGD(torch.optim.SGD):
         with torch.cuda.device(dev):
             table = torch.empty((len(rows) * _lib.CVB_SGD_TABLE_ENTRY_BYTES,), dtype=torch.uint8, device=dev)
             _lib.check(_lib.lib().cvb_sgd_table_upload((_lib.CvbSgdEntry * len(rows))(*rows), len(rows), n_groups, table.data_ptr(),
-                                                       torch.cuda.current_stream().cuda_stream), 'cvb_sgd_table_upload')
+                                                       _stream()), 'cvb_sgd_table_upload')
         self.table_builds += 1
         return table, len(rows)
 
@@ -164,9 +165,7 @@ class SGD(torch.optim.SGD):
         table, n = self._table
         with torch.cuda.device(table.device):
             _lib.check(_lib.lib().cvb_sgd_step(table.data_ptr(), n, (_lib.CvbSgdGroup * len(hyper))(*hyper), len(hyper),
-                                               grad_scale.data_ptr() if grad_scale is not None else None,
-                                               found_inf.data_ptr() if found_inf is not None else None,
-                                               torch.cuda.current_stream().cuda_stream), 'cvb_sgd_step')
+                                               _p(grad_scale), _p(found_inf), _stream()), 'cvb_sgd_step')
         return loss
 
     def state_dict(self):

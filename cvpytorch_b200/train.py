@@ -31,14 +31,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+from ._lib import _p, _stream
 
 
 def _ptrs(ts):
