@@ -7,8 +7,8 @@
 //                       then target), compacted with a block scan, with the clamped cell, tbox = gxy - clamped cell, the anchor and the class.
 //   2. v5_rank_kernel   the stable sort of the candidates by cell: rank = #(cell, index) pairs before the candidate's (exact, no atomics).
 //   3. v5_term_kernel   one thread per candidate: CIoU of the decoded prediction, 1 - CIoU and the class BCE sum.
-//   4. v5_seg_kernel    one thread per sorted position; the first of each cell's run takes the last candidate in candidate order (the
-//                       reference's index_put_ on the CPU: last write wins) for tobj = (1 - gr) + gr * clamp(CIoU, 0), and the objectness
+//   4. v5_seg_kernel    one thread per sorted position; the first of each cell's run takes the last candidate in candidate order (last write
+//                       wins, as the reference's index_put_ does while it runs serially) for tobj = (1 - gr) + gr * clamp(CIoU, 0), and the objectness
 //                       correction BCE(x, tobj) - BCE(x, 0) of that cell.
 //   5. v5_obj_kernel    every objectness logit: BCE(x, 0), summed per CTA (block_sum).
 //   6. v5_final_kernel  one CTA: the per-level means from fp64 sums (block_sum) -> loss, lbox, lobj, lcls.

@@ -4,7 +4,9 @@ objectness and class BCE terms, in fp32 torch so that torch.autograd gives the r
 Differences from the reference, all where the reference cannot run or is undefined:
   - the in-place clamp of the grid cell uses integer bounds (the reference's float bounds raise on current torch; older torch did this);
   - a class outside [0, nc) gets no one-hot entry and an image index outside [0, B) matches nothing (the reference raises IndexError);
-  - the objectness target of a cell hit by several candidates is the last one's, in candidate order (index_put_ on the CPU; run on the CPU).
+  - the objectness target of a cell hit by several candidates is the last one's, in candidate order.  The reference's index_put_ leaves
+    the winner of duplicate indices unspecified: on the CPU it is the last write only while the copy runs serially, which stops at a
+    few thousand candidates (a 64-image batch with 2 to 20 targets per image passes it).
 """
 import torch
 import torch.nn.functional as F
@@ -75,8 +77,7 @@ def bbox_ciou(box1, box2, eps=1e-7):
 
 
 def yolov5_loss(preds, targets, anchors, num_classes, hyp_box=0.05, hyp_obj=1.0, hyp_cls=0.5, balance=(4.0, 1.0, 0.4), gr=1.0, anchor_t=4.0):
-    """preds: fp32 NCHW [B, na (5 + nc), ny, nx] (requires_grad for the gradient; on the CPU, where index_put_ keeps the last write of a
-    cell).  -> (loss [1], items [3], the build_targets lists)."""
+    """preds: fp32 NCHW [B, na (5 + nc), ny, nx] (requires_grad for the gradient).  -> (loss [1], items [3], the build_targets lists)."""
     na, no = anchors.shape[1], num_classes + 5
     B, dev = preds[0].shape[0], preds[0].device
     p = [x.view(B, na, no, x.shape[2], x.shape[3]).permute(0, 1, 3, 4, 2) for x in preds]
@@ -96,7 +97,11 @@ def yolov5_loss(preds, targets, anchors, num_classes, hyp_box=0.05, hyp_obj=1.0,
             iou = bbox_ciou(torch.cat((pxy, pwh), 1).T, tbox)
             lbox += (1.0 - iou).mean()
             score_iou = iou.detach().clamp(0).type(tobj.dtype)
-            tobj[b, a, gj, gi] = (1.0 - gr) + gr * score_iou
+            cell = ((b * na + a) * pi.shape[2] + gj) * pi.shape[3] + gi  # (the last candidate of each cell sets its target)
+            order = torch.arange(n, device=dev)
+            last = torch.full((tobj.numel(),), -1, dtype=torch.long, device=dev).scatter_reduce(0, cell, order, 'amax')
+            win = last[cell] == order
+            tobj[b[win], a[win], gj[win], gi[win]] = ((1.0 - gr) + gr * score_iou)[win]
             if num_classes > 1:
                 t = torch.zeros_like(ps[:, 5:])
                 ok = (c >= 0) & (c < num_classes)

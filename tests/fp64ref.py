@@ -83,19 +83,97 @@ def choose_box128(B, H, W):
 
 
 def wgrad_split(B, Ho, Wo, cin, cout, k, sms):
-    """Restates cvb_train_conv_wgrad's launch: -> (m_tiles, splits, per), `per` = 128-pixel tiles one CTA accumulates before its atomics."""
+    """Restates cvb_train_conv_wgrad's launch: -> (m_tiles, splits, per), `per` = 128-pixel tiles one CTA accumulates before its atomics.
+    cout = 16 or 32 runs as one 64-wide block."""
     tw, th, nb = choose_box128(B, Ho, Wo)
     m_tiles = -(-Wo // tw) * -(-Ho // th) * -(-B // nb)
     npan = 4 if (cout // 64) % 4 == 0 else (2 if (cout // 64) % 2 == 0 else 1)
-    splits = (2 * sms) // (k * k * -(-cin // 128) * (cout // (64 * npan)))
+    nblocks = 1 if cout < 64 else cout // (64 * npan)
+    splits = (2 * sms) // (k * k * -(-cin // 128) * nblocks)
     splits = min(max(splits, 1), m_tiles)
     return m_tiles, splits, -(-m_tiles // splits)
 
 
+def red_chain(npix, C, sms):
+    """Longest fp32 addition chain of one channel's sum in bn_stats_kernel / bn_silu_bwd_reduce_kernel (csrc/train_kernels.cu red_grid):
+    the pixels of one thread (+1 for the paired loads), the CTA's pixel lanes, one atomic per CTA."""
+    lanes = 256 // (C // 8)
+    grid = min(max(-(-npix // (lanes * 4)), 1), sms * 4)
+    return -(-(-(-npix // grid)) // lanes) + 1 + lanes + grid
+
+
 def wgrad_gamma(B, Ho, Wo, cin, cout, k, sms):
-    """One CTA chains 8 MMAs (K = 16 pixels each) per tile it owns; `splits` CTAs then add their partial sums with fp32 atomics."""
+    """One CTA chains 8 MMAs (K = 16 pixels each) per tile it owns; `splits` CTAs then add their partial sums with fp32 atomics (every
+    width: cout = 16 / 32 runs as one 64-wide block)."""
     _, splits, per = wgrad_split(B, Ho, Wo, cin, cout, k, sms)
     return (8 * per + 16 + splits) * U23
+
+
+# ---------------------------------------------------------------------------------------------------- BatchNorm + SiLU training passes
+# Each kernel is compared with float64 of the operation it computes, from the statistics / sums the previous kernel produced; the bounds
+# propagate the summation bound gs (relative to the sum of |terms|: (red_chain + 2) * 2^-24 for the pivoted fp32 sums, see
+# tests/test_train_gpu.py) and one 2^-24 rounding per fp32 operation.  y, da: [npix, C] bf16; stat [4][C] = mean, rstd, scale, shift.
+def bn_stats_check(y, gamma, beta, rm0, rv0, eps, mom, stat, rm, rv, gs):
+    """cvb_train_bn_stats' statistics and running statistics (rm0 / rv0 before, rm / rv after) -> {name: worst |error| / bound}."""
+    u = U24
+    y64, n = y.double(), float(y.shape[0])
+    mean, var = y64.mean(0), y64.var(0, unbiased=False)
+    d = y64 - y64[0]
+    d_abs, d_sq, d_mean = d.abs().mean(0), (d * d).mean(0), d.mean(0)
+    del d
+    e_mean = gs * d_abs + u * mean.abs()
+    e_var = gs * d_sq + 2 * d_mean.abs() * gs * d_abs
+    rstd = 1 / torch.sqrt(var + eps)
+    e_rstd = rstd * (0.5 * e_var / (var + eps) + 2 * u)
+    g64, b64 = gamma.double(), beta.double()
+    scale = g64 * rstd
+    e_scale = g64 * e_rstd + u * scale
+    e_shift = mean.abs() * e_scale + scale * e_mean + 2 * u * ((mean * scale).abs() + b64.abs())
+    r = {'mean': check(stat[0], mean, e_mean, 'mean'), 'rstd': check(stat[1], rstd, e_rstd, 'rstd'),
+         'scale': check(stat[2], scale, e_scale, 'scale'), 'shift': check(stat[3], b64 - mean * scale, e_shift, 'shift')}
+    m = float(torch.tensor(mom, dtype=torch.float32))
+    var_unb = var * n / max(n - 1, 1)
+    rm_ref, rv_ref = (1 - m) * rm0.double() + m * mean, (1 - m) * rv0.double() + m * var_unb
+    r['running_mean'] = check(rm, rm_ref, m * e_mean + 4 * u * ((1 - m) * rm0.double().abs() + m * mean.abs()), 'running_mean')
+    r['running_var'] = check(rv, rv_ref, m * (e_var * n / max(n - 1, 1) + u * var_unb) + 4 * u * rv_ref, 'running_var')
+    return r
+
+
+def bn_silu_fwd_check(y, stat, a):
+    """a = silu(y * scale + shift) with the kernel's scale / shift: one fma, __expf, an addition and a division, bf16 store."""
+    z = y.double() * stat[2].double() + stat[3].double()
+    a_ref = z * torch.sigmoid(z)
+    return {'a': check(a, a_ref, BF16_REL * a_ref.abs() + (1 + BF16_REL) * (a_ref.abs() * sigmoid_rel_err(z) + 1.1 * U24 * z.abs()), 'a')}
+
+
+def bn_silu_bwd_check(da, is_dz, y, gamma, stat, sums, dy, gs, gs_sum=None):
+    """cvb_train_bn_silu_bwd with the kernel's mean / rstd / scale / shift: dz = g * silu'(z) (or g when is_dz), xhat = (y - mean) * rstd;
+    sums = (sum dz, sum dz * xhat), dy.  gs_sum: the summation bound of sum dz alone (default gs; 0 where that sum is exact)."""
+    u = U24
+    gs_sum = gs if gs_sum is None else gs_sum
+    y64, n = y.double(), float(y.shape[0])
+    xhat = (y64 - stat[0].double()) * stat[1].double()
+    g64d = da.double()
+    if is_dz:
+        dz, e_dz = g64d, torch.zeros_like(g64d)
+    else:
+        z = y64 * stat[2].double() + stat[3].double()
+        dz = g64d * silu_grad64(z)
+        e_dz = g64d.abs() * silu_grad_err(z) + u * dz.abs()
+        del z
+    tag = ' (g = dz)' if is_dz else ''
+    r = {'sum dz' + tag: check(sums[0], dz.sum(0), gs_sum * dz.abs().sum(0) + e_dz.sum(0), 'sum dz' + tag)}
+    dzx = (dz * xhat).abs()
+    r['sum dz*xhat' + tag] = check(sums[1], (dz * xhat).sum(0), (gs + 3 * u) * dzx.sum(0) + (e_dz * xhat.abs()).sum(0), 'sum dz*xhat' + tag)
+    del dzx
+    # dy = gamma * rstd * (dz - S0 / n - xhat * S1 / n) from the kernel's sums: about eight fp32 roundings of terms of that size
+    S0, S1 = sums[0].double() / n, sums[1].double() / n
+    g64 = gamma.double()
+    gr = (g64 * stat[1].double()).abs()
+    dy_ref = g64 * stat[1].double() * (dz - S0 - xhat * S1)
+    bound = BF16_REL * dy_ref.abs() + (1 + BF16_REL) * gr * (e_dz + 8 * u * (dz.abs() + S0.abs() + (xhat * S1).abs()))
+    r['dy' + tag] = check(dy, dy_ref, bound, 'dy' + tag)
+    return r
 
 
 # ---------------------------------------------------------------------------------------------------- split-fp16 inference conv

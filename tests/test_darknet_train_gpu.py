@@ -50,17 +50,6 @@ def _kpad(c):
     return -(-c // 64) * 64
 
 
-def _wgrad_gamma(B, Ho, Wo, cin, cout, k, sms):
-    """fp64ref.wgrad_gamma for every width: cout = 16 / 32 runs as one 64-wide block."""
-    if cout >= 64:
-        return R.wgrad_gamma(B, Ho, Wo, cin, cout, k, sms)
-    TW, TH, NB = R.choose_box128(B, Ho, Wo)
-    m_tiles = -(-Wo // TW) * -(-Ho // TH) * -(-B // NB)
-    splits = min(max((2 * sms) // (k * k * -(-cin // 128)), 1), m_tiles)
-    per = -(-m_tiles // splits)
-    return (8 * per + 16 + splits) * R.U23
-
-
 # (B, H, W, cin, cout, k, stride): 16 / 32-channel K chunks and N tiles in every pass; odd maps, B = 5, a 1x1 map under stride 2, and the
 # stem / stage1 shapes of YOLOX-n and -s at a small image
 @pytest.mark.parametrize('B,H,W,cin,cout,k,stride', [(2, 13, 9, 16, 32, 3, 1), (5, 7, 11, 32, 64, 3, 2), (3, 26, 18, 16, 32, 3, 2), (2, 9, 7, 64, 32, 1, 1),
@@ -104,7 +93,7 @@ def test_narrow_conv_forward_backward_data_backward_weight(cuda, B, H, W, cin, c
     dwr, dwa = R.conv_wgrad(xd, dy, wd.shape, stride, k // 2)
     g_f = R.mma_gamma(k * k * _kpad(cin))
     g_d = R.mma_gamma((k * k if stride == 1 else 4) * _kpad(cout))
-    g_w = _wgrad_gamma(B, Ho, Wo, cin, cout, k, _sms())
+    g_w = R.wgrad_gamma(B, Ho, Wo, cin, cout, k, _sms())
     r = {'y': R.check(yh, yr, R.BF16_REL * yr.abs() + (1 + R.BF16_REL) * g_f * ya, 'forward'),
          'dx': R.check(dxh, dxr, R.BF16_REL * dxr.abs() + (1 + R.BF16_REL) * g_d * dxa, 'backward-data'),
          'dw': R.check(dw, dwr, g_w * dwa, 'backward-weight')}

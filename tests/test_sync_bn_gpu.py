@@ -25,7 +25,6 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fp64ref as R  # noqa: E402
-from test_train_gpu import _red_chain  # noqa: E402
 from test_yolox_train_gpu import _compare, _leaves, _network_models, _network_state, _oracle_named  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -82,7 +81,7 @@ def test_sync_bn_merged_statistics_and_backward_vs_float64(cuda, C, shards, shif
     e_mean, e_m2 = torch.zeros_like(mean), torch.zeros_like(mean)
     for ys in parts:
         ys64, ns = ys.double(), ys.shape[0]
-        gs = (_red_chain(ns, C, _sms()) + 2) * u
+        gs = (R.red_chain(ns, C, _sms()) + 2) * u
         d = ys64 - ys64[0]
         d_abs, d_sq, d_mean = d.abs().sum(0), (d * d).sum(0), d.mean(0)
         e_ms = gs * d_abs / ns
@@ -120,7 +119,7 @@ def test_sync_bn_merged_statistics_and_backward_vs_float64(cuda, C, shards, shif
         tag = ' (g = dz)' if is_dz else ''
         e_tot0, e_tot1 = 0, 0
         for i, (a, b) in enumerate(zip(bounds, bounds[1:])):
-            gs = (_red_chain(b - a, C, _sms()) + 2) * u
+            gs = (R.red_chain(b - a, C, _sms()) + 2) * u
             dzs, dzxs = dz[a:b], dz[a:b] * xhat[a:b]
             e0 = gs * dzs.abs().sum(0) + e_dz[a:b].sum(0)
             e1 = (gs + 3 * u) * dzxs.abs().sum(0) + (e_dz[a:b] * xhat[a:b].abs()).sum(0)

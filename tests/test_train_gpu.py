@@ -17,7 +17,7 @@ per = 2) and 16x40x40 3x3 64->64 (200 tiles of 8x1x16 over 2 * 132 / 9 = 29 spli
 per = 1.
 
 BatchNorm: the statistics are fp32 sums of y - y[0] over a tree of additions (pixels of one thread, the CTA's pixel lanes, one atomic per CTA;
-the longest chain, _red_chain, is 362..724 additions for 102 401 pixels, 19..259 for 129), finalised in double.  A chain of L fp32
+the longest chain, fp64ref.red_chain, is 362..724 additions for 102 401 pixels, 19..259 for 129), finalised in double.  A chain of L fp32
 additions is off by at most L * 2^-24 * sum|terms|; that bound is propagated to mean, variance, rstd, scale, shift and the running statistics
 in test_bn_statistics_silu_forward_backward_vs_float64.  At 102 401 pixels it allows 1e-5..2e-5 relative of rstd per
 (1 + ((y[0] - mean) / std)^2), at 129 pixels 1e-6..8e-6; the one-pass E[y^2] - mean^2 instead loses (mean / std)^2 times the same error."""
@@ -157,14 +157,6 @@ def test_bn_silu_forward_backward_and_fused_silu_grad_epilogue(cuda):
     assert _rel(fused, ref) < 8e-3, _rel(fused, ref)  # (`plain` was rounded to bf16 before the multiplication, `fused` after)
 
 
-def _red_chain(npix, C, sms):
-    """Longest fp32 addition chain of one channel's sum in bn_stats_kernel / bn_silu_bwd_reduce_kernel (csrc/train_kernels.cu red_grid):
-    the pixels of one thread (+1 for the paired loads), the CTA's pixel lanes, one atomic per CTA."""
-    lanes = 256 // (C // 8)
-    grid = min(max(-(-npix // (lanes * 4)), 1), sms * 4)
-    return -(-(-(-npix // grid)) // lanes) + 1 + lanes + grid
-
-
 @pytest.mark.parametrize('shift', [0, 10, 100])
 @pytest.mark.parametrize('npix', [2, 7, 129, 102401])
 @pytest.mark.parametrize('C', [8, 24, 64, 192, 1024, 2048])
@@ -193,60 +185,12 @@ def test_bn_statistics_silu_forward_backward_vs_float64(cuda, C, npix, shift):
     for is_dz in (0, 1):
         _lib.check(L.cvb_train_bn_silu_bwd(T._p(da), is_dz, T._p(y), npix, C, T._p(stat), T._p(gamma), T._p(sums[is_dz]), T._p(dy[is_dz]), T._stream()), 'bwd')
     torch.cuda.synchronize()
-    gs = (_red_chain(npix, C, _sms()) + 2) * u  # + the subtraction of the pivot and the square
-    r = {}
-
-    # statistics: mean, variance of the bf16 values in float64; the kernel sums d = y - y[0]
-    y64, n = y.double(), float(npix)
-    mean, var = y64.mean(0), y64.var(0, unbiased=False)
-    d = y64 - y64[0]
-    d_abs, d_sq, d_mean = d.abs().mean(0), (d * d).mean(0), d.mean(0)
-    del d
-    e_mean = gs * d_abs + u * mean.abs()
-    e_var = gs * d_sq + 2 * d_mean.abs() * gs * d_abs
-    rstd = 1 / torch.sqrt(var + eps)
-    e_rstd = rstd * (0.5 * e_var / (var + eps) + 2 * u)
-    g64, b64 = gamma.double(), beta.double()
-    scale = g64 * rstd
-    e_scale = g64 * e_rstd + u * scale
-    e_shift = mean.abs() * e_scale + scale * e_mean + 2 * u * ((mean * scale).abs() + b64.abs())
-    r['mean'] = R.check(stat[0], mean, e_mean, 'mean')
-    r['rstd'] = R.check(stat[1], rstd, e_rstd, 'rstd')
-    r['scale'] = R.check(stat[2], scale, e_scale, 'scale')
-    r['shift'] = R.check(stat[3], b64 - mean * scale, e_shift, 'shift')
-    m = float(np.float32(mom))
-    var_unb = var * n / max(n - 1, 1)
-    rm_ref, rv_ref = (1 - m) * rm0.double() + m * mean, (1 - m) * rv0.double() + m * var_unb
-    r['running_mean'] = R.check(rm, rm_ref, m * e_mean + 4 * u * ((1 - m) * rm0.double().abs() + m * mean.abs()), 'running_mean')
-    r['running_var'] = R.check(rv, rv_ref, m * (e_var * n / max(n - 1, 1) + u * var_unb) + 4 * u * rv_ref, 'running_var')
-
-    # forward a = silu(y * scale + shift) with the kernel's scale / shift: one fma, __expf, an addition and a division, bf16 store
-    s32, t32 = stat[2].double(), stat[3].double()
-    z = y64 * s32 + t32
-    a_ref = z * torch.sigmoid(z)
-    r['a'] = R.check(a, a_ref, R.BF16_REL * a_ref.abs() + (1 + R.BF16_REL) * (a_ref.abs() * R.sigmoid_rel_err(z) + 1.1 * u * z.abs()), 'a')
-    del a_ref
-
-    # backward with the kernel's mean / rstd / scale / shift: dz = g * silu'(z) (or g), xhat = (y - mean) * rstd
-    xhat = (y64 - stat[0].double()) * stat[1].double()
-    g64d = da.double()
+    gs = (R.red_chain(npix, C, _sms()) + 2) * u  # + the subtraction of the pivot and the square
+    # statistics: mean, variance of the bf16 values in float64 (the kernel sums d = y - y[0]); forward; backward for both kinds of g
+    r = R.bn_stats_check(y, gamma, beta, rm0, rv0, eps, mom, stat, rm, rv, gs)
+    r.update(R.bn_silu_fwd_check(y, stat, a))
     for is_dz in (0, 1):
-        if is_dz:
-            dz, e_dz = g64d, torch.zeros_like(g64d)
-        else:
-            dz = g64d * R.silu_grad64(z)
-            e_dz = g64d.abs() * R.silu_grad_err(z) + u * dz.abs()
-        tag = ' (g = dz)' if is_dz else ''
-        r['sum dz' + tag] = R.check(sums[is_dz][0], dz.sum(0), gs * dz.abs().sum(0) + e_dz.sum(0), 'sum dz' + tag)
-        dzx = (dz * xhat).abs()
-        r['sum dz*xhat' + tag] = R.check(sums[is_dz][1], (dz * xhat).sum(0), (gs + 3 * u) * dzx.sum(0) + (e_dz * xhat.abs()).sum(0), 'sum dz*xhat' + tag)
-        # dy = gamma * rstd * (dz - S0 / n - xhat * S1 / n) from the kernel's sums: about eight fp32 roundings of terms of that size
-        S0, S1 = sums[is_dz][0].double() / n, sums[is_dz][1].double() / n
-        gr = (g64 * stat[1].double()).abs()
-        dy_ref = g64 * stat[1].double() * (dz - S0 - xhat * S1)
-        bound = R.BF16_REL * dy_ref.abs() + (1 + R.BF16_REL) * gr * (e_dz + 8 * u * (dz.abs() + S0.abs() + (xhat * S1).abs()))
-        r['dy' + tag] = R.check(dy[is_dz], dy_ref, bound, 'dy' + tag)
-        del dz, e_dz, dzx, dy_ref, bound
+        r.update(R.bn_silu_bwd_check(da, is_dz, y, gamma, stat, sums[is_dz], dy[is_dz], gs))
     print('worst error / bound', {k: round(v, 3) for k, v in r.items()})
 
 

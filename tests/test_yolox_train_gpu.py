@@ -42,17 +42,6 @@ def _kpad(c):
     return -(-c // 64) * 64
 
 
-def _wgrad_gamma(B, Ho, Wo, cin, cout, k, sms):
-    """fp64ref.wgrad_gamma for every width: cout = 16 / 32 runs as one 64-wide block."""
-    if cout >= 64:
-        return R.wgrad_gamma(B, Ho, Wo, cin, cout, k, sms)
-    TW, TH, NB = R.choose_box128(B, Ho, Wo)
-    m_tiles = -(-Wo // TW) * -(-Ho // TH) * -(-B // NB)
-    splits = min(max((2 * sms) // (k * k * -(-cin // 128)), 1), m_tiles)
-    per = -(-m_tiles // splits)
-    return (8 * per + 16 + splits) * R.U23
-
-
 @pytest.mark.parametrize('B,h,w,Ca,Cb', [(2, 3, 5, 32, 32), (2, 6, 10, 16, 32), (1, 1, 1, 16, 16), (3, 7, 9, 64, 128), (16, 40, 40, 128, 128)])
 def test_upsample_cat_forward_backward(cuda, B, h, w, Ca, Cb):
     """Forward bit-exact against F.interpolate(nearest) + torch.cat; backward: db bit-exact, da within one bf16 rounding of the float64 2x2
@@ -104,7 +93,7 @@ def test_padded_1x1_conv_forward_backward_data_backward_weight(cuda, B, H, W, ci
     dxr, dxa = (nhwc(t) for t in R.conv_dgrad(dy, w, x.shape, 1, pad))
     dwr, dwa = R.conv_wgrad(x, dy, w.shape, 1, pad)
     g_f, g_d = R.mma_gamma(_kpad(cin)), R.mma_gamma(_kpad(cout))
-    g_w = _wgrad_gamma(B, Ho, Wo, cin, cout, 1, torch.cuda.get_device_properties(0).multi_processor_count)
+    g_w = R.wgrad_gamma(B, Ho, Wo, cin, cout, 1, torch.cuda.get_device_properties(0).multi_processor_count)
     r = {'y': R.check(yh, yr, R.BF16_REL * yr.abs() + (1 + R.BF16_REL) * g_f * ya, 'forward'),
          'dx': R.check(dxh, dxr, R.BF16_REL * dxr.abs() + (1 + R.BF16_REL) * g_d * dxa, 'backward-data'),
          'dw': R.check(dw, dwr, g_w * dwa, 'backward-weight')}
