@@ -209,12 +209,16 @@ __device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) { return ((
 // three products -> dm (the 256-wide tiles, whose two accumulators would not fit the register file).
 // Descriptor low words in 16-byte units (a16: hi activation view, a16 + lo16: lo view, b16: hi weight tile, + bl16: lo tile); the
 // high words are loop invariants.
-template <int BLOCK_N, int KSTEPS, bool SPLIT>
+// PRED: only the first `ksteps` K steps are issued (the halo loader's row-window stems skip their zero weight columns).  The run-time
+// predicate between the wgmmas of a tap makes ptxas fence the accumulator registers (warpgroup.arrive, C7519) before every K step, so the
+// ping-pong kernels, which have no halo loader, issue the KSTEPS steps as one straight wgmma sequence.  The cooperative kernels keep it:
+// without it ptxas serializes their wgmmas (C7515), which costs more than the fences.
+template <int BLOCK_N, int KSTEPS, bool SPLIT, bool PRED>
 __device__ __forceinline__ void issue_tap(float (&dm)[BLOCK_N / 2], float (&dc)[SPLIT ? BLOCK_N / 2 : 1], uint32_t a16, uint32_t lo16,
                                           uint32_t a_hi, uint32_t b16, uint32_t bl16, uint32_t b_hi, int ksteps) {
 #pragma unroll
   for (int k = 0; k < KSTEPS; ++k) {
-    if (k < ksteps) {
+    if (!PRED || k < ksteps) {
       const uint64_t ah = desc64(a16 + 2 * k, a_hi), al = desc64(a16 + lo16 + 2 * k, a_hi);
       const uint64_t bh = desc64(b16 + 2 * k, b_hi), bl = desc64(b16 + bl16 + 2 * k, b_hi);
       wgmma_m64k16<BLOCK_N, 0, 0>(dm, ah, bh);
@@ -235,9 +239,11 @@ __device__ __forceinline__ void issue_tap(float (&dm)[BLOCK_N / 2], float (&dc)[
 //   3 act = ReLU, no residual, no up-partial   4 act = ReLU, residual tile by TMA added BEFORE the activation (ResNet bottleneck)
 // PP selects the ping-pong schedule (one-CTA-per-SM plans, not for the fused decode or the halo loader): a tile is 64 pixels, the
 // CTA's tiles alternate between the two warpgroups, and a warpgroup runs its epilogue while the other one's MMAs run (DESIGN.md 4.1).
-// Only the cooperative narrow kernels may share an SM; a ping-pong plan always runs one CTA per SM and gets the full register budget.
-template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0, bool PP = false>
-__global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
+// CTAS: the CTAs per SM the register budget is sized for.  Only the cooperative narrow kernels may share an SM, and they exist with both
+// bounds: the two-CTA plans need the 96-register cap, the one-CTA plans would spill under it for nothing.  A ping-pong plan always runs
+// one CTA per SM and gets the full register budget.
+template <int BLOCK_N, int BLOCK_K, bool OUT_F32, bool YOLO, int EPI = 0, bool PP = false, int CTAS = 1>
+__global__ void __launch_bounds__(kThreads, CTAS) conv_tc_kernel(const __grid_constant__ ConvKArgs a) {
   constexpr ConvGeom G = conv_geom(BLOCK_N, BLOCK_K, OUT_F32, YOLO, PP);
   constexpr int SWZ = G.swz;
   constexpr int A_BYTES = G.a_bytes;
@@ -254,6 +260,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
   constexpr bool SPLIT = BLOCK_N <= 128;
   static_assert(EPI == 0 || (!OUT_F32 && !YOLO), "epilogue specialisations exist for the split16 output only");
   static_assert(!(PP && YOLO), "the fused decode runs the cooperative schedule");
+  static_assert(CTAS == 1 || (CTAS == 2 && BLOCK_N <= 64 && !PP && !YOLO), "only the cooperative narrow kernels may share an SM");
   // run-time mode flags, folded to constants in the specialised kernels
   const bool resid_tma = (EPI == 2 || EPI == 4) ? true : ((EPI == 1 || EPI == 3) ? false : a.resid_tma != 0);
   const int act_mode = (EPI == 1 || EPI == 2) ? CVB_ACT_SILU : ((EPI == 3 || EPI == 4) ? CVB_ACT_RELU : a.act);
@@ -532,7 +539,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
                   bb = bres16 + (uint32_t)hb * 2u * kB16;
                 }
                 wgmma_fence();
-                issue_tap<BLOCK_N, KSTEPS, SPLIT>(dm, dc, a16, lo16, a_hi, bb, kB16, kHiStd, ksteps);
+                issue_tap<BLOCK_N, KSTEPS, SPLIT, !PP>(dm, dc, a16, lo16, a_hi, bb, kB16, kHiStd, ksteps);
                 // the A slot is released with the last tap of the copy, the weight slot with its tap
                 unit_issued((y == ny - 1 && x == nx - 1) ? stage : -1, resident ? -1 : hb);
                 if (!resident && ++hb == SB) {
@@ -557,7 +564,7 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
           CVB_PROF_WAIT(5, mbar_wait(&full[stage], phase, 300 + stage));
           const uint32_t b16 = resident ? bres_it16 : a_ring16 + ((2u * A_BYTES) >> 4);
           wgmma_fence();
-          issue_tap<BLOCK_N, KSTEPS, SPLIT>(dm, dc, a_ring16 + wg16, lo16, kHiStd, b16, kB16, kHiStd, ksteps);
+          issue_tap<BLOCK_N, KSTEPS, SPLIT, !PP>(dm, dc, a_ring16 + wg16, lo16, kHiStd, b16, kB16, kHiStd, ksteps);
           unit_issued(stage, -1);  // frees this smem stage once the MMAs above have read it
           a_ring16 += stage16;
           if (++stage == STAGES) {
@@ -1021,21 +1028,36 @@ __global__ void __launch_bounds__(kThreads, (BLOCK_N <= 64 && !PP ? 2 : 1)) conv
 }
 
 // ---------------------------------------------------------------------------------------------- host
-template <int BN, int BK, bool PP>
+template <int BN, int BK, bool PP, int CTAS = 1>
 static const void* kernel_epi(bool f32, int epi) {
-  if (f32) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, true, false, 0, PP>);
+  if (f32) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, true, false, 0, PP, CTAS>);
   switch (epi) {
-    case 1: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 1, PP>);
-    case 2: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 2, PP>);
-    case 3: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 3, PP>);
-    case 4: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 4, PP>);
-    default: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 0, PP>);
+    case 1: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 1, PP, CTAS>);
+    case 2: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 2, PP, CTAS>);
+    case 3: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 3, PP, CTAS>);
+    case 4: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 4, PP, CTAS>);
+    default: return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 0, PP, CTAS>);
   }
 }
 
-// the kernel instantiation, or nullptr.  pp: the ping-pong schedule, instantiated for block_n <= 128 (at 256 its generic and residual
-// epilogues spill more than the cooperative kernel's)
-static const void* lookup_kernel(int bn, int bk, bool f32, bool yolo = false, int epi = 0, bool pp = false) {
+// The cooperative block_n <= 64 kernels.  ctas == 1: the one-CTA register bound, instantiated for the epilogues a one-CTA-per-SM
+// cooperative plan gets in auto mode (no residual tile: the narrow layers with a residual run ping-pong); the residual epilogues keep the
+// two-CTA bound.
+template <int BN, int BK>
+static const void* kernel_narrow(bool f32, int epi, int ctas) {
+  if (ctas == 1) {
+    if (f32) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, true, false, 0, false, 1>);
+    if (epi == 0) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 0, false, 1>);
+    if (epi == 1) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 1, false, 1>);
+    if (epi == 3) return reinterpret_cast<const void*>(&conv_tc_kernel<BN, BK, false, false, 3, false, 1>);
+  }
+  return kernel_epi<BN, BK, false, 2>(f32, epi);
+}
+
+// The kernel instantiation, or nullptr.  pp: the ping-pong schedule, instantiated for block_n <= 128 (at 256 its generic and residual
+// epilogues spill more than the cooperative kernel's).  ctas: CTAs per SM of the plan (selects the register bound of the cooperative
+// narrow kernels).
+static const void* lookup_kernel(int bn, int bk, bool f32, bool yolo = false, int epi = 0, bool pp = false, int ctas = 1) {
   if (yolo) {  // fused-decode epilogue: one anchor per 128-wide n-tile
     if (pp) return nullptr;
     if (bn == 128 && bk == 32) return reinterpret_cast<const void*>(&conv_tc_kernel<128, 32, true, true>);
@@ -1046,13 +1068,16 @@ static const void* lookup_kernel(int bn, int bk, bool f32, bool yolo = false, in
   if (bn == BN && bk == BK) return kernel_epi<BN, BK, false>(f32, epi);
 #define CVB_CASE_PP(BN, BK) \
   if (bn == BN && bk == BK) return pp ? kernel_epi<BN, BK, true>(f32, epi) : kernel_epi<BN, BK, false>(f32, epi);
-  CVB_CASE_PP(32, 16) CVB_CASE_PP(32, 32) CVB_CASE_PP(32, 64)
-  CVB_CASE_PP(64, 16) CVB_CASE_PP(64, 32) CVB_CASE_PP(64, 64)
+#define CVB_CASE_NARROW(BN, BK) \
+  if (bn == BN && bk == BK) return pp ? kernel_epi<BN, BK, true>(f32, epi) : kernel_narrow<BN, BK>(f32, epi, ctas);
+  CVB_CASE_NARROW(32, 16) CVB_CASE_NARROW(32, 32) CVB_CASE_NARROW(32, 64)
+  CVB_CASE_NARROW(64, 16) CVB_CASE_NARROW(64, 32) CVB_CASE_NARROW(64, 64)
   CVB_CASE_PP(128, 16) CVB_CASE_PP(128, 32) CVB_CASE_PP(128, 64)
   if (pp) return nullptr;
   CVB_CASE(256, 16) CVB_CASE(256, 32) CVB_CASE(256, 64)
 #undef CVB_CASE
 #undef CVB_CASE_PP
+#undef CVB_CASE_NARROW
   return nullptr;
 }
 
@@ -1857,9 +1882,9 @@ static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& 
       else if (a.resid_tma && a.resid_first && a.resid_scale == 1.0f) epi = 4;
     }
   }
-  const void* fn = epi ? lookup_kernel(bn, S.bk, P.f32, false, epi, S.pp) : nullptr;
+  const void* fn = epi ? lookup_kernel(bn, S.bk, P.f32, false, epi, S.pp, S.ctas) : nullptr;
   *epi_out = fn ? epi : 0;
-  return fn ? fn : lookup_kernel(bn, S.bk, P.f32, P.yolo, 0, S.pp);
+  return fn ? fn : lookup_kernel(bn, S.bk, P.f32, P.yolo, 0, S.pp, S.ctas);
 }
 
 // programmatic dependent launch (prologue of conv N+1 overlapping the tail of conv N): measured neutral on the YOLOv5-s step (6.57 vs
@@ -1901,10 +1926,10 @@ static int set_launch(const ConvProblem& P, int bn, const SchedPlan& S, CvbConvP
   static const bool dbg = [] { const char* e = getenv("CVB_PLAN_DEBUG"); return e && atoi(e) != 0; }();
   if (dbg)
     fprintf(stderr, "[cvb plan] cin=%d cout=%d k=%dx%d s=%d out=%dx%dx%d bn=%d bk=%d stages=%d resident=%d out_bufs=%d ctas/sm=%d "
-            "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s epi=%d pdl=%d\n", P.cin, P.cout,
+            "smem=%d grid=%d tiles=%lld resid_tma=%d halo=%d copies=%d sb=%d slot=%u kskip=%d schedule=%s epi=%d f32=%d yolo=%d pdl=%d\n", P.cin, P.cout,
             P.d.kh, P.d.kw, P.d.stride, P.d.out.B, P.Ho, P.Wo, bn, S.bk, a.stages, a.b_resident, a.out_bufs, S.ctas, p->smem, p->grid, total,
             a.resid_tma, a.halo, a.n_copies, a.sb_stages, a.halo ? (unsigned)a.sm.slot : 0u, a.kskip, S.pp ? "pingpong" : "cooperative",
-            p->epi, (int)pdl_on());
+            p->epi, (int)P.f32, (int)P.yolo, (int)pdl_on());
   return CVB_OK;
 }
 
