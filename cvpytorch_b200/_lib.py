@@ -165,6 +165,9 @@ SYMBOLS = {
     'cvb_fcos_nms': (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_float, c_int32, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_yolox_workspace_bytes': (c_size_t, [c_int32, c_int32]),
+    'cvb_yolov6_decode': (c_int32, [POINTER(CvbView), POINTER(CvbView), c_int32, c_float, c_void_p, c_int64, c_int64, c_void_p, c_float, c_int32,
+                                    c_void_p]),
+    'cvb_depth_to_space2': (c_int32, [POINTER(CvbView), POINTER(CvbView), c_void_p]),
     'cvb_yolox_decode': (c_int32, [POINTER(CvbView), POINTER(CvbView), c_int32, c_float, c_void_p, c_int64, c_int64, c_void_p]),
     'cvb_yolox_nms': (c_int32, [c_void_p, c_int32, c_int32, c_float, c_double, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'cvb_rescale_clip_boxes': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

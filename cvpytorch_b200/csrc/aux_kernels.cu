@@ -389,6 +389,107 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
   }
 }
 
+// ------------------------------------------------------------------ YOLOv6 anchor-free decode
+// Grid (pixel chunks, B); one warp per z row (one anchor per pixel), its no = 5 + nc <= 96 floats in three coalesced 32-lane chunks:
+// lanes 0..3 the box, lane 4 the objectness 1.0, the rest sigmoid(class logit).  Box: anchor (x + 0.5, y + 0.5), x1y1 = a - lt,
+// x2y2 = a + rb, centre (x1y1 + x2y2) / 2, size x2y2 - x1y1, times stride -- dist2bbox(..., 'xywh') of yolov6_loss.py:205-216 in its
+// fp32 operation order.  HIST / MULTI: the NMS pre-pass of yolo_decode_kernel with obj = 1, so score = cls * 1 = cls bit for bit.
+constexpr int kV6DecodePix = 256;  // pixels per CTA
+constexpr int kV6DecodeThreads = 256;
+
+template <bool HIST, bool MULTI>
+__global__ void __launch_bounds__(kV6DecodeThreads) yolov6_decode_kernel(const float* __restrict__ cls, int cls_pitch, const float* __restrict__ reg,
+                                                                         int reg_pitch, int ny, int nx, int nc, float stride,
+                                                                         float* __restrict__ z, long long z_rows, long long z_off,
+                                                                         uint32_t* __restrict__ hist, float* __restrict__ rowmax, float conf) {
+  extern __shared__ uint32_t s_hist[];  // [kNmsBins] when HIST
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int NW = kV6DecodeThreads / 32;
+  const int b = blockIdx.y;
+  const int npix = ny * nx;
+  const int pix0 = blockIdx.x * kV6DecodePix;
+  const int cpix = min(npix, pix0 + kV6DecodePix) - pix0;
+  const int no = nc + 5;
+  if (HIST) {
+    for (int i = threadIdx.x; i < kNmsBins; i += kV6DecodeThreads) s_hist[i] = 0;
+    __syncthreads();
+  }
+  const bool v0 = lane < no, v1 = 32 + lane < no, v2 = 64 + lane < no;
+  const bool is_cls = v0 && lane >= 5;
+  float* rmb = HIST ? rowmax + (size_t)b * z_rows + z_off : nullptr;
+  for (int p = warp; p < cpix; p += NW) {  // warp-uniform loop
+    const int pix = pix0 + p;
+    const size_t q = (size_t)b * npix + pix;
+    const float* cr = cls + q * cls_pitch;
+    const float c0 = is_cls ? __ldg(cr + lane - 5) : 0.0f;
+    const float c1 = v1 ? __ldg(cr + lane + 27) : 0.0f;
+    const float c2 = v2 ? __ldg(cr + lane + 59) : 0.0f;
+    float o0;
+    if (lane < 4) {
+      const int d = lane & 1;  // 0: x, 1: y
+      const float lt = __ldg(reg + q * reg_pitch + d), rb = __ldg(reg + q * reg_pitch + d + 2);
+      const int py = pix / nx;
+      const float a = __fadd_rn((float)(d ? py : pix - py * nx), 0.5f);
+      const float x1 = __fsub_rn(a, lt), x2 = __fadd_rn(a, rb);
+      o0 = __fmul_rn(lane < 2 ? __fmul_rn(__fadd_rn(x1, x2), 0.5f) : __fsub_rn(x2, x1), stride);
+    } else {
+      o0 = lane == 4 ? 1.0f : sigmoid_fast(c0);
+    }
+    const float y1 = sigmoid_fast(c1), y2 = sigmoid_fast(c2);
+    float* dst = z + ((size_t)b * z_rows + z_off + pix) * no + lane;
+    if (v0) dst[0] = o0;
+    if (v1) dst[32] = y1;
+    if (v2) dst[64] = y2;
+    if (HIST) {
+      const float obj = 1.0f;  // > conf for every conf_thres < 1 (the NMS refuses larger ones)
+      const float s0 = is_cls ? yolo_score(o0, obj) : 0.0f;
+      const float s1 = v1 ? yolo_score(y1, obj) : 0.0f;
+      const float s2 = v2 ? yolo_score(y2, obj) : 0.0f;
+      if (MULTI) {
+        if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
+        if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
+        if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
+      }
+      float rbest = fmaxf(fmaxf(s0, s1), s2);
+      if (!(rbest > conf)) rbest = 0.0f;
+#pragma unroll
+      for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
+      if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
+      if (lane == 0) rmb[pix] = rbest;
+    }
+  }
+  if (HIST) {
+    __syncthreads();
+    uint32_t* gh = hist + (size_t)b * kNmsBins;
+    for (int i = threadIdx.x; i < kNmsBins; i += kV6DecodeThreads) {
+      const uint32_t c = s_hist[i];
+      if (c) atomicAdd(&gh[i], c);
+    }
+  }
+}
+
+// ------------------------------------------------------------------ 2x depth-to-space (ConvTranspose2d k = s = 2 after its 1x1 GEMM)
+// src [B,h,w,4c] split16 with channel (py*2+px)*c + o  ->  dst [B,2h,2w,c] split16 pixel (2y+py, 2x+px) channel o.  One thread per (output
+// pixel, 8-channel vector); the hi and lo planes are copied as they are, so the values are the GEMM's bit for bit.
+__global__ void __launch_bounds__(256) depth_to_space2_kernel(const __half* __restrict__ src, int sp, long long splane, int h, int w, int c,
+                                                              __half* __restrict__ dst, int dp, long long dplane, long long n) {
+  const int cv = c / 8;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % cv);
+    long long r = i / cv;
+    const int ox = (int)(r % (2 * w));
+    r /= 2 * w;
+    const int oy = (int)(r % (2 * h));
+    const long long b = r / (2 * h);
+    const size_t s = (((size_t)b * h + (oy >> 1)) * w + (ox >> 1)) * sp + (size_t)(((oy & 1) * 2 + (ox & 1)) * c + v * 8);
+    const size_t d = (((size_t)b * 2 * h + oy) * 2 * w + ox) * dp + (size_t)v * 8;
+    const uint4 hi = *reinterpret_cast<const uint4*>(src + s);
+    const uint4 lo = *reinterpret_cast<const uint4*>(src + s + splane);
+    *reinterpret_cast<uint4*>(dst + d) = hi;
+    *reinterpret_cast<uint4*>(dst + d + dplane) = lo;
+  }
+}
+
 // ------------------------------------------------------------------ 3x3 / stride 2 / pad 1 max pool (ResNet stem)
 // one thread per (output pixel, 8-channel vector); max over hi+lo values, result re-split exactly (max is one of the inputs).  A NaN
 // is taken and then kept, like F.max_pool2d; the running maximum starts as -inf (hi = 0xFC00) so an all -inf window gives -inf.
@@ -1008,6 +1109,57 @@ extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const
   kernel<<<dim3(ceil_div(raw->H * raw->W, kDecodePix), raw->B), kDecodeThreads, smem, as_stream(stream)>>>(
       static_cast<const float*>(raw->base), raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows, z_off, xperm, hist, rowmax,
       conf_thres, fast_div_magic(raw->W, (unsigned long long)raw->H * raw->W));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_yolov6_decode(const CvbView* cls, const CvbView* reg, int32_t nc, float stride, float* z, int64_t z_rows, int64_t z_off,
+                                 void* nms_workspace, float conf_thres, int32_t multi_label, void* stream) {
+  CVB_REQUIRE(cls && cls->base && reg && reg->base && z, "yolov6_decode: null argument");
+  CVB_REQUIRE(nc >= 1 && nc <= 91, "yolov6_decode: 1..91 classes supported (nc=%d)", nc);
+  CVB_REQUIRE(cls->plane_stride == 0 && reg->plane_stride == 0, "yolov6_decode: cls and reg must be fp32 views");
+  CVB_REQUIRE(cls->C >= nc && cls->c_pitch >= cls->C && reg->C >= 4 && reg->c_pitch >= reg->C, "yolov6_decode: cls needs >= nc and reg >= 4 channels");
+  CVB_REQUIRE(cls->B == reg->B && cls->H == reg->H && cls->W == reg->W, "yolov6_decode: cls [%d,%d,%d] and reg [%d,%d,%d] differ", cls->B, cls->H,
+              cls->W, reg->B, reg->H, reg->W);
+  CVB_REQUIRE(z_off >= 0 && z_off + (long long)cls->H * cls->W <= z_rows, "yolov6_decode: level rows [%lld, %lld) outside z's %lld rows",
+              (long long)z_off, (long long)z_off + (long long)cls->H * cls->W, (long long)z_rows);
+  CVB_REQUIRE((long long)cls->H * cls->W < 0x7fffffffLL, "yolov6_decode: level too large");
+  static const cudaError_t multi_smem_err = opt_in_smem(yolov6_decode_kernel<true, true>, kNmsBins * (int)sizeof(uint32_t));
+  static const cudaError_t single_smem_err = opt_in_smem(yolov6_decode_kernel<true, false>, kNmsBins * (int)sizeof(uint32_t));
+  CVB_CHECK_CUDA(multi_smem_err);
+  CVB_CHECK_CUDA(single_smem_err);
+  uint32_t* hist = static_cast<uint32_t*>(nms_workspace);
+  float* rowmax = hist ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(cls->B)) : nullptr;
+  const size_t smem = hist ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
+  const bool multi = multi_label && nc > 1;
+  const auto kernel = !hist ? yolov6_decode_kernel<false, false> : multi ? yolov6_decode_kernel<true, true> : yolov6_decode_kernel<true, false>;
+  kernel<<<dim3(ceil_div(cls->H * cls->W, kV6DecodePix), cls->B), kV6DecodeThreads, smem, as_stream(stream)>>>(
+      static_cast<const float*>(cls->base), cls->c_pitch, static_cast<const float*>(reg->base), reg->c_pitch, cls->H, cls->W, nc, stride, z, z_rows,
+      z_off, hist, rowmax, conf_thres);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_depth_to_space2(const CvbView* src, const CvbView* dst, void* stream) {
+  int rc = check_split_view(src, "depth_to_space2 src");
+  if (!rc) rc = check_split_view(dst, "depth_to_space2 dst");
+  if (rc) return rc;
+  CVB_REQUIRE(src->plane_stride > 0 && dst->plane_stride > 0, "depth_to_space2: src and dst must be split16 views");
+  CVB_REQUIRE(dst->C % 8 == 0 && src->C == 4 * dst->C, "depth_to_space2: src must have 4 x dst's channels (src %d, dst %d), a multiple of 8",
+              src->C, dst->C);
+  CVB_REQUIRE(src->B == dst->B && dst->H == 2 * src->H && dst->W == 2 * src->W, "depth_to_space2: dst [%d,%d,%d] is not src [%d,%d,%d] at twice the size",
+              dst->B, dst->H, dst->W, src->B, src->H, src->W);
+  CVB_REQUIRE(src->c_pitch % 8 == 0 && dst->c_pitch % 8 == 0 && is_aligned(src->base, 16) && is_aligned(dst->base, 16) &&
+                  src->plane_stride % 16 == 0 && dst->plane_stride % 16 == 0,
+              "depth_to_space2: alignment");
+  const long long n = (long long)dst->B * dst->H * dst->W * (dst->C / 8);
+  if (n == 0) return CVB_OK;
+  long long grid = (n + 255) / 256;
+  if (grid > kSmCount * 16) grid = kSmCount * 16;
+  depth_to_space2_kernel<<<(int)grid, 256, 0, as_stream(stream)>>>(static_cast<const __half*>(src->base), src->c_pitch, src->plane_stride / 2, src->H,
+                                                                   src->W, dst->C, static_cast<__half*>(dst->base), dst->c_pitch, dst->plane_stride / 2, n);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;

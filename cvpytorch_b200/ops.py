@@ -293,6 +293,21 @@ def yolo_decode(raw_view, na, no, anchors_px, stride, z, z_rows, z_off, xperm=No
                                           1 if (multi_label and no - 5 > 1) else 0, _stream()), 'cvb_yolo_decode')
 
 
+def yolov6_decode(cls_view, reg_view, nc, stride, z, z_rows, z_off, nms_ws=None, conf_thres=0.001, multi_label=True):
+    """One YOLOv6 head level (fp32 NHWC class logits and ltrb distances) -> rows z_off .. z_off + h*w of z [B, z_rows, 5 + nc].
+    nms_ws: NmsWorkspace previously reset with nms_reset(); the decode then also fills the NMS score histogram (yolo_nms hist_ready)."""
+    _require_cuda(z, 'yolov6_decode')
+    assert z.dtype == torch.float32 and z.is_contiguous() and tuple(z.shape[1:]) == (z_rows, nc + 5)
+    _lib.check(_lib.lib().cvb_yolov6_decode(byref(cls_view), byref(reg_view), nc, float(stride), z.data_ptr(), z_rows, z_off,
+                                            nms_ws.ws_ptr if nms_ws is not None else None, float(conf_thres), 1 if multi_label else 0,
+                                            _stream()), 'cvb_yolov6_decode')
+
+
+def depth_to_space2(src_view, dst_view):
+    """split16 [B,h,w,4c] (channel (py*2+px)*c + o) -> split16 [B,2h,2w,c] (pixel (2y+py, 2x+px)), values copied exactly."""
+    _lib.check(_lib.lib().cvb_depth_to_space2(byref(src_view), byref(dst_view), _stream()), 'cvb_depth_to_space2')
+
+
 def nms_reset(ws):
     _lib.check(_lib.lib().cvb_nms_workspace_reset(ws.ws_ptr, ws.ws_bytes, ws.B, _stream()), 'cvb_nms_workspace_reset')
 

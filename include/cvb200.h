@@ -252,6 +252,24 @@ typedef struct CvbNmsParams {
   int32_t hist_ready;  /* 1: histogram + per-row best scores were already produced by cvb_yolo_decode (all levels) */
 } CvbNmsParams;
 
+/*
+ * YOLOv6 anchor-free decode of one level (src/models/detects/yolov6_detect.py:36-50 with generate_anchors(..., mode='af') and
+ * dist2bbox(..., 'xywh')).  cls / reg: fp32 NHWC views [B,h,w,>=nc] (class logits) and [B,h,w,>=4] (ltrb distances), the outputs of the
+ * head's cls_preds / reg_preds 1x1 convs.  Writes z[b, z_off + y*w + x, :] = (cx, cy, w, h, 1.0, sigmoid(cls_0..nc-1)) with anchor
+ * (x + 0.5, y + 0.5), box = ((a - lt + a + rb) / 2, rb + lt) * stride in the reference's fp32 operation order; nc <= 91.
+ * nms_workspace (optional): as for cvb_yolo_decode -- the histogram and per-row best scores of cvb_yolo_nms(hist_ready = 1).  With the
+ * objectness exactly 1.0 the YOLOv5 NMS keeps the rows and scores of the YOLOv6 one (src/models/yolov6.py:32-107).
+ */
+int cvb_yolov6_decode(const CvbView* cls, const CvbView* reg, int32_t nc, float stride, float* z, int64_t z_rows, int64_t z_off,
+                      void* nms_workspace, float conf_thres, int32_t multi_label, void* stream);
+
+/*
+ * 2x depth-to-space of split16 activations: src [B,h,w,4c] with channel (py*2+px)*c + o -> dst [B,2h,2w,c] pixel (2y+py, 2x+px), channel o;
+ * hi and lo planes copied unchanged.  With a 1x1 GEMM whose 4c output columns are packed [py][px][cout] it is
+ * nn.ConvTranspose2d(c, c, 2, stride=2) (BiFusion.upsample, src/models/modules/yolo_modules.py:245-267).  c % 8 == 0.
+ */
+int cvb_depth_to_space2(const CvbView* src, const CvbView* dst, void* stream);
+
 size_t cvb_nms_workspace_bytes(int32_t B, int32_t A, int32_t nc);
 /* zero the per-image histogram / counters (only needed before cvb_yolo_decode(..., nms_workspace, ...)) */
 int cvb_nms_workspace_reset(void* workspace, size_t workspace_bytes, int32_t B, void* stream);
