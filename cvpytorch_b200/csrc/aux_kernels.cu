@@ -301,10 +301,7 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
   const int npix = ny * nx;
   const int pix0 = blockIdx.x * kDecodePix;
   const int cpix = min(npix, pix0 + kDecodePix) - pix0;
-  if (HIST) {
-    for (int i = threadIdx.x; i < kNmsBins; i += kDecodeThreads) s_hist[i] = 0;
-    __syncthreads();
-  }
+  if (HIST) nms_hist_clear<kDecodeThreads>(s_hist);
   const float* rbase = raw + ((size_t)b * npix + pix0) * pitch;
   const size_t zb = ((size_t)b * z_rows + z_off) * no;  // z element of the level's first row in image b
   const size_t xb = (size_t)b * na * npix * no;
@@ -360,33 +357,17 @@ __global__ void __launch_bounds__(kDecodeThreads) yolo_decode_kernel(const float
           const float obj = __shfl_sync(0xffffffffu, o0, 4);
           float rbest = 0.0f;
           if (ok && obj > conf) {  // warp-uniform
-            const float s0 = is_cls ? yolo_score(o0, obj) : 0.0f;
-            const float s1 = v1 ? yolo_score(y1, obj) : 0.0f;
-            const float s2 = v2 ? yolo_score(y2, obj) : 0.0f;
-            if (MULTI) {
-              if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
-              if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
-              if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
-            }
-            rbest = fmaxf(fmaxf(s0, s1), s2);
-            if (!(rbest > conf)) rbest = 0.0f;
-#pragma unroll
-            for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
-            if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
+            nms_count_score(s_hist, is_cls ? yolo_score(o0, obj) : 0.0f, conf, MULTI, rbest);
+            nms_count_score(s_hist, v1 ? yolo_score(y1, obj) : 0.0f, conf, MULTI, rbest);
+            nms_count_score(s_hist, v2 ? yolo_score(y2, obj) : 0.0f, conf, MULTI, rbest);
+            rbest = nms_finish_row(s_hist, rbest, conf, MULTI, lane);
           }
           if (ok && lane == 0) rmb[a * npix + pix] = rbest;
         }
       }
     }
   }
-  if (HIST) {
-    __syncthreads();
-    uint32_t* gh = hist + (size_t)b * kNmsBins;
-    for (int i = threadIdx.x; i < kNmsBins; i += kDecodeThreads) {
-      const uint32_t c = s_hist[i];
-      if (c) atomicAdd(&gh[i], c);
-    }
-  }
+  if (HIST) nms_hist_flush<kDecodeThreads>(s_hist, hist + (size_t)b * kNmsBins);
 }
 
 // ------------------------------------------------------------------ YOLOv6 anchor-free decode
@@ -410,10 +391,7 @@ __global__ void __launch_bounds__(kV6DecodeThreads) yolov6_decode_kernel(const f
   const int pix0 = blockIdx.x * kV6DecodePix;
   const int cpix = min(npix, pix0 + kV6DecodePix) - pix0;
   const int no = nc + 5;
-  if (HIST) {
-    for (int i = threadIdx.x; i < kNmsBins; i += kV6DecodeThreads) s_hist[i] = 0;
-    __syncthreads();
-  }
+  if (HIST) nms_hist_clear<kV6DecodeThreads>(s_hist);
   const bool v0 = lane < no, v1 = 32 + lane < no, v2 = 64 + lane < no;
   const bool is_cls = v0 && lane >= 5;
   float* rmb = HIST ? rowmax + (size_t)b * z_rows + z_off : nullptr;
@@ -442,30 +420,15 @@ __global__ void __launch_bounds__(kV6DecodeThreads) yolov6_decode_kernel(const f
     if (v2) dst[64] = y2;
     if (HIST) {
       const float obj = 1.0f;  // > conf for every conf_thres < 1 (the NMS refuses larger ones)
-      const float s0 = is_cls ? yolo_score(o0, obj) : 0.0f;
-      const float s1 = v1 ? yolo_score(y1, obj) : 0.0f;
-      const float s2 = v2 ? yolo_score(y2, obj) : 0.0f;
-      if (MULTI) {
-        if (s0 > conf) atomicAdd(&s_hist[nms_score_bin(s0)], 1u);
-        if (s1 > conf) atomicAdd(&s_hist[nms_score_bin(s1)], 1u);
-        if (s2 > conf) atomicAdd(&s_hist[nms_score_bin(s2)], 1u);
-      }
-      float rbest = fmaxf(fmaxf(s0, s1), s2);
-      if (!(rbest > conf)) rbest = 0.0f;
-#pragma unroll
-      for (int o2 = 16; o2 > 0; o2 >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o2));
-      if (!MULTI && lane == 0 && rbest > conf) atomicAdd(&s_hist[nms_score_bin(rbest)], 1u);
+      float rbest = 0.0f;
+      nms_count_score(s_hist, is_cls ? yolo_score(o0, obj) : 0.0f, conf, MULTI, rbest);
+      nms_count_score(s_hist, v1 ? yolo_score(y1, obj) : 0.0f, conf, MULTI, rbest);
+      nms_count_score(s_hist, v2 ? yolo_score(y2, obj) : 0.0f, conf, MULTI, rbest);
+      rbest = nms_finish_row(s_hist, rbest, conf, MULTI, lane);
       if (lane == 0) rmb[pix] = rbest;
     }
   }
-  if (HIST) {
-    __syncthreads();
-    uint32_t* gh = hist + (size_t)b * kNmsBins;
-    for (int i = threadIdx.x; i < kNmsBins; i += kV6DecodeThreads) {
-      const uint32_t c = s_hist[i];
-      if (c) atomicAdd(&gh[i], c);
-    }
-  }
+  if (HIST) nms_hist_flush<kV6DecodeThreads>(s_hist, hist + (size_t)b * kNmsBins);
 }
 
 // ------------------------------------------------------------------ 2x depth-to-space (ConvTranspose2d k = s = 2 after its 1x1 GEMM)
@@ -1089,6 +1052,22 @@ extern "C" int cvb_sppf_pool(const CvbView* x, const CvbView* y1, const CvbView*
   return CVB_OK;
 }
 
+// What both decode entry points launch: K<HIST, MULTI> with HIST iff there is an NMS workspace and MULTI iff multi_label with nc > 1
+// (the rule of cvb_yolo_nms), the workspace's histograms and rowmax, and the shared-memory histogram of HIST, to which both HIST
+// instantiations are opted in once (thread-safe static initialisation).
+template <auto kPlain, auto kSingle, auto kMulti>
+static int decode_prepass(void* ws, int B, bool multi, decltype(kPlain)* kernel, uint32_t** hist, float** rowmax, size_t* smem) {
+  static const cudaError_t single_smem_err = opt_in_smem(kSingle, kNmsBins * (int)sizeof(uint32_t));
+  static const cudaError_t multi_smem_err = opt_in_smem(kMulti, kNmsBins * (int)sizeof(uint32_t));
+  CVB_CHECK_CUDA(single_smem_err);
+  CVB_CHECK_CUDA(multi_smem_err);
+  *kernel = !ws ? kPlain : multi ? kMulti : kSingle;
+  *hist = static_cast<uint32_t*>(ws);
+  *rowmax = nms_ws_rowmax(ws, B);
+  *smem = ws ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
+  return CVB_OK;
+}
+
 extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const float* anchors_px, float stride, float* z, int64_t z_rows,
                                int64_t z_off, float* xperm, void* nms_workspace, float conf_thres, int32_t multi_label, void* stream) {
   CVB_REQUIRE(raw && raw->base && anchors_px, "yolo_decode: null argument");
@@ -1097,15 +1076,14 @@ extern "C" int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const
   CVB_REQUIRE(nms_workspace == nullptr || z != nullptr, "yolo_decode: histogram needs the decoded output");
   CVB_REQUIRE((long long)raw->H * raw->W * na < 0x7fffffffLL, "yolo_decode: level too large");
   CVB_REQUIRE(no <= 96, "yolo_decode: at most 91 classes supported (no=%d)", no);
-  // one-time, thread-safe (C++11 static initialisation) opt-in to the large dynamic shared memory carve-out
-  static const cudaError_t multi_smem_err = opt_in_smem(yolo_decode_kernel<true, true>, kNmsBins * (int)sizeof(uint32_t));
-  static const cudaError_t single_smem_err = opt_in_smem(yolo_decode_kernel<true, false>, kNmsBins * (int)sizeof(uint32_t));
-  CVB_CHECK_CUDA(multi_smem_err);
-  CVB_CHECK_CUDA(single_smem_err);
-  uint32_t* hist = static_cast<uint32_t*>(nms_workspace);
-  float* rowmax = hist ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(raw->B)) : nullptr;
-  const size_t smem = hist ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
-  const auto kernel = !hist ? yolo_decode_kernel<false, false> : multi_label ? yolo_decode_kernel<true, true> : yolo_decode_kernel<true, false>;
+  if (int rc = z ? check_level_rows("yolo_decode", z_off, (long long)na * raw->H * raw->W, z_rows) : CVB_OK) return rc;
+  auto kernel = yolo_decode_kernel<false, false>;
+  uint32_t* hist;
+  float* rowmax;
+  size_t smem;
+  if (int rc = decode_prepass<yolo_decode_kernel<false, false>, yolo_decode_kernel<true, false>, yolo_decode_kernel<true, true>>(
+          nms_workspace, raw->B, multi_label && no - 5 > 1, &kernel, &hist, &rowmax, &smem))
+    return rc;
   kernel<<<dim3(ceil_div(raw->H * raw->W, kDecodePix), raw->B), kDecodeThreads, smem, as_stream(stream)>>>(
       static_cast<const float*>(raw->base), raw->H, raw->W, raw->c_pitch, na, no, anchors_px, stride, z, z_rows, z_off, xperm, hist, rowmax,
       conf_thres, fast_div_magic(raw->W, (unsigned long long)raw->H * raw->W));
@@ -1122,18 +1100,15 @@ extern "C" int cvb_yolov6_decode(const CvbView* cls, const CvbView* reg, int32_t
   CVB_REQUIRE(cls->C >= nc && cls->c_pitch >= cls->C && reg->C >= 4 && reg->c_pitch >= reg->C, "yolov6_decode: cls needs >= nc and reg >= 4 channels");
   CVB_REQUIRE(cls->B == reg->B && cls->H == reg->H && cls->W == reg->W, "yolov6_decode: cls [%d,%d,%d] and reg [%d,%d,%d] differ", cls->B, cls->H,
               cls->W, reg->B, reg->H, reg->W);
-  CVB_REQUIRE(z_off >= 0 && z_off + (long long)cls->H * cls->W <= z_rows, "yolov6_decode: level rows [%lld, %lld) outside z's %lld rows",
-              (long long)z_off, (long long)z_off + (long long)cls->H * cls->W, (long long)z_rows);
   CVB_REQUIRE((long long)cls->H * cls->W < 0x7fffffffLL, "yolov6_decode: level too large");
-  static const cudaError_t multi_smem_err = opt_in_smem(yolov6_decode_kernel<true, true>, kNmsBins * (int)sizeof(uint32_t));
-  static const cudaError_t single_smem_err = opt_in_smem(yolov6_decode_kernel<true, false>, kNmsBins * (int)sizeof(uint32_t));
-  CVB_CHECK_CUDA(multi_smem_err);
-  CVB_CHECK_CUDA(single_smem_err);
-  uint32_t* hist = static_cast<uint32_t*>(nms_workspace);
-  float* rowmax = hist ? reinterpret_cast<float*>(static_cast<uint8_t*>(nms_workspace) + nms_ws_rowmax_offset(cls->B)) : nullptr;
-  const size_t smem = hist ? (size_t)kNmsBins * sizeof(uint32_t) : 0;
-  const bool multi = multi_label && nc > 1;
-  const auto kernel = !hist ? yolov6_decode_kernel<false, false> : multi ? yolov6_decode_kernel<true, true> : yolov6_decode_kernel<true, false>;
+  if (int rc = check_level_rows("yolov6_decode", z_off, (long long)cls->H * cls->W, z_rows)) return rc;
+  auto kernel = yolov6_decode_kernel<false, false>;
+  uint32_t* hist;
+  float* rowmax;
+  size_t smem;
+  if (int rc = decode_prepass<yolov6_decode_kernel<false, false>, yolov6_decode_kernel<true, false>, yolov6_decode_kernel<true, true>>(
+          nms_workspace, cls->B, multi_label && nc > 1, &kernel, &hist, &rowmax, &smem))
+    return rc;
   kernel<<<dim3(ceil_div(cls->H * cls->W, kV6DecodePix), cls->B), kV6DecodeThreads, smem, as_stream(stream)>>>(
       static_cast<const float*>(cls->base), cls->c_pitch, static_cast<const float*>(reg->base), reg->c_pitch, cls->H, cls->W, nc, stride, z, z_rows,
       z_off, hist, rowmax, conf_thres);

@@ -192,16 +192,6 @@ __device__ __forceinline__ float silu_fast(float x) {
     }                                          \
   } while (0)
 
-// NMS score histogram in shared memory: ++hist[nms_score_bin(sc)] iff `on` (must match that definition in internal.h) -- one predicated red.shared, no branch
-// (a C++ `if (on) atomicAdd(...)` compiles to a ~14-instruction divergent region per score, which dominated the fused-decode epilogue)
-__device__ __forceinline__ void hist_inc_if(uint32_t hist_smem_addr, float sc, bool on) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b32 t;\n\tsetp.ne.b32 p, %2, 0;\n\tshr.b32 t, %1, 17;\n\tmin.u32 t, t, %3;\n\tmad.lo.u32 t, t, 4, %0;\n\t"
-      "@p red.shared.add.u32 [t], 1;\n\t}\n"
-      ::"r"(hist_smem_addr), "r"(__float_as_uint(sc)), "r"((uint32_t)on), "n"(kNmsBins - 1)
-      : "memory");
-}
-
 __device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
 // The MMAs of one (filter tap, K chunk) for the 64 accumulator rows of this warpgroup: KSTEPS K steps of 16 over the hi / lo
@@ -1225,6 +1215,7 @@ static int validate_desc(const CvbConvDesc& desc, ConvProblem* P) {
     CVB_REQUIRE(out.C == d->yolo->na * 128 && d->cout_pad == out.C, "conv(yolo): weights must be packed one anchor per 128-wide n-tile (C = na*128)");
     CVB_REQUIRE(!d->residual.base && !d->up_partial.base && d->act == CVB_ACT_NONE, "conv(yolo): no residual / partial / activation");
     CVB_REQUIRE(is_aligned(d->yolo->z, 4), "conv(yolo): z must be 4-byte aligned");
+    if (int rc = check_level_rows("conv(yolo)", d->yolo->z_off, (long long)d->yolo->na * in.H * in.W, d->yolo->z_rows)) return rc;
   }
   const int cout = out.C;
   CVB_REQUIRE(cin % 16 == 0, "conv: cin=%d must be a multiple of 16", cin);
@@ -1851,12 +1842,12 @@ static const void* fill_epilogue(const ConvProblem& P, int bn, const SchedPlan& 
     a.y_no = y.no;
     a.y_nx = P.yolo_nx;
     a.y_nx_magic = (uint32_t)((0x100000000ULL + (unsigned long long)P.yolo_nx - 1) / (unsigned long long)P.yolo_nx);
-    a.y_multi = y.multi_label ? 1 : 0;
+    a.y_multi = y.multi_label && y.no - 5 > 1 ? 1 : 0;
     a.y_stride = y.stride;
     a.y_conf = y.conf_thres;
     for (int i = 0; i < 8; ++i) a.y_anchor[i] = y.anchors_px[i];
     a.y_hist = static_cast<unsigned int*>(y.nms_workspace);
-    a.y_rowmax = y.nms_workspace ? reinterpret_cast<float*>(static_cast<uint8_t*>(y.nms_workspace) + nms_ws_rowmax_offset(d->out.B)) : nullptr;
+    a.y_rowmax = nms_ws_rowmax(y.nms_workspace, d->out.B);
   }
   {
     // one accumulation chain per tile: the hi*hi products (and, at block_n = 256, the cross terms too: one register accumulator) of

@@ -90,6 +90,50 @@ constexpr int kNmsBins = 16384;
 #ifdef __CUDACC__
 // Histogram bin of a score: its fp32 bits >> 17, monotone in non-negative scores; sign-bit patterns clamp to the last bin.
 __device__ __forceinline__ uint32_t nms_score_bin(float score) { return min(__float_as_uint(score) >> 17, (uint32_t)(kNmsBins - 1)); }
+
+// ++hist[nms_score_bin(sc)] of a shared-memory histogram iff `on`, as one predicated red.shared with no branch (a C++ `if (on)
+// atomicAdd(...)` compiles to a ~14-instruction divergent region per score, which dominated the fused-decode epilogue).  The bin
+// formula must match nms_score_bin above.
+__device__ __forceinline__ void hist_inc_if(uint32_t hist_smem_addr, float sc, bool on) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 t;\n\tsetp.ne.b32 p, %2, 0;\n\tshr.b32 t, %1, 17;\n\tmin.u32 t, t, %3;\n\tmad.lo.u32 t, t, 4, %0;\n\t"
+      "@p red.shared.add.u32 [t], 1;\n\t}\n"
+      ::"r"(hist_smem_addr), "r"(__float_as_uint(sc)), "r"((uint32_t)on), "n"(kNmsBins - 1)
+      : "memory");
+}
+
+// The NMS score pre-pass: what a decode kernel or the NMS counting pass builds for every z row, and what cvb_yolo_nms then trusts
+// (hist_ready = 1).  Each lane of the row's warp counts its scores into `best` (starting from 0) with nms_count_score, then
+// nms_finish_row gives the row's rowmax entry.  multi: one histogram entry per score > conf; else one per row with a best score > conf.
+__device__ __forceinline__ void nms_count_score(uint32_t* hist, float sc, float conf, bool multi, float& best) {
+  if (multi && sc > conf) atomicAdd(&hist[nms_score_bin(sc)], 1u);
+  best = fmaxf(best, sc);
+}
+
+// Warp-wide: the row's best score if it is > conf, else 0 (every lane gets it).
+__device__ __forceinline__ float nms_finish_row(uint32_t* hist, float best, float conf, bool multi, int lane) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if (!(best > conf)) best = 0.0f;
+  if (!multi && lane == 0 && best > conf) atomicAdd(&hist[nms_score_bin(best)], 1u);
+  return best;
+}
+
+// A CTA's shared-memory histogram: zeroed before the CTA counts into it, and its non-empty bins added to the image's global
+// histogram once at the end (keeps the hot bins out of global atomics).
+template <int kThreads>
+__device__ __forceinline__ void nms_hist_clear(uint32_t* s_hist) {
+  for (int i = threadIdx.x; i < kNmsBins; i += kThreads) s_hist[i] = 0;
+  __syncthreads();
+}
+template <int kThreads>
+__device__ __forceinline__ void nms_hist_flush(const uint32_t* s_hist, uint32_t* g_hist) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < kNmsBins; i += kThreads) {
+    const uint32_t c = s_hist[i];
+    if (c) atomicAdd(&g_hist[i], c);
+  }
+}
 #endif
 constexpr int kNmsCap = 65536;   // candidate key capacity per image (phase B)
 constexpr int kNmsCapA = 4096;   // phase-A candidate capacity = one shared-memory sort chunk
@@ -99,6 +143,13 @@ constexpr int kNmsCapA = 4096;   // phase-A candidate capacity = one shared-memo
 // builds the histogram (decode kernel or the NMS count pass) and lets the emit passes skip rows below the threshold bin.
 inline size_t nms_ws_head_bytes(int B) { return align_up((size_t)B * kNmsBins * 4, 256) + 6 * align_up((size_t)B * 4, 256); }
 inline size_t nms_ws_rowmax_offset(int B) { return nms_ws_head_bytes(B) + (size_t)B * (kNmsCap + kNmsCapA) * 8; }
+inline float* nms_ws_rowmax(void* ws, int B) { return ws ? reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + nms_ws_rowmax_offset(B)) : nullptr; }
+
+// A decode level writes the z rows [z_off, z_off + rows) of each image, which must lie inside the image's z_rows.
+inline int check_level_rows(const char* op, long long z_off, long long rows, long long z_rows) {
+  CVB_REQUIRE(z_off >= 0 && z_off + rows <= z_rows, "%s: level rows [%lld, %lld) outside z's %lld rows", op, z_off, z_off + rows, z_rows);
+  return CVB_OK;
+}
 
 #ifdef __CUDACC__
 // The one fp32 -> split16 (hi, lo) conversion, for a pair of values (one F2FP per plane).  hi = fp16_rn(x) and lo = fp16_rn(x - hi), both

@@ -61,7 +61,7 @@ static NmsWs carve_ws(void* ws, int B, int phase) {
   p += 6 * slot;
   uint64_t* keysB = reinterpret_cast<uint64_t*>(p);
   uint64_t* keysA = keysB + (size_t)B * kCap;
-  w.rowmax = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + nms_ws_rowmax_offset(B));
+  w.rowmax = nms_ws_rowmax(ws, B);
   w.phase = phase;
   if (phase == 0) {
     w.cnt = cntA;
@@ -297,12 +297,13 @@ __device__ __forceinline__ int greedy_chunk(GreedyChunk<kChunk>& G, bool alive, 
 
 // ------------------------------------------------------------------ counting pass (only when the decode kernel did not build the histogram)
 // Grid (ceil(A / kRowsPerCta), B); each warp walks rows of ONE image: histogram of score bits (spread global atomics) and the
-// per-row best score (rowmax) that lets the emit passes skip rows.
+// per-row best score (rowmax) that lets the emit passes skip rows.  MULTI: multi-label histogram.  At most 32 registers (8 CTAs per SM):
+// uncapped, the multi-label kernel takes 44.
 constexpr int kRowsPerCta = 64;
 constexpr int kScanThreads = 256;
 
-__global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __restrict__ pred, int A, int nc, float conf, int multi_label,
-                                                                 NmsWs ws) {
+template <bool MULTI>
+__global__ void __launch_bounds__(kScanThreads, 8) nms_count_kernel(const float* __restrict__ pred, int A, int nc, float conf, NmsWs ws) {
   const int no = nc + 5;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
@@ -326,27 +327,10 @@ __global__ void __launch_bounds__(kScanThreads) nms_count_kernel(const float* __
         continue;
       }
       const float* r = pred + ((size_t)b * A + anchor) * no;
-      const float ob = obj[i];
       float rbest = 0.0f;
-      if (multi_label) {
-        for (int c = lane; c < nc; c += 32) {
-          const float sc = yolo_score(__ldg(r + 5 + c), ob);
-          if (sc > conf) {
-            atomicAdd(&hist[nms_score_bin(sc)], 1u);
-            rbest = fmaxf(rbest, sc);
-          }
-        }
-      } else {
-        // best class only: conf, j = x[:, 5:].max(1)
-        for (int c = lane; c < nc; c += 32) rbest = fmaxf(rbest, yolo_score(__ldg(r + 5 + c), ob));
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) rbest = fmaxf(rbest, __shfl_xor_sync(0xffffffffu, rbest, o));
-      if (!(rbest > conf)) rbest = 0.0f;
-      if (lane == 0) {
-        rowmax[anchor] = rbest;
-        if (!multi_label && rbest > conf) atomicAdd(&hist[nms_score_bin(rbest)], 1u);
-      }
+      for (int c = lane; c < nc; c += 32) nms_count_score(hist, yolo_score(__ldg(r + 5 + c), obj[i]), conf, MULTI, rbest);
+      rbest = nms_finish_row(hist, rbest, conf, MULTI, lane);
+      if (lane == 0) rowmax[anchor] = rbest;
     }
   }
 }
@@ -661,6 +645,7 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   CVB_REQUIRE(workspace_bytes >= cvb_nms_workspace_bytes(p->B, p->A, p->nc), "nms: workspace too small");
   CVB_REQUIRE(is_aligned(workspace, 256), "nms: workspace must be 256-byte aligned");
   cudaStream_t st = as_stream(stream);
+  const int multi_label = p->multi_label && p->nc > 1;  // the reference's multi_label &= nc > 1 (include/cvb200.h)
   NmsWs wsA = carve_ws(workspace, p->B, 0), wsB = carve_ws(workspace, p->B, 1);
   if (!p->hist_ready) CVB_CHECK_CUDA(cudaMemsetAsync(workspace, 0, nms_ws_head_bytes(p->B), st));
   if (status) CVB_CHECK_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), st));
@@ -679,13 +664,13 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   CVB_CHECK_CUDA(emit_smem_err);
   CVB_CHECK_CUDA(greedy_smem_err);
   if (!p->hist_ready) {
-    nms_count_kernel<<<sgrid, kScanThreads, 0, st>>>(prediction, p->A, p->nc, p->conf_thres, p->multi_label, wsB);
+    (multi_label ? nms_count_kernel<true> : nms_count_kernel<false>)<<<sgrid, kScanThreads, 0, st>>>(prediction, p->A, p->nc, p->conf_thres, wsB);
     count_launch();
   }
   // ---- phase A: the top ~3k candidates of every image (one shared-memory sort chunk), early exit at max_det
   const int targetA = p->max_nms < kTargetA ? p->max_nms : kTargetA;
   nms_threshold_kernel<<<p->B, 256, 0, st>>>(wsA, targetA);
-  nms_emit_kernel<<<egrid, kScanThreads, stage_bytes, st>>>(prediction, p->A, p->nc, p->conf_thres, p->multi_label, wsA, status);
+  nms_emit_kernel<<<egrid, kScanThreads, stage_bytes, st>>>(prediction, p->A, p->nc, p->conf_thres, multi_label, wsA, status);
   bitonic_local_sort_kernel<<<dim3(1, p->B), 1024, 0, st>>>(wsA);
   nms_greedy_kernel<<<p->B, kGreedyThreads, gsmem, st>>>(prediction, p->A, p->nc, wsA, p->iou_thres, p->max_nms, p->max_det, p->max_wh, det,
                                                          det_idx, det_count);
@@ -693,7 +678,7 @@ extern "C" int cvb_yolo_nms(const float* prediction, const CvbNmsParams* p, floa
   count_launch(4);
   // ---- phase B: full top-max_nms path for the images phase A could not finish (every kernel returns at once otherwise)
   nms_threshold_kernel<<<p->B, 256, 0, st>>>(wsB, p->max_nms);
-  nms_emit_kernel<<<egrid, kScanThreads, stage_bytes, st>>>(prediction, p->A, p->nc, p->conf_thres, p->multi_label, wsB, status);
+  nms_emit_kernel<<<egrid, kScanThreads, stage_bytes, st>>>(prediction, p->A, p->nc, p->conf_thres, multi_label, wsB, status);
   count_launch(2);
   {
     // one CTA per SM: co-residency is guaranteed (required by the grid barriers); resolved once, thread-safe static initialisation

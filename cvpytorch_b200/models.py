@@ -231,7 +231,44 @@ def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=Non
     return out
 
 
-class YOLOv5(_Standalone):
+class _YoloNmsModel(_Standalone):
+    """What the YOLO drop-ins whose cached graph ends in ops.yolo_nms (YOLOv5, YOLOv6) share: ``predict``, ``nms_status`` and the
+    post-processing of forward(mode='val').  A subclass defines ``_graph_for(imgs)``, whose graph reads its input from holder['x'] and
+    leaves the NMS result in its NmsWorkspace 'ws'."""
+
+    def predict(self, imgs):
+        """Device-only inference: returns (det [B,max_det,6] (x1,y1,x2,y2,conf,cls), det_idx [B,max_det] (row*nc + cls), det_count [B])
+        device tensors, no host sync.  The tensors are the GRAPH-OWNED output buffers (overwritten by the next call with the same shape).
+        ``nms_status(imgs)`` returns the device status word of the last run ([0] != 0: the NMS candidate capacity overflowed and the
+        result is invalid); ``forward()`` checks it and raises."""
+        G = self._graph_for(imgs)
+        G['holder']['x'] = imgs.contiguous().float()
+        G['g'].run()
+        return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
+
+    def nms_status(self, imgs):
+        """Device int32[4] status of the NMS stage of the graph that serves `imgs` ([0] = candidate-capacity overflow flag)."""
+        return self._graph_for(imgs)['ws'].status
+
+    def _val(self, imgs, targets):
+        """forward(imgs, targets, 'val'): (losses, per-image {'boxes', 'labels', 'scores'}) with the boxes rescaled and clipped to each
+        image's original geometry, as the reference (yolov5.py:258-282, yolov6.py:209-227)."""
+        det, _, cnt = self.predict(imgs)
+        # the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps the
+        # unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict under cfg.distributed)
+        losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
+        det_h, cnt_h = ops.val_rows_to_host(det.clone(), cnt, targets, imgs.shape[2:])
+        if int(self.nms_status(imgs)[0]) != 0:  # (the copy above already synchronised)
+            raise _lib.CvbError(f'{type(self).__name__} NMS: candidate capacity overflow (more keys in the threshold bin than the workspace '
+                                'holds); the detections of this batch would be truncated non-deterministically')
+        outputs = []
+        for b in range(det_h.shape[0]):
+            pred = det_h[b, :cnt_h[b]]
+            outputs.append({"boxes": pred[:, :4].clone(), "labels": pred[:, 5], "scores": pred[:, 4]})
+        return losses, outputs
+
+
+class YOLOv5(_YoloNmsModel):
     """Model-level drop-in for src.models.yolov5.YOLOv5.  forward(imgs, targets, mode) keeps the reference contract: mode 'val' (eval()) ->
     (losses_dict, outputs list of {'boxes','labels','scores'}) from the cached inference graph; mode 'train' (train()) -> the loss dict
     {'loss', 'box_loss', 'obj_loss', 'cls_loss'} from the training kernels and the YOLOv5Loss over the same parameters."""
@@ -311,20 +348,6 @@ class YOLOv5(_Standalone):
         G['g'].run()
         return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
 
-    def predict(self, imgs):
-        """Device-only inference: returns (det [B,300,6], det_idx [B,300], det_count [B]) device tensors, no host sync.
-        The tensors are the GRAPH-OWNED output buffers (overwritten by the next call with the same shape).  ``nms_status(imgs)``
-        returns the device status word of the last run ([0] != 0: the NMS candidate capacity overflowed and the result is invalid);
-        ``forward()`` checks it and raises."""
-        G = self._graph_for(imgs)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
-
-    def nms_status(self, imgs):
-        """Device int32[4] status of the NMS stage of the graph that serves `imgs` ([0] = candidate-capacity overflow flag)."""
-        return self._graph_for(imgs)['ws'].status
-
     def _training_modules(self):
         """(yolov5_train.YOLOv5CSPDarknet, YOLOv5Neck, YOLOv5Detect) over this model's own parameters, buffers and BatchNorm modules.  Widths
         the training kernels refuse (YOLOv5-m, -x) raise NotImplementedError."""
@@ -366,22 +389,4 @@ class YOLOv5(_Standalone):
             return self.forward_train(imgs, targets)
         if mode != 'val':
             raise RuntimeError(f"YOLOv5 (H100): unknown mode {mode!r}")
-        det, _, cnt = self.predict(imgs)
-        losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
-        # yolov5.py:258: the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps
-        # the unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict under cfg.distributed)
-        # yolov5.py:267-282 on the device (cvb_rescale_clip_boxes: same fp32 subtract / divide / clip as the numpy lines), then ONE
-        # device->host copy instead of one per image
-        rows = det.clone()
-        pads, scales, wh = ops.targets_to_device_geometry(targets, rows.shape[0], imgs.shape[2:], rows.device)
-        ops.rescale_clip_boxes(rows, cnt, pads, scales, wh)
-        det_h = rows.cpu()
-        cnt_h = cnt.cpu().tolist()
-        if int(self.nms_status(imgs)[0]) != 0:  # (the .cpu() above already synchronised)
-            raise _lib.CvbError('YOLOv5 NMS: candidate capacity overflow (more keys in the threshold bin than the workspace holds); '
-                                'the detections of this batch would be truncated non-deterministically')
-        outputs = []
-        for b in range(det_h.shape[0]):
-            pred = det_h[b, :cnt_h[b]]
-            outputs.append({"boxes": pred[:, :4].clone(), "labels": pred[:, 5], "scores": pred[:, 4]})
-        return losses, outputs
+        return self._val(imgs, targets)

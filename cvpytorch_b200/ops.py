@@ -128,7 +128,7 @@ def yolo_decode_desc(na, no, anchors_px, stride, z, z_rows, z_off, nms_ws=None, 
     y.z_rows, y.z_off = int(z_rows), int(z_off)
     y.nms_workspace = nms_ws.ws_ptr if nms_ws is not None else None
     y.conf_thres = float(conf_thres)
-    y.multi_label = 1 if (multi_label and no - 5 > 1) else 0
+    y.multi_label = 1 if multi_label else 0
     return y
 
 
@@ -290,7 +290,7 @@ def yolo_decode(raw_view, na, no, anchors_px, stride, z, z_rows, z_off, xperm=No
                                           z.data_ptr() if z is not None else None, z_rows, z_off,
                                           xperm.data_ptr() if xperm is not None else None,
                                           nms_ws.ws_ptr if nms_ws is not None else None, float(conf_thres),
-                                          1 if (multi_label and no - 5 > 1) else 0, _stream()), 'cvb_yolo_decode')
+                                          1 if multi_label else 0, _stream()), 'cvb_yolo_decode')
 
 
 def yolov6_decode(cls_view, reg_view, nc, stride, z, z_rows, z_off, nms_ws=None, conf_thres=0.001, multi_label=True):
@@ -340,7 +340,7 @@ def yolo_nms(prediction, ws, conf_thres=0.001, iou_thres=0.6, multi_label=True, 
     p = CvbNmsParams()
     p.B, p.A, p.nc = B, A, no - 5
     p.conf_thres, p.iou_thres = conf_thres, iou_thres
-    p.multi_label = 1 if (multi_label and no - 5 > 1) else 0
+    p.multi_label = 1 if multi_label else 0
     p.max_nms, p.max_det, p.max_wh = max_nms, ws.max_det, max_wh
     p.hist_ready = 1 if hist_ready else 0
     _lib.check(_lib.lib().cvb_yolo_nms(prediction.data_ptr(), byref(p), ws.det.data_ptr(), ws.det_idx.data_ptr(),
@@ -464,6 +464,15 @@ def targets_to_device_geometry(targets, B, default_hw, device):
         if 'height' in t:
             wh[i, 1] = float(t['height'])
     return pads.to(device), scales.to(device), wh.to(device)
+
+
+def val_rows_to_host(rows, count, targets, default_hw):
+    """The val post-processing of the YOLO drop-ins: the boxes of rows [B,M,>=4] (a device tensor the caller owns) are rescaled and
+    clipped in place to each image's original geometry (targets' pads / scales / width / height), then ONE device->host copy instead
+    of one per image.  Returns (rows on the host, count as a list)."""
+    pads, scales, wh = targets_to_device_geometry(targets, rows.shape[0], default_hw, rows.device)
+    rescale_clip_boxes(rows, count, pads, scales, wh)
+    return rows.cpu(), count.cpu().tolist()
 
 
 def confusion_matrix(gt, pred, num_classes, out=None):

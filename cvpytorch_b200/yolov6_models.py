@@ -24,8 +24,9 @@ the NMS pre-pass, after which the YOLOv5 NMS (ops.yolo_nms, hist_ready) selects 
 import torch
 import torch.nn as nn
 
-from . import _lib, ops
+from . import ops
 from .engine import GraphBuilder
+from .models import _YoloNmsModel
 from .modules import ConvModule, _build, _EmitModule, _Standalone, folded
 from .yolo_blocks import RepBlock, RepVGGBlock
 
@@ -357,7 +358,7 @@ class YOLOv6Loss(nn.Module):
         raise NotImplementedError('YOLOv6 (H100): training and the YOLOv6 loss are not on the H100 path')
 
 
-class YOLOv6(_Standalone):
+class YOLOv6(_YoloNmsModel):
     """Model-level drop-in for the reference's YOLOv6 (YAML route conf/det/yolov6/coco_yolov6_{n,s}.yml, USE_MODEL): same state_dict keys
     as its YOLODetector; forward(imgs, targets, 'val') runs the cached inference graph with the val contract of src/models/yolov6.py."""
 
@@ -401,18 +402,6 @@ class YOLOv6(_Standalone):
         return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device),
                            float(self.conf_thres), float(self.iou_thres), int(self.max_det))
 
-    def predict(self, imgs):
-        """Device-only inference: (det [B,300,6] (x1,y1,x2,y2,conf,cls), det_idx [B,300] (row*nc + cls), det_count [B]), no host sync.
-        The tensors are the graph-owned output buffers (overwritten by the next call with the same shape)."""
-        G = self._graph_for(imgs)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
-
-    def nms_status(self, imgs):
-        """Device int32[4] status of the NMS stage of the graph that serves `imgs` ([0] = candidate-capacity overflow flag)."""
-        return self._graph_for(imgs)['ws'].status
-
     def forward(self, imgs, targets=None, mode='infer', **kwargs):
         if mode == 'infer':
             return
@@ -422,18 +411,4 @@ class YOLOv6(_Standalone):
             raise RuntimeError(f"YOLOv6 (H100): unknown mode {mode!r}")
         if isinstance(imgs, (list, tuple)):
             imgs = torch.stack(list(imgs))
-        det, _, cnt = self.predict(imgs)
-        losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}  # yolov6.py:209 (a 0 loss in 'val')
-        # yolov6.py:214-227 on the device (cvb_rescale_clip_boxes), then ONE device->host copy
-        rows = det.clone()
-        pads, scales, wh = ops.targets_to_device_geometry(targets, rows.shape[0], imgs.shape[2:], rows.device)
-        ops.rescale_clip_boxes(rows, cnt, pads, scales, wh)
-        det_h, cnt_h = rows.cpu(), cnt.cpu().tolist()
-        if int(self.nms_status(imgs)[0]) != 0:  # (the .cpu() above already synchronised)
-            raise _lib.CvbError('YOLOv6 NMS: candidate capacity overflow (more keys in the threshold bin than the workspace holds); '
-                                'the detections of this batch would be truncated non-deterministically')
-        outputs = []
-        for b in range(det_h.shape[0]):
-            pred = det_h[b, :cnt_h[b]]
-            outputs.append({"boxes": pred[:, :4].clone(), "labels": pred[:, 5], "scores": pred[:, 4]})
-        return losses, outputs
+        return self._val(imgs, targets)

@@ -356,12 +356,9 @@ class YOLOX(_Standalone):
         losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
         # yolox.py:156: the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps
         # the unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict under cfg.distributed)
-        # yolox.py:165-178 on the device (cvb_rescale_clip_boxes), then ONE device->host copy of the kept prefix
+        # yolox.py:165-178 on the device, then ONE device->host copy of the kept prefix
         kmax = max(int(cnt.max()), 1)
-        rows = det[:, :kmax].contiguous()
-        pads, scales, wh = ops.targets_to_device_geometry(targets, rows.shape[0], imgs.shape[2:], rows.device)
-        ops.rescale_clip_boxes(rows, cnt, pads, scales, wh)
-        det_h, cnt_h = rows.cpu(), cnt.cpu().tolist()
+        det_h, cnt_h = ops.val_rows_to_host(det[:, :kmax].contiguous(), cnt, targets, imgs.shape[2:])
         outputs = []
         for i in range(det_h.shape[0]):
             pred = det_h[i, :cnt_h[i]]

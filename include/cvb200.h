@@ -80,7 +80,7 @@ typedef struct CvbYoloDecode {
   int64_t z_rows, z_off;
   void* nms_workspace;     /* prepared with cvb_nms_workspace_reset (sized for A = z_rows), or NULL */
   float conf_thres;
-  int32_t multi_label;
+  int32_t multi_label;     /* as CvbNmsParams.multi_label (ignored with one class) */
 } CvbYoloDecode;
 
 typedef struct CvbConvDesc {
@@ -224,6 +224,7 @@ int cvb_sppf_pool(const CvbView* x, const CvbView* y1, const CvbView* y2, const 
  *   NMS score histogram and the per-row best score (conf_thres / multi_label as later passed to cvb_yolo_nms with
  *   hist_ready = 1; z_rows must then be the A of that call, the workspace must have been sized for it), which saves one full
  *   pass over the prediction tensor and lets the NMS emit passes skip rows below their threshold.
+ *   With z, the level's rows [z_off, z_off + na*ny*nx) must lie inside [0, z_rows); the fused head (CvbYoloDecode) checks the same.
  * replaces: YOLOv5Detect.forward src/models/detects/yolov5_detect.py:42-55, _make_grid :60-65.
  */
 int cvb_yolo_decode(const CvbView* raw, int32_t na, int32_t no, const float* anchors_px /*[na*2]*/, float stride,
@@ -245,7 +246,9 @@ typedef struct CvbNmsParams {
   int32_t B, A, nc;
   float conf_thres;    /* compared in fp32: x > float(conf_thres) like the reference's tensor > scalar */
   double iou_thres;    /* compared in double: torchvision's CPU kernel tests float IoU > double threshold */
-  int32_t multi_label; /* 1: one candidate per (box,class) pair; 0: best class only */
+  int32_t multi_label; /* 1: one candidate per (box,class) pair; 0: best class only.  Ignored when nc == 1 (the reference's
+                          multi_label &= nc > 1, yolov5.py:82): one class gives the same candidates either way.  The decode entry
+                          points that build the histogram for hist_ready = 1 apply the same rule. */
   int32_t max_nms;     /* 30000 */
   int32_t max_det;     /* 300   */
   float max_wh;        /* 4096 class offset; 0 = agnostic */
@@ -256,7 +259,8 @@ typedef struct CvbNmsParams {
  * YOLOv6 anchor-free decode of one level (src/models/detects/yolov6_detect.py:36-50 with generate_anchors(..., mode='af') and
  * dist2bbox(..., 'xywh')).  cls / reg: fp32 NHWC views [B,h,w,>=nc] (class logits) and [B,h,w,>=4] (ltrb distances), the outputs of the
  * head's cls_preds / reg_preds 1x1 convs.  Writes z[b, z_off + y*w + x, :] = (cx, cy, w, h, 1.0, sigmoid(cls_0..nc-1)) with anchor
- * (x + 0.5, y + 0.5), box = ((a - lt + a + rb) / 2, rb + lt) * stride in the reference's fp32 operation order; nc <= 91.
+ * (x + 0.5, y + 0.5), box = ((a - lt + a + rb) / 2, rb + lt) * stride in the reference's fp32 operation order; nc <= 91.  The rows
+ * [z_off, z_off + h*w) must lie inside [0, z_rows).
  * nms_workspace (optional): as for cvb_yolo_decode -- the histogram and per-row best scores of cvb_yolo_nms(hist_ready = 1).  With the
  * objectness exactly 1.0 the YOLOv5 NMS keeps the rows and scores of the YOLOv6 one (src/models/yolov6.py:32-107).
  */

@@ -732,6 +732,45 @@ def test_fast_decode_vs_formula(cuda, no, multi, hist, na, nx, xperm):
         nms_consistency(zl, h, rowmax[:, z_off:z_off + na * npix], conf, multi and no - 5 > 1, f'decode no={no}')
 
 
+@pytest.mark.parametrize('producer', ['yolov6_decode', 'count_pass'])
+@pytest.mark.parametrize('nc,multi', [(80, True), (80, False), (1, True), (1, False)])
+def test_prepass_producers_vs_z(cuda, producer, nc, multi):
+    """The histogram / rowmax of the other two producers of the NMS pre-pass against their own z: cvb_yolov6_decode and the NMS counting
+    pass (yolo_nms with hist_ready=False).  With one class both multi_label values must build the best-class pre-pass (the reference's
+    multi_label &= nc > 1, applied by the C entry points), and the counting pass's NMS rows equal the oracle's for both."""
+    from cvpytorch_b200 import ops
+    from oracle import nms_oracle as NO
+    B, ny, nx, z_off, conf = 2, 10, 13, 2, 0.05
+    no, A = nc + 5, ny * nx + z_off + 3
+    g = torch.Generator().manual_seed(90 + nc)
+    ws = ops.NmsWorkspace(B, A, nc)
+    if producer == 'yolov6_decode':
+        cls, reg = ops.F32Tensor(B, ny, nx, (nc + 31) // 32 * 32), ops.F32Tensor(B, ny, nx, 32)
+        cls.data.copy_(torch.randn(cls.data.shape, generator=g) * 3)
+        reg.data.copy_(torch.rand(reg.data.shape, generator=g) * 4)
+        z = torch.full((B, A, no), float('nan'), device='cuda')
+        ops.nms_reset(ws)
+        ops.yolov6_decode(cls.view(0, nc), reg.view(0, 4), nc, 8.0, z, A, z_off, ws, conf, multi)
+        rows = slice(z_off, z_off + ny * nx)
+    else:
+        z = torch.rand(B, A, no, generator=g)
+        z[..., :2] *= 640
+        z[..., 2:4] *= 64
+        z = z.cuda()
+        det, idx, cnt = ops.yolo_nms(z, ws, conf, 0.6, multi)
+        rows = slice(0, A)
+    torch.cuda.synchronize()
+    h, rowmax = _ws_regions(ws, B, A)
+    nms_consistency(z[:, rows], h, rowmax[:, rows], conf, multi and nc > 1, f'{producer} nc={nc} multi={multi}')
+    if producer == 'count_pass':
+        assert int(ws.status[0]) == 0
+        ref = NO.non_max_suppression(z.cpu().numpy(), conf, 0.6, multi_label=multi)
+        for b in range(B):
+            k = int(cnt[b])
+            assert k == ref[b][0].shape[0] and torch.equal(idx[b, :k].cpu().long(), torch.from_numpy(ref[b][1]))
+            assert torch.equal(det[b, :k].cpu(), torch.from_numpy(ref[b][0]))
+
+
 def test_decode_checks_teeth(cuda):
     """The decode checks reject one z element moved by twice its bound, one NaN, and a histogram count or a rowmax off by one step."""
     from cvpytorch_b200 import ops

@@ -5,9 +5,15 @@ Rows, indices and counts are compared with np.array_equal: these kernels have no
 scores come from bit patterns (histogram bin = fp32 bits >> 17), so the sort size, the threshold bin and the phase that finishes
 an image are chosen by the test, and each test asserts from the workspace (`done` / `cnt` / `total` / `tbin`, `status`,
 `det_count`) that it reached the path it is named after."""
+import os
+import sys
+
 import numpy as np
 import pytest
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from test_post_gpu import _ws_regions  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -84,19 +90,18 @@ def big_scene(n, A=None, nc=4):
 
 # ------------------------------------------------------------------------------------------------ YOLOv5 harness
 def ws_regions(ws):
-    """Views of every region of an NmsWorkspace (layout: csrc/internal.h and carve_ws in csrc/nms.cu)."""
-    B, A = ws.B, ws.A
+    """Views of every region of an NmsWorkspace: the histogram and rowmax of test_post_gpu._ws_regions, and the per-image slots and
+    key arrays between them (carve_ws in csrc/nms.cu)."""
+    B = ws.B
     al = lambda x, a: (x + a - 1) // a * a
     hist_bytes, slot = al(B * BINS * 4, 256), al(B * 4, 256)
     head = hist_bytes + 6 * slot
     raw = ws.ws[ws.ws_ptr - ws.ws.data_ptr():]
-    r = {'hist': raw[:B * BINS * 4].view(torch.int32).view(B, BINS)}
+    r = dict(zip(('hist', 'rowmax'), _ws_regions(ws, B, ws.A)))
     for i, name in enumerate(('cntB', 'tbinB', 'cntA', 'tbinA', 'done', 'total')):
         r[name] = raw[hist_bytes + i * slot:hist_bytes + i * slot + B * 4].view(torch.int32)
     r['keysB'] = raw[head:head + B * CAP_B * 8].view(torch.int64).view(B, CAP_B)
     r['keysA'] = raw[head + B * CAP_B * 8:head + B * (CAP_B + CAP_A) * 8].view(torch.int64).view(B, CAP_A)
-    rm = head + B * (CAP_B + CAP_A) * 8
-    r['rowmax'] = raw[rm:rm + B * A * 4].view(torch.float32).view(B, A)
     return r
 
 
@@ -364,6 +369,28 @@ def test_yolov5_rejected_arguments(cuda):
         call(nc=321)
     with pytest.raises(CvbError, match='nms: workspace must be 256-byte aligned'):
         call(shift=16)
+
+    # a decode level must write inside z's rows: [z_off, z_off + rows) within [0, z_rows), rows = na * ny * nx (YOLOv5) or ny * nx (YOLOv6)
+    na, no, ny, nx, A = 3, 85, 4, 5, 60
+    anchors = torch.tensor([[10., 13.], [16., 30.], [33., 23.]])
+    z = torch.zeros((1, A + 1, no), device='cuda')
+    raw = ops.F32Tensor(1, ny, nx, 256)
+    for off in (-1, 1):
+        with pytest.raises(CvbError, match=rf"yolo_decode: level rows \[{off}, {off + A}\) outside z's {A} rows"):
+            ops.yolo_decode(raw.view(0, na * no), na, no, anchors.cuda(), 8.0, z, A, off, None, None, 0.05, True)
+    ops.yolo_decode(raw.view(0, na * no), na, no, anchors.cuda(), 8.0, z, A + 1, 1, None, None, 0.05, True)
+    cls, reg = ops.F32Tensor(1, ny, nx, 96), ops.F32Tensor(1, ny, nx, 32)
+    with pytest.raises(CvbError, match=r"yolov6_decode: level rows \[1, 21\) outside z's 20 rows"):
+        ops.yolov6_decode(cls.view(0, 80), reg.view(0, 4), 80, 8.0, z[:, :20].contiguous(), 20, 1)
+    tin = ops.SplitTensor(1, ny, nx, 64)
+    wy, by = ops.pack_yolo_head_weights(torch.zeros(na * no, 64, 1, 1, dtype=torch.float64), torch.zeros(na * no, dtype=torch.float64), na, no)
+    for off in (-1, 1):
+        y = ops.yolo_decode_desc(na, no, anchors, 8.0, z, A, off)
+        with pytest.raises(CvbError, match=rf"conv\(yolo\): level rows \[{off}, {off + A}\) outside z's {A} rows"):
+            ops.ConvPlan(tin.view(), ops.CvbView(z.data_ptr(), 1, ny, nx, na * 128, na * 128, 0), wy, by, 1, yolo=y)
+    ops.ConvPlan(tin.view(), ops.CvbView(z.data_ptr(), 1, ny, nx, na * 128, na * 128, 0), wy, by, 1, yolo=ops.yolo_decode_desc(
+        na, no, anchors, 8.0, z, A + 1, 1))
+    torch.cuda.synchronize()
 
 
 # ================================================================================================ YOLOX
