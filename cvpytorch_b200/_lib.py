@@ -71,6 +71,17 @@ class CvbCocoEvalParams(ctypes.Structure):
                 ('rec_thrs', c_double * CVB_COCO_REC_THRS)]
 
 
+CVB_YOLOV6_MAX_LEVELS = 8
+CVB_YOLOV6_ATSS, CVB_YOLOV6_TAL = 0, 1
+CVB_YOLOV6_GIOU, CVB_YOLOV6_SIOU = 0, 1
+
+
+class CvbYolov6LossParams(ctypes.Structure):
+    _fields_ = [('B', c_int32), ('nc', c_int32), ('nlev', c_int32), ('h', c_int32 * CVB_YOLOV6_MAX_LEVELS), ('w', c_int32 * CVB_YOLOV6_MAX_LEVELS),
+                ('strides', c_float * CVB_YOLOV6_MAX_LEVELS), ('grid_cell_size', c_float), ('grid_cell_offset', c_float), ('ori_img_size', c_float),
+                ('assigner', c_int32), ('iou_type', c_int32), ('loss_weight', c_double * 3)]
+
+
 CVB_SEG_U8, CVB_SEG_I32, CVB_SEG_I64 = 0, 1, 2
 CVB_SEG_ERR_NEGATIVE, CVB_SEG_ERR_OVERFLOW = 1, 2
 CVB_SEG_MAX_N = (1 << 31) - 1  # pixels per cvb_seg_confusion_update call
@@ -123,6 +134,11 @@ SYMBOLS = {
     'cvb_train_fcos_loss_bwd': (c_int32, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), POINTER(c_float),
                                           c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, POINTER(c_void_p),
                                           POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    'cvb_train_yolov6_loss_workspace_bytes': (c_size_t, [POINTER(CvbYolov6LossParams), c_int32]),
+    'cvb_train_yolov6_loss_fwd': (c_int32, [POINTER(CvbYolov6LossParams), c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'cvb_train_yolov6_loss_bwd': (c_int32, [POINTER(CvbYolov6LossParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p]),
     'cvb_ema_table_upload':(c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
     'cvb_ema_update': (c_int32, [c_void_p, c_int32, c_float, c_float, c_void_p]),
     'cvb_sgd_table_upload': (c_int32, [POINTER(CvbSgdEntry), c_int32, c_int32, c_void_p, c_void_p]),

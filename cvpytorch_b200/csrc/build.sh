@@ -17,11 +17,11 @@ FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler
 TMP="$(mktemp -d)"
 trap 'rm -rf "$TMP"' EXIT
 pids=()
-for src in api conv_tc aux_kernels nms train_kernels yolox_loss yolov5_loss fcos_loss ema sgd coco_eval seg_eval seg_loss; do
+for src in api conv_tc aux_kernels nms train_kernels yolox_loss yolov5_loss fcos_loss yolov6_loss ema sgd coco_eval seg_eval seg_loss; do
   FILE_FLAGS=()
   # the losses, the EMA and SGD follow the reference's fp32 operation order, and the COCO evaluation pycocotools' float64 one: no contracted
   # multiply-adds
-  [[ "$src" == yolox_loss || "$src" == yolov5_loss || "$src" == fcos_loss || "$src" == ema || "$src" == sgd || "$src" == coco_eval ]] && FILE_FLAGS=(--fmad=false)
+  [[ "$src" == yolox_loss || "$src" == yolov5_loss || "$src" == fcos_loss || "$src" == yolov6_loss || "$src" == ema || "$src" == sgd || "$src" == coco_eval ]] && FILE_FLAGS=(--fmad=false)
   "$NVCC" "${FLAGS[@]}" "${FILE_FLAGS[@]}" "${EXTRA[@]}" "$@" -c "$HERE/$src.cu" -o "$TMP/$src.o" &
   pids+=($!)
 done

@@ -525,6 +525,45 @@ int cvb_train_fcos_loss_bwd(const float* const* cls, const float* const* cnt, co
                             const int32_t* matched_gt, const int32_t* num_pos, const float* grad_out, float* const* gcls, float* const* gcnt,
                             float* const* greg, void* stream);
 
+/* YOLOv6 training loss (src/losses/det/yolov6_loss.py with src/models/assigners/{atss,tal}_assigner.py; csrc/yolov6_loss.cu): target
+ * packing, the ATSS (topk 9) or task-aligned (topk 13, alpha 1, beta 6) assignment, the 1 - GIoU / 1 - SIoU box loss (eps 1e-10) and its
+ * gradient with respect to pred_distri.  Anchors: per level l (1 <= nlev <= 8) an h[l] x w[l] grid of stride strides[l] (a positive
+ * integer), in level order and row-major within a level (A = sum h w); the anchor point is ((column + grid_cell_offset) stride, (row +
+ * grid_cell_offset) stride) and the ATSS anchor box that point -+ grid_cell_size stride / 2.  pred_scores fp32 [B, A, nc] (class
+ * probabilities), pred_distri fp32 [B, A, 4] (l, t, r, b in stride units, 16-byte aligned).  gt fp64 [nt, 6] = (image, label, cx, cy, w, h),
+ * the box normalised by ori_img_size; a row's image is int()-truncated and rows outside [0, B) are dropped (the reference wraps -1).  Each
+ * image's rows keep their input order; a row whose x1 + y1 + x2 + y2 <= 0 is not a GT (mask_gt = 0).  A label outside [0, nc) gives a zero
+ * class score (the reference raises).  Ties: among equal distances (ATSS) or metrics (TAL) at the top-k boundary the lowest anchor index
+ * is taken.  An anchor claimed by several GTs goes to the first IoU maximum over all of its image's rows.
+ * cvb_train_yolov6_loss_fwd: out fp64 [3] = loss_weight[k] L with L = sum over positives of soft label (1 - IoU) / target_scores_sum (not
+ *   divided when that sum is 0), or 0 * sum(pred_distri) without positives.  Per anchor, kept for the backward: fg_mask u8 [B, A],
+ *   gt_idx int32 [B, A] (the GT's row within its image, 0 for background), labels int32 [B, A] (nc for background), target_boxes fp64
+ *   [B, A, 4] (x1, y1, x2, y2 pixels; background: the image's first row), target_scores fp64 [B, A] (the soft label summed over classes,
+ *   0 for background); stats fp64 [4] = (sum soft label (1 - IoU), target_scores_sum, num_pos, sum pred_distri).  workspace:
+ *   cvb_train_yolov6_loss_workspace_bytes(p, nt) bytes (0 for invalid params), 256-byte aligned.  No host sync; bitwise reproducible.
+ * cvb_train_yolov6_loss_bwd: grad_distri fp32 [B, A, 4] (every element written) = d(sum_k grad_out[k] out[k]) / d(pred_distri) under
+ *   the forward's assignment; grad_out fp64 [3] on the device.  pred_scores gets no gradient (the reference's class loss is unused).
+ */
+#define CVB_YOLOV6_MAX_LEVELS 8
+#define CVB_YOLOV6_ATSS 0
+#define CVB_YOLOV6_TAL 1
+#define CVB_YOLOV6_GIOU 0
+#define CVB_YOLOV6_SIOU 1
+typedef struct {
+  int32_t B, nc, nlev;
+  int32_t h[CVB_YOLOV6_MAX_LEVELS], w[CVB_YOLOV6_MAX_LEVELS];
+  float strides[CVB_YOLOV6_MAX_LEVELS];
+  float grid_cell_size, grid_cell_offset, ori_img_size;
+  int32_t assigner, iou_type;  /* CVB_YOLOV6_ATSS / _TAL; CVB_YOLOV6_GIOU / _SIOU */
+  double loss_weight[3];       /* (iou, dfl, class) */
+} CvbYolov6LossParams;
+size_t cvb_train_yolov6_loss_workspace_bytes(const CvbYolov6LossParams* p, int32_t nt);
+int cvb_train_yolov6_loss_fwd(const CvbYolov6LossParams* p, const float* pred_scores, const float* pred_distri, const double* gt, int32_t nt,
+                              uint8_t* fg_mask, int32_t* gt_idx, int32_t* labels, double* target_boxes, double* target_scores, double* stats,
+                              double* out, void* workspace, size_t ws_bytes, void* stream);
+int cvb_train_yolov6_loss_bwd(const CvbYolov6LossParams* p, const float* pred_distri, const uint8_t* fg_mask, const double* target_boxes,
+                              const double* target_scores, const double* stats, const double* grad_out, float* grad_distri, void* stream);
+
 size_t cvb_train_yolox_loss_workspace_bytes(int32_t B, int32_t A);
 int cvb_train_yolox_loss_fwd(const float* const* preds, const int32_t* shapes, const float* strides, int32_t nlev, int32_t nc, const float* targets,
                              int32_t B, int32_t max_gt, int32_t* matched_gt, float* matched_iou, float* out, void* workspace, size_t ws_bytes,
