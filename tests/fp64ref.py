@@ -192,6 +192,23 @@ def conv_out64(d):
     return split64(d) if d.dtype == torch.float16 else d.double().permute(0, 3, 1, 2)
 
 
+def split_conv_sums(pairs, k, s=1, p=0, dil=1, w_window=0, out_h=None):
+    """The conv kernel's dot products in float64, without bias or epilogue: for each (x [B, C, H, W], w [cout, K] in the packed K order)
+    of `pairs`, the NCHW conv with the kernel's geometry (see split_conv_reference).  -> ([conv of each pair], taps, K per tap)."""
+    x0, w0 = pairs[0]
+    cout = w0.shape[0]
+    if w_window:
+        C = x0.shape[1]
+        Ho = x0.shape[2] if out_h is None else out_h
+
+        def conv(x, w):
+            x = F.pad(x, (0, 0, p, max(0, Ho + k - 1 - p - x.shape[2])))[:, :, :Ho + k - 1]
+            return F.conv2d(x, w.view(cout, k, w_window, C).permute(0, 3, 1, 2))
+        return [conv(x, w) for x, w in pairs], k, w_window * C
+    cin = x0.shape[1]
+    return [F.conv2d(x, w.view(cout, k, k, cin).permute(0, 3, 1, 2), None, s, p, dil) for x, w in pairs], k * k, cin
+
+
 def split_conv_reference(tin, wp, bp, k, s=1, p=0, dil=1, act='silu', residual=None, resid_first=0, resid_scale=1.0, up=None,
                          w_window=0, block_n=128, cout=None, out_h=None):
     """float64 reference of the fused conv kernel (csrc/conv_tc.cu) and the element-wise bound of its error -> (ref, bound), NCHW.
@@ -223,18 +240,7 @@ def split_conv_reference(tin, wp, bp, k, s=1, p=0, dil=1, act='silu', residual=N
     x = split64(tin)
     cout = wp.shape[1] if cout is None else cout
     w = (wp[0].double() + wp[1].double())[:cout]
-    if w_window:
-        C = x.shape[1]
-        Ho = x.shape[2] if out_h is None else out_h
-        w = w.view(cout, k, w_window, C).permute(0, 3, 1, 2)
-        x = F.pad(x, (0, 0, p, max(0, Ho + k - 1 - p - x.shape[2])))[:, :, :Ho + k - 1]
-        taps, k_tap = k, w_window * C
-        ref, absref = F.conv2d(x, w), F.conv2d(x.abs(), w.abs())
-    else:
-        cin = x.shape[1]
-        w = w.view(cout, k, k, cin).permute(0, 3, 1, 2)
-        taps, k_tap = k * k, cin
-        ref, absref = F.conv2d(x, w, None, s, p, dil), F.conv2d(x.abs(), w.abs(), None, s, p, dil)
+    (ref, absref), taps, k_tap = split_conv_sums([(x, w), (x.abs(), w.abs())], k, s, p, dil, w_window, out_h)
     b = bp[:cout].double().view(1, -1, 1, 1)
     ref, absref = ref + b, absref + b.abs()
     Ho, Wo = ref.shape[2:]

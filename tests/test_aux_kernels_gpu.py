@@ -529,8 +529,12 @@ def test_yolox_decode(cuda, nc, H, W):
       cx = (p0 + px) * stride: two roundings, gamma_2 (|p0| + px) stride;  w = expf(p2) * stride: (2^-22 + u) w;
       x1 = cx - w / 2 (w / 2 exact): e_cx + e_w / 2 + u |x1|;  obj = sigmoid_fast: sigmoid_fast_rel_err;
       class_conf = the largest class sigmoid: the largest class bound;  score = obj * conf: e_obj conf + obj e_conf + u score."""
+    _yolox_case(nc, 3, H, W, 16.0)
+
+
+def _yolox_case(nc, B, H, W, stride):
     ops = _ops()
-    B, stride, off = 3, 16.0, 5
+    off = 5
     A = off + H * W + 4
     g = _gen(nc * 10 + H * W)
     ro = ops.F32Tensor(B, H, W, 8)
