@@ -116,6 +116,13 @@ SYMBOLS = {
     'cvb_train_conv_wgrad_pad': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_train_pred_conv': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     'cvb_train_pred_grad': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_bn_relu_fwd': (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_bn_relu_bwd': (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_repvgg_fwd': (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_repvgg_bwd': (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_convt_scatter': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_convt_gather': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_train_yolox_loss_workspace_bytes': (c_size_t, [c_int32, c_int32]),
     'cvb_train_yolox_loss_fwd': (c_int32, [POINTER(c_void_p), POINTER(c_int32), POINTER(c_float), c_int32, c_int32, c_void_p, c_int32, c_int32,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -6,13 +6,15 @@
 // its autograd backward (what trainer.py:177-207 runs through cuDNN / ATen):
 //   forward   y = conv(x, W)                         tconv_kernel            (M = 128 pixels, N = cout tile, K = taps x cin)
 //             batch mean / var of y                  bn_stats_kernel + bn_finalize_kernel
-//             a = silu(gamma * (y - mean) * rstd + beta)     bn_silu_fwd_kernel
-//   backward  dz = da * silu'(z);  sum(dz), sum(dz * xhat)   bn_silu_bwd_reduce_kernel   (or dz straight from the consumer's dgrad epilogue)
-//             dy = gamma * rstd * (dz - mean(dz) - xhat * mean(dz * xhat))   bn_silu_bwd_apply_kernel
+//             a = silu(gamma * (y - mean) * rstd + beta)     bn_act_fwd_kernel<kActSilu>
+//   backward  dz = da * silu'(z);  sum(dz), sum(dz * xhat)   bn_act_bwd_reduce_kernel   (or dz straight from the consumer's dgrad epilogue)
+//             dy = gamma * rstd * (dz - mean(dz) - xhat * mean(dz * xhat))   bn_act_bwd_apply_kernel
 //             dx = conv(dy, W rotated by 180 degrees, in/out swapped)   tconv_kernel again (optionally with the PRODUCER's SiLU' in the epilogue)
 //             dW[co][tap][ci] = sum_pixels dy[p][co] * x[p + tap][ci]    twgrad_kernel   (K = pixels: both operands MN-major in shared memory)
 // nn.SyncBatchNorm (statistics over every rank's pixels): bn_stats_kernel + bn_partial_kernel -> all-gather of the fp64 records ->
-// bn_merge_kernel; backward bn_silu_bwd_reduce_kernel -> all-reduce of the two sums -> bn_silu_bwd_apply_kernel with the global count.
+// bn_merge_kernel; backward bn_act_bwd_reduce_kernel -> all-reduce of the two sums -> bn_act_bwd_apply_kernel with the global count.
+// YOLOv6 adds the same passes with ReLU (<kActRelu>), the RepVGG branch sum relu(bn3(y3) + bn1(y1) [+ bnid(x)]) with its backward
+// (repvgg_*_kernel) and the ConvTranspose2d(c, c, 2, stride 2) scatter / gather around a 1x1 GEMM of 4c columns (convt_*_kernel).
 //
 // Layout: activations and gradients are NHWC bf16, dense (pitch == C; C = 16, 32 or a multiple of 64, and TMA zero-fills a box's channels
 // past a 16- or 32-channel C); weights bf16 [cout][kh*kw][kpad(cin)] (K-major rows, zero-padded to 64 channels), fp32 master weights / fp32
@@ -496,8 +498,26 @@ __global__ void bn_merge_kernel(const double* __restrict__ recs, int world, int 
   if (c == 0) *count = n;
 }
 
-// a = silu(y * scale + shift)
-__global__ void __launch_bounds__(kEwThreads) bn_silu_fwd_kernel(const __nv_bfloat16* __restrict__ y, long long nvec, int C, const float* __restrict__ stat,
+__device__ __forceinline__ float silu_grad(float z) {
+  const float g = 1.0f / (1.0f + __expf(-z));
+  return g * fmaf(z, 1.0f - g, 1.0f);
+}
+
+// The activation after a training BatchNorm: SiLU (YOLOX, YOLOv5, the YOLOv6 head) or ReLU (the YOLOv6 backbone and neck).  The ReLU
+// gradient passes where z > 0, torch's rule; z is the same fp32 fmaf(y, scale, shift) in the forward and both backward passes.
+enum : int { kActSilu = 0, kActRelu = 1 };
+template <int ACT>
+__device__ __forceinline__ float act_fwd(float z) {
+  return ACT == kActRelu ? fmaxf(z, 0.0f) : z / (1.0f + __expf(-z));
+}
+template <int ACT>
+__device__ __forceinline__ float act_grad(float z) {
+  return ACT == kActRelu ? (z > 0.0f ? 1.0f : 0.0f) : silu_grad(z);
+}
+
+// a = act(y * scale + shift)
+template <int ACT>
+__global__ void __launch_bounds__(kEwThreads) bn_act_fwd_kernel(const __nv_bfloat16* __restrict__ y, long long nvec, int C, const float* __restrict__ stat,
                                                                  __nv_bfloat16* __restrict__ out) {
   const int cv = C / 8;
   const long long stride = (long long)gridDim.x * kEwThreads;
@@ -513,7 +533,7 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_fwd_kernel(const __nv_bflo
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const float z = fmaf(f[k], __ldg(stat + 2 * C + c0 + k), __ldg(stat + 3 * C + c0 + k));
-        f[k] = z / (1.0f + __expf(-z));
+        f[k] = act_fwd<ACT>(z);
       }
       reinterpret_cast<uint4*>(out)[i] = float_to_bf16x8(f);
     }
@@ -524,20 +544,16 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_fwd_kernel(const __nv_bflo
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const float z = fmaf(f[k], __ldg(stat + 2 * C + c0 + k), __ldg(stat + 3 * C + c0 + k));
-        f[k] = z / (1.0f + __expf(-z));
+        f[k] = act_fwd<ACT>(z);
       }
       reinterpret_cast<uint4*>(out)[i2] = float_to_bf16x8(f);
     }
   }
 }
 
-__device__ __forceinline__ float silu_grad(float z) {
-  const float g = 1.0f / (1.0f + __expf(-z));
-  return g * fmaf(z, 1.0f - g, 1.0f);
-}
-
-// sums[c] += sum_p dz, sums[C + c] += sum_p dz * xhat   (dz = g * silu'(z) when `g` is d(loss)/d(a); dz = g when g_is_dz)
-__global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, long long npix,
+// sums[c] += sum_p dz, sums[C + c] += sum_p dz * xhat   (dz = g * act'(z) when `g` is d(loss)/d(a); dz = g when g_is_dz)
+template <int ACT>
+__global__ void __launch_bounds__(kEwThreads) bn_act_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, long long npix,
                                                                         int C, const float* __restrict__ stat, int g_is_dz, float* __restrict__ sums) {
   __shared__ float s_part[kRedSmemFloats];
   const int cv = C / 8;
@@ -566,7 +582,7 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_reduce_kernel(const __
       bf16x8_to_float(ug, fg);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float dz = g_is_dz ? fg[i] : fg[i] * silu_grad(fmaf(fy[i], sc[i], sh[i]));
+        const float dz = g_is_dz ? fg[i] : fg[i] * act_grad<ACT>(fmaf(fy[i], sc[i], sh[i]));
         a1[i] += dz;
         a2[i] = fmaf(dz, (fy[i] - mean[i]) * rstd[i], a2[i]);
       }
@@ -576,8 +592,8 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_reduce_kernel(const __
 }
 
 // dy = gamma * rstd * (dz - sum_dz / N - xhat * sum_dzx / N);  1 / N = inv_n, or (DEV_COUNT: N over every rank) 1 / *count, read on the device
-template <bool DEV_COUNT>
-__global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, long long nvec, int C,
+template <int ACT, bool DEV_COUNT>
+__global__ void __launch_bounds__(kEwThreads) bn_act_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, long long nvec, int C,
                                                                        const float* __restrict__ stat, const float* __restrict__ gamma, const float* __restrict__ sums,
                                                                        float inv_n, const double* __restrict__ count, int g_is_dz, __nv_bfloat16* __restrict__ dy) {
   if (DEV_COUNT) inv_n = (float)(1.0 / __ldg(count));
@@ -601,7 +617,7 @@ __global__ void __launch_bounds__(kEwThreads) bn_silu_bwd_apply_kernel(const __n
       for (int k = 0; k < 8; ++k) {
         const int c = c0 + k;
         const float mean = __ldg(stat + c), rstd = __ldg(stat + C + c);
-        const float dz = g_is_dz ? fg[k] : fg[k] * silu_grad(fmaf(fy[k], __ldg(stat + 2 * C + c), __ldg(stat + 3 * C + c)));
+        const float dz = g_is_dz ? fg[k] : fg[k] * act_grad<ACT>(fmaf(fy[k], __ldg(stat + 2 * C + c), __ldg(stat + 3 * C + c)));
         const float xhat = (fy[k] - mean) * rstd;
         fg[k] = __ldg(gamma + c) * rstd * (dz - __ldg(sums + c) * inv_n - xhat * __ldg(sums + C + c) * inv_n);
       }
@@ -906,6 +922,199 @@ __global__ void __launch_bounds__(kEwThreads) pred_bias_grad_kernel(const float*
     __syncthreads();
   }
   if (threadIdx.x == 0) dbias[c] = part[0];
+}
+
+// ------------------------------------------------------------------------------------------------ YOLOv6: RepVGG blocks, BiFusion upsample
+// RepVGG block in training form (src/models/modules/yolo_modules.py:268-327): a = relu(bn3(y3) + bn1(y1) [+ bnid(x)]), each BatchNorm with
+// its own batch statistics (stat [4][C] of cvb_train_bn_stats).  ID: the identity branch exists (cin == cout, stride 1).  The sum is
+// (z3 + z1) + zid in fp32, every z_b = fmaf(y_b, scale_b, shift_b).  One item = one 8-channel vector.
+struct RepvggStats {
+  const float* s3;
+  const float* s1;
+  const float* sid;
+};
+
+template <bool ID>
+__global__ void __launch_bounds__(kEwThreads) repvgg_fwd_kernel(const __nv_bfloat16* __restrict__ y3, const __nv_bfloat16* __restrict__ y1,
+                                                                const __nv_bfloat16* __restrict__ x, long long nvec, int C, RepvggStats st,
+                                                                __nv_bfloat16* __restrict__ out) {
+  const int cv = C / 8;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < nvec; i += (long long)gridDim.x * kEwThreads) {
+    const int c0 = (int)(i % cv) * 8;
+    float f3[8], f1[8], fx[8];
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y3) + i), f3);
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y1) + i), f1);
+    if (ID) bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(x) + i), fx);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int c = c0 + k;
+      float z = fmaf(f3[k], __ldg(st.s3 + 2 * C + c), __ldg(st.s3 + 3 * C + c)) + fmaf(f1[k], __ldg(st.s1 + 2 * C + c), __ldg(st.s1 + 3 * C + c));
+      if (ID) z += fmaf(fx[k], __ldg(st.sid + 2 * C + c), __ldg(st.sid + 3 * C + c));
+      f3[k] = act_fwd<kActRelu>(z);
+    }
+    reinterpret_cast<uint4*>(out)[i] = float_to_bf16x8(f3);
+  }
+}
+
+// Backward, reduce half: dz = g * [a > 0] (a: the forward's saved output) is every branch's BatchNorm-output gradient, so
+// sums [4][C] = (sum dz = each branch's dbeta, sum dz * xhat3, sum dz * xhat1, sum dz * xhatid = the three dgammas).
+template <bool ID>
+__global__ void __launch_bounds__(kEwThreads) repvgg_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ a,
+                                                                       const __nv_bfloat16* __restrict__ y3, const __nv_bfloat16* __restrict__ y1,
+                                                                       const __nv_bfloat16* __restrict__ x, long long npix, int C, RepvggStats st,
+                                                                       float* __restrict__ sums) {
+  __shared__ float s_part[kRedSmemFloats];
+  const int cv = C / 8;
+  const int v = threadIdx.x % cv;
+  const int pl = threadIdx.x / cv, np = kEwThreads / cv;
+  const bool active = pl < np;
+  const long long chunk = (npix + gridDim.x - 1) / gridDim.x;
+  const long long p0 = (long long)blockIdx.x * chunk, p1 = min(npix, p0 + chunk);
+  float sdz[8], s3[8], s1[8], sid[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) sdz[i] = s3[i] = s1[i] = sid[i] = 0.0f;
+  if (active) {
+    for (long long p = p0 + pl; p < p1; p += np) {
+      const long long off = p * C;
+      float fg[8], fa[8], f3[8], f1[8], fx[8];
+      bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(g + off) + v), fg);
+      bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(a + off) + v), fa);
+      bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y3 + off) + v), f3);
+      bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y1 + off) + v), f1);
+      if (ID) bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(x + off) + v), fx);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int c = v * 8 + i;
+        const float dz = fa[i] > 0.0f ? fg[i] : 0.0f;
+        sdz[i] += dz;
+        s3[i] = fmaf(dz, (f3[i] - __ldg(st.s3 + c)) * __ldg(st.s3 + C + c), s3[i]);
+        s1[i] = fmaf(dz, (f1[i] - __ldg(st.s1 + c)) * __ldg(st.s1 + C + c), s1[i]);
+        if (ID) sid[i] = fmaf(dz, (fx[i] - __ldg(st.sid + c)) * __ldg(st.sid + C + c), sid[i]);
+      }
+    }
+  }
+  red_finish(sdz, s3, v, pl, np, active, C, s_part, sums);
+  __syncthreads();  // (s_part is reused)
+  red_finish(s1, sid, v, pl, np, active, C, s_part, sums + 2 * C);
+}
+
+// ... apply half: dy_b = gamma_b * rstd_b * (dz - sum dz / N - xhat_b * sum(dz * xhat_b) / N) for b = 3x3, 1x1 and (ID) the identity
+// branch, whose dy is its contribution to d(loss)/d(x).
+template <bool ID>
+__global__ void __launch_bounds__(kEwThreads) repvgg_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ a,
+                                                                      const __nv_bfloat16* __restrict__ y3, const __nv_bfloat16* __restrict__ y1,
+                                                                      const __nv_bfloat16* __restrict__ x, long long nvec, int C, RepvggStats st,
+                                                                      const float* __restrict__ gamma3, const float* __restrict__ gamma1,
+                                                                      const float* __restrict__ gamma_id, const float* __restrict__ sums, float inv_n,
+                                                                      __nv_bfloat16* __restrict__ dy3, __nv_bfloat16* __restrict__ dy1,
+                                                                      __nv_bfloat16* __restrict__ dx_id) {
+  const int cv = C / 8;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < nvec; i += (long long)gridDim.x * kEwThreads) {
+    const int c0 = (int)(i % cv) * 8;
+    float fg[8], fa[8], f3[8], f1[8], fx[8];
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(g) + i), fg);
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(a) + i), fa);
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y3) + i), f3);
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(y1) + i), f1);
+    if (ID) bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(x) + i), fx);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int c = c0 + k;
+      const float dz = fa[k] > 0.0f ? fg[k] : 0.0f;
+      const float mdz = __ldg(sums + c) * inv_n;
+      const float r3 = __ldg(st.s3 + C + c), r1 = __ldg(st.s1 + C + c);
+      f3[k] = __ldg(gamma3 + c) * r3 * (dz - mdz - (f3[k] - __ldg(st.s3 + c)) * r3 * __ldg(sums + C + c) * inv_n);
+      f1[k] = __ldg(gamma1 + c) * r1 * (dz - mdz - (f1[k] - __ldg(st.s1 + c)) * r1 * __ldg(sums + 2 * C + c) * inv_n);
+      if (ID) {
+        const float ri = __ldg(st.sid + C + c);
+        fx[k] = __ldg(gamma_id + c) * ri * (dz - mdz - (fx[k] - __ldg(st.sid + c)) * ri * __ldg(sums + 3 * C + c) * inv_n);
+      }
+    }
+    reinterpret_cast<uint4*>(dy3)[i] = float_to_bf16x8(f3);
+    reinterpret_cast<uint4*>(dy1)[i] = float_to_bf16x8(f1);
+    if (ID) reinterpret_cast<uint4*>(dx_id)[i] = float_to_bf16x8(fx);
+  }
+}
+
+// BiFusion's ConvTranspose2d(c, c, 2, stride=2, bias) (src/models/modules/yolo_modules.py:245-265) around a 1x1 GEMM u [B,h,w,4c] whose
+// column (py * 2 + px) * c + o is output pixel (2y + py, 2x + px), channel o.  Scatter: out [B,2h,2w,c] = u + bias (fp32 sum, one bf16
+// rounding).  Item = one 8-channel vector of out.
+__global__ void __launch_bounds__(kEwThreads) convt_scatter_kernel(const __nv_bfloat16* __restrict__ u, int B, int h, int w, int C,
+                                                                   const float* __restrict__ bias, __nv_bfloat16* __restrict__ out) {
+  const int cv = C / 8, W2 = 2 * w;
+  const long long n = (long long)B * 4 * h * w * cv;
+  for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kEwThreads) {
+    const int v = (int)(i % cv);
+    const long long p = i / cv;
+    const int X = (int)(p % W2);
+    const long long t = p / W2;
+    const int Y = (int)(t % (2 * h));
+    const long long img = t / (2 * h);
+    const long long src = ((img * h + Y / 2) * w + X / 2) * 4 * cv + ((Y & 1) * 2 + (X & 1)) * cv + v;
+    float f[8];
+    bf16x8_to_float(__ldg(reinterpret_cast<const uint4*>(u) + src), f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] += __ldg(bias + 8 * v + k);
+    reinterpret_cast<uint4*>(out)[i] = float_to_bf16x8(f);
+  }
+}
+
+// Gather: g = d(loss)/d(out) [B,2h,2w,c] -> du [B,h,w,4c] in the GEMM layout (a permutation: exact), and dbias partials: CTA b sums its
+// fixed pixel range of g per channel (pixel lanes in order, then a fixed shared-memory tree over the lanes) into partial[b][c].
+// convt_bias_finish_kernel adds the kConvtParts partials in order: dbias is bitwise reproducible.
+constexpr int kConvtParts = 256;
+
+__global__ void __launch_bounds__(kEwThreads) convt_gather_kernel(const __nv_bfloat16* __restrict__ g, int B, int h, int w, int C,
+                                                                  __nv_bfloat16* __restrict__ du, float* __restrict__ partial) {
+  __shared__ float s_part[kEwThreads * 8];
+  const int cv = C / 8, W2 = 2 * w;
+  const int v = threadIdx.x % cv;
+  const int pl = threadIdx.x / cv, np = kEwThreads / cv;
+  const bool active = pl < np;
+  const long long npix = (long long)B * 4 * h * w;
+  const long long chunk = (npix + gridDim.x - 1) / gridDim.x;
+  const long long p0 = (long long)blockIdx.x * chunk, p1 = min(npix, p0 + chunk);
+  float acc[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) acc[k] = 0.0f;
+  if (active) {
+    for (long long p = p0 + pl; p < p1; p += np) {
+      const int X = (int)(p % W2);
+      const long long t = p / W2;
+      const int Y = (int)(t % (2 * h));
+      const long long img = t / (2 * h);
+      const uint4 q = __ldg(reinterpret_cast<const uint4*>(g) + p * cv + v);
+      reinterpret_cast<uint4*>(du)[((img * h + Y / 2) * w + X / 2) * 4 * cv + ((Y & 1) * 2 + (X & 1)) * cv + v] = q;
+      float f[8];
+      bf16x8_to_float(q, f);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += f[k];
+    }
+  }
+  // fixed tree over the pixel lanes: lane pl takes lane pl + s for s = the largest power of two below np, then halving
+  if (active) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s_part[pl * C + v * 8 + k] = acc[k];
+  }
+  __syncthreads();
+  int s0 = 1;
+  while (2 * s0 < np) s0 *= 2;
+  for (int s = s0; s > 0; s >>= 1) {
+    if (pl < s && pl + s < np) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) s_part[pl * C + v * 8 + k] += s_part[(pl + s) * C + v * 8 + k];
+    }
+    __syncthreads();
+  }
+  for (int c = threadIdx.x; c < C; c += kEwThreads) partial[(long long)blockIdx.x * C + c] = s_part[c];
+}
+
+__global__ void convt_bias_finish_kernel(const float* __restrict__ partial, int C, float* __restrict__ dbias) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float t = 0.0f;
+  for (int b = 0; b < kConvtParts; ++b) t += partial[(long long)b * C + c];
+  dbias[c] = t;
 }
 
 // fp32 master weights [cout][cin][kh][kw] (nn.Conv2d) -> bf16 [cout][kh*kw][cin] (forward / wgrad layout) and the backward-data operand
@@ -1281,22 +1490,28 @@ extern "C" int cvb_train_bn_stats(const void* y, int64_t npix, int32_t C, const 
   return CVB_OK;
 }
 
-extern "C" int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream) {
-  CVB_REQUIRE(y && stat && out && C % 8 == 0, "train_bn_silu_fwd: bad argument");
+template <int ACT>
+static int bn_act_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream) {
   const long long nvec = npix * (C / 8);
   const int grid = ew_grid(nvec);
   if (grid == 0) return CVB_ERR_NO_DEVICE;
-  bn_silu_fwd_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(y), nvec, C, stat, static_cast<__nv_bfloat16*>(out));
+  bn_act_fwd_kernel<ACT><<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(y), nvec, C, stat, static_cast<__nv_bfloat16*>(out));
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
 }
 
+extern "C" int cvb_train_bn_silu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream) {
+  CVB_REQUIRE(y && stat && out && C % 8 == 0, "train_bn_silu_fwd: bad argument");
+  return bn_act_fwd<kActSilu>(y, npix, C, stat, out, stream);
+}
+
+template <int ACT = kActSilu>
 static int bn_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, cudaStream_t st) {
   CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 2 * (size_t)C * sizeof(float), st));
   const int grid = red_grid(npix, kEwThreads / (C / 8));
   if (grid == 0) return CVB_ERR_NO_DEVICE;
-  bn_silu_bwd_reduce_kernel<<<grid, kEwThreads, 0, st>>>(
+  bn_act_bwd_reduce_kernel<ACT><<<grid, kEwThreads, 0, st>>>(
       static_cast<const __nv_bfloat16*>(g), static_cast<const __nv_bfloat16*>(y), npix, C, stat, g_is_dz, sums);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -1304,6 +1519,7 @@ static int bn_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t 
 }
 
 // count == nullptr: 1 / npix (this device's pixels); otherwise 1 / *count, the global count bn_merge_kernel left on the device
+template <int ACT = kActSilu>
 static int bn_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, const float* sums,
                         const double* count, void* dy, cudaStream_t st) {
   const long long nvec = npix * (C / 8);
@@ -1313,9 +1529,9 @@ static int bn_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t n
   const auto* yb = static_cast<const __nv_bfloat16*>(y);
   auto* dyb = static_cast<__nv_bfloat16*>(dy);
   if (count == nullptr)
-    bn_silu_bwd_apply_kernel<false><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, (float)(1.0 / (double)npix), nullptr, g_is_dz, dyb);
+    bn_act_bwd_apply_kernel<ACT, false><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, (float)(1.0 / (double)npix), nullptr, g_is_dz, dyb);
   else
-    bn_silu_bwd_apply_kernel<true><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, 0.0f, count, g_is_dz, dyb);
+    bn_act_bwd_apply_kernel<ACT, true><<<grid, kEwThreads, 0, st>>>(gb, yb, nvec, C, stat, gamma, sums, 0.0f, count, g_is_dz, dyb);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return CVB_OK;
@@ -1481,6 +1697,131 @@ extern "C" int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int
   if (grid == 0) return CVB_ERR_NO_DEVICE;
   pred_grad_nhwc_kernel<<<grid, kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, cout, cout_pad, static_cast<__nv_bfloat16*>(dy));
   pred_bias_grad_kernel<<<cout, kEwThreads, 0, st>>>(g, B, c_tot, hw, c_off, dbias);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(2);
+  return CVB_OK;
+}
+
+// ---- YOLOv6: BatchNorm + ReLU, RepVGG branch sum, ConvTranspose2d scatter / gather
+// every bf16 operand 16-byte aligned, C a multiple of 8 up to 2048 (one lane per 8 channels of a kEwThreads-thread CTA)
+static bool aligned16(const void* p) { return p == nullptr || is_aligned(p, 16); }
+
+extern "C" int cvb_train_bn_relu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream) {
+  CVB_REQUIRE(y && stat && out, "train_bn_relu_fwd: null pointer");
+  const int rc = check_bn_shape("train_bn_relu_fwd", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(y, 16) && is_aligned(out, 16) && is_aligned(stat, 4), "train_bn_relu_fwd: y / out must be 16-byte, stat 4-byte aligned");
+  return bn_act_fwd<kActRelu>(y, npix, C, stat, out, stream);
+}
+
+extern "C" int cvb_train_bn_relu_bwd(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, float* sums, void* dy,
+                                     void* stream) {
+  CVB_REQUIRE(g && y && stat && gamma && sums && dy, "train_bn_relu_bwd: null pointer");
+  const int rc = check_bn_shape("train_bn_relu_bwd", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(y, 16) && is_aligned(dy, 16), "train_bn_relu_bwd: g / y / dy must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(stat, 4) && is_aligned(gamma, 4) && is_aligned(sums, 4), "train_bn_relu_bwd: stat / gamma / sums must be 4-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  const int r = bn_bwd_reduce<kActRelu>(g, 0, y, npix, C, stat, sums, st);
+  return r != CVB_OK ? r : bn_bwd_apply<kActRelu>(g, 0, y, npix, C, stat, gamma, sums, nullptr, dy, st);
+}
+
+// the identity branch's operands come together: all of (x, stat_id[, gamma_id, dx_id]) or none
+static int check_repvgg(const char* fn, int64_t npix, int32_t C, const void* x, const float* stat_id, const void* const* bf16s, int nb,
+                        const float* const* f32s, int nf) {
+  const int rc = check_bn_shape(fn, npix, C);
+  if (rc != CVB_OK) return rc;
+  for (int i = 0; i < nb; ++i) CVB_REQUIRE(aligned16(bf16s[i]), "%s: bf16 tensors must be 16-byte aligned", fn);
+  for (int i = 0; i < nf; ++i) CVB_REQUIRE(f32s[i] == nullptr || is_aligned(f32s[i], 4), "%s: fp32 stat / gamma / sums must be 4-byte aligned", fn);
+  CVB_REQUIRE((x == nullptr) == (stat_id == nullptr), "%s: x and stat_id go together (both NULL: no identity branch)", fn);
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_repvgg_fwd(const void* y3, const void* y1, const void* x, int64_t npix, int32_t C, const float* stat3, const float* stat1,
+                                    const float* stat_id, void* out, void* stream) {
+  CVB_REQUIRE(y3 && y1 && stat3 && stat1 && out, "train_repvgg_fwd: null pointer");
+  const void* bf[] = {y3, y1, x, out};
+  const float* f32[] = {stat3, stat1, stat_id};
+  const int rc = check_repvgg("train_repvgg_fwd", npix, C, x, stat_id, bf, 4, f32, 3);
+  if (rc != CVB_OK) return rc;
+  const long long nvec = npix * (C / 8);
+  const int grid = ew_grid(nvec);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  const RepvggStats st{stat3, stat1, stat_id};
+  const auto* b3 = static_cast<const __nv_bfloat16*>(y3);
+  const auto* b1 = static_cast<const __nv_bfloat16*>(y1);
+  const auto* bx = static_cast<const __nv_bfloat16*>(x);
+  auto* bo = static_cast<__nv_bfloat16*>(out);
+  if (x)
+    repvgg_fwd_kernel<true><<<grid, kEwThreads, 0, as_stream(stream)>>>(b3, b1, bx, nvec, C, st, bo);
+  else
+    repvgg_fwd_kernel<false><<<grid, kEwThreads, 0, as_stream(stream)>>>(b3, b1, nullptr, nvec, C, st, bo);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_repvgg_bwd(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
+                                    const float* stat3, const float* stat1, const float* stat_id, const float* gamma3, const float* gamma1,
+                                    const float* gamma_id, float* sums, void* dy3, void* dy1, void* dx_id, void* stream) {
+  CVB_REQUIRE(g && a && y3 && y1 && stat3 && stat1 && gamma3 && gamma1 && sums && dy3 && dy1, "train_repvgg_bwd: null pointer");
+  const void* bf[] = {g, a, y3, y1, x, dy3, dy1, dx_id};
+  const float* f32[] = {stat3, stat1, stat_id, gamma3, gamma1, gamma_id, sums};
+  const int rc = check_repvgg("train_repvgg_bwd", npix, C, x, stat_id, bf, 8, f32, 7);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE((x == nullptr) == (gamma_id == nullptr) && (x == nullptr) == (dx_id == nullptr),
+              "train_repvgg_bwd: x, stat_id, gamma_id and dx_id go together (all NULL: no identity branch)");
+  cudaStream_t st = as_stream(stream);
+  CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 4 * (size_t)C * sizeof(float), st));
+  const int rgrid = red_grid(npix, kEwThreads / (C / 8));
+  const long long nvec = npix * (C / 8);
+  const int agrid = ew_grid(nvec);
+  if (rgrid == 0 || agrid == 0) return CVB_ERR_NO_DEVICE;
+  const RepvggStats s{stat3, stat1, stat_id};
+  const auto* bg = static_cast<const __nv_bfloat16*>(g);
+  const auto* ba = static_cast<const __nv_bfloat16*>(a);
+  const auto* b3 = static_cast<const __nv_bfloat16*>(y3);
+  const auto* b1 = static_cast<const __nv_bfloat16*>(y1);
+  const auto* bx = static_cast<const __nv_bfloat16*>(x);
+  auto* d3 = static_cast<__nv_bfloat16*>(dy3);
+  auto* d1 = static_cast<__nv_bfloat16*>(dy1);
+  auto* dx = static_cast<__nv_bfloat16*>(dx_id);
+  const float inv_n = (float)(1.0 / (double)npix);
+  if (x) {
+    repvgg_bwd_reduce_kernel<true><<<rgrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, npix, C, s, sums);
+    repvgg_bwd_apply_kernel<true><<<agrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, nvec, C, s, gamma3, gamma1, gamma_id, sums, inv_n, d3, d1, dx);
+  } else {
+    repvgg_bwd_reduce_kernel<false><<<rgrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, npix, C, s, sums);
+    repvgg_bwd_apply_kernel<false><<<agrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, nvec, C, s, gamma3, gamma1, nullptr, sums, inv_n, d3, d1, nullptr);
+  }
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(2);
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_convt_scatter(const void* u, int32_t B, int32_t h, int32_t w, int32_t C, const float* bias, void* out, void* stream) {
+  CVB_REQUIRE(u && bias && out, "train_convt_scatter: null pointer");
+  CVB_REQUIRE(B > 0 && h > 0 && w > 0 && C > 0 && C % 8 == 0, "train_convt_scatter: B, h, w must be > 0 and C a multiple of 8 (B=%d h=%d w=%d C=%d)", B,
+              h, w, C);
+  CVB_REQUIRE(is_aligned(u, 16) && is_aligned(out, 16) && is_aligned(bias, 4), "train_convt_scatter: u / out must be 16-byte, bias 4-byte aligned");
+  const int grid = ew_grid((long long)B * 4 * h * w * (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  convt_scatter_kernel<<<grid, kEwThreads, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(u), B, h, w, C, bias, static_cast<__nv_bfloat16*>(out));
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+extern "C" int cvb_train_convt_gather(const void* g, int32_t B, int32_t h, int32_t w, int32_t C, float* scratch, void* du, float* dbias, void* stream) {
+  CVB_REQUIRE(g && scratch && du && dbias, "train_convt_gather: null pointer");
+  CVB_REQUIRE(B > 0 && h > 0 && w > 0 && C > 0 && C % 8 == 0 && C / 8 <= kEwThreads,
+              "train_convt_gather: B, h, w must be > 0 and C a multiple of 8 up to 2048 (B=%d h=%d w=%d C=%d)", B, h, w, C);
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(du, 16) && is_aligned(scratch, 4) && is_aligned(dbias, 4),
+              "train_convt_gather: g / du must be 16-byte, scratch / dbias 4-byte aligned");
+  if (sm_count() == 0) return CVB_ERR_NO_DEVICE;
+  cudaStream_t st = as_stream(stream);
+  convt_gather_kernel<<<kConvtParts, kEwThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(g), B, h, w, C, static_cast<__nv_bfloat16*>(du), scratch);
+  convt_bias_finish_kernel<<<ceil_div(C, 128), 128, 0, st>>>(scratch, C, dbias);
   CVB_CHECK_CUDA(cudaGetLastError());
   count_launch(2);
   return CVB_OK;

@@ -236,6 +236,16 @@ class _YoloNmsModel(_Standalone):
     post-processing of forward(mode='val').  A subclass defines ``_graph_for(imgs)``, whose graph reads its input from holder['x'] and
     leaves the NMS result in its NmsWorkspace 'ws'."""
 
+    @staticmethod
+    def pack_targets(imgs, targets):
+        """trans_specific_format (yolov5.py:221-245, detectors/yolo_detector.py:23-50): the per-image target dicts -> gts [nt, 6] rows (image, label, cx, cy, w, h) on the
+        images' device.  A tensor is taken as already packed."""
+        if isinstance(targets, torch.Tensor):
+            return targets
+        rows = [torch.cat([torch.full((t['labels'].shape[0], 1), float(i), device=imgs.device), t['labels'].to(imgs.device, torch.float32).view(-1, 1),
+                           t['boxes'].to(imgs.device, torch.float32).view(-1, 4)], 1) for i, t in enumerate(targets)]
+        return torch.cat(rows, 0) if rows else torch.zeros((0, 6), device=imgs.device)
+
     def predict(self, imgs):
         """Device-only inference: returns (det [B,max_det,6] (x1,y1,x2,y2,conf,cls), det_idx [B,max_det] (row*nc + cls), det_count [B])
         device tensors, no host sync.  The tensors are the GRAPH-OWNED output buffers (overwritten by the next call with the same shape).
@@ -357,16 +367,6 @@ class YOLOv5(_YoloNmsModel):
             return (yolov5_train.YOLOv5CSPDarknet(**strip(bcfg)), yolov5_train.YOLOv5Neck(**{k: v for k, v in ncfg.items() if k != 'name'}),
                     yolov5_train.YOLOv5Detect(**{k: v for k, v in dcfg.items() if k != 'name'}))
         return train.bound_training_modules(self, (self.backbone, self.neck, self.detect), build)
-
-    @staticmethod
-    def pack_targets(imgs, targets):
-        """trans_specific_format (yolov5.py:221-245): the per-image target dicts -> gts [nt, 6] rows (image, label, cx, cy, w, h) on the
-        images' device.  A tensor is taken as already packed."""
-        if isinstance(targets, torch.Tensor):
-            return targets
-        rows = [torch.cat([torch.full((t['labels'].shape[0], 1), float(i), device=imgs.device), t['labels'].to(imgs.device, torch.float32).view(-1, 1),
-                           t['boxes'].to(imgs.device, torch.float32).view(-1, 4)], 1) for i, t in enumerate(targets)]
-        return torch.cat(rows, 0) if rows else torch.zeros((0, 6), device=imgs.device)
 
     def forward_train(self, imgs, targets):
         """The reference's training forward (yolov5.py:247-262) on the H100 training kernels: backbone -> neck -> detect -> YOLOv5Loss over this

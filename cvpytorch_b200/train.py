@@ -165,14 +165,31 @@ def _sync_group(bn):
     return group if dist.get_world_size(group) > 1 else None
 
 
-def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None):
-    """a = silu(bn_train(conv(x, weight))) -> (a, (y, stat, g32, wb), count): what _bn_silu_backward and the backward convolutions need (the
-    conv output, the BN statistics, fp32 gamma and the backward-data weights) and, with a process group (SyncBatchNorm), the global pixel count
-    on the device (None otherwise).  Updates the running statistics."""
+def bn_stats(y, gamma, beta, running_mean, running_var, eps, momentum):
+    """Batch statistics of y NHWC bf16 [..., C] -> (stat fp32 [4, C] = mean, rstd, scale, shift; fp32 gamma).  Updates the running statistics."""
+    C = y.shape[-1]
+    stat = torch.empty((4, C), dtype=torch.float32, device=y.device)
+    scratch = torch.empty((2, C), dtype=torch.float32, device=y.device)
+    g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
+    _lib.check(_lib.lib().cvb_train_bn_stats(_p(y), y.numel() // C, C, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                             _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
+    return stat, g32
+
+
+def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None, act='silu'):
+    """a = act(bn_train(conv(x, weight))) (act 'silu', or 'relu' without a process group) -> (a, (y, stat, g32, wb), count): what
+    _bn_silu_backward / _bn_relu_backward and the backward convolutions need (the conv output, the BN statistics, fp32 gamma and the
+    backward-data weights) and, with a process group (SyncBatchNorm), the global pixel count on the device (None otherwise).  Updates the
+    running statistics."""
     cout = weight.shape[0]
     L = _lib.lib()
     wf, wb = pack_weights(weight)
     y = conv(x, wf, cout, k, stride=stride, pad=pad)
+    if act == 'relu':
+        stat, g32 = bn_stats(y, gamma, beta, running_mean, running_var, eps, momentum)
+        a = torch.empty_like(y)
+        _lib.check(L.cvb_train_bn_relu_fwd(_p(y), y.numel() // cout, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_relu_fwd')
+        return a, (y, stat, g32, wb), None
     npix = y.shape[0] * y.shape[1] * y.shape[2]
     stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
     scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
@@ -216,15 +233,25 @@ def _bn_silu_backward(g, g_is_dz, y, stat, g32, group=None, count=None):
     return dy, dgamma, dbeta
 
 
+def _bn_relu_backward(g, y, stat, g32):
+    """g = d(loss)/d(a), a = relu(bn(y)) -> (dy, dgamma, dbeta)."""
+    g = g.contiguous()
+    cout = y.shape[3]
+    sums = torch.empty((2, cout), dtype=torch.float32, device=y.device)
+    dy = torch.empty_like(y)
+    _lib.check(_lib.lib().cvb_train_bn_relu_bwd(_p(g), _p(y), y.numel() // cout, cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()), 'cvb_train_bn_relu_bwd')
+    return dy, sums[1].clone(), sums[0].clone()
+
+
 class _ConvBnSiLU(torch.autograd.Function):
-    """a = silu(bn_train(conv(x, W))) with the backward the reference obtains from torch.autograd, on the H100 kernels."""
+    """a = silu(bn_train(conv(x, W))) (or relu: act='relu') with the backward the reference obtains from torch.autograd, on the H100 kernels."""
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None, act='silu'):
         _check_cuda(x, 'BaseConv (H100 training)')
-        a, saved, count = _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride, pad)
+        a, saved, count = _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride, pad, act)
         ctx.save_for_backward(x, *saved)
-        ctx.k, ctx.stride, ctx.pad = k, stride, pad
+        ctx.k, ctx.stride, ctx.pad, ctx.act = k, stride, pad, act
         ctx.group, ctx.count = group, count
         ctx.need_dx = x.requires_grad
         return a
@@ -234,7 +261,10 @@ class _ConvBnSiLU(torch.autograd.Function):
         x, y, stat, g32, wb = ctx.saved_tensors
         k = ctx.k
         B, H, W, cin = x.shape
-        dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32, ctx.group, ctx.count)
+        if ctx.act == 'relu':
+            dy, dgamma, dbeta = _bn_relu_backward(da, y, stat, g32)
+        else:
+            dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32, ctx.group, ctx.count)
         dw = conv_wgrad(x, dy, k, ctx.stride, ctx.pad)
         dx = None
         if ctx.need_dx:
@@ -242,7 +272,7 @@ class _ConvBnSiLU(torch.autograd.Function):
                 dx = conv_dgrad_s2(dy, wb, cin, H, W)
             else:  # backward-data of a padding-p conv: the same conv over dy with the rotated weights and padding k - 1 - p
                 dx = conv(dy, wb, cin, k, pad=None if ctx.pad is None else k - 1 - ctx.pad)
-        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None
+        return dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None
 
 
 class _BottleneckChain(torch.autograd.Function):
@@ -276,6 +306,7 @@ class _ConvBnSiLULayer(nn.Module):
     """conv (no bias) -> BatchNorm (batch statistics) -> SiLU as one _ConvBnSiLU, with the reference's conv / bn / act children.
     forward: NHWC bf16 in -> NHWC bf16 out.  `padding` None: k // 2 through cvb_train_conv (stride 1 or 2); otherwise cvb_train_conv_pad."""
     drop_in = None  # the public module named in the eval() refusal
+    act = 'silu'  # the activation after the BatchNorm: 'silu', or 'relu' (yolov6_train.ConvModule)
 
     def __init__(self, in_channels, out_channels, ksize, stride=1, padding=None):
         super().__init__()
@@ -295,7 +326,7 @@ class _ConvBnSiLULayer(nn.Module):
 
     def _layer(self, x, weight):
         _require_training(self, f'{type(self).__module__}.{self.drop_in} is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
-        return _ConvBnSiLU.apply(x, weight, *self._bn_inputs(), self.ksize, self.stride, self.padding)
+        return _ConvBnSiLU.apply(x, weight, *self._bn_inputs(), self.ksize, self.stride, self.padding, self.act)
 
 
 class BaseConv(_ConvBnSiLULayer):

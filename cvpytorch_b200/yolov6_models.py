@@ -12,7 +12,8 @@ Mirrors (paths relative to the reference checkout; same constructor arguments an
 
 Only the n and s widths run: every width of these two is a multiple of 16 (the conv kernel's cin % 16 == 0).  yolov6_t (24-channel
 stem), yolov6_m / l / x (the reference head sets reg_max = 16 whatever use_dfl is, so its own eval forward fails at
-reg_output.reshape([b, 4, l])), use_dfl=True, fuse_ab=True and training raise NotImplementedError.
+reg_output.reshape([b, 4, l])), use_dfl=True and fuse_ab=True raise NotImplementedError.  forward(mode='train') runs the training mirrors
+of yolov6_train.py on the training kernels and the H100 YOLOv6Loss.
 
 Graph notes: the stem RepVGGBlock(3, c, stride 2) is one 3x3/s1 conv over the space-to-depth map (row-window loader of the YOLOv5
 stem; only taps -1 and 0 are non-zero, ``repvgg_stem_weights_to_s2d``).  RepVGG blocks are folded to one 3x3 conv (yolo_blocks.py).
@@ -24,7 +25,7 @@ the NMS pre-pass, after which the YOLOv5 NMS (ops.yolo_nms, hist_ready) selects 
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, train, yolov6_train
 from .engine import GraphBuilder
 from .models import _YoloNmsModel
 from .modules import ConvModule, _build, _EmitModule, _Standalone, folded
@@ -338,6 +339,9 @@ class YOLOv6Detect(_EmitModule):
         assert off == A
 
 
+_TRAIN_BACKBONES = {'YOLOv6EfficientRep': yolov6_train.YOLOv6EfficientRep}
+_TRAIN_NECKS = {'YOLOv6RepBiPAN': yolov6_train.YOLOv6RepBiPAN}
+_TRAIN_HEADS = {'YOLOv6Effidehead': yolov6_train.YOLOv6Effidehead}
 _BACKBONES = {'YOLOv6EfficientRep': YOLOv6EfficientRep}
 _NECKS = {'YOLOv6RepBiPAN': YOLOv6RepBiPAN}
 _HEADS = {'YOLOv6Effidehead': YOLOv6Effidehead}
@@ -346,7 +350,8 @@ _DETECTS = {'YOLOv6Detect': YOLOv6Detect}
 
 class YOLOv6Loss(nn.Module):
     """Holds the reference YOLOv6Loss's one parameter (``proj``, src/losses/det/yolov6_loss.py:45) so that the model's state_dict keys are
-    the reference's (``loss.0.proj``).  YOLOv6 training is not on the H100 path: calling it raises."""
+    the reference's (``loss.0.proj``).  It is not called: YOLOv6.forward(mode='train') computes the loss with a yolov6_train.YOLOv6Loss
+    built from the same config."""
 
     def __init__(self, num_classes=80, fpn_strides=[8, 16, 32], grid_cell_size=5.0, grid_cell_offset=0.5, ori_img_size=640, warmup_epoch=4,
                  use_dfl=False, reg_max=16, iou_type='giou', loss_weight={'class': 1.0, 'iou': 2.5, 'dfl': 0.5}):
@@ -355,12 +360,19 @@ class YOLOv6Loss(nn.Module):
         self.proj = nn.Parameter(torch.linspace(0, reg_max, reg_max + 1), requires_grad=False)
 
     def forward(self, *a, **k):
-        raise NotImplementedError('YOLOv6 (H100): training and the YOLOv6 loss are not on the H100 path')
+        raise NotImplementedError("YOLOv6 (H100): this holder only keeps the loss's state_dict key; YOLOv6.forward(mode='train') computes the "
+                                  'loss (cvpytorch_b200.yolov6_train.YOLOv6Loss)')
 
 
 class YOLOv6(_YoloNmsModel):
     """Model-level drop-in for the reference's YOLOv6 (YAML route conf/det/yolov6/coco_yolov6_{n,s}.yml, USE_MODEL): same state_dict keys
-    as its YOLODetector; forward(imgs, targets, 'val') runs the cached inference graph with the val contract of src/models/yolov6.py."""
+    as its YOLODetector; forward(imgs, targets, 'val') runs the cached inference graph with the val contract of src/models/yolov6.py, and
+    forward(imgs, targets, 'train') the training step of detectors/yolo_detector.py + single_stage.py: backbone -> neck -> head on the
+    training kernels (yolov6_train), then the loss -> {'iou', 'dfl', 'class', 'loss'} fp64 device scalars.
+
+    As the reference's YAML route: the loss is called without epoch_num, so ATSS assigns at every epoch (while warmup_epoch > 0); the class
+    loss is discarded, so head.cls_convs.* and head.cls_preds.* get no gradient (.grad stays None; their BatchNorm running statistics still
+    update, their forward runs)."""
 
     def __init__(self, dictionary=None, model_cfg=None):
         super().__init__()
@@ -381,6 +393,11 @@ class YOLOv6(_YoloNmsModel):
         if lcfg.pop('name', 'YOLOv6Loss') != 'YOLOv6Loss':
             raise NotImplementedError('YOLOv6 (H100): only the YOLOv6Loss keys are mirrored')
         self.loss = nn.ModuleList([YOLOv6Loss(**lcfg)])
+        self._cfgs = (dict(get('BACKBONE')), dict(get('NECK')), dict(get('HEAD')), sub)
+        # the training loss (parameter-only: kept out of the module tree, so the state_dict keeps the reference's keys) and the training
+        # modules, built on the first training forward over this model's own parameters and buffers (train.bound_training_modules)
+        self.__dict__['_train_loss'] = yolov6_train.YOLOv6Loss(**lcfg)
+        self.__dict__['_train_modules'] = None
         self.conf_thres, self.iou_thres, self.max_det = 0.03, 0.65, 300  # src/models/yolov6.py:150-151, :32
 
     def build_graph(self, B, H, W, device):
@@ -402,11 +419,34 @@ class YOLOv6(_YoloNmsModel):
         return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device),
                            float(self.conf_thres), float(self.iou_thres), int(self.max_det))
 
+    def _training_modules(self):
+        """(yolov6_train.YOLOv6EfficientRep, YOLOv6RepBiPAN, YOLOv6Effidehead) over this model's own parameters, buffers and BatchNorms."""
+        def build():
+            bcfg, ncfg, hcfg, sub = self._cfgs
+            return (_build(_TRAIN_BACKBONES, dict(bcfg, **sub)), _build(_TRAIN_NECKS, dict(ncfg, **sub)), _build(_TRAIN_HEADS, dict(hcfg, **sub)))
+        return train.bound_training_modules(self, (self.backbone, self.neck, self.head), build)
+
+    def forward_train(self, imgs, targets):
+        """The reference's training forward on the H100 training kernels -> {'iou', 'dfl', 'class', 'loss'} (fp64 device scalars, no host sync)."""
+        if isinstance(imgs, (list, tuple)):
+            imgs = torch.stack(list(imgs))
+        if not imgs.is_cuda:
+            raise NotImplementedError("YOLOv6 (H100): mode='train' has no CPU fallback: pass CUDA images")
+        if not self.training:
+            raise RuntimeError("YOLOv6 (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
+        if any(train._sync_group(m) is not None for m in self.modules() if isinstance(m, nn.SyncBatchNorm)):
+            raise NotImplementedError('YOLOv6 (H100) training: BatchNorm statistics over several ranks (nn.SyncBatchNorm) are not on the training path')
+        gt = self.pack_targets(imgs, targets)
+        bb, nk, hd = self._training_modules()
+        losses = self._train_loss(hd.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gt)  # (no epoch_num: loss_forward, single_stage.py:97-103)
+        losses['loss'] = losses['iou'] + losses['dfl'] + losses['class']
+        return losses
+
     def forward(self, imgs, targets=None, mode='infer', **kwargs):
         if mode == 'infer':
             return
         if mode == 'train':
-            raise NotImplementedError("YOLOv6 (H100): mode='train' (YOLOv6 training and its loss) is not on the H100 path")
+            return self.forward_train(imgs, targets)
         if mode != 'val':
             raise RuntimeError(f"YOLOv6 (H100): unknown mode {mode!r}")
         if isinstance(imgs, (list, tuple)):

@@ -445,6 +445,34 @@ int cvb_train_pred_conv(const void* x, int32_t B, int32_t H, int32_t W, int32_t 
 int cvb_train_pred_grad(const float* g, int32_t B, int32_t c_tot, int32_t h, int32_t w, int32_t c_off, int32_t cout, int32_t cout_pad, void* dy, float* dbias,
                         void* stream);
 
+/* YOLOv6 training (EfficientRep backbone, Rep-BiPAN neck: src/models/modules/yolo_modules.py:218-327).  NHWC bf16 operands, 16-byte
+ * aligned; C a multiple of 8 up to 2048; stat [4][C] = (mean, rstd, scale, shift) as cvb_train_bn_stats writes it.
+ * cvb_train_bn_relu_fwd: out = relu(y * scale + shift) (conv -> BatchNorm -> ReLU, the ConvModules of the backbone and neck).
+ * cvb_train_bn_relu_bwd: g = d(loss)/d(out) -> sums [2][C] = (dbeta, dgamma) and dy = gamma * rstd * (dz - dbeta / N - xhat * dgamma / N),
+ *   dz = g where z = fmaf(y, scale, shift) > 0 (the fp32 expression of the forward; torch's ReLU rule: no gradient at z = 0).
+ * cvb_train_repvgg_fwd: a RepVGG block in training form: out = relu(z3 + z1 [+ zid]) with z3 = bn(y3; stat3) of the 3x3 branch's conv
+ *   output, z1 = bn(y1; stat1) of the 1x1 branch's and zid = bn(x; stat_id) of the block input (the identity branch, when cin == cout
+ *   and stride 1; x = stat_id = NULL without it).  Each stat is a cvb_train_bn_stats call on its own branch.  Summed in fp32 in that order.
+ * cvb_train_repvgg_bwd: g = d(loss)/d(out), a = the forward's out -> dz = g where a > 0; sums [4][C] = (sum dz: every branch's dbeta,
+ *   sum dz * xhat3, sum dz * xhat1, sum dz * xhatid: the three dgammas; the last row is 0 without the identity branch) and dy3, dy1,
+ *   dx_id = each branch's batch-norm backward (dx_id is the identity branch's share of d(loss)/d(x)).  x, stat_id, gamma_id and dx_id
+ *   are all NULL without the identity branch.  One reduce and one apply pass.
+ * cvb_train_convt_scatter: nn.ConvTranspose2d(C, C, 2, stride 2, bias) after its 1x1 GEMM u [B,h,w,4C], column (py * 2 + px) * C + o =
+ *   output pixel (2y + py, 2x + px), channel o -> out [B,2h,2w,C] = u + bias (fp32 sum, one bf16 rounding).
+ * cvb_train_convt_gather: g = d(loss)/d(out) [B,2h,2w,C] -> du [B,h,w,4C] in the GEMM layout (a permutation, exact; the backward convs
+ *   of the 1x1 GEMM read it) and dbias [C] = the sum of g over images and pixels, fp32 in a fixed order (256 partial sums, scratch fp32
+ *   [256][C], added in order): bitwise reproducible.
+ */
+int cvb_train_bn_relu_fwd(const void* y, int64_t npix, int32_t C, const float* stat, void* out, void* stream);
+int cvb_train_bn_relu_bwd(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, float* sums, void* dy, void* stream);
+int cvb_train_repvgg_fwd(const void* y3, const void* y1, const void* x, int64_t npix, int32_t C, const float* stat3, const float* stat1,
+                         const float* stat_id, void* out, void* stream);
+int cvb_train_repvgg_bwd(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C, const float* stat3,
+                         const float* stat1, const float* stat_id, const float* gamma3, const float* gamma1, const float* gamma_id, float* sums,
+                         void* dy3, void* dy1, void* dx_id, void* stream);
+int cvb_train_convt_scatter(const void* u, int32_t B, int32_t h, int32_t w, int32_t C, const float* bias, void* out, void* stream);
+int cvb_train_convt_gather(const void* g, int32_t B, int32_t h, int32_t w, int32_t C, float* scratch, void* du, float* dbias, void* stream);
+
 /* SyncBatchNorm (nn.SyncBatchNorm in training mode: batch statistics over every rank's pixels).  The caller runs the collectives between
  * the calls; nothing here synchronises the host, so the whole sequence can be captured in a CUDA graph.
  * cvb_train_bn_partial: y [npix][C] bf16 (16-byte aligned, C % 8 == 0, C <= 2048) -> record fp64 [2C + 1] = (mean [C], M2 [C] = sum of
