@@ -21,7 +21,7 @@ import torch.nn as nn
 
 from . import _lib, ops
 from .engine import GraphBuilder
-from .modules import _build, _Standalone, folded
+from .modules import _build, _Model, _Standalone, folded
 
 
 # =============================================================================================== ResNet-50
@@ -321,24 +321,20 @@ def build_detect(cfg):
     return _build(_DETECTS, cfg)
 
 
-class FCOS(_Standalone):
+class FCOS(_Model):
     """Model-level drop-in for src.models.fcos.FCOS (inference path)."""
 
     def __init__(self, dictionary=None, model_cfg=None):
-        super().__init__()
-        self.dictionary = dictionary
-        self.model_cfg = model_cfg
+        super().__init__(dictionary, model_cfg)
         self.dummy_input = torch.zeros(1, 3, 800, 800)
-        self.num_classes = len(self.dictionary)
-        get = (lambda k: model_cfg[k]) if isinstance(model_cfg, dict) else (lambda k: getattr(model_cfg, k))
-        hcfg = dict(get('HEAD'))
+        hcfg = dict(self._cfg('HEAD'))
         hcfg['num_classes'] = self.num_classes  # setup_extra_params (fcos.py:48-49)
-        bcfg = dict(get('BACKBONE'))
+        bcfg = dict(self._cfg('BACKBONE'))
         bcfg['pretrained'] = False  # no network on the box; weights come from load_state_dict
         self.backbone = build_backbone(bcfg)
-        self.neck = build_neck(dict(get('NECK')))
+        self.neck = build_neck(dict(self._cfg('NECK')))
         self.head = build_head(hcfg)
-        self.detect = build_detect(dict(get('DETECT')))
+        self.detect = build_detect(dict(self._cfg('DETECT')))
         self.loss = None
         self.conf_thres = 0.05
         self.iou_thres = 0.6
@@ -353,26 +349,15 @@ class FCOS(_Standalone):
         ws = self.detect.emit(g, head_outs, self.num_classes, scales)
         return dict(g=g, holder=holder, ws=ws, feats=feats, levels=levels, head=head_outs)
 
-    def _graph_for(self, imgs):
-        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device))
-
     def predict(self, imgs):
         """Device-only inference: (scores [B,K], classes [B,K] (1-based), boxes [B,K,4], loc [B,K], count [B]); no host sync.
         Graph-owned buffers (overwritten by the next call).  ``self._graph_for(imgs)['ws'].status[0] != 0`` flags a top-k
         capacity overflow of the last run; ``forward()`` checks it and raises."""
-        G = self._graph_for(imgs)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        ws = G['ws']
+        ws = self._replay(imgs.contiguous().float())['ws']
         return ws.out_scores, ws.out_classes, ws.out_boxes, ws.out_loc, ws.out_count
 
-    def forward(self, imgs, targets=None, mode='infer', **kwargs):
-        if mode == 'infer':
-            return  # the reference does nothing in 'infer' mode (fcos.py:120-121)
-        if mode != 'val':
-            raise RuntimeError("FCOS (H100): only mode='val' (inference) is implemented; training stays on the reference")
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs), 0)
+    def _val(self, imgs, targets):
+        """fcos.py:124-166: (losses, per-image {'boxes', 'labels', 'scores'})."""
         sc, cl, bx, _, cnt = self.predict(imgs)
         sc, cl, bx, cnt = sc.cpu(), cl.cpu(), bx.cpu(), cnt.cpu().tolist()
         if int(self._graph_for(imgs)['ws'].status[0]) != 0:
@@ -399,6 +384,4 @@ class FCOS(_Standalone):
             bn[:, [1, 3]] = bn[:, [1, 3]].clip(0, height)
             keep = sc[i, :k] > 0.05
             outputs.append({"boxes": torch.tensor(bn)[keep], "labels": cl[i, :k][keep].long(), "scores": sc[i, :k][keep]})
-        # fcos.py:124-166 returns the loss dict next to the outputs; a zero 'loss' entry keeps the unchanged trainer alive under
-        # cfg.distributed (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict)
-        return {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}, outputs
+        return self._val_losses(imgs.device), outputs

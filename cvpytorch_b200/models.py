@@ -19,7 +19,7 @@ import torch.nn as nn
 
 from . import _lib, ops, train, yolov5_train
 from .engine import GraphBuilder
-from .modules import ConvModule, CSPLayer, DownsamplingModule, SPPF, UpsamplingModule, _build, _Standalone, folded
+from .modules import ConvModule, CSPLayer, DownsamplingModule, SPPF, UpsamplingModule, _build, _Model, _Standalone, folded
 
 
 # =============================================================================================== backbone
@@ -231,10 +231,18 @@ def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=Non
     return out
 
 
-class _YoloNmsModel(_Standalone):
-    """What the YOLO drop-ins whose cached graph ends in ops.yolo_nms (YOLOv5, YOLOv6) share: ``predict``, ``nms_status`` and the
-    post-processing of forward(mode='val').  A subclass defines ``_graph_for(imgs)``, whose graph reads its input from holder['x'] and
-    leaves the NMS result in its NmsWorkspace 'ws'."""
+class _YoloModel(_Model):
+    """What the YOLO drop-ins share: the training forward (YOLOv5, YOLOX, YOLOv6) and, for the ones whose cached graph ends in ops.yolo_nms
+    (YOLOv5, YOLOv6), ``predict``, ``nms_status`` and the post-processing of forward(mode='val').  A trainer defines ``_parts`` (the names of
+    its inference modules), ``_build_training_parts()`` (their training modules) and ``_loss_step(outputs, targets)``.  YOLOX replaces
+    ``pack_targets``, ``predict`` and ``_val``; its graph ends in ops.yolox_nms, which has no status word, so ``nms_status`` does not apply."""
+
+    def _loss_cfg(self, name):
+        """The LOSS section's constructor arguments (the model's own loss when the section is missing); another loss raises NotImplementedError."""
+        lcfg = dict(self._cfg('LOSS', None) or {'name': name})
+        if lcfg.pop('name', name) != name:
+            raise NotImplementedError(f'{type(self).__name__} (H100): only the {name} is on the training path')
+        return lcfg
 
     @staticmethod
     def pack_targets(imgs, targets):
@@ -246,15 +254,30 @@ class _YoloNmsModel(_Standalone):
                            t['boxes'].to(imgs.device, torch.float32).view(-1, 4)], 1) for i, t in enumerate(targets)]
         return torch.cat(rows, 0) if rows else torch.zeros((0, 6), device=imgs.device)
 
+    def _training_modules(self):
+        """The training modules of ``_parts`` over this model's own parameters, buffers and BatchNorm modules (train.bound_training_modules).
+        Widths the training kernels refuse raise NotImplementedError."""
+        return train.bound_training_modules(self, tuple(getattr(self, p) for p in self._parts), self._build_training_parts)
+
+    def forward_train(self, imgs, targets):
+        """The reference's training forward on the H100 training kernels: backbone -> neck -> head over this model's parameters, then
+        ``_loss_step`` (device tensors, no host sync)."""
+        name = type(self).__name__
+        if not self.training:
+            raise RuntimeError(f"{name} (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
+        if not imgs.is_cuda:
+            raise _lib.CvbError(f'{name} (H100) training: CUDA images required (the training path has no CPU fallback)')
+        gts = self.pack_targets(imgs, targets)
+        bb, nk, hd = self._training_modules()
+        return self._loss_step(hd.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gts)
+
     def predict(self, imgs):
         """Device-only inference: returns (det [B,max_det,6] (x1,y1,x2,y2,conf,cls), det_idx [B,max_det] (row*nc + cls), det_count [B])
         device tensors, no host sync.  The tensors are the GRAPH-OWNED output buffers (overwritten by the next call with the same shape).
         ``nms_status(imgs)`` returns the device status word of the last run ([0] != 0: the NMS candidate capacity overflowed and the
         result is invalid); ``forward()`` checks it and raises."""
-        G = self._graph_for(imgs)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
+        ws = self._replay(imgs.contiguous().float())['ws']
+        return ws.det, ws.det_idx, ws.det_count
 
     def nms_status(self, imgs):
         """Device int32[4] status of the NMS stage of the graph that serves `imgs` ([0] = candidate-capacity overflow flag)."""
@@ -264,9 +287,6 @@ class _YoloNmsModel(_Standalone):
         """forward(imgs, targets, 'val'): (losses, per-image {'boxes', 'labels', 'scores'}) with the boxes rescaled and clipped to each
         image's original geometry, as the reference (yolov5.py:258-282, yolov6.py:209-227)."""
         det, _, cnt = self.predict(imgs)
-        # the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps the
-        # unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict under cfg.distributed)
-        losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
         det_h, cnt_h = ops.val_rows_to_host(det.clone(), cnt, targets, imgs.shape[2:])
         if int(self.nms_status(imgs)[0]) != 0:  # (the copy above already synchronised)
             raise _lib.CvbError(f'{type(self).__name__} NMS: candidate capacity overflow (more keys in the threshold bin than the workspace '
@@ -275,10 +295,10 @@ class _YoloNmsModel(_Standalone):
         for b in range(det_h.shape[0]):
             pred = det_h[b, :cnt_h[b]]
             outputs.append({"boxes": pred[:, :4].clone(), "labels": pred[:, 5], "scores": pred[:, 4]})
-        return losses, outputs
+        return self._val_losses(imgs.device), outputs
 
 
-class YOLOv5(_YoloNmsModel):
+class YOLOv5(_YoloModel):
     """Model-level drop-in for src.models.yolov5.YOLOv5.  forward(imgs, targets, mode) keeps the reference contract: mode 'val' (eval()) ->
     (losses_dict, outputs list of {'boxes','labels','scores'}) from the cached inference graph; mode 'train' (train()) -> the loss dict
     {'loss', 'box_loss', 'obj_loss', 'cls_loss'} from the training kernels and the YOLOv5Loss over the same parameters."""
@@ -286,19 +306,16 @@ class YOLOv5(_YoloNmsModel):
                [[1.87500, 3.81250], [3.87500, 2.81250], [3.68750, 7.43750]],
                [[3.62500, 2.81250], [4.87500, 6.18750], [11.65625, 10.18750]]]
     cfg = {"nano": [0.33, 0.25], "tiny": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
+    _parts = ('backbone', 'neck', 'detect')
 
     def __init__(self, dictionary=None, model_cfg=None):
-        super().__init__()
-        self.dictionary = dictionary
-        self.model_cfg = model_cfg
+        super().__init__(dictionary, model_cfg)
         self.dummy_input = torch.zeros(1, 3, 640, 640)
-        self.num_classes = len(self.dictionary)
         self.category = [v for d in self.dictionary for v in d.keys()]
         self.weight = [d[v] for d in self.dictionary for v in d.keys() if v in self.category]
-        get = (lambda k: model_cfg[k]) if isinstance(model_cfg, dict) else (lambda k: getattr(model_cfg, k))
-        self.depth_mul, self.width_mul = self.cfg[get('TYPE').split("_")[1]]
-        bcfg, ncfg, dcfg = dict(get('BACKBONE')), dict(get('NECK')), dict(get('DETECT'))
-        bcfg.setdefault('subtype', get('TYPE'))
+        self.depth_mul, self.width_mul = self.cfg[self._cfg('TYPE').split("_")[1]]
+        bcfg, ncfg, dcfg = dict(self._cfg('BACKBONE')), dict(self._cfg('NECK')), dict(self._cfg('DETECT'))
+        bcfg.setdefault('subtype', self._cfg('TYPE'))
         ncfg.update(depth_mul=self.depth_mul, width_mul=self.width_mul)
         dcfg.update(depth_mul=self.depth_mul, width_mul=self.width_mul, anchors=self.anchors, num_classes=self.num_classes)
         self.backbone = build_backbone(bcfg)
@@ -307,10 +324,7 @@ class YOLOv5(_YoloNmsModel):
         self.conf_thres = 0.001   # yolov5.py:189
         self.iou_thres = 0.6      # yolov5.py:190
         self.max_det = 300
-        lcfg = model_cfg.get('LOSS') if isinstance(model_cfg, dict) else getattr(model_cfg, 'LOSS', None)
-        lcfg = dict(lcfg) if lcfg else {'name': 'YOLOv5Loss'}
-        if lcfg.pop('name', 'YOLOv5Loss') != 'YOLOv5Loss':
-            raise NotImplementedError('YOLOv5 (H100): only the YOLOv5Loss is on the training path')
+        lcfg = self._loss_cfg('YOLOv5Loss')
         lcfg.update(anchors=self.anchors, num_classes=self.num_classes)  # yolov5.py:210-219 (setup_extra_params)
         self.loss = yolov5_train.YOLOv5Loss(**lcfg)  # (no parameters or buffers: the state_dict keys stay the inference model's)
         for m in self.modules():
@@ -353,40 +367,17 @@ class YOLOv5(_YoloNmsModel):
             raise RuntimeError('inference only: call .eval() first')
         if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[3] != 3 or not frames_u8.is_cuda:
             raise ValueError('predict_frames expects a uint8 CUDA tensor [B,H,W,3]')
-        G = self._graph_for(frames_u8)
-        G['holder']['x'] = frames_u8.contiguous()
-        G['g'].run()
-        return G['ws'].det, G['ws'].det_idx, G['ws'].det_count
+        ws = self._replay(frames_u8.contiguous())['ws']
+        return ws.det, ws.det_idx, ws.det_count
 
-    def _training_modules(self):
-        """(yolov5_train.YOLOv5CSPDarknet, YOLOv5Neck, YOLOv5Detect) over this model's own parameters, buffers and BatchNorm modules.  Widths
-        the training kernels refuse (YOLOv5-m, -x) raise NotImplementedError."""
-        def build():
-            strip = lambda c: {k: v for k, v in c.items() if k not in ('name', 'depth_mul', 'width_mul')}  # noqa: E731
-            bcfg, ncfg, dcfg = self._cfgs
-            return (yolov5_train.YOLOv5CSPDarknet(**strip(bcfg)), yolov5_train.YOLOv5Neck(**{k: v for k, v in ncfg.items() if k != 'name'}),
-                    yolov5_train.YOLOv5Detect(**{k: v for k, v in dcfg.items() if k != 'name'}))
-        return train.bound_training_modules(self, (self.backbone, self.neck, self.detect), build)
+    def _build_training_parts(self):
+        """(yolov5_train.YOLOv5CSPDarknet, YOLOv5Neck, YOLOv5Detect); the training kernels refuse YOLOv5-m and -x."""
+        strip = lambda c: {k: v for k, v in c.items() if k not in ('name', 'depth_mul', 'width_mul')}  # noqa: E731
+        bcfg, ncfg, dcfg = self._cfgs
+        return (yolov5_train.YOLOv5CSPDarknet(**strip(bcfg)), yolov5_train.YOLOv5Neck(**{k: v for k, v in ncfg.items() if k != 'name'}),
+                yolov5_train.YOLOv5Detect(**{k: v for k, v in dcfg.items() if k != 'name'}))
 
-    def forward_train(self, imgs, targets):
-        """The reference's training forward (yolov5.py:247-262) on the H100 training kernels: backbone -> neck -> detect -> YOLOv5Loss over this
-        model's parameters; returns {loss [1], box_loss, obj_loss, cls_loss} (device tensors, no host sync)."""
-        if not self.training:
-            raise RuntimeError("YOLOv5 (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs))
-        if not imgs.is_cuda:
-            raise _lib.CvbError('YOLOv5 (H100) training: CUDA images required (the training path has no CPU fallback)')
-        gts = self.pack_targets(imgs, targets)
-        bb, nk, dt = self._training_modules()
-        loss, items = self.loss(dt.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gts)
+    def _loss_step(self, outputs, gts):
+        """yolov5.py:247-262: {loss [1], box_loss, obj_loss, cls_loss}."""
+        loss, items = self.loss(outputs, gts)
         return {'loss': loss, 'box_loss': items[0], 'obj_loss': items[1], 'cls_loss': items[2]}
-
-    def forward(self, imgs, targets=None, mode='infer', **kwargs):
-        if mode == 'infer':
-            return  # the reference returns None here (yolov5.py:247-249)
-        if mode == 'train':
-            return self.forward_train(imgs, targets)
-        if mode != 'val':
-            raise RuntimeError(f"YOLOv5 (H100): unknown mode {mode!r}")
-        return self._val(imgs, targets)

@@ -132,6 +132,60 @@ class _Standalone(nn.Module):
         return res if len(self.out_stages) > 1 else res[0]
 
 
+class _Model(_Standalone):
+    """Base of the model-level drop-ins (YOLOv5, YOLOX, YOLOv6, FCOS, EncoderDecoder): the reference's ``(dictionary=, model_cfg=)``
+    constructor and ``forward(imgs, targets, mode)`` contract.  A subclass defines ``build_graph(B, H, W, device)`` (whose graph reads its
+    input from holder['x']) and ``_val(imgs, targets)``; it overrides ``forward_train`` when it trains and ``_infer`` when its 'infer'
+    result is not the detectors' None."""
+
+    def __init__(self, dictionary, model_cfg):
+        super().__init__()
+        self.dictionary, self.model_cfg = dictionary, model_cfg
+        self.num_classes = len(dictionary)
+
+    def _cfg(self, key, *default):
+        """``model_cfg[key]`` of a dict or an attribute config.  Without a default, a missing key raises KeyError naming it."""
+        try:
+            return self.model_cfg[key] if isinstance(self.model_cfg, dict) else getattr(self.model_cfg, key)
+        except (KeyError, AttributeError):
+            if default:
+                return default[0]
+            raise KeyError(f'{type(self).__name__}: model_cfg has no {key!r} entry') from None
+
+    def forward(self, imgs, targets=None, mode='infer', **kwargs):
+        if mode == 'infer':
+            return self._infer(imgs)
+        if mode not in ('train', 'val'):
+            raise RuntimeError(f'{type(self).__name__} (H100): unknown mode {mode!r}')
+        if isinstance(imgs, (list, tuple)):
+            imgs = torch.stack(list(imgs))
+        return self.forward_train(imgs, targets) if mode == 'train' else self._val(imgs, targets)
+
+    def _infer(self, imgs):
+        return None  # what the reference detectors return in 'infer' mode (yolov5.py:247-249, yolox.py:144-149, fcos.py:120-121)
+
+    def forward_train(self, imgs, targets):
+        raise RuntimeError(f"{type(self).__name__} (H100): only mode='val' (inference) is implemented; training stays on the reference")
+
+    def _graph_for(self, imgs, *key):
+        """The cached graph of ``build_graph`` for the NCHW images ``imgs``, keyed by their shape and ``key``."""
+        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device), *key)
+
+    def _replay(self, x, *args):
+        """Runs the graph ``_graph_for(x, *args)`` on the input ``x`` and returns its dict."""
+        G = self._graph_for(x, *args)
+        G['holder']['x'] = x
+        G['g'].run()
+        return G
+
+    @staticmethod
+    def _val_losses(device):
+        # the reference returns its loss dict next to the val outputs; that loss is a training diagnostic and is not computed on the H100
+        # path.  A zero 'loss' entry keeps the unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty
+        # dict under cfg.distributed)
+        return {'loss': torch.zeros((), dtype=torch.float32, device=device)}
+
+
 def _build(table, cfg):
     """Reference factory contract (src/models/{backbones,necks,heads,detects}/__init__.py): deepcopy the cfg, pop 'name',
     Class(**cfg); an unknown name raises NotImplementedError."""

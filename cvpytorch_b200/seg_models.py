@@ -17,7 +17,7 @@ import torch.nn as nn
 from . import ops
 from .engine import GraphBuilder
 from .fcos_models import ResNet
-from .modules import ConvModule, DepthwiseSeparableConvModule, _build, _Standalone, folded
+from .modules import ConvModule, DepthwiseSeparableConvModule, _build, _Model, _Standalone, folded
 
 
 class ASPPModules(nn.ModuleList):
@@ -109,23 +109,19 @@ def build_head(cfg):
     return _build(_HEADS, cfg)
 
 
-class EncoderDecoder(_Standalone):
+class EncoderDecoder(_Model):
     """Model-level drop-in for src.models.segmentors.encoder_decoder.EncoderDecoder (inference: mode='val' -> int64 [B,H,W])."""
 
     def __init__(self, dictionary=None, model_cfg=None, *args, **kwargs):
-        super().__init__()
-        self.dictionary = dictionary
-        self.model_cfg = model_cfg
+        super().__init__(dictionary, model_cfg)
         self.input_size = [1024, 2048]
         self.dummy_input = torch.zeros(1, 3, self.input_size[0], self.input_size[1])
-        self.num_classes = len(self.dictionary)
-        get = (lambda k: model_cfg.get(k) if isinstance(model_cfg, dict) else getattr(model_cfg, k))
-        if get('NECK') is not None or get('AUX_HEAD') is not None:
+        if self._cfg('NECK', None) is not None or self._cfg('AUX_HEAD', None) is not None:
             raise NotImplementedError('NECK / AUX_HEAD are not on the H100 hot path')
-        bcfg = dict(get('BACKBONE'))
+        bcfg = dict(self._cfg('BACKBONE'))
         bcfg['pretrained'] = False
         self.backbone = build_backbone(bcfg)
-        self.head = build_head(dict(get('HEAD')))
+        self.head = build_head(dict(self._cfg('HEAD')))
 
     def build_graph(self, B, H, W, device, out_hw=None):
         g = GraphBuilder(B, device)
@@ -146,19 +142,15 @@ class EncoderDecoder(_Standalone):
         """Device-only inference: int64 label map [B, Ho, Wo] (Ho, Wo default to the input size); no host sync.
         The returned tensor is the GRAPH-OWNED output buffer: the next call with the same shape overwrites it (zero-copy);
         ``forward()`` returns a fresh tensor like the reference does."""
-        G = self._graph_for(imgs, out_hw)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        return G['labels']
+        return self._replay(imgs.contiguous().float(), out_hw)['labels']
 
-    def forward(self, imgs, targets=None, mode='infer', epoch_num=0, step_num=0, **kwargs):
-        if mode == 'val':
-            out_hw = tuple(targets.shape[-2:]) if targets is not None else None
-            # encoder_decoder.py:131-133: argmax(bilinear(preds -> targets size)); a fresh tensor per call like the reference (a caller may
-            # keep predictions of several batches), the zero-copy graph buffer is only handed out by predict()
-            return self.predict(imgs, out_hw).clone()
-        if mode == 'infer':
-            # the reference's 'infer' branch calls torch.argmax on a *list* and raises TypeError (SURVEY.md 3.3); the usable
-            # inference path is 'val'.  Here 'infer' returns the label map at input resolution.
-            return self.predict(imgs).clone()
-        raise RuntimeError("EncoderDecoder (H100): training stays on the reference implementation")
+    def _infer(self, imgs):
+        # the reference's 'infer' branch calls torch.argmax on a *list* and raises TypeError (SURVEY.md 3.3); the usable
+        # inference path is 'val'.  Here 'infer' returns the label map at input resolution.
+        return self.predict(imgs).clone()
+
+    def _val(self, imgs, targets):
+        out_hw = tuple(targets.shape[-2:]) if targets is not None else None
+        # encoder_decoder.py:131-133: argmax(bilinear(preds -> targets size)); a fresh tensor per call like the reference (a caller may
+        # keep predictions of several batches), the zero-copy graph buffer is only handed out by predict()
+        return self.predict(imgs, out_hw).clone()

@@ -27,7 +27,7 @@ import torch.nn as nn
 
 from . import ops, train, yolov6_train
 from .engine import GraphBuilder
-from .models import _YoloNmsModel
+from .models import _YoloModel
 from .modules import ConvModule, _build, _EmitModule, _Standalone, folded
 from .yolo_blocks import RepBlock, RepVGGBlock
 
@@ -364,7 +364,7 @@ class YOLOv6Loss(nn.Module):
                                   'loss (cvpytorch_b200.yolov6_train.YOLOv6Loss)')
 
 
-class YOLOv6(_YoloNmsModel):
+class YOLOv6(_YoloModel):
     """Model-level drop-in for the reference's YOLOv6 (YAML route conf/det/yolov6/coco_yolov6_{n,s}.yml, USE_MODEL): same state_dict keys
     as its YOLODetector; forward(imgs, targets, 'val') runs the cached inference graph with the val contract of src/models/yolov6.py, and
     forward(imgs, targets, 'train') the training step of detectors/yolo_detector.py + single_stage.py: backbone -> neck -> head on the
@@ -374,26 +374,23 @@ class YOLOv6(_YoloNmsModel):
     loss is discarded, so head.cls_convs.* and head.cls_preds.* get no gradient (.grad stays None; their BatchNorm running statistics still
     update, their forward runs)."""
 
+    _parts = ('backbone', 'neck', 'head')
+
     def __init__(self, dictionary=None, model_cfg=None):
-        super().__init__()
-        self.dictionary, self.model_cfg = dictionary, model_cfg
+        super().__init__(dictionary, model_cfg)
         self.dummy_input = torch.zeros(1, 3, 640, 640)
-        self.num_classes = len(self.dictionary)
         self.category = [v for d in self.dictionary for v in d.keys()]
         self.weight = [d[v] for d in self.dictionary for v in d.keys() if v in self.category]
-        get = (lambda k: model_cfg.get(k)) if isinstance(model_cfg, dict) else (lambda k: getattr(model_cfg, k, None))
-        self.subtype = get('TYPE')
+        self.subtype = self._cfg('TYPE')
         check_subtype(self.subtype)
         sub = dict(subtype=self.subtype)  # yolo_detector.py:19-21
-        self.backbone = _build(_BACKBONES, dict(dict(get('BACKBONE')), **sub))
-        self.neck = _build(_NECKS, dict(dict(get('NECK')), **sub))
-        self.head = _build(_HEADS, dict(dict(get('HEAD')), **sub))
-        self.detect = _build(_DETECTS, dict(get('DETECT')))
-        lcfg = dict(get('LOSS') or {'name': 'YOLOv6Loss'})
-        if lcfg.pop('name', 'YOLOv6Loss') != 'YOLOv6Loss':
-            raise NotImplementedError('YOLOv6 (H100): only the YOLOv6Loss keys are mirrored')
+        self.backbone = _build(_BACKBONES, dict(dict(self._cfg('BACKBONE')), **sub))
+        self.neck = _build(_NECKS, dict(dict(self._cfg('NECK')), **sub))
+        self.head = _build(_HEADS, dict(dict(self._cfg('HEAD')), **sub))
+        self.detect = _build(_DETECTS, dict(self._cfg('DETECT')))
+        lcfg = self._loss_cfg('YOLOv6Loss')
         self.loss = nn.ModuleList([YOLOv6Loss(**lcfg)])
-        self._cfgs = (dict(get('BACKBONE')), dict(get('NECK')), dict(get('HEAD')), sub)
+        self._cfgs = (dict(self._cfg('BACKBONE')), dict(self._cfg('NECK')), dict(self._cfg('HEAD')), sub)
         # the training loss (parameter-only: kept out of the module tree, so the state_dict keeps the reference's keys) and the training
         # modules, built on the first training forward over this model's own parameters and buffers (train.bound_training_modules)
         self.__dict__['_train_loss'] = yolov6_train.YOLOv6Loss(**lcfg)
@@ -416,39 +413,22 @@ class YOLOv6(_YoloNmsModel):
 
     def _graph_for(self, imgs):
         # the thresholds are baked into the decode histogram / NMS steps of a graph: part of the key, so that changing them takes effect
-        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device),
-                           float(self.conf_thres), float(self.iou_thres), int(self.max_det))
+        return super()._graph_for(imgs, float(self.conf_thres), float(self.iou_thres), int(self.max_det))
 
-    def _training_modules(self):
-        """(yolov6_train.YOLOv6EfficientRep, YOLOv6RepBiPAN, YOLOv6Effidehead) over this model's own parameters, buffers and BatchNorms."""
-        def build():
-            bcfg, ncfg, hcfg, sub = self._cfgs
-            return (_build(_TRAIN_BACKBONES, dict(bcfg, **sub)), _build(_TRAIN_NECKS, dict(ncfg, **sub)), _build(_TRAIN_HEADS, dict(hcfg, **sub)))
-        return train.bound_training_modules(self, (self.backbone, self.neck, self.head), build)
+    def _build_training_parts(self):
+        """(yolov6_train.YOLOv6EfficientRep, YOLOv6RepBiPAN, YOLOv6Effidehead)."""
+        bcfg, ncfg, hcfg, sub = self._cfgs
+        return (_build(_TRAIN_BACKBONES, dict(bcfg, **sub)), _build(_TRAIN_NECKS, dict(ncfg, **sub)), _build(_TRAIN_HEADS, dict(hcfg, **sub)))
 
     def forward_train(self, imgs, targets):
         """The reference's training forward on the H100 training kernels -> {'iou', 'dfl', 'class', 'loss'} (fp64 device scalars, no host sync)."""
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs))
         if not imgs.is_cuda:
             raise NotImplementedError("YOLOv6 (H100): mode='train' has no CPU fallback: pass CUDA images")
-        if not self.training:
-            raise RuntimeError("YOLOv6 (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
         if any(train._sync_group(m) is not None for m in self.modules() if isinstance(m, nn.SyncBatchNorm)):
             raise NotImplementedError('YOLOv6 (H100) training: BatchNorm statistics over several ranks (nn.SyncBatchNorm) are not on the training path')
-        gt = self.pack_targets(imgs, targets)
-        bb, nk, hd = self._training_modules()
-        losses = self._train_loss(hd.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gt)  # (no epoch_num: loss_forward, single_stage.py:97-103)
+        return super().forward_train(imgs, targets)
+
+    def _loss_step(self, outputs, gt):
+        losses = self._train_loss(outputs, gt)  # (no epoch_num: loss_forward, single_stage.py:97-103)
         losses['loss'] = losses['iou'] + losses['dfl'] + losses['class']
         return losses
-
-    def forward(self, imgs, targets=None, mode='infer', **kwargs):
-        if mode == 'infer':
-            return
-        if mode == 'train':
-            return self.forward_train(imgs, targets)
-        if mode != 'val':
-            raise RuntimeError(f"YOLOv6 (H100): unknown mode {mode!r}")
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs))
-        return self._val(imgs, targets)

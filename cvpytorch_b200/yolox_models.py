@@ -20,8 +20,9 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _lib, ops, train
+from . import ops, train
 from .engine import GraphBuilder
+from .models import _YoloModel
 from .modules import ConvModule, CSPLayer, SPPF, _build, _EmitModule, _emit_csp, _Standalone, folded
 
 
@@ -246,37 +247,31 @@ def build_head(cfg):
     return _build(_HEADS, cfg)
 
 
-class YOLOX(_Standalone):
+class YOLOX(_YoloModel):
     """Model-level drop-in for src.models.yolox.YOLOX: mode='val' runs the cached inference graph (eval()), mode='train' the training
     kernels and the YOLOXLoss (train()) over the same parameters."""
     cfg = {"nano": [0.33, 0.25], "tiny": [0.33, 0.375], "s": [0.33, 0.5], "m": [0.67, 0.75], "l": [1.0, 1.0], "x": [1.33, 1.25]}
     input_norm = dict(mean=(0.406, 0.456, 0.485), std=(0.225, 0.224, 0.229), reverse_channels=True)
+    _parts = ('backbone', 'neck', 'head')
 
     def __init__(self, dictionary=None, model_cfg=None):
-        super().__init__()
-        self.dictionary, self.model_cfg = dictionary, model_cfg
+        super().__init__(dictionary, model_cfg)
         self.dummy_input = torch.zeros(1, 3, 640, 640)
-        self.num_classes = len(self.dictionary)
-        get = (lambda k: model_cfg.get(k) if isinstance(model_cfg, dict) else getattr(model_cfg, k))
-        self.depth_mul, self.width_mul = self.cfg[get('TYPE').split('_')[1]]
-        bcfg = dict(get('BACKBONE'))
+        self.depth_mul, self.width_mul = self.cfg[self._cfg('TYPE').split('_')[1]]
+        bcfg = dict(self._cfg('BACKBONE'))
         bcfg.pop('depth_mul', None)
         bcfg.pop('width_mul', None)
         bcfg['pretrained'] = False
         if bcfg.get('name') == 'CspDarkNet' and 'subtype' not in bcfg:
-            bcfg['subtype'] = get('TYPE')  # the composite of SURVEY.md 3.5: CSPDarknet(subtype='yolox_s')
-        ncfg = dict(get('NECK'), depth_mul=self.depth_mul, width_mul=self.width_mul)
-        hcfg = dict(get('HEAD'), depth_mul=self.depth_mul, width_mul=self.width_mul, num_classes=self.num_classes)
+            bcfg['subtype'] = self._cfg('TYPE')  # the composite of SURVEY.md 3.5: CSPDarknet(subtype='yolox_s')
+        ncfg = dict(self._cfg('NECK'), depth_mul=self.depth_mul, width_mul=self.width_mul)
+        hcfg = dict(self._cfg('HEAD'), depth_mul=self.depth_mul, width_mul=self.width_mul, num_classes=self.num_classes)
         self.backbone = build_backbone(bcfg)
         self.neck = build_neck(ncfg)
         self.head = build_head(hcfg)
         self.stride = [8, 16, 32]
         self.conf_thr, self.nms_thr = 0.01, 0.65   # src/models/yolox.py:94-95
-        lcfg = model_cfg.get('LOSS') if isinstance(model_cfg, dict) else getattr(model_cfg, 'LOSS', None)
-        lcfg = dict(lcfg) if lcfg else {'name': 'YOLOXLoss'}
-        if lcfg.pop('name', 'YOLOXLoss') != 'YOLOXLoss':
-            raise NotImplementedError('YOLOX (H100): only the YOLOXLoss is on the training path')
-        lcfg['num_classes'] = self.num_classes
+        lcfg = dict(self._loss_cfg('YOLOXLoss'), num_classes=self.num_classes)
         self.loss = train.YOLOXLoss(**lcfg)  # (no parameters or buffers: the state_dict keys stay the inference model's)
         # the training modules (train.CSPDarknet / YOLOXNeck / YOLOXHead), built on the first training forward over this model's own
         # parameters and buffers; kept out of the module tree so that state_dict(), parameters() and .to() see each tensor once
@@ -298,24 +293,16 @@ class YOLOX(_Standalone):
         g.fn(lambda: ops.yolox_nms(ws, self.conf_thr, self.nms_thr))
         return dict(g=g, holder=holder, outs=outs, ws=ws)
 
-    def _graph_for(self, imgs):
-        return self._graph([imgs], lambda: self.build_graph(imgs.shape[0], imgs.shape[2], imgs.shape[3], imgs.device))
-
     def predict(self, imgs):
         """Device-only inference: (det [B,A,7] rows (x1,y1,x2,y2,obj,class_conf,class_pred) in kept order, count [B]); no host sync."""
-        G = self._graph_for(imgs)
-        G['holder']['x'] = imgs.contiguous().float()
-        G['g'].run()
-        return G['ws'].det, G['ws'].count
+        ws = self._replay(imgs.contiguous().float())['ws']
+        return ws.det, ws.count
 
-    def _training_modules(self):
-        """(train.CSPDarknet, train.YOLOXNeck, train.YOLOXHead) over this model's own parameters, buffers and BatchNorm modules
-        (train.bound_training_modules).  Widths the training kernels refuse (YOLOX-t, -m, -x) raise NotImplementedError."""
-        def build():
-            strip = lambda c: {k: v for k, v in c.items() if k != 'name'}  # noqa: E731
-            bcfg, ncfg, hcfg = self._cfgs
-            return train.CSPDarknet(**strip(bcfg)), train.YOLOXNeck(**strip(ncfg)), train.YOLOXHead(**strip(hcfg))
-        return train.bound_training_modules(self, (self.backbone, self.neck, self.head), build)
+    def _build_training_parts(self):
+        """(train.CSPDarknet, train.YOLOXNeck, train.YOLOXHead); the training kernels refuse YOLOX-t, -m and -x."""
+        strip = lambda c: {k: v for k, v in c.items() if k != 'name'}  # noqa: E731
+        bcfg, ncfg, hcfg = self._cfgs
+        return train.CSPDarknet(**strip(bcfg)), train.YOLOXNeck(**strip(ncfg)), train.YOLOXHead(**strip(hcfg))
 
     def pack_targets(self, imgs, targets):
         """trans_specific_format (yolox.py:112-139): the per-image target dicts -> gt [B, max_labels, 5] rows (label, box) on the images'
@@ -330,32 +317,12 @@ class YOLOX(_Standalone):
             gt[i, :n, 1:] = t['boxes'].to(imgs.device, torch.float32)
         return gt
 
-    def forward_train(self, imgs, targets):
-        """The reference's training forward (yolox.py:150-157, 186-187) on the H100 training kernels: backbone -> neck -> head -> loss,
-        over this model's parameters; returns the loss dict {loss, conf_loss, cls_loss, iou_loss, num_fg} (device scalars, no host sync)."""
-        if not self.training:
-            raise RuntimeError("YOLOX (H100): mode='train' runs the training kernels (batch statistics); call .train() first")
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs))
-        if not imgs.is_cuda:
-            raise _lib.CvbError('YOLOX (H100) training: CUDA images required (the training path has no CPU fallback)')
-        gt = self.pack_targets(imgs, targets)
-        bb, nk, hd = self._training_modules()
-        return self.loss(hd.forward_nhwc(nk.forward_nhwc(bb.forward_nhwc(imgs))), gt)
+    def _loss_step(self, outputs, gt):
+        """yolox.py:150-157, 186-187: the loss dict {loss, conf_loss, cls_loss, iou_loss, num_fg}."""
+        return self.loss(outputs, gt)
 
-    def forward(self, imgs, targets=None, mode='infer', **kwargs):
-        if mode == 'infer':
-            return  # the reference returns None here (yolox.py:144-149)
-        if mode == 'train':
-            return self.forward_train(imgs, targets)
-        if mode != 'val':
-            raise RuntimeError(f"YOLOX (H100): unknown mode {mode!r}")
-        if isinstance(imgs, (list, tuple)):
-            imgs = torch.stack(list(imgs))
+    def _val(self, imgs, targets):
         det, cnt = self.predict(imgs)
-        losses = {'loss': torch.zeros((), dtype=torch.float32, device=imgs.device)}
-        # yolox.py:156: the val-mode loss of the reference is a training diagnostic and is not computed on the H100 path; a zero 'loss' entry keeps
-        # the unchanged trainer alive (trainer.py:216-219 -> reduce_dict -> torch.stack needs a non-empty dict under cfg.distributed)
         # yolox.py:165-178 on the device, then ONE device->host copy of the kept prefix
         kmax = max(int(cnt.max()), 1)
         det_h, cnt_h = ops.val_rows_to_host(det[:, :kmax].contiguous(), cnt, targets, imgs.shape[2:])
@@ -366,4 +333,4 @@ class YOLOX(_Standalone):
                 outputs.append({"boxes": torch.empty((0, 4)), "labels": torch.empty((0, 1)), "scores": torch.empty((0, 1))})
                 continue
             outputs.append({"boxes": pred[:, :4].clone(), "labels": pred[:, 6], "scores": pred[:, 4] * pred[:, 5]})
-        return losses, outputs
+        return self._val_losses(imgs.device), outputs

@@ -95,18 +95,25 @@ def test_factories_follow_reference_contract():
 
 
 def test_standalone_dropins_reject_cpu_input_and_training_without_caching():
-    """Every drop-in that runs on its own -- the 3 backbones, the 7 components, the bricks, the yolo_blocks blocks and the 4 models'
-    'val' forward -- raises CvbError on CPU tensors and RuntimeError in training mode (that check first), and caches no graph."""
+    """Every drop-in that runs on its own -- the 3 backbones, the 7 components, the bricks, the yolo_blocks blocks and the 5 models'
+    'val' forward, on a tensor and on a list of images -- raises CvbError on CPU tensors and RuntimeError in training mode (that check
+    first), and caches no graph.  The models' other modes: 'infer' returns None (the detectors) or runs the graph (EncoderDecoder), 'train'
+    in eval mode names .train() (the YOLO trainers; YOLOv6 refuses CPU images first) or is refused (FCOS, EncoderDecoder), and an unknown
+    mode raises RuntimeError."""
+    from test_yolov6_host import use_model
+
     from cvpytorch_b200 import _lib, synth
     from cvpytorch_b200 import fcos_models as FM
     from cvpytorch_b200 import models as M
     from cvpytorch_b200 import seg_models as SM
     from cvpytorch_b200 import yolo_blocks as YB
+    from cvpytorch_b200 import yolov6_models as Y6
     from cvpytorch_b200 import yolox_models as XM
     from cvpytorch_b200.modules import Conv, ConvModule
     cls80 = [{f'c{i}': 1.0} for i in range(80)]
-    v5, yx = M.YOLOv5(cls80, dict(synth.YOLOV5S_CFG)), XM.YOLOX(cls80, dict(synth.YOLOX_CFG))
+    v5, yx, v6 = M.YOLOv5(cls80, dict(synth.YOLOV5S_CFG)), XM.YOLOX(cls80, dict(synth.YOLOX_CFG)), Y6.YOLOv6(cls80, use_model('n'))
     fc, dl = FM.FCOS(cls80, dict(synth.FCOS_CFG)), SM.EncoderDecoder([{f'c{i}': 1.0} for i in range(19)], dict(synth.DEEPLAB_CFG))
+    models = (v5, yx, v6, fc, dl)
     img = torch.zeros(1, 3, 64, 64)
     maps = lambda *cs: [torch.zeros(1, c, 8 >> i, 8 >> i) for i, c in enumerate(cs)]  # noqa: E731
     x = torch.zeros(1, 32, 8, 8)
@@ -116,7 +123,8 @@ def test_standalone_dropins_reject_cpu_input_and_training_without_caching():
               (ConvModule(24, 32, 3, padding=1, norm_cfg=dict(type='BN')), torch.zeros(1, 24, 8, 8)), (Conv(24, 32, 3), torch.zeros(1, 24, 8, 8)),
               (YB.RepVGGBlock(32, 32), x), (YB.BottleRep(32, 32), x), (YB.RepBlock(32, 32, n=2), x), (YB.Conv_C3(32, 32), x),
               (YB.BepC3(32, 32, n=2), x), (YB.EELAN(32, 16, 32), x)]
-    calls = [(m, lambda m=m, t=t: m(t)) for m, t in inputs] + [(m, lambda m=m: m(img, None, 'val')) for m in (v5, yx, fc, dl)]
+    calls = ([(m, lambda m=m, t=t: m(t)) for m, t in inputs] + [(m, lambda m=m: m(img, None, 'val')) for m in models]
+             + [(m, lambda m=m: m([img[0], img[0]], None, 'val')) for m in models])
     for m, call in calls:
         m.eval()
         with pytest.raises(_lib.CvbError):
@@ -127,6 +135,39 @@ def test_standalone_dropins_reject_cpu_input_and_training_without_caching():
             call()
         assert not isinstance(e.value, _lib.CvbError), type(m).__name__
         assert m._graphs == {}, type(m).__name__
+    for m in models:
+        m.eval()
+        with pytest.raises(RuntimeError, match='unknown mode'):
+            m(img, None, 'bogus')
+    assert all(m(img, None, 'infer') is None for m in (v5, yx, v6, fc))
+    with pytest.raises(_lib.CvbError):
+        dl(img, None, 'infer')  # the label map of the cached graph
+    for m in (v5, yx):
+        with pytest.raises(RuntimeError, match=r'\.train\(\)'):
+            m(img, None, 'train')
+    with pytest.raises(NotImplementedError, match='no CPU fallback'):
+        v6(img, None, 'train')
+    for m in (fc, dl):
+        for mode in (True, False):
+            with pytest.raises(RuntimeError, match='training stays on the reference'):
+                m.train(mode)(img, None, 'train')
+    assert all(m._graphs == {} for m in models)
+
+
+def test_models_name_a_missing_config_section():
+    """A dict or attribute model_cfg without a required section fails at construction with a KeyError that names the section."""
+    from types import SimpleNamespace
+
+    from test_yolov6_host import use_model
+
+    from cvpytorch_b200 import fcos_models as FM, models as M, seg_models as SM, synth, yolov6_models as Y6, yolox_models as XM
+    cls80 = [{f'c{i}': 1.0} for i in range(80)]
+    for cls, cfg, key in ((M.YOLOv5, synth.YOLOV5S_CFG, 'NECK'), (XM.YOLOX, synth.YOLOX_CFG, 'HEAD'), (Y6.YOLOv6, use_model('n'), 'DETECT'),
+                          (FM.FCOS, synth.FCOS_CFG, 'BACKBONE'), (SM.EncoderDecoder, synth.DEEPLAB_CFG, 'HEAD')):
+        rest = {k: v for k, v in cfg.items() if k != key}
+        for model_cfg in (rest, SimpleNamespace(**rest)):
+            with pytest.raises(KeyError, match=key):
+                cls(cls80, model_cfg)
 
 
 def test_model_surface_and_loud_failure_without_cuda():

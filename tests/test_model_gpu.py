@@ -124,6 +124,9 @@ def test_forward_val_contract(model):
     targets2 = [{'labels': torch.zeros(1), 'boxes': torch.zeros(1, 4), 'scales': torch.tensor([0.4, 0.5]), 'pads': torch.tensor([3.0, 7.0]),
                  'height': torch.tensor(300), 'width': torch.tensor(240)} for _ in range(2)]
     _, outs2 = model(x, targets2, 'val')
+    _, outs_list = model(list(x), targets2, 'val')  # a list of images is stacked
+    for a, b in zip(outs_list, outs2, strict=True):
+        assert all(torch.equal(a[k], b[k]) for k in ('boxes', 'labels', 'scores'))
     det, _, cnt = model.predict(x)
     for b, o in enumerate(outs2):
         bb = det[b, :int(cnt[b]), :4].cpu().numpy().copy()
