@@ -105,6 +105,12 @@ SYMBOLS = {
     'cvb_train_bn_merge': (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_train_bn_silu_bwd_reduce': (c_int32, [c_void_p, c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_bn_silu_bwd_apply': (c_int32, [c_void_p, c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_bn_relu_bwd_reduce': (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_bn_relu_bwd_apply': (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'cvb_train_repvgg_bwd_reduce': (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                              c_void_p]),
+    'cvb_train_repvgg_bwd_apply': (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'cvb_train_focus_s2d': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     'cvb_train_spp_pool_fwd': (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     'cvb_train_spp_pool_bwd': (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),

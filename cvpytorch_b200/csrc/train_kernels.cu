@@ -15,6 +15,7 @@
 // bn_merge_kernel; backward bn_act_bwd_reduce_kernel -> all-reduce of the two sums -> bn_act_bwd_apply_kernel with the global count.
 // YOLOv6 adds the same passes with ReLU (<kActRelu>), the RepVGG branch sum relu(bn3(y3) + bn1(y1) [+ bnid(x)]) with its backward
 // (repvgg_*_kernel) and the ConvTranspose2d(c, c, 2, stride 2) scatter / gather around a 1x1 GEMM of 4c columns (convt_*_kernel).
+// Synced, a RepVGG block takes one record per branch (the identity branch's on the block input) and one all-reduce of its [4][C] sums.
 //
 // Layout: activations and gradients are NHWC bf16, dense (pitch == C; C = 16, 32 or a multiple of 64, and TMA zero-fills a box's channels
 // past a 16- or 32-channel C); weights bf16 [cout][kh*kw][kpad(cin)] (K-major rows, zero-padded to 64 channels), fp32 master weights / fp32
@@ -999,15 +1000,16 @@ __global__ void __launch_bounds__(kEwThreads) repvgg_bwd_reduce_kernel(const __n
 }
 
 // ... apply half: dy_b = gamma_b * rstd_b * (dz - sum dz / N - xhat_b * sum(dz * xhat_b) / N) for b = 3x3, 1x1 and (ID) the identity
-// branch, whose dy is its contribution to d(loss)/d(x).
-template <bool ID>
+// branch, whose dy is its contribution to d(loss)/d(x).  1 / N = inv_n, or (DEV_COUNT: N over every rank) 1 / *count, read on the device.
+template <bool ID, bool DEV_COUNT>
 __global__ void __launch_bounds__(kEwThreads) repvgg_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ a,
                                                                       const __nv_bfloat16* __restrict__ y3, const __nv_bfloat16* __restrict__ y1,
                                                                       const __nv_bfloat16* __restrict__ x, long long nvec, int C, RepvggStats st,
                                                                       const float* __restrict__ gamma3, const float* __restrict__ gamma1,
                                                                       const float* __restrict__ gamma_id, const float* __restrict__ sums, float inv_n,
-                                                                      __nv_bfloat16* __restrict__ dy3, __nv_bfloat16* __restrict__ dy1,
-                                                                      __nv_bfloat16* __restrict__ dx_id) {
+                                                                      const double* __restrict__ count, __nv_bfloat16* __restrict__ dy3,
+                                                                      __nv_bfloat16* __restrict__ dy1, __nv_bfloat16* __restrict__ dx_id) {
+  if (DEV_COUNT) inv_n = (float)(1.0 / __ldg(count));
   const int cv = C / 8;
   for (long long i = blockIdx.x * (long long)kEwThreads + threadIdx.x; i < nvec; i += (long long)gridDim.x * kEwThreads) {
     const int c0 = (int)(i % cv) * 8;
@@ -1726,6 +1728,27 @@ extern "C" int cvb_train_bn_relu_bwd(const void* g, const void* y, int64_t npix,
   return r != CVB_OK ? r : bn_bwd_apply<kActRelu>(g, 0, y, npix, C, stat, gamma, sums, nullptr, dy, st);
 }
 
+// SyncBatchNorm halves of cvb_train_bn_relu_bwd (a collective sums `sums` over the ranks between them)
+extern "C" int cvb_train_bn_relu_bwd_reduce(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream) {
+  CVB_REQUIRE(g && y && stat && sums, "train_bn_relu_bwd_reduce: null pointer");
+  const int rc = check_bn_shape("train_bn_relu_bwd_reduce", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(y, 16), "train_bn_relu_bwd_reduce: g / y must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(stat, 4) && is_aligned(sums, 4), "train_bn_relu_bwd_reduce: stat / sums must be 4-byte aligned");
+  return bn_bwd_reduce<kActRelu>(g, 0, y, npix, C, stat, sums, as_stream(stream));
+}
+
+extern "C" int cvb_train_bn_relu_bwd_apply(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, const float* sums,
+                                           const double* count, void* dy, void* stream) {
+  CVB_REQUIRE(g && y && stat && gamma && sums && count && dy, "train_bn_relu_bwd_apply: null pointer");
+  const int rc = check_bn_shape("train_bn_relu_bwd_apply", npix, C);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE(is_aligned(g, 16) && is_aligned(y, 16) && is_aligned(dy, 16), "train_bn_relu_bwd_apply: g / y / dy must be 16-byte aligned");
+  CVB_REQUIRE(is_aligned(stat, 4) && is_aligned(gamma, 4) && is_aligned(sums, 4) && is_aligned(count, 8),
+              "train_bn_relu_bwd_apply: stat / gamma / sums must be 4-byte, count 8-byte aligned");
+  return bn_bwd_apply<kActRelu>(g, 0, y, npix, C, stat, gamma, sums, count, dy, as_stream(stream));
+}
+
 // the identity branch's operands come together: all of (x, stat_id[, gamma_id, dx_id]) or none
 static int check_repvgg(const char* fn, int64_t npix, int32_t C, const void* x, const float* stat_id, const void* const* bf16s, int nb,
                         const float* const* f32s, int nf) {
@@ -1761,6 +1784,56 @@ extern "C" int cvb_train_repvgg_fwd(const void* y3, const void* y1, const void* 
   return CVB_OK;
 }
 
+// The two halves of the RepVGG backward, shared by the fused entry and the SyncBatchNorm split.  Arguments checked by the caller.
+static int repvgg_bwd_reduce(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C, const RepvggStats& s,
+                             float* sums, cudaStream_t st) {
+  CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 4 * (size_t)C * sizeof(float), st));
+  const int grid = red_grid(npix, kEwThreads / (C / 8));
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  const auto* bg = static_cast<const __nv_bfloat16*>(g);
+  const auto* ba = static_cast<const __nv_bfloat16*>(a);
+  const auto* b3 = static_cast<const __nv_bfloat16*>(y3);
+  const auto* b1 = static_cast<const __nv_bfloat16*>(y1);
+  if (x)
+    repvgg_bwd_reduce_kernel<true><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, static_cast<const __nv_bfloat16*>(x), npix, C, s, sums);
+  else
+    repvgg_bwd_reduce_kernel<false><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, npix, C, s, sums);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
+// count == nullptr: 1 / npix (this device's pixels); otherwise 1 / *count, the global count cvb_train_bn_merge left on the device
+static int repvgg_bwd_apply(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C, const RepvggStats& s,
+                            const float* gamma3, const float* gamma1, const float* gamma_id, const float* sums, const double* count, void* dy3,
+                            void* dy1, void* dx_id, cudaStream_t st) {
+  const long long nvec = npix * (C / 8);
+  const int grid = ew_grid(nvec);
+  if (grid == 0) return CVB_ERR_NO_DEVICE;
+  const auto* bg = static_cast<const __nv_bfloat16*>(g);
+  const auto* ba = static_cast<const __nv_bfloat16*>(a);
+  const auto* b3 = static_cast<const __nv_bfloat16*>(y3);
+  const auto* b1 = static_cast<const __nv_bfloat16*>(y1);
+  const auto* bx = static_cast<const __nv_bfloat16*>(x);
+  auto* d3 = static_cast<__nv_bfloat16*>(dy3);
+  auto* d1 = static_cast<__nv_bfloat16*>(dy1);
+  auto* dx = static_cast<__nv_bfloat16*>(dx_id);
+  const float inv_n = (float)(1.0 / (double)npix);
+  if (x && count)
+    repvgg_bwd_apply_kernel<true, true><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, nvec, C, s, gamma3, gamma1, gamma_id, sums, 0.0f, count, d3, d1, dx);
+  else if (x)
+    repvgg_bwd_apply_kernel<true, false><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, nvec, C, s, gamma3, gamma1, gamma_id, sums, inv_n, nullptr, d3, d1, dx);
+  else if (count)
+    repvgg_bwd_apply_kernel<false, true><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, nvec, C, s, gamma3, gamma1, nullptr, sums, 0.0f, count, d3, d1,
+                                                                      nullptr);
+  else
+    repvgg_bwd_apply_kernel<false, false><<<grid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, nvec, C, s, gamma3, gamma1, nullptr, sums, inv_n, nullptr, d3,
+                                                                       d1, nullptr);
+  CVB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return CVB_OK;
+}
+
 extern "C" int cvb_train_repvgg_bwd(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
                                     const float* stat3, const float* stat1, const float* stat_id, const float* gamma3, const float* gamma1,
                                     const float* gamma_id, float* sums, void* dy3, void* dy1, void* dx_id, void* stream) {
@@ -1772,31 +1845,36 @@ extern "C" int cvb_train_repvgg_bwd(const void* g, const void* a, const void* y3
   CVB_REQUIRE((x == nullptr) == (gamma_id == nullptr) && (x == nullptr) == (dx_id == nullptr),
               "train_repvgg_bwd: x, stat_id, gamma_id and dx_id go together (all NULL: no identity branch)");
   cudaStream_t st = as_stream(stream);
-  CVB_CHECK_CUDA(cudaMemsetAsync(sums, 0, 4 * (size_t)C * sizeof(float), st));
-  const int rgrid = red_grid(npix, kEwThreads / (C / 8));
-  const long long nvec = npix * (C / 8);
-  const int agrid = ew_grid(nvec);
-  if (rgrid == 0 || agrid == 0) return CVB_ERR_NO_DEVICE;
   const RepvggStats s{stat3, stat1, stat_id};
-  const auto* bg = static_cast<const __nv_bfloat16*>(g);
-  const auto* ba = static_cast<const __nv_bfloat16*>(a);
-  const auto* b3 = static_cast<const __nv_bfloat16*>(y3);
-  const auto* b1 = static_cast<const __nv_bfloat16*>(y1);
-  const auto* bx = static_cast<const __nv_bfloat16*>(x);
-  auto* d3 = static_cast<__nv_bfloat16*>(dy3);
-  auto* d1 = static_cast<__nv_bfloat16*>(dy1);
-  auto* dx = static_cast<__nv_bfloat16*>(dx_id);
-  const float inv_n = (float)(1.0 / (double)npix);
-  if (x) {
-    repvgg_bwd_reduce_kernel<true><<<rgrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, npix, C, s, sums);
-    repvgg_bwd_apply_kernel<true><<<agrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, bx, nvec, C, s, gamma3, gamma1, gamma_id, sums, inv_n, d3, d1, dx);
-  } else {
-    repvgg_bwd_reduce_kernel<false><<<rgrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, npix, C, s, sums);
-    repvgg_bwd_apply_kernel<false><<<agrid, kEwThreads, 0, st>>>(bg, ba, b3, b1, nullptr, nvec, C, s, gamma3, gamma1, nullptr, sums, inv_n, d3, d1, nullptr);
-  }
-  CVB_CHECK_CUDA(cudaGetLastError());
-  count_launch(2);
-  return CVB_OK;
+  const int r = repvgg_bwd_reduce(g, a, y3, y1, x, npix, C, s, sums, st);
+  return r != CVB_OK ? r : repvgg_bwd_apply(g, a, y3, y1, x, npix, C, s, gamma3, gamma1, gamma_id, sums, nullptr, dy3, dy1, dx_id, st);
+}
+
+// SyncBatchNorm halves of cvb_train_repvgg_bwd: one collective sums the [4][C] sums of all three branches over the ranks between them
+extern "C" int cvb_train_repvgg_bwd_reduce(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
+                                           const float* stat3, const float* stat1, const float* stat_id, float* sums, void* stream) {
+  CVB_REQUIRE(g && a && y3 && y1 && stat3 && stat1 && sums, "train_repvgg_bwd_reduce: null pointer");
+  const void* bf[] = {g, a, y3, y1, x};
+  const float* f32[] = {stat3, stat1, stat_id, sums};
+  const int rc = check_repvgg("train_repvgg_bwd_reduce", npix, C, x, stat_id, bf, 5, f32, 4);
+  if (rc != CVB_OK) return rc;
+  return repvgg_bwd_reduce(g, a, y3, y1, x, npix, C, RepvggStats{stat3, stat1, stat_id}, sums, as_stream(stream));
+}
+
+extern "C" int cvb_train_repvgg_bwd_apply(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
+                                          const float* stat3, const float* stat1, const float* stat_id, const float* gamma3, const float* gamma1,
+                                          const float* gamma_id, const float* sums, const double* count, void* dy3, void* dy1, void* dx_id,
+                                          void* stream) {
+  CVB_REQUIRE(g && a && y3 && y1 && stat3 && stat1 && gamma3 && gamma1 && sums && count && dy3 && dy1, "train_repvgg_bwd_apply: null pointer");
+  const void* bf[] = {g, a, y3, y1, x, dy3, dy1, dx_id};
+  const float* f32[] = {stat3, stat1, stat_id, gamma3, gamma1, gamma_id, sums};
+  const int rc = check_repvgg("train_repvgg_bwd_apply", npix, C, x, stat_id, bf, 8, f32, 7);
+  if (rc != CVB_OK) return rc;
+  CVB_REQUIRE((x == nullptr) == (gamma_id == nullptr) && (x == nullptr) == (dx_id == nullptr),
+              "train_repvgg_bwd_apply: x, stat_id, gamma_id and dx_id go together (all NULL: no identity branch)");
+  CVB_REQUIRE(is_aligned(count, 8), "train_repvgg_bwd_apply: count must be 8-byte aligned");
+  return repvgg_bwd_apply(g, a, y3, y1, x, npix, C, RepvggStats{stat3, stat1, stat_id}, gamma3, gamma1, gamma_id, sums, count, dy3, dy1, dx_id,
+                          as_stream(stream));
 }
 
 extern "C" int cvb_train_convt_scatter(const void* u, int32_t B, int32_t h, int32_t w, int32_t C, const float* bias, void* out, void* stream) {

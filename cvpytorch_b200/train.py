@@ -176,39 +176,40 @@ def bn_stats(y, gamma, beta, running_mean, running_var, eps, momentum):
     return stat, g32
 
 
-def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None, act='silu'):
-    """a = act(bn_train(conv(x, weight))) (act 'silu', or 'relu' without a process group) -> (a, (y, stat, g32, wb), count): what
-    _bn_silu_backward / _bn_relu_backward and the backward convolutions need (the conv output, the BN statistics, fp32 gamma and the
-    backward-data weights) and, with a process group (SyncBatchNorm), the global pixel count on the device (None otherwise).  Updates the
-    running statistics."""
-    cout = weight.shape[0]
+def batch_stats(y, gamma, beta, running_mean, running_var, eps, momentum, group=None):
+    """bn_stats over this device's pixels (group None) or, with a process group (SyncBatchNorm), over every rank's -> (stat, fp32 gamma,
+    count): count is the global pixel count, fp64 [1] on the device, with a process group (None otherwise).  Updates the running statistics."""
+    if group is None:
+        return (*bn_stats(y, gamma, beta, running_mean, running_var, eps, momentum), None)
     L = _lib.lib()
+    C = y.shape[-1]
+    npix = y.numel() // C
+    stat = torch.empty((4, C), dtype=torch.float32, device=y.device)
+    scratch = torch.empty((2, C), dtype=torch.float32, device=y.device)
+    g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
+    # every rank's (mean, M2, count) record, gathered in rank order and merged on the device
+    world = dist.get_world_size(group)
+    rec = torch.empty((2 * C + 1,), dtype=torch.float64, device=y.device)
+    _lib.check(L.cvb_train_bn_partial(_p(y), npix, C, _p(scratch), _p(rec), _stream()), 'cvb_train_bn_partial')
+    recs = torch.empty((world * (2 * C + 1),), dtype=torch.float64, device=y.device)  # (flat: gloo's all-gather wants world x the input)
+    dist.all_gather_into_tensor(recs, rec, group=group)
+    count = torch.empty((1,), dtype=torch.float64, device=y.device)
+    _lib.check(L.cvb_train_bn_merge(_p(recs), world, C, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
+                                    _p(stat), _p(count), _stream()), 'cvb_train_bn_merge')
+    return stat, g32, count
+
+
+def _conv_bn_silu(x, weight, gamma, beta, running_mean, running_var, eps, momentum, group, k, stride=1, pad=None, act='silu'):
+    """a = act(bn_train(conv(x, weight))) (act 'silu' or 'relu') -> (a, (y, stat, g32, wb), count): what _bn_silu_backward /
+    _bn_relu_backward and the backward convolutions need (the conv output, the BN statistics, fp32 gamma and the backward-data weights)
+    and, with a process group (SyncBatchNorm), the global pixel count on the device (None otherwise).  Updates the running statistics."""
+    cout = weight.shape[0]
     wf, wb = pack_weights(weight)
     y = conv(x, wf, cout, k, stride=stride, pad=pad)
-    if act == 'relu':
-        stat, g32 = bn_stats(y, gamma, beta, running_mean, running_var, eps, momentum)
-        a = torch.empty_like(y)
-        _lib.check(L.cvb_train_bn_relu_fwd(_p(y), y.numel() // cout, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_relu_fwd')
-        return a, (y, stat, g32, wb), None
-    npix = y.shape[0] * y.shape[1] * y.shape[2]
-    stat = torch.empty((4, cout), dtype=torch.float32, device=x.device)
-    scratch = torch.empty((2, cout), dtype=torch.float32, device=x.device)
-    g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-    count = None
-    if group is None:
-        _lib.check(L.cvb_train_bn_stats(_p(y), npix, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
-                                        _p(scratch), _p(stat), _stream()), 'cvb_train_bn_stats')
-    else:  # every rank's (mean, M2, count) record, gathered in rank order and merged on the device
-        world = dist.get_world_size(group)
-        rec = torch.empty((2 * cout + 1,), dtype=torch.float64, device=x.device)
-        _lib.check(L.cvb_train_bn_partial(_p(y), npix, cout, _p(scratch), _p(rec), _stream()), 'cvb_train_bn_partial')
-        recs = torch.empty((world * (2 * cout + 1),), dtype=torch.float64, device=x.device)  # (flat: gloo's all-gather wants world x the input)
-        dist.all_gather_into_tensor(recs, rec, group=group)
-        count = torch.empty((1,), dtype=torch.float64, device=x.device)
-        _lib.check(L.cvb_train_bn_merge(_p(recs), world, cout, _p(g32), _p(b32), float(eps), float(momentum), _p(running_mean), _p(running_var),
-                                        _p(stat), _p(count), _stream()), 'cvb_train_bn_merge')
+    stat, g32, count = batch_stats(y, gamma, beta, running_mean, running_var, eps, momentum, group)
     a = torch.empty_like(y)
-    _lib.check(L.cvb_train_bn_silu_fwd(_p(y), npix, cout, _p(stat), _p(a), _stream()), 'cvb_train_bn_silu_fwd')
+    fwd = 'cvb_train_bn_relu_fwd' if act == 'relu' else 'cvb_train_bn_silu_fwd'
+    _lib.check(getattr(_lib.lib(), fwd)(_p(y), y.numel() // cout, cout, _p(stat), _p(a), _stream()), fwd)
     return a, (y, stat, g32, wb), count
 
 
@@ -233,14 +234,23 @@ def _bn_silu_backward(g, g_is_dz, y, stat, g32, group=None, count=None):
     return dy, dgamma, dbeta
 
 
-def _bn_relu_backward(g, y, stat, g32):
-    """g = d(loss)/d(a), a = relu(bn(y)) -> (dy, dgamma, dbeta)."""
+def _bn_relu_backward(g, y, stat, g32, group=None, count=None):
+    """g = d(loss)/d(a), a = relu(bn(y)) -> (dy, dgamma, dbeta).  With a process group (SyncBatchNorm): as _bn_silu_backward."""
     g = g.contiguous()
     cout = y.shape[3]
+    npix = y.numel() // cout
+    L = _lib.lib()
     sums = torch.empty((2, cout), dtype=torch.float32, device=y.device)
     dy = torch.empty_like(y)
-    _lib.check(_lib.lib().cvb_train_bn_relu_bwd(_p(g), _p(y), y.numel() // cout, cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()), 'cvb_train_bn_relu_bwd')
-    return dy, sums[1].clone(), sums[0].clone()
+    if group is None:
+        _lib.check(L.cvb_train_bn_relu_bwd(_p(g), _p(y), npix, cout, _p(stat), _p(g32), _p(sums), _p(dy), _stream()), 'cvb_train_bn_relu_bwd')
+        return dy, sums[1].clone(), sums[0].clone()
+    _lib.check(L.cvb_train_bn_relu_bwd_reduce(_p(g), _p(y), npix, cout, _p(stat), _p(sums), _stream()), 'cvb_train_bn_relu_bwd_reduce')
+    dgamma, dbeta = sums[1].clone(), sums[0].clone()
+    dist.all_reduce(sums, group=group)
+    _lib.check(L.cvb_train_bn_relu_bwd_apply(_p(g), _p(y), npix, cout, _p(stat), _p(g32), _p(sums), _p(count), _p(dy), _stream()),
+               'cvb_train_bn_relu_bwd_apply')
+    return dy, dgamma, dbeta
 
 
 class _ConvBnSiLU(torch.autograd.Function):
@@ -262,7 +272,7 @@ class _ConvBnSiLU(torch.autograd.Function):
         k = ctx.k
         B, H, W, cin = x.shape
         if ctx.act == 'relu':
-            dy, dgamma, dbeta = _bn_relu_backward(da, y, stat, g32)
+            dy, dgamma, dbeta = _bn_relu_backward(da, y, stat, g32, ctx.group, ctx.count)
         else:
             dy, dgamma, dbeta = _bn_silu_backward(da, False, y, stat, g32, ctx.group, ctx.count)
         dw = conv_wgrad(x, dy, k, ctx.stride, ctx.pad)

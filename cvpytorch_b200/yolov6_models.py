@@ -25,7 +25,7 @@ the NMS pre-pass, after which the YOLOv5 NMS (ops.yolo_nms, hist_ready) selects 
 import torch
 import torch.nn as nn
 
-from . import ops, train, yolov6_train
+from . import ops, yolov6_train
 from .engine import GraphBuilder
 from .models import _YoloModel
 from .modules import ConvModule, _build, _EmitModule, _Standalone, folded
@@ -424,8 +424,6 @@ class YOLOv6(_YoloModel):
         """The reference's training forward on the H100 training kernels -> {'iou', 'dfl', 'class', 'loss'} (fp64 device scalars, no host sync)."""
         if not imgs.is_cuda:
             raise NotImplementedError("YOLOv6 (H100): mode='train' has no CPU fallback: pass CUDA images")
-        if any(train._sync_group(m) is not None for m in self.modules() if isinstance(m, nn.SyncBatchNorm)):
-            raise NotImplementedError('YOLOv6 (H100) training: BatchNorm statistics over several ranks (nn.SyncBatchNorm) are not on the training path')
         return super().forward_train(imgs, targets)
 
     def _loss_step(self, outputs, gt):

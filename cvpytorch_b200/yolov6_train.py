@@ -18,8 +18,14 @@ cvb_train_bn_stats and one pass sums the branches and applies ReLU (cvb_train_re
 of a 3x3 / stride-2 / pad-1 conv: its weight is zero-padded in torch, so autograd returns the 1x1 gradient.  The stem RepVGGBlock(3, c,
 stride 2) runs over train.focus_s2d's map with both branch weights remapped in torch (stem_weight_to_s2d).  BiFusion's transposed conv is a
 1x1 GEMM of 4c columns followed by cvb_train_convt_scatter; its backward gathers d(out) back (cvb_train_convt_gather).  YOLOv6-n's
-96-channel bifusion1.cv3 input is zero-padded to 128 channels, and so is its weight (autograd slices the gradient).  BatchNorms that span
-several ranks (nn.SyncBatchNorm) raise NotImplementedError.
+96-channel bifusion1.cv3 input is zero-padded to 128 channels, and so is its weight (autograd slices the gradient).
+
+nn.SyncBatchNorm (convert_sync_batchnorm, as the reference trainer does under cfg.distributed) normalises over every rank of its process
+group, decided at every forward by train._sync_group.  A ReLU ConvModule takes train._conv_bn_silu's record -> all-gather -> merge path and
+cvb_train_bn_relu_bwd_reduce -> all-reduce -> _apply.  A RepVGG block gathers and merges one record per branch (the identity branch's on the
+block input) and all-reduces one [4][C] buffer in backward (cvb_train_repvgg_bwd_reduce / _apply); its three BatchNorms must all be local
+or all share one process group, otherwise it raises NotImplementedError.  Without a process group (or in a world of one) the step issues
+the same launches as with nn.BatchNorm2d.
 
 The loss: head outputs are cast with .float().contiguous(), so fp16 / bf16 outputs under autocast work and their
 gradients flow back through the cast.  The reference returns {'iou': 2.5 L, 'dfl': 0.5 L, 'class': 1.0 L} of its box loss L (its class
@@ -30,12 +36,13 @@ raises); a level with fewer than 9 anchors takes all of them as ATSS candidates 
 boundary the lowest anchor index wins (torch.topk's order is undefined).
 """
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib, train
 from .train import (_bn_momentum, _check_cuda, _ConvBnSiLULayer, _p, _require_training, _require_widths, _set_bn, _SppfChain, _stream, _sync_group,
-                    _workspace, bn_stats, conv, conv_dgrad_s2, conv_wgrad, focus_s2d, pack_weights)
+                    _workspace, batch_stats, conv, conv_dgrad_s2, conv_wgrad, focus_s2d, pack_weights)
 from .yolov5_train import _PredConv
 
 LOSS_WEIGHT = {'class': 1.0, 'iou': 2.5, 'dfl': 0.5}
@@ -153,10 +160,9 @@ _WIDTHS = 'channels must be 16, 32 or multiples of 64'
 
 
 def _bn_args(bn):
-    """Counts the step -> (running_mean, running_var, eps, momentum) of a BatchNorm with batch statistics on this device's pixels."""
-    if _sync_group(bn) is not None:
-        raise NotImplementedError('YOLOv6 (H100) training: BatchNorm statistics over several ranks (nn.SyncBatchNorm) are not on the training path')
-    return bn.running_mean, bn.running_var, bn.eps, _bn_momentum(bn)
+    """Counts the step -> (running_mean, running_var, eps, momentum, process group) of a BatchNorm with batch statistics: the group whose
+    ranks' pixels it normalises over (train._sync_group), or None (this device's pixels)."""
+    return bn.running_mean, bn.running_var, bn.eps, _bn_momentum(bn), _sync_group(bn)
 
 
 def stem_weight_to_s2d(w):
@@ -177,36 +183,53 @@ def stem_weight_to_s2d(w):
 _S2D_INDEX = {}
 
 
-def repvgg_forward(x, w3, w1, bn3, bn1, bnid, stride):
-    """a = relu(bn3(conv3x3(x, w3)) + bn1(conv(x, w1)) [+ bnid(x)]) with batch statistics -> (a, saved tensors of repvgg_backward).  w1 is
-    [cout, cin, 1, 1], or 3x3 (the zero-padded stride-2 1x1 branch).  bn*: (gamma, beta, running_mean, running_var, eps, momentum); bnid None:
-    no identity branch.  Updates the running statistics."""
+def repvgg_forward(x, w3, w1, bn3, bn1, bnid, stride, group=None):
+    """a = relu(bn3(conv3x3(x, w3)) + bn1(conv(x, w1)) [+ bnid(x)]) with batch statistics -> (a, saved tensors of repvgg_backward, count).
+    w1 is [cout, cin, 1, 1], or 3x3 (the zero-padded stride-2 1x1 branch).  bn*: (gamma, beta, running_mean, running_var, eps, momentum);
+    bnid None: no identity branch.  group: the process group of all three BatchNorms (SyncBatchNorm: each branch's statistics span its
+    ranks, and count is the global pixel count on the device, which the branches share), or None (this device's pixels; count None).
+    Updates the running statistics."""
     B, H, W, cin = x.shape
     cout = w3.shape[0]
     wf3, wb3 = pack_weights(w3)
     wf1, wb1 = pack_weights(w1)
     y3 = conv(x, wf3, cout, 3, stride=stride)
     y1 = conv(x, wf1, cout, w1.shape[2], stride=stride)
-    st3, g3 = bn_stats(y3, *bn3)
-    st1, g1 = bn_stats(y1, *bn1)
-    stid, gid = bn_stats(x, *bnid) if bnid is not None else (None, None)
+    st3, g3, count = batch_stats(y3, *bn3, group)
+    st1, g1, _ = batch_stats(y1, *bn1, group)
+    stid, gid, _ = batch_stats(x, *bnid, group) if bnid is not None else (None, None, None)
     a = torch.empty_like(y3)
     _lib.check(_lib.lib().cvb_train_repvgg_fwd(_p(y3), _p(y1), _p(x) if bnid is not None else None, a.numel() // cout, cout, _p(st3), _p(st1), _p(stid),
                                                _p(a), _stream()), 'cvb_train_repvgg_fwd')
-    return a, (y3, y1, st3, st1, stid, g3, g1, gid, wb3, wb1)
+    return a, (y3, y1, st3, st1, stid, g3, g1, gid, wb3, wb1), count
 
 
-def repvgg_backward(g, x, a, saved, need_dx, stride):
-    """g = d(loss)/d(a) -> (dx or None, dw3, dw1, dgamma3, dgamma1, dgamma_id or None, dbeta): dbeta is every branch's beta gradient."""
+def repvgg_backward(g, x, a, saved, need_dx, stride, group=None, count=None):
+    """g = d(loss)/d(a) -> (dx or None, dw3, dw1, dgamma3, dgamma1, dgamma_id or None, dbeta): dbeta is every branch's beta gradient.  With
+    a process group (SyncBatchNorm): dgamma and dbeta stay this rank's sums (DDP averages them like every other gradient); the dy of every
+    branch takes the sums over every rank (one all-reduce of the [4][C] sums) and the forward's global pixel count `count`."""
     y3, y1, st3, st1, stid, g3, g1, gid, wb3, wb1 = saved
     B, H, W, cin = x.shape
     cout = y3.shape[3]
+    npix = a.numel() // cout
     ident = stid is not None
+    L = _lib.lib()
+    g = g.contiguous()
     sums = torch.empty((4, cout), dtype=torch.float32, device=x.device)
     dy3, dy1 = torch.empty_like(y3), torch.empty_like(y1)
     dxid = torch.empty_like(x) if ident else None
-    _lib.check(_lib.lib().cvb_train_repvgg_bwd(_p(g.contiguous()), _p(a), _p(y3), _p(y1), _p(x) if ident else None, a.numel() // cout, cout, _p(st3), _p(st1),
-                                               _p(stid), _p(g3), _p(g1), _p(gid), _p(sums), _p(dy3), _p(dy1), _p(dxid), _stream()), 'cvb_train_repvgg_bwd')
+    xid = _p(x) if ident else None
+    if group is None:
+        _lib.check(L.cvb_train_repvgg_bwd(_p(g), _p(a), _p(y3), _p(y1), xid, npix, cout, _p(st3), _p(st1), _p(stid), _p(g3), _p(g1), _p(gid), _p(sums),
+                                          _p(dy3), _p(dy1), _p(dxid), _stream()), 'cvb_train_repvgg_bwd')
+        local = sums
+    else:
+        _lib.check(L.cvb_train_repvgg_bwd_reduce(_p(g), _p(a), _p(y3), _p(y1), xid, npix, cout, _p(st3), _p(st1), _p(stid), _p(sums), _stream()),
+                   'cvb_train_repvgg_bwd_reduce')
+        local = sums.clone()
+        dist.all_reduce(sums, group=group)
+        _lib.check(L.cvb_train_repvgg_bwd_apply(_p(g), _p(a), _p(y3), _p(y1), xid, npix, cout, _p(st3), _p(st1), _p(stid), _p(g3), _p(g1), _p(gid),
+                                                _p(sums), _p(count), _p(dy3), _p(dy1), _p(dxid), _stream()), 'cvb_train_repvgg_bwd_apply')
     k1 = 3 if wb1.shape[1] == 9 else 1  # (the stride-2 1x1 branch runs as a zero-padded 3x3)
     dw3 = conv_wgrad(x, dy3, 3, stride)
     dw1 = conv_wgrad(x, dy1, k1, stride)
@@ -218,26 +241,27 @@ def repvgg_backward(g, x, a, saved, need_dx, stride):
             dx = conv(dy3, wb3, cin, 3) + conv(dy1, wb1, cin, k1)
             if ident:
                 dx = dx + dxid
-    return dx, dw3, dw1, sums[1].clone(), sums[2].clone(), sums[3].clone() if ident else None, sums[0]
+    return dx, dw3, dw1, local[1].clone(), local[2].clone(), local[3].clone() if ident else None, local[0]
 
 
 class _RepVGG(torch.autograd.Function):
     """One RepVGG block in training form (forward: repvgg_forward, backward: repvgg_backward).  meta = (running statistics, eps and momentum
-    of the three BatchNorms (None: no identity branch), stride)."""
+    of the three BatchNorms (None: no identity branch), stride, process group of the block's BatchNorms or None)."""
 
     @staticmethod
     def forward(ctx, x, w3, w1, g3, b3, g1, b1, gid, bid, meta):
         _check_cuda(x, 'RepVGGBlock (H100 training)')
-        m3, m1, mid, stride = meta
-        a, saved = repvgg_forward(x, w3, w1, (g3, b3, *m3), (g1, b1, *m1), (gid, bid, *mid) if mid is not None else None, stride)
+        m3, m1, mid, stride, group = meta
+        a, saved, count = repvgg_forward(x, w3, w1, (g3, b3, *m3), (g1, b1, *m1), (gid, bid, *mid) if mid is not None else None, stride, group)
         ctx.save_for_backward(x, a, *saved)
         ctx.stride, ctx.need_dx = stride, x.requires_grad
+        ctx.group, ctx.count = group, count
         return a
 
     @staticmethod
     def backward(ctx, g):
         x, a, *saved = ctx.saved_tensors
-        dx, dw3, dw1, dg3, dg1, dgid, dbeta = repvgg_backward(g, x, a, saved, ctx.need_dx, ctx.stride)
+        dx, dw3, dw1, dg3, dg1, dgid, dbeta = repvgg_backward(g, x, a, saved, ctx.need_dx, ctx.stride, ctx.group, ctx.count)
         return dx, dw3, dw1, dg3, dbeta.clone(), dg1, dbeta.clone(), dgid, dbeta.clone() if dgid is not None else None, None
 
 
@@ -276,7 +300,15 @@ class RepVGGBlock(nn.Module):
     def _block(self, x, w3, w1, stride):
         _require_training(self, 'cvpytorch_b200.yolov6_train.RepVGGBlock is the TRAINING drop-in (batch statistics); use the inference modules for eval()')
         bn3, bn1, bnid = self.rbr_dense.bn, self.rbr_1x1.bn, self.rbr_identity
-        meta = (_bn_args(bn3), _bn_args(bn1), _bn_args(bnid) if bnid is not None else None, stride)
+        groups = {'rbr_dense.bn': _sync_group(bn3), 'rbr_1x1.bn': _sync_group(bn1)}
+        if bnid is not None:
+            groups['rbr_identity'] = _sync_group(bnid)
+        group = groups['rbr_dense.bn']
+        if any(g is not group for g in groups.values()):
+            raise NotImplementedError(f'H100 training RepVGGBlock({self.in_channels}, {self.out_channels}, stride {self.stride}): its BatchNorms must all '
+                                      'be local or all span the same process group (convert_sync_batchnorm converts all three); got ' +
+                                      ', '.join(f'{k}: {"local" if g is None else "synced"}' for k, g in groups.items()))
+        meta = tuple(_bn_args(bn)[:4] if bn is not None else None for bn in (bn3, bn1, bnid)) + (stride, group)
         return _RepVGG.apply(x, w3, w1, bn3.weight, bn3.bias, bn1.weight, bn1.bias, bnid.weight if bnid is not None else None,
                              bnid.bias if bnid is not None else None, meta)
 
@@ -335,10 +367,6 @@ class ConvModule(_ConvBnSiLULayer):
         _require_widths((in_channels + in_pad, out_channels), lambda bad: f'H100 training ConvModule: {_WIDTHS} (got {in_channels} -> {out_channels})')
         super().__init__(in_channels, out_channels, kernel_size, stride)
         self.in_pad = in_pad
-
-    def _bn_inputs(self):
-        bn = self.bn
-        return (bn.weight, bn.bias, *_bn_args(bn), None)
 
     def forward(self, x):
         w = self.conv.weight

@@ -486,6 +486,15 @@ int cvb_train_convt_gather(const void* g, int32_t B, int32_t h, int32_t w, int32
  * cvb_train_bn_silu_bwd_reduce: the first half of cvb_train_bn_silu_bwd: sums [2][C] = this rank's (dbeta, dgamma).
  * cvb_train_bn_silu_bwd_apply: the second half, from the sums summed over every rank and N = *count (device fp64, e.g. cvb_train_bn_merge's):
  *   dy = gamma * rstd * (dz - sums[0] / N - xhat * sums[1] / N).
+ * cvb_train_bn_relu_bwd_reduce / _apply: the same two halves of cvb_train_bn_relu_bwd (dz = g where the forward's fp32 fmaf(y, scale, shift)
+ *   is > 0).  Operands as cvb_train_bn_relu_bwd; count fp64 [1], 8-byte aligned.  1 / N is the fp32 rounding of the fp64 1.0 / *count, the
+ *   expression of the fused entry with N = npix, so an apply fed the fused entry's sums and count = npix writes its dy bit for bit.
+ * cvb_train_repvgg_bwd_reduce: the first half of cvb_train_repvgg_bwd: sums [4][C] = this rank's (sum dz, sum dz * xhat3, sum dz * xhat1,
+ *   sum dz * xhatid; the last row 0 without the identity branch).  stat3 / stat1 / stat_id: the merged statistics of each branch (three
+ *   cvb_train_bn_partial -> all-gather -> cvb_train_bn_merge sequences; the identity branch's on the block input x).  One all-reduce of
+ *   the [4][C] sums then serves all three branches.
+ * cvb_train_repvgg_bwd_apply: the second half, from the sums summed over every rank and N = *count (the branches of a block share one
+ *   pixel count): dy3, dy1, dx_id as cvb_train_repvgg_bwd.  x, stat_id, gamma_id and dx_id are all NULL without the identity branch.
  */
 int cvb_train_bn_partial(const void* y, int64_t npix, int32_t C, float* sums_scratch, double* record, void* stream);
 int cvb_train_bn_merge(const double* records, int32_t world, int32_t C, const float* gamma, const float* beta, float eps, float momentum,
@@ -493,6 +502,14 @@ int cvb_train_bn_merge(const double* records, int32_t world, int32_t C, const fl
 int cvb_train_bn_silu_bwd_reduce(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream);
 int cvb_train_bn_silu_bwd_apply(const void* g, int32_t g_is_dz, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma,
                                 const float* sums, const double* count, void* dy, void* stream);
+int cvb_train_bn_relu_bwd_reduce(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, float* sums, void* stream);
+int cvb_train_bn_relu_bwd_apply(const void* g, const void* y, int64_t npix, int32_t C, const float* stat, const float* gamma, const float* sums,
+                                const double* count, void* dy, void* stream);
+int cvb_train_repvgg_bwd_reduce(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
+                                const float* stat3, const float* stat1, const float* stat_id, float* sums, void* stream);
+int cvb_train_repvgg_bwd_apply(const void* g, const void* a, const void* y3, const void* y1, const void* x, int64_t npix, int32_t C,
+                               const float* stat3, const float* stat1, const float* stat_id, const float* gamma3, const float* gamma1,
+                               const float* gamma_id, const float* sums, const double* count, void* dy3, void* dy1, void* dx_id, void* stream);
 
 /* YOLOX training loss (src/losses/det/yolox_loss.py:73-436; csrc/yolox_loss.cu): SimOTA assignment, the IoU / objectness / class losses
  * and their gradient with respect to the head outputs.  preds[l]: fp32 NCHW [B, 5 + nc, h_l, w_l] (read in place), shapes[4 l ..] =
